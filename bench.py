@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- masked-token train step (MaskGitTransformer base-256) on N B200s, one JSON line on rank 0.
+"""bench.py -- masked-token train step (MaskGitTransformer base-256) on N H100s, one JSON line on rank 0.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -56,7 +56,7 @@ def mask_batch(tokens, class_ids, mask_id, codebook, gen=None):
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons while the timed region runs (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons while the timed region runs."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -100,25 +100,19 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def gemm_traffic_from_profile():
-    """Average DRAM bytes (read + write) per tcgen05-GEMM launch from the committed `ncu --set full` capture of the step's
-    GEMMs (profiles/r02_ncu_kernels.txt: one line per captured launch, sizes in GB / MB), or None."""
-    path = os.path.join(ROOT, "profiles", "r02_ncu_kernels.txt")
-    if not os.path.exists(path):
-        return None
-    tot, n = 0.0, 0
-    for line in open(path):
-        if not line.startswith("gemm_tcgen05_kernel"):
-            continue
-        try:
-            rd = line.split("dram_read=")[1].split()[0]
-            wr = line.split("dram_write=")[1].split()[0]
-            unit = lambda v: float(v[:-2]) * {"GB": 1e9, "MB": 1e6, "KB": 1e3}[v[-2:]]
-            tot += unit(rd) + unit(wr)
-            n += 1
-        except Exception:
-            pass
-    return tot / n if n else None
+def dump_outputs(out_dir, loss, model, per_tensor=4096):
+    """The loss of the last timed step and, for every parameter, the same seeded sample of at most `per_tensor` entries of
+    its updated value (a few MB in all), so that two builds can be compared output for output."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss)], dtype=np.float32))
+    g = torch.Generator().manual_seed(0)
+    for name, p in model.named_parameters():
+        flat = p.detach().float().reshape(-1)
+        n = flat.numel()
+        idx = torch.randperm(n, generator=g)[:per_tensor].sort().values if n > per_tensor else torch.arange(n)
+        np.save(os.path.join(out_dir, f"param.{name}.npy"), flat[idx.to(flat.device)].cpu().numpy())
 
 
 def measured_peaks():
@@ -126,7 +120,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", d.get("bf16_tflops")), d.get("hbm_gbs"), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md: ~1.4 PF sustained, 6.65 TB/s)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
 def reference_kind():
@@ -165,7 +159,7 @@ def reference_module_step_fn(batch, device="cpu"):
 def cpu_reference_step_fn(batch, device="cpu"):
     """The reference arm's step: the unmodified reference modules when the oracle/_ref snapshot is present, else the
     oracle port (same torch op sequence, fp32 eager): fwd + bwd + AdamW on `batch` samples.  With device="cuda" the same
-    eager ops run under bf16 autocast on the GPU -- what the reference executes on this B200 (the real bar)."""
+    eager ops run under bf16 autocast on the GPU -- what the reference executes on this GPU (the real bar)."""
     if reference_kind() == "reference":
         return reference_module_step_fn(batch, device)
     from oracle import transformer_oracle as T
@@ -247,14 +241,14 @@ def _timeit(fn, n=10, warm=3):
 
 def kernel_rooflines(dev, peak_tf, peak_hbm):
     """Every named kernel of the hot path timed alone at its BASELINE-config shape (CUDA events on the launching stream,
-    inputs >> L2 or freshly produced), with its ALGORITHMIC bytes / FLOPs (DESIGN.md section 4) against the measured
-    peaks.  The ncu --set full captures of the same launches are committed under profiles/ (r02_ncu_kernels.txt)."""
+    inputs >> L2 or freshly produced), with its ALGORITHMIC bytes / FLOPs (DESIGN.md section 4) against the peaks
+    given."""
     from open_muse_b200 import ops
 
     B, S, H, I, nh = 256, 257, 512, 2048, 8
     T = B * S
     out = []
-    FP32_SIMT_TF = 148 * 128 * 2 * 1.965e9 / 1e12  # 148 SMs x 128 FMA lanes at the max SM clock
+    FP32_SIMT_TF = 132 * 128 * 2 * 1.98e9 / 1e12  # H100 SXM: 132 SMs x 128 FMA lanes at the max SM clock
 
     def add(name, ms, nbytes=None, flops=None, bound=None, peak=None):
         if nbytes is not None:
@@ -316,9 +310,9 @@ def kernel_rooflines(dev, peak_tf, peak_hbm):
         wt, xin, dyy = bf(N, K), bf(T, K), bf(T, N)
         res = torch.randn(T, N, device=dev) if "residual" in name else None
         f = 2.0 * T * N * K
-        add(f"gemm_tcgen05_kernel fwd {name} [T,{K}]x[{N},{K}]", _timeit(lambda: ops.linear_fwd(xin, wt, res=res)), flops=f)
-        add(f"gemm_tcgen05_kernel dgrad {name}", _timeit(lambda: ops.linear_dgrad(dyy, wt)), flops=f)
-        add(f"gemm_tcgen05_kernel wgrad {name} (deterministic split-K)", _timeit(lambda: ops.linear_wgrad_det(dyy, xin)), flops=f)
+        add(f"gemm_wgmma_kernel fwd {name} [T,{K}]x[{N},{K}]", _timeit(lambda: ops.linear_fwd(xin, wt, res=res)), flops=f)
+        add(f"gemm_wgmma_kernel dgrad {name}", _timeit(lambda: ops.linear_dgrad(dyy, wt)), flops=f)
+        add(f"gemm_wgmma_kernel wgrad {name} (deterministic split-K)", _timeit(lambda: ops.linear_wgrad_det(dyy, xin)), flops=f)
         del wt, xin, dyy, res
     # ---- tokenizer search and the decode-step kernel
     n = 128 * 256
@@ -418,7 +412,7 @@ def secondary_metrics(dev, base_model, peak_tf, peak_hbm):
                               "decode_images_per_s": 128 / (ms_dec * 1e-3),
                               "model_tflops": (128.76 + 186.55) * 128 / (ms_enc + ms_dec),
                               "config": "MaskGitVQGAN f16-256 (class defaults) encode -> ids -> decode_code, fp32-faithful bf16x3 "
-                                        "tcgen05 convolutions, bit-exact arg-min"}
+                                        "wgmma convolutions, bit-exact arg-min"}
     del vq, pix
     torch.cuda.empty_cache()
     # ---- the reference recipe in torch eager on this GPU (bf16 autocast): what the unmodified reference runs here
@@ -435,7 +429,7 @@ def secondary_metrics(dev, base_model, peak_tf, peak_hbm):
         out["torch_eager_same_gpu"] = {"value": PER_GPU_BATCH / dt, "unit": "images/s", "ms_per_step": dt * 1e3,
                                        "kind": reference_kind(),
                                        "config": "the reference train step (fwd + bwd + AdamW, bf16 autocast, cuBLAS/ATen kernels) "
-                                                 f"at batch {PER_GPU_BATCH} on this B200"}
+                                                 f"at batch {PER_GPU_BATCH} on this GPU"}
         del rstep
     except Exception as e:  # informational leg: never sinks the bench line
         out["torch_eager_same_gpu"] = {"error": f"{type(e).__name__}: {e}"}
@@ -475,6 +469,9 @@ def main():
                     help="torch.optim.AdamW(fused=True) or open_muse_b200.FusedAdamW (AdamW + bf16 operand packing in one pass)")
     ap.add_argument("--pdl", type=int, default=None, choices=[0, 1],
                     help="programmatic dependent launch for the library's kernels (default: the library's own default / MUSE_B200_PDL)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (its loss and a fixed, seeded "
+                         "sample of every updated parameter) as float32 DIR/<name>.npy")
     ap.add_argument("--ref-device", default="cpu", choices=["cpu", "cuda"],
                     help="--impl reference only: cpu (the reference arm) or cuda (same eager ops under bf16 autocast, informational)")
     args = ap.parse_args()
@@ -498,7 +495,7 @@ def main():
             os.environ["TORCH_NCCL_ASYNC_ERROR_HANDLING"] = "0"
         if args.nccl_sms > 0:
             # the gradient all-reduce needs ~11 GB/s here (144 MB per 13 ms of backward): a few NCCL channels (= CTAs = SMs)
-            # are plenty on NVLink 5, and the persistent GEMMs give exactly those SMs up instead of stalling behind them
+            # are plenty over NVLink, and the persistent GEMMs give exactly those SMs up instead of stalling behind them
             os.environ.setdefault("NCCL_MAX_NCHANNELS", str(args.nccl_sms))
             os.environ.setdefault("NCCL_MIN_NCHANNELS", str(min(2, args.nccl_sms)))
             ops.reserve_sms(args.nccl_sms)
@@ -600,6 +597,7 @@ def main():
     loss_host = [torch.empty((), dtype=torch.float32).pin_memory() for _ in range(2)]
     loss_evt = [torch.cuda.Event() for _ in range(2)]
     seen = []
+    last_loss = [None]
 
     # inputs: step i+1's tokens are copied host -> device on a copy stream (two staging slots) while step i computes
     copy_stream = torch.cuda.Stream()
@@ -622,6 +620,7 @@ def main():
         k = i & 1
         torch.cuda.current_stream().wait_event(staged[k])
         loss = run(stage[k][0], stage[k][1])
+        last_loss[0] = loss
         consumed[k].record()
         if i + 1 < args.steps:
             prefetch(i + 1)
@@ -639,9 +638,11 @@ def main():
     ms_e2e = timed(e2e_step, args.steps)
     assert len(seen) == args.steps and all(math.isfinite(v) for v in seen), seen
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss[0], model)
     model._packed.key = None  # graph replays update the parameters without bumping their version counters: re-pack for eager use
 
-    # ---- roofline of the dominant kernel (tcgen05 GEMM), measured live with CUDA events around every launch
+    # ---- roofline of the dominant kernel (wgmma GEMM), measured live with CUDA events around every launch
     peak_tf, peak_hbm, peak_src = measured_peaks()
     ops.profile_gemms(True)
     for i in range(2):
@@ -651,9 +652,9 @@ def main():
     roof = None
     if gemm_n:
         ach = gemm_flops / (gemm_ms * 1e-3) / 1e12
-        roof = {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all Linear fwd/dgrad/wgrad GEMMs of the step)",
+        roof = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all Linear fwd/dgrad/wgrad GEMMs of the step)",
                 "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
-                "traffic": gemm_traffic_from_profile(), "algorithmic_flops_per_launch": gemm_flops / gemm_n,
+                "algorithmic_flops_per_launch": gemm_flops / gemm_n,
                 "peak_source": peak_src, "launches_per_step": gemm_n // 2,
                 "gemm_share_of_step": (gemm_ms / 2) / ms_dev}
 
@@ -679,7 +680,7 @@ def main():
         ms_enc = timed(lambda i: tokenise(), 3)
         full = {"value": B / (ms_full * 1e-3), "unit": "images/s", "ms_per_step": ms_full, "vq_encode_ms": ms_enc,
                 "vq_encode_images_per_s": B / (ms_enc * 1e-3),
-                "note": "pixels resident in HBM -> MaskGitVQGAN f16-256 get_code (fp32-faithful bf16x3 tcgen05 convs) -> "
+                "note": "pixels resident in HBM -> MaskGitVQGAN f16-256 get_code (fp32-faithful bf16x3 wgmma convs) -> "
                         "masking -> train step; random-init tokeniser"}
         # fast tokenizer mode: single-pass bf16 convolutions (the accuracy class of the reference's own TF32 GPU path)
         with torch.no_grad():

@@ -1,4 +1,4 @@
-/* muse_b200.h - C ABI of libmuse_b200.so: the B200 (sm_100a) hot path of huggingface/open-muse.
+/* muse_b200.h - C ABI of libmuse_b200.so: the H100 (sm_90a) hot path of huggingface/open-muse.
  *
  * The reference (pure PyTorch, no FFI of its own) reaches the device through torch ops; each
  * entry point below replaces the torch call(s) cited next to it (paths relative to the reference
@@ -251,7 +251,7 @@ int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* be
                              float* partials_ws, float* scale_shift_ws, int B, int HW, int C, int groups, float eps,
                              int precomputed_tiles, int apply_silu, void* stream);  /* apply_silu 0: plain GroupNorm
                              (AttnBlock.norm of the taming VQGAN, modeling_taming_vqgan.py:137-150) */
-/* Conv2dSame (:33-45) on the tcgen05 tensor cores with fp32-level accuracy (3 bf16 products hi*hi + lo*hi + hi*lo,
+/* Conv2dSame (:33-45) on the Hopper (wgmma) tensor cores with fp32-level accuracy (3 bf16 products hi*hi + lo*hi + hi*lo,
  * fp32 accumulation): x_hi/x_lo bf16 [B,H,W,Cin], w_hi/w_lo bf16 [Cout, ksize*ksize*Cin] (tap-major, then input
  * channel), optional bias [Cout] and residual [B,H,W,Cout] -> y fp32 [B,H,W,Cout].
  * muse_conv2d_tc_supported says whether the geometry is handled (Cin % 64 == 0, W a multiple or a divisor of 128 ...);

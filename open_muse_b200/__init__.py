@@ -1,4 +1,4 @@
-"""open_muse_b200 -- the B200 (sm_100a) hot path of huggingface/open-muse behind the reference's Python surface.
+"""open_muse_b200 -- the H100 (sm_90a) hot path of huggingface/open-muse behind the reference's Python surface.
 
     from open_muse_b200 import MaskGitTransformer, MaskGitVQGAN
 

@@ -1,4 +1,4 @@
-"""Builds libmuse_b200.so (hand-written sm_100a CUDA behind a C ABI) in-tree with nvcc.
+"""Builds libmuse_b200.so (hand-written sm_90a CUDA behind a C ABI) in-tree with nvcc.
 
 No torch headers are involved: the library's ABI is plain C (include/muse_b200.h) and the Python
 host side binds it with ctypes.  Objects are compiled in parallel and cached by source mtime.
@@ -18,7 +18,7 @@ BUILD_DIR = PKG_DIR / "csrc" / "build"
 LIB_PATH = PKG_DIR / "libmuse_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -64,7 +64,7 @@ def build(verbose: bool = False, force: bool = False) -> Path:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(run, jobs))
     if jobs or force or not LIB_PATH.exists():
-        run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB_PATH), *map(str, objs)])
+        run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB_PATH), *map(str, objs)])
     return LIB_PATH
 
 
@@ -74,7 +74,7 @@ XCHECK_LIB = XCHECK_DIR / "libmuse_b200_xcheck.so"
 
 def build_xcheck(verbose: bool = False, force: bool = False) -> Path:
     """TEST-ONLY cross-check library (tests/xcheck): the first-generation mma.sync GEMM / attention kernels the GPU tests
-    compare the tcgen05 product kernels against.  Never linked into libmuse_b200.so."""
+    compare the wgmma product kernels against.  Never linked into libmuse_b200.so."""
     nvcc = _nvcc()
     src_dir = XCHECK_DIR / "csrc"
     out_dir = src_dir / "build"
@@ -94,7 +94,7 @@ def build_xcheck(verbose: bool = False, force: bool = False) -> Path:
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed:\n{' '.join(cmd)}\n{r.stdout}\n{r.stderr}")
     if jobs or force or not XCHECK_LIB.exists():
-        r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(XCHECK_LIB), *map(str, objs)],
+        r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(XCHECK_LIB), *map(str, objs)],
                            capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc link failed:\n{r.stdout}\n{r.stderr}")

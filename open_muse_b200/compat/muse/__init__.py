@@ -1,6 +1,6 @@
 """Drop-in ``muse`` package: put ``open_muse_b200/compat`` on PYTHONPATH and the reference's
 ``from muse import MaskGitTransformer, MaskGitVQGAN, PipelineMuse`` / ``from muse.sampling import cosine_schedule``
-(training/train_maskgit_imagenet.py:30-33) resolve to the B200 implementations."""
+(training/train_maskgit_imagenet.py:30-33) resolve to the H100 implementations."""
 __version__ = "0.0.1"
 
 from open_muse_b200 import (  # noqa: F401
@@ -24,7 +24,7 @@ class _OutOfScopeTokenizer:
     config actually selects them."""
 
     def __init__(self, *a, **k):
-        raise NotImplementedError(f"open_muse_b200: {type(self).__name__} is not part of the B200 hot path; use "
+        raise NotImplementedError(f"open_muse_b200: {type(self).__name__} is not part of the H100 hot path; use "
                                   "MaskGitVQGAN (model.vq_model.type: maskgit_vqgan) or VQGANModel (taming)")
 
     @classmethod

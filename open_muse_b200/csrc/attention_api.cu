@@ -1,5 +1,5 @@
 // Attention entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its
-// autograd backward, head_dim 64 or 48, no mask, no dropout.  Every shape runs on the tcgen05 / TMEM kernels of
+// autograd backward, head_dim 64 or 48, no mask, no dropout.  Every shape runs on the wgmma / TMA kernels of
 // attention_tc.cu (balanced row tiles cover ragged sequence lengths such as 257 = 256 + class token and the 77 text
 // states of cross-attention); there is no second implementation in this library.
 #include "common.cuh"

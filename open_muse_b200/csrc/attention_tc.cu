@@ -1,31 +1,32 @@
-// tcgen05 / TMEM / TMA attention for head_dim 64 and 48 (sm_100a): forward, dQ and dK/dV kernels.
+// wgmma / TMA attention for head_dim 64 and 48 (sm_90a): forward, dQ and dK/dV kernels.
 // Replaces the reference's materialised attention (muse/modeling_transformer.py:221-241) and its autograd backward.
 //
-// One CTA = one (batch, head) x one 128-row tile of the "owned" sequence dimension; its 128 threads each own one
-// TMEM lane (= one row).  Thread 0 also drives TMA and issues the MMAs; the CTA is internally sequential
-// (load -> score MMA -> row-wise softmax math -> accumulate MMA) and the SM overlaps TWO co-resident CTAs
-// (each <= 256 TMEM columns and <= ~112 KB smem), so tensor core, TMA and the softmax lanes of different CTAs overlap.
+// One CTA = one (batch, head) x one 128-row tile of the "owned" sequence dimension.  Every warpgroup of the CTA issues
+// wgmma on 64-row halves of the tile.  Score-like products (S, dP) land in an fp32 [128 x 64] shared-memory tile from
+// which the softmax math reads whole rows (one row per thread, as written below); the accumulating products (O, dQ, dK,
+// dV) stay in the wgmma accumulator registers for the whole loop and are stored once at the end.
 //
-//   forward  : owned = q rows.   S = Q K_j^T -> online softmax (fp32) -> P (bf16, smem) -> O += P V_j      (TMEM: S 128 + O 64)
-//   dQ       : owned = q rows.   S, dP = dO V_j^T -> sweep 1: D = sum P*dP ; sweep 2: dS -> dQ += dS K_j  (TMEM: 64+64+64)
+//   forward  : owned = q rows.   S = Q K_j^T -> online softmax (fp32) -> P (bf16, smem) -> O += P V_j
+//   dQ       : owned = q rows.   S, dP = dO V_j^T -> sweep 1: D = sum P*dP ; sweep 2: dS -> dQ += dS K_j
 //   dK/dV    : owned = kv rows.  S^T = K Q_i^T, dP^T = V dO_i^T -> P^T, dS^T -> dV += P^T dO_i, dK += dS^T Q_i
-//                                                                                       (TMEM: 64+64+64+64)
 // Operands are read straight from the strided [tokens, 3H] QKV projection through 3-D TMA tensor maps
 // {64 head columns, S rows, B} (rows past the end of a sequence are zero-filled by the TMA unit), with the same
-// 128-byte-swizzled tiles serving as K-major or MN-major MMA operands depending on the product.
+// 128-byte-swizzled tiles serving as K-major or MN-major MMA operands depending on the product.  The looped tiles sit in
+// a TMA ring that is refilled while the current tile is being processed.
 // The owned dimension is cut into ceil(S / 128) tiles of EQUAL height R = ceil(S / tiles) (S = 257 with the class token ->
 // three tiles of 86 rows; S = 256 -> two of 128; the 77 text states of cross-attention -> one of 77): a tile starts at row
 // i * R, its CTA still loads a 128-row box (rows past R belong to the next tile or are zero-filled past the sequence), the
-// MMAs run on all 128 lanes, but only rows < R are kept, and warps whose 32 lanes all lie past R skip the softmax math.
+// MMAs run on all 128 rows, but only rows < R are kept, and warps whose 32 rows all lie past R skip the softmax math.
 // No row is ever handed to another kernel.  The looped dimension handles ragged tails by shrinking the MMA N/K to a
 // multiple of 16.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace muse {
 
 int make_tmap3(CUtensorMap* map, const void* base, long long cols, long long rows, long long batches,
-               long long row_pitch_elems, int box_rows);  // gemm_tcgen05.cu
+               long long row_pitch_elems, int box_rows);  // gemm_wgmma.cu
 
 namespace {
 
@@ -44,37 +45,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
-
-// 16-column TMEM load (used for ragged 16-wide tails)
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
 // exp2 on the SFU without the denormal/range fix-ups of exp2f (inputs here are <= 0 or bounded scores)
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -113,14 +83,71 @@ struct TcParams {
   float* dvec;                       // [B, nh, Sq]
 };
 
+// ------------------------------------------------------------------------------------------------ wgmma helpers
+constexpr int SP = 68;  // row pitch (floats) of the fp32 score tiles: float4 row reads by 8 consecutive rows hit 32 banks
+constexpr int SCORE_BYTES = 128 * SP * 4;
+
+// d (+)= A[64 rows x 16*ksteps] * B, A a K-major tile, B K-major (TB = 0, N rows) or MN-major (TB = 1, N columns).
+template <int N, int TB>
+__device__ __forceinline__ void mma_tile(float (&d)[N / 2], uint32_t a, uint32_t b, int ksteps, int accumulate) {
+  ptx::wgmma_fence();
+  for (int ks = 0; ks < ksteps; ++ks)
+    ptx::Wgmma<N, 0, TB>::run(d, desc_kmajor(a, ks), TB ? desc_mnmajor(b, ks) : desc_kmajor(b, ks), (accumulate || ks > 0) ? 1 : 0);
+  ptx::wgmma_commit();
+  ptx::wgmma_wait<0>();
+}
+
+// the fragment row / column of d[4j] for the calling thread of its warpgroup (d[4j + 2] is 8 rows further down)
+__device__ __forceinline__ int frag_row() { return ((threadIdx.x & 127) >> 5) * 16 + ((threadIdx.x & 31) >> 2); }
+__device__ __forceinline__ int frag_col() { return 2 * (threadIdx.x & 3); }
+
+template <int N>
+__device__ __forceinline__ void scores_n(uint32_t a, uint32_t b, int ksteps, float* dst, int row0) {
+  float d[N / 2];
+  mma_tile<N, 0>(d, a, b, ksteps, 0);
+  const int r = row0 + frag_row(), c = frag_col();
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(dst + r * SP + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(dst + (r + 8) * SP + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+// rows [row0, row0 + 64) of A B^T (both K-major, N = n16 <= 64 rows of B) -> the fp32 score tile
+__device__ __forceinline__ void scores_to_smem(uint32_t a, uint32_t b, int n16, int ksteps, float* dst, int row0) {
+  switch (n16) {
+    case 16: scores_n<16>(a, b, ksteps, dst, row0); break;
+    case 32: scores_n<32>(a, b, ksteps, dst, row0); break;
+    case 48: scores_n<48>(a, b, ksteps, dst, row0); break;
+    default: scores_n<64>(a, b, ksteps, dst, row0); break;
+  }
+}
+
+// bf16 store of an [64 x HD] accumulator fragment: rows row0 + (fragment row) of `base` (row stride rs), if < rows_ok
+template <int HD>
+__device__ __forceinline__ void store_acc(const float (&d)[HD / 2], bf16* base, long long rs, int row0, int rows_ok,
+                                          const float* row_scale) {
+  const int r = row0 + frag_row(), c = frag_col();
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int rr = r + 8 * hr;
+    if (rr >= rows_ok) continue;
+    const float sc = row_scale ? row_scale[rr] : 1.f;
+    bf16* dst = base + rr * rs;
+#pragma unroll
+    for (int j = 0; j < HD / 8; ++j)
+      *reinterpret_cast<uint32_t*>(dst + 8 * j + c) = pack_bf16(d[4 * j + 2 * hr] * sc, d[4 * j + 2 * hr + 1] * sc);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ forward
-// TMEM columns: S [0,64)  O [64,128) -> 128 columns per CTA; smem 48 KB -> FOUR co-resident CTAs per SM overlap each
-// other's TMA / MMA / softmax latencies (a 128-wide score tile with 2 CTAs/SM measured slower than the mma.sync kernel).
+// 128 threads = one warpgroup, which issues the MMAs of both 64-row halves (O of both halves in registers).
+// smem: Q 16K | K 8K | V 8K | P 16K | S fp32 | per-row scale | barriers -> two co-resident CTAs per SM overlap each other's
+// TMA / MMA / softmax phases.
 constexpr int FWD_BN = 64;
-constexpr int FWD_SMEM = 16384 /*Q*/ + 8192 /*K*/ + 8192 /*V*/ + 16384 /*P*/ + 64;  // 5 mbarriers + the TMEM holder
+constexpr int FWD_SMEM = 16384 /*Q*/ + 8192 /*K*/ + 8192 /*V*/ + 16384 /*P*/ + SCORE_BYTES + 512 + 64;
 
 template <int HD>
-__global__ void __launch_bounds__(128, 4)
+__global__ void __launch_bounds__(128, 2)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const TcParams p) {
   pdl_trigger();
@@ -131,12 +158,11 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint8_t* sK = smem + 16384;
   uint8_t* sV = smem + 24576;
   uint8_t* sP = smem + 32768;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 49152);
+  float* sS = reinterpret_cast<float*>(smem + 49152);
+  float* sRow = reinterpret_cast<float*>(smem + 49152 + SCORE_BYTES);  // per-row alpha, then 1 / l
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 49152 + SCORE_BYTES + 512);
   uint64_t* bar_kv = bars;      // Q (first use) + K tile landed
-  uint64_t* bar_s = bars + 1;   // score MMA done
-  uint64_t* bar_o = bars + 2;   // accumulate MMA done
-  uint64_t* bar_v = bars + 3;   // V tile landed
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* bar_v = bars + 1;   // V tile landed
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int q0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
@@ -144,22 +170,11 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const bool warp_active = warp * 32 < rows_here;  // warps whose rows all belong to the next tile skip the softmax math
   if (tid == 0) {
     ptx::mbar_init(bar_kv, 1);
-    ptx::mbar_init(bar_s, 1);
-    ptx::mbar_init(bar_o, 1);
     ptx::mbar_init(bar_v, 1);
     ptx::fence_barrier_init();
   }
-  if (warp == 0) {
-    ptx::tmem_alloc(tmem_holder, 128);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  pdl_wait();  // everything above touches only shared memory / TMEM / kernel parameters
-  const uint32_t tmem = *tmem_holder;
-  const uint32_t t_s = tmem + (static_cast<uint32_t>(warp * 32) << 16);        // S: columns [0,64)
-  const uint32_t t_o = t_s + 64;                                                // O: columns [64,128)
+  pdl_wait();  // everything above touches only shared memory / kernel parameters
   const int ntiles = ceil_div(p.Skv, FWD_BN);
 
   if (tid == 0) {
@@ -171,52 +186,35 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
   const float sl2 = p.scale * kLog2e;
   float m = -INFINITY, l = 0.f;
-
-  // The score MMA of tile j+1 is issued right behind the accumulate MMA of tile j (the scores of tile j are in registers by
-  // then), so one tcgen05.commit covers both and the CTA waits for ONE tensor-core round trip per tile instead of two:
-  // bar_s(j+1) completing means P V_j has landed as well (MMAs of a CTA complete in issue order), which is what frees the
-  // P buffer, the V tile and the running output for iteration j+1.
-  if (tid == 0) {
-    ptx::mbar_wait(bar_kv, 0);
-    ptx::tc_fence_after();
-    const uint32_t idesc0 = ptx::make_idesc_bf16(128, (min(FWD_BN, p.Skv) + 15) & ~15, 0, 0);
+  float o[2][HD / 2];
 #pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks)
-      ptx::umma_f16(tmem, desc_kmajor(ptx::smem_u32(sQ), ks), desc_kmajor(ptx::smem_u32(sK), ks), idesc0, ks > 0);
-    ptx::umma_commit(bar_s);
-  }
+  for (int i = 0; i < HD / 2; ++i) { o[0][i] = 0.f; o[1][i] = 0.f; }
+
   for (int j = 0; j < ntiles; ++j) {
     const uint32_t par = j & 1;
     const int nvalid = min(FWD_BN, p.Skv - j * FWD_BN);
     const int n16 = (nvalid + 15) & ~15;
-    ptx::mbar_wait(bar_s, par);  // S_j is complete -- and so is P V_{j-1}
-    ptx::tc_fence_after();
-    if (tid == 0) {
-      if (j + 1 < ntiles) {  // the score MMA has consumed K_j: fetch K_{j+1} under the softmax math
-        ptx::mbar_expect_tx(bar_kv, 8192);
-        tma_load_3d(sK, &tmK, bar_kv, h * HD, (j + 1) * FWD_BN, b);
-      }
-      if (j > 0) {  // the accumulate MMA of tile j-1 has consumed V_{j-1}
-        ptx::mbar_expect_tx(bar_v, 8192);
-        tma_load_3d(sV, &tmV, bar_v, h * HD, j * FWD_BN, b);
-      }
+    ptx::mbar_wait(bar_kv, par);
+    scores_to_smem(ptx::smem_u32(sQ), ptx::smem_u32(sK), n16, HD / 16, sS, 0);
+    scores_to_smem(ptx::smem_u32(sQ) + 8192, ptx::smem_u32(sK), n16, HD / 16, sS, 64);
+    __syncthreads();  // S_j is in shared memory and K_j has been consumed
+    if (tid == 0 && j + 1 < ntiles) {  // fetch K_{j+1} under the softmax math
+      ptx::mbar_expect_tx(bar_kv, 8192);
+      tma_load_3d(sK, &tmK, bar_kv, h * HD, (j + 1) * FWD_BN, b);
     }
+    float alpha = 1.f;
     if (warp_active) {
-    // the whole score row (<= 64 columns) fits in registers: one TMEM read, max, exp2, pack.  The instruction count
-    // per score element is what bounds this kernel (issue slots, not the tensor core), so the ragged-tail masking is
-    // kept out of the full-tile path and the softmax scale is folded into one FFMA per element.
+    // the whole score row (<= 64 columns) fits in registers.  The instruction count per score element is what bounds
+    // this loop, so the ragged-tail masking is kept out of the full-tile path and the softmax scale is folded into one
+    // FFMA per element.
     float sc[64];
 #pragma unroll
-    for (int c = 0; c < 64; c += 16) {
+    for (int c = 0; c < 64; c += 4) {
       if (c < n16) {
-        uint32_t r16[16];
-        tmem_ld_32x32b_x16(t_s + c, r16);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) sc[c + i] = __uint_as_float(r16[i]);
+        const float4 v = *reinterpret_cast<const float4*>(sS + tid * SP + c);
+        sc[c] = v.x; sc[c + 1] = v.y; sc[c + 2] = v.z; sc[c + 3] = v.w;
       } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) sc[c + i] = -INFINITY;
+        sc[c] = sc[c + 1] = sc[c + 2] = sc[c + 3] = -INFINITY;
       }
     }
     if (nvalid < FWD_BN) {
@@ -228,11 +226,10 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int i = 0; i < 64; ++i) raw = fmaxf(raw, sc[i]);
     // Lazy running maximum: the reference point m only moves when the tile's maximum exceeds it by more than 8 (log2
     // units), i.e. P entries stay below 2^8 -- harmless in bf16 / fp32 -- and the final 1 / l normalisation and the LSE
-    // (m + log2 l) are exact for any reference point.  Most tiles then leave m alone, alpha is exactly 1 for the whole warp
-    // and the TMEM round trip that rescales the running output is skipped (warp-uniform vote below).
+    // (m + log2 l) are exact for any reference point.  Most tiles then leave m alone and alpha is exactly 1.
     const float cand = raw * sl2;
     const float mx = (cand > m + 8.0f) ? cand : m;
-    const float alpha = ex2(m - mx);  // 0 on the first tile (m = -inf), 1 when the reference point stays
+    alpha = ex2(m - mx);  // 0 on the first tile (m = -inf), 1 when the reference point stays
     m = mx;
     float l4[4] = {0.f, 0.f, 0.f, 0.f};  // four independent chains instead of one 64-long dependent add chain
 #pragma unroll
@@ -250,115 +247,49 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         st_operand_chunk(sP, tid, i, u);
       }
     }
-    // rescale the running output (P V_{j-1} has finished: see the bar_s wait above)
-    if (j > 0 && !__all_sync(0xffffffffu, alpha == 1.0f)) {
-#pragma unroll
-      for (int c = 0; c + 32 <= HD; c += 32) {
-        uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(t_o + c, r);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-        tmem_st_32x32b_x32(t_o + c, r);
-      }
-      if constexpr (HD % 32 != 0) {  // HD = 48: the last 16 columns
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(t_o + (HD & ~31), r);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-        tmem_st_32x32b_x16(t_o + (HD & ~31), r);
-      }
-      tmem_st_wait();
-    }
     }  // warp_active
+    sRow[tid] = alpha;
     ptx::fence_proxy_async();
-    ptx::tc_fence_before();
-    __syncthreads();  // every thread holds its scores in registers and has written its part of P
-    if (tid == 0) {
-      ptx::mbar_wait(bar_v, par);
-      ptx::tc_fence_after();
-      const uint32_t idesc = ptx::make_idesc_bf16(128, HD, 0, 1);
-      const int ksteps = n16 >> 4;
-      for (int ks = 0; ks < ksteps; ++ks)
-        ptx::umma_f16(tmem + 64, desc_kmajor(ptx::smem_u32(sP), ks), desc_mnmajor(ptx::smem_u32(sV), ks), idesc,
-                      (j > 0 || ks > 0) ? 1u : 0u);
-      if (j + 1 < ntiles) {
-        ptx::mbar_wait(bar_kv, par ^ 1);  // K_{j+1} landed (requested at the top of this iteration)
-        ptx::tc_fence_after();
-        const int nn16 = (min(FWD_BN, p.Skv - (j + 1) * FWD_BN) + 15) & ~15;
-        const uint32_t idesc_s = ptx::make_idesc_bf16(128, nn16, 0, 0);
+    __syncthreads();  // P_j is visible to the tensor core, every row's alpha to every thread
+    if (j > 0) {  // rescale the running output
 #pragma unroll
-        for (int ks = 0; ks < HD / 16; ++ks)
-          ptx::umma_f16(tmem, desc_kmajor(ptx::smem_u32(sQ), ks), desc_kmajor(ptx::smem_u32(sK), ks), idesc_s, ks > 0);
-        ptx::umma_commit(bar_s);
-      } else {
-        ptx::umma_commit(bar_o);
+      for (int hh = 0; hh < 2; ++hh) {
+        const float a0 = sRow[hh * 64 + frag_row()], a1 = sRow[hh * 64 + frag_row() + 8];
+#pragma unroll
+        for (int i = 0; i < HD / 2; i += 4) {
+          o[hh][i] *= a0; o[hh][i + 1] *= a0; o[hh][i + 2] *= a1; o[hh][i + 3] *= a1;
+        }
       }
+    }
+    ptx::mbar_wait(bar_v, par);
+    mma_tile<HD, 1>(o[0], ptx::smem_u32(sP), ptx::smem_u32(sV), n16 >> 4, j > 0);
+    mma_tile<HD, 1>(o[1], ptx::smem_u32(sP) + 8192, ptx::smem_u32(sV), n16 >> 4, j > 0);
+    __syncthreads();  // P_j and V_j have been consumed
+    if (tid == 0 && j + 1 < ntiles) {
+      ptx::mbar_expect_tx(bar_v, 8192);
+      tma_load_3d(sV, &tmV, bar_v, h * HD, (j + 1) * FWD_BN, b);
     }
   }
-  ptx::mbar_wait(bar_o, 0);  // the last accumulate MMA
-  ptx::tc_fence_after();
   // epilogue: O / l -> bf16 rows, LSE
   const int row = q0 + tid;
-  const bool row_ok = tid < rows_here;
-  const float inv = 1.f / l;
-  bf16* orow = p.out0 + (static_cast<long long>(b) * p.Sq + row) * p.out0_rs + h * HD;
-#pragma unroll
-  for (int c = 0; c + 32 <= HD; c += 32) {
-    uint32_t r[32];
-    ptx::tmem_ld_32x32b_x32(t_o + c, r);
-    ptx::tmem_ld_wait();
-    if (row_ok) {
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        uint4 u;
-        u.x = pack_bf16(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-        u.y = pack_bf16(__uint_as_float(r[i + 2]) * inv, __uint_as_float(r[i + 3]) * inv);
-        u.z = pack_bf16(__uint_as_float(r[i + 4]) * inv, __uint_as_float(r[i + 5]) * inv);
-        u.w = pack_bf16(__uint_as_float(r[i + 6]) * inv, __uint_as_float(r[i + 7]) * inv);
-        *reinterpret_cast<uint4*>(orow + c + i) = u;
-      }
-    }
-  }
-  if constexpr (HD % 32 != 0) {  // HD = 48: the last 16 columns
-    uint32_t r[16];
-    tmem_ld_32x32b_x16(t_o + (HD & ~31), r);
-    ptx::tmem_ld_wait();
-    if (row_ok) {
-#pragma unroll
-      for (int i = 0; i < 16; i += 8) {
-        uint4 u;
-        u.x = pack_bf16(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-        u.y = pack_bf16(__uint_as_float(r[i + 2]) * inv, __uint_as_float(r[i + 3]) * inv);
-        u.z = pack_bf16(__uint_as_float(r[i + 4]) * inv, __uint_as_float(r[i + 5]) * inv);
-        u.w = pack_bf16(__uint_as_float(r[i + 6]) * inv, __uint_as_float(r[i + 7]) * inv);
-        *reinterpret_cast<uint4*>(orow + (HD & ~31) + i) = u;
-      }
-    }
-  }
-  if (row_ok) p.lse[(static_cast<long long>(b) * p.nh + h) * p.Sq + row] = (m + log2f(l)) * kLn2;
-  ptx::tc_fence_before();
+  sRow[tid] = 1.f / l;
+  if (tid < rows_here) p.lse[(static_cast<long long>(b) * p.nh + h) * p.Sq + row] = (m + log2f(l)) * kLn2;
   __syncthreads();
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem, 128);
-  }
+  bf16* obase = p.out0 + (static_cast<long long>(b) * p.Sq + q0) * p.out0_rs + h * HD;
+  store_acc<HD>(o[0], obase, p.out0_rs, 0, rows_here, sRow);
+  store_acc<HD>(o[1], obase, p.out0_rs, 64, rows_here, sRow);
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dQ
-// 256 threads: warps w and w+4 share TMEM lanes (rows) 32*(w%4).. and split the 64 score columns in two halves.
-// Software pipeline inside the CTA: as soon as every thread has pulled its S / dP columns out of TMEM into registers
-// (barrier A), thread 0 issues the score MMAs of the NEXT step, so the tensor core works while the exp2 / FMA math of
-// the current step runs; the dQ MMA of a step is never waited for by the step that issued it (dS is double-buffered,
-// K/V tiles sit in a 3-stage TMA ring with prefetch distance 2).
-// TMEM columns: S [0,64)  dP [64,128)  dQ [128,192).
-// smem: Q 16K | dO 16K | 3 x {K_j 8K, V_j 8K} | 2 x dS 16K (the partial-D exchange buffer aliases dS[0])
+// 256 threads = two warpgroups; warpgroup g issues the MMAs of rows [64 g, 64 g + 64) and keeps that half of dQ in
+// registers.  In the softmax math, warps w and w+4 share rows 32*(w%4).. and split the 64 score columns in two halves.
+// K/V tiles sit in a 3-stage TMA ring with prefetch distance 2.
+// smem: Q 16K | dO 16K | 3 x {K_j 8K, V_j 8K} | dS 16K (the partial-D exchange buffer aliases it) | S, dP fp32
 constexpr int BWD_BN = 64;
-constexpr int DQ_SMEM = 16384 * 2 + 3 * 16384 + 2 * 16384 + 64;
+constexpr int DQ_SMEM = 16384 * 2 + 3 * 16384 + 16384 + 2 * SCORE_BYTES + 64;
 
 template <int HD>
-__global__ void __launch_bounds__(288, 2)
+__global__ void __launch_bounds__(256, 1)
 attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const TcParams p) {
@@ -369,43 +300,27 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   uint8_t* sQ = smem;
   uint8_t* sdO = smem + 16384;
   uint8_t* sKV = smem + 32768;             // 3 stages x {K 8 KB, V 8 KB}
-  uint8_t* sdS = smem + 32768 + 49152;     // 2 buffers x 16 KB
+  uint8_t* sdS = smem + 32768 + 49152;
   float* sDp = reinterpret_cast<float*>(sdS);  // [2][128] partial D (only used between the two sweeps)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 32768 + 49152 + 32768);
+  float* sS = reinterpret_cast<float*>(sdS + 16384);
+  float* sdP = sS + 128 * SP;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + 16384 + 2 * SCORE_BYTES);
   uint64_t* bar_kv = bars;       // [3] TMA landed
-  uint64_t* bar_s = bars + 3;    //     score MMAs done
-  uint64_t* bar_o = bars + 4;    // [2] dQ MMA done
-  uint64_t* bar_free = bars + 6; //     all math threads pulled their scores out of TMEM (count 256)
-  uint64_t* bar_ds = bars + 7;   // [2] dS operand written (count 256)
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 9);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = tid >> 7;                     // warpgroup: MMA rows [64 g, 64 g + 64)
   const int half = warp >> 2;                 // column half handled by this thread
-  const int r = (warp & 3) * 32 + lane;       // row (TMEM lane) handled by this thread
+  const int r = (warp & 3) * 32 + lane;       // row handled by this thread
   const int q0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
   const int rows_here = min(p.tile_rows, p.Sq - q0);
   const bool warp_active = (warp & 3) * 32 < rows_here;  // other warps keep the barrier protocol but skip the math
   const bool row_ok = r < rows_here;
   if (tid == 0) {
     for (int i = 0; i < 3; ++i) ptx::mbar_init(&bar_kv[i], 1);
-    ptx::mbar_init(bar_s, 1);
-    ptx::mbar_init(&bar_o[0], 1);
-    ptx::mbar_init(&bar_o[1], 1);
-    ptx::mbar_init(bar_free, 256);
-    ptx::mbar_init(&bar_ds[0], 256);
-    ptx::mbar_init(&bar_ds[1], 256);
     ptx::fence_barrier_init();
   }
-  if (warp == 0) {
-    ptx::tmem_alloc(tmem_holder, 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  pdl_wait();  // everything above touches only shared memory / TMEM / kernel parameters
-  const uint32_t tmem = *tmem_holder;
-  const uint32_t t_row = tmem + (static_cast<uint32_t>((warp & 3) * 32) << 16);
+  pdl_wait();  // everything above touches only shared memory / kernel parameters
   const int ntiles = ceil_div(p.Skv, BWD_BN);
   const int nsteps = 2 * ntiles;
   const int row = q0 + r;
@@ -413,69 +328,25 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   const float lse2 = row_ok ? p.lse[stat_idx] * kLog2e : 0.f;
   const float sl2 = p.scale * kLog2e;
 
-  auto n16_of = [&](int step) { return (min(BWD_BN, p.Skv - (step % ntiles) * BWD_BN) + 15) & ~15; };
-  auto issue_scores = [&](int step) {  // thread 0: S = Q K^T and dP = dO V^T of `step` into TMEM [0,128)
-    uint8_t* sK = sKV + (step % 3) * 16384;
-    const uint32_t idesc = ptx::make_idesc_bf16(128, n16_of(step), 0, 0);
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks)
-      ptx::umma_f16(tmem, desc_kmajor(ptx::smem_u32(sQ), ks), desc_kmajor(ptx::smem_u32(sK), ks), idesc, ks > 0);
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks)
-      ptx::umma_f16(tmem + 64, desc_kmajor(ptx::smem_u32(sdO), ks), desc_kmajor(ptx::smem_u32(sK + 8192), ks), idesc, ks > 0);
-    ptx::umma_commit(bar_s);
-  };
   auto load_kv = [&](int step) {       // thread 0: TMA of the K/V tile of `step` into its ring stage
     uint8_t* sK = sKV + (step % 3) * 16384;
     const int jn = step % ntiles;
     tma_load_3d(sK, &tmK, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
     tma_load_3d(sK + 8192, &tmV, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
   };
-
-  // ---- warp 8: control thread (TMA + MMA issue), never touches the softmax math -----------------------------------
-  if (warp == 8) {
-    if (lane == 0) {
-      ptx::mbar_expect_tx(&bar_kv[0], 16384 * 2 + 8192 * 2);
-      tma_load_3d(sQ, &tmQ, &bar_kv[0], h * HD, q0, b);
-      tma_load_3d(sdO, &tmdO, &bar_kv[0], h * HD, q0, b);
-      load_kv(0);
-      if (nsteps > 1) {
-        ptx::mbar_expect_tx(&bar_kv[1], 8192 * 2);
-        load_kv(1);
-      }
-      ptx::mbar_wait(&bar_kv[0], 0);
-      ptx::tc_fence_after();
-      issue_scores(0);
-      for (int st = 0; st < nsteps; ++st) {
-        const int u = st - ntiles;
-        ptx::mbar_wait(bar_free, st & 1);  // scores of step st are in registers: TMEM [0,128) may be overwritten
-        ptx::tc_fence_after();
-        if (st + 1 < nsteps) {
-          if (st + 2 < nsteps) {
-            // ring stage (st+2)%3 was last read by the dQ MMA of step st-1
-            if (st - 1 >= ntiles) ptx::mbar_wait(&bar_o[(u - 1) & 1], ((u - 1) >> 1) & 1);
-            ptx::mbar_expect_tx(&bar_kv[(st + 2) % 3], 8192 * 2);
-            load_kv(st + 2);
-          }
-          ptx::mbar_wait(&bar_kv[(st + 1) % 3], ((st + 1) / 3) & 1);
-          ptx::tc_fence_after();
-          issue_scores(st + 1);
-        }
-        if (u >= 0) {
-          ptx::mbar_wait(&bar_ds[u & 1], (u >> 1) & 1);  // dS of this step is in shared memory
-          const uint32_t idesc = ptx::make_idesc_bf16(128, HD, 0, 1);
-          uint8_t* sK = sKV + (st % 3) * 16384;
-          uint8_t* dS = sdS + (u & 1) * 16384;
-          const int ksteps = n16_of(st) >> 4;
-          for (int ks = 0; ks < ksteps; ++ks)  // dQ += dS K_j   (K_j consumed as an MN-major operand)
-            ptx::umma_f16(tmem + 128, desc_kmajor(ptx::smem_u32(dS), ks), desc_mnmajor(ptx::smem_u32(sK), ks), idesc,
-                          (u > 0 || ks > 0) ? 1u : 0u);
-          ptx::umma_commit(&bar_o[u & 1]);
-        }
-      }
+  if (tid == 0) {
+    ptx::mbar_expect_tx(&bar_kv[0], 16384 * 2 + 8192 * 2);
+    tma_load_3d(sQ, &tmQ, &bar_kv[0], h * HD, q0, b);
+    tma_load_3d(sdO, &tmdO, &bar_kv[0], h * HD, q0, b);
+    load_kv(0);
+    if (nsteps > 1) {
+      ptx::mbar_expect_tx(&bar_kv[1], 8192 * 2);
+      load_kv(1);
     }
-  } else {
-  // ---- warps 0-7: math threads ------------------------------------------------------------------------------------
+  }
+  float dq[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) dq[i] = 0.f;
   float dsum = 0.f;
   for (int st = 0; st < nsteps; ++st) {
     const int j = st % ntiles;
@@ -483,27 +354,28 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const int u = st - ntiles;  // index among the sweep-2 steps
     const int nvalid = min(BWD_BN, p.Skv - j * BWD_BN);
     const int n16 = (nvalid + 15) & ~15;
-    ptx::mbar_wait(bar_s, st & 1);
-    ptx::tc_fence_after();
-    uint32_t s_reg[32], d_reg[32];
+    if (tid == 0 && st + 2 < nsteps) {  // ring stage (st+2)%3 was last read in step st-1, which every thread has left
+      ptx::mbar_expect_tx(&bar_kv[(st + 2) % 3], 8192 * 2);
+      load_kv(st + 2);
+    }
+    ptx::mbar_wait(&bar_kv[st % 3], (st / 3) & 1);
+    uint8_t* sK = sKV + (st % 3) * 16384;
+    scores_to_smem(ptx::smem_u32(sQ) + g * 8192, ptx::smem_u32(sK), n16, HD / 16, sS, g * 64);
+    scores_to_smem(ptx::smem_u32(sdO) + g * 8192, ptx::smem_u32(sK) + 8192, n16, HD / 16, sdP, g * 64);
+    math_sync();  // S and dP of this step are in shared memory
+    float s_reg[32], d_reg[32];
     if (warp_active) {
 #pragma unroll
-    for (int cc = 0; cc < 32; cc += 16) {
-      const int c = half * 32 + cc;
-      if (c < n16) {
-        uint32_t a16[16], b16[16];
-        tmem_ld_32x32b_x16(t_row + c, a16);
-        tmem_ld_32x32b_x16(t_row + 64 + c, b16);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) { s_reg[cc + i] = a16[i]; d_reg[cc + i] = b16[i]; }
+      for (int cc = 0; cc < 32; cc += 4) {
+        const int c = half * 32 + cc;
+        if (c < n16) {
+          const float4 a4 = *reinterpret_cast<const float4*>(sS + r * SP + c);
+          const float4 b4 = *reinterpret_cast<const float4*>(sdP + r * SP + c);
+          s_reg[cc] = a4.x; s_reg[cc + 1] = a4.y; s_reg[cc + 2] = a4.z; s_reg[cc + 3] = a4.w;
+          d_reg[cc] = b4.x; d_reg[cc + 1] = b4.y; d_reg[cc + 2] = b4.z; d_reg[cc + 3] = b4.w;
+        }
       }
     }
-    ptx::tmem_ld_wait();
-    }
-    ptx::tc_fence_before();
-    ptx::mbar_arrive(bar_free);  // (A) this thread holds its scores in registers
-    uint8_t* dS = sdS + (u & 1) * 16384;
-    if (sweep2 && u >= 2) ptx::mbar_wait(&bar_o[u & 1], ((u >> 1) - 1) & 1);  // dQ MMA of step st-2 read this buffer
     const float neg_d_scaled = -dsum * p.scale;
 #pragma unroll
     for (int cc = 0; cc < 32; cc += 16) {
@@ -513,90 +385,49 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         for (int i8 = 0; i8 < 16; i8 += 8) {
           float pr[8];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) pr[i] = ex2(fmaf(__uint_as_float(s_reg[cc + i8 + i]), sl2, -lse2));
+          for (int i = 0; i < 8; ++i) pr[i] = ex2(fmaf(s_reg[cc + i8 + i], sl2, -lse2));
           if (nvalid < BWD_BN) {  // ragged last tile only
 #pragma unroll
             for (int i = 0; i < 8; ++i) pr[i] = (c + i8 + i < nvalid) ? pr[i] : 0.f;
           }
           if (!sweep2) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) dsum = fmaf(pr[i], __uint_as_float(d_reg[cc + i8 + i]), dsum);
+            for (int i = 0; i < 8; ++i) dsum = fmaf(pr[i], d_reg[cc + i8 + i], dsum);
           } else {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) pr[i] *= fmaf(__uint_as_float(d_reg[cc + i8 + i]), p.scale, neg_d_scaled);
+            for (int i = 0; i < 8; ++i) pr[i] *= fmaf(d_reg[cc + i8 + i], p.scale, neg_d_scaled);
             uint4 v;
             v.x = pack_bf16(pr[0], pr[1]); v.y = pack_bf16(pr[2], pr[3]);
             v.z = pack_bf16(pr[4], pr[5]); v.w = pack_bf16(pr[6], pr[7]);
-            st_operand_chunk(dS, r, c + i8, v);
+            st_operand_chunk(sdS, r, c + i8, v);
           }
         }
       }
     }
     if (sweep2) {
       ptx::fence_proxy_async();
-      ptx::mbar_arrive(&bar_ds[u & 1]);  // (B) this thread's part of dS is visible to the tensor core
+      math_sync();  // dS is visible to the tensor core
+      mma_tile<HD, 1>(dq, ptx::smem_u32(sdS) + g * 8192, ptx::smem_u32(sK), n16 >> 4, u > 0);  // dQ += dS K_j
     }
     if (st == ntiles - 1) {  // D = sum over both column halves, identical in both threads of the row
       sDp[half * 128 + r] = dsum;
       math_sync();
       dsum = sDp[r] + sDp[128 + r];
       if (half == 0 && row_ok) p.dvec[stat_idx] = dsum;  // for the dK/dV kernels
-      math_sync();  // sDp aliases dS[0]: everyone has read it before sweep 2 writes dS
     }
+    math_sync();  // end of step: score tiles, dS and the ring stage are free again
   }
-  }  // math threads
-  // all dQ MMAs must have landed: last use of each completion barrier
-  if (warp < 8) {
-    const int U = ntiles;
-    const int ua = U - 1;
-    ptx::mbar_wait(&bar_o[ua & 1], (ua >> 1) & 1);
-    if (U >= 2) { const int ub = U - 2; ptx::mbar_wait(&bar_o[ub & 1], (ub >> 1) & 1); }
-    ptx::tc_fence_after();
-  }
-  if (warp < 8) {
-    // the two threads of a row write columns [0, 32) and [32, HD) of dQ
-    bf16* orow = p.out0 + (static_cast<long long>(b) * p.Sq + row) * p.out0_rs + h * HD + half * 32;
-    uint32_t rr[32];
-    if (HD == 64 || half == 0) {
-      ptx::tmem_ld_32x32b_x32(t_row + 128 + half * 32, rr);
-      ptx::tmem_ld_wait();
-    } else {
-      uint32_t r16[16];
-      tmem_ld_32x32b_x16(t_row + 128 + 32, r16);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 16; ++i) rr[i] = r16[i];
-    }
-    const int ncol = (HD == 64 || half == 0) ? 32 : HD - 32;
-    if (row_ok) {
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        if (i >= ncol) break;
-        uint4 v;
-        v.x = pack_bf16(__uint_as_float(rr[i]), __uint_as_float(rr[i + 1]));
-        v.y = pack_bf16(__uint_as_float(rr[i + 2]), __uint_as_float(rr[i + 3]));
-        v.z = pack_bf16(__uint_as_float(rr[i + 4]), __uint_as_float(rr[i + 5]));
-        v.w = pack_bf16(__uint_as_float(rr[i + 6]), __uint_as_float(rr[i + 7]));
-        *reinterpret_cast<uint4*>(orow + i) = v;
-      }
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem, 256);
-  }
+  store_acc<HD>(dq, p.out0 + (static_cast<long long>(b) * p.Sq + q0) * p.out0_rs + h * HD, p.out0_rs, g * 64, rows_here,
+                nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dK, dV
-// Same software pipeline as the dQ kernel, looping over 64-row q tiles.
-// TMEM columns: S^T [0,64)  dP^T [64,128)  dK [128,192)  dV [192,256).
-// smem: K_j 16K | V_j 16K | 3 x {Q_i 8K, dO_i 8K} | P^T 16K | dS^T 16K | lse/D 512 B
-constexpr int DKDV_SMEM = 16384 * 2 + 3 * 16384 + 16384 * 2 + 512 + 128;
+// Same structure as the dQ kernel, looping over 64-row q tiles; dK and dV of the warpgroup's 64 kv rows in registers.
+// smem: K_j 16K | V_j 16K | 3 x {Q_i 8K, dO_i 8K} | P^T 16K | dS^T 16K | lse/D 512 B | S^T, dP^T fp32
+constexpr int DKDV_SMEM = 16384 * 2 + 3 * 16384 + 16384 * 2 + 512 + 2 * SCORE_BYTES + 64;
 
 template <int HD>
-__global__ void __launch_bounds__(288, 2)
+__global__ void __launch_bounds__(256, 1)
 attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                         const TcParams p) {
@@ -610,15 +441,13 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
   uint8_t* sPT = smem + 32768 + 49152;
   uint8_t* sdST = sPT + 16384;
   float* sLD = reinterpret_cast<float*>(sdST + 16384);  // [lse 64 | D 64] of the current q tile
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sdST + 16384 + 512);
+  float* sS = sLD + 128;
+  float* sdP = sS + 128 * SP;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sdST + 16384 + 512 + 2 * SCORE_BYTES);
   uint64_t* bar_ld = bars;       // [3] TMA landed
-  uint64_t* bar_s = bars + 3;    //     score MMAs done
-  uint64_t* bar_o = bars + 4;    //     dV / dK MMAs done
-  uint64_t* bar_free = bars + 5; //     scores pulled out of TMEM by all math threads (count 256)
-  uint64_t* bar_ps = bars + 6;   //     P^T / dS^T operands written (count 256)
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 7);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = tid >> 7;
   const int half = warp >> 2;
   const int r = (warp & 3) * 32 + lane;
   const int kv0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
@@ -626,120 +455,66 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
   const bool warp_active = (warp & 3) * 32 < rows_here;
   if (tid == 0) {
     for (int i = 0; i < 3; ++i) ptx::mbar_init(&bar_ld[i], 1);
-    ptx::mbar_init(bar_s, 1);
-    ptx::mbar_init(bar_o, 1);
-    ptx::mbar_init(bar_free, 256);
-    ptx::mbar_init(bar_ps, 256);
     ptx::fence_barrier_init();
   }
-  if (warp == 0) {
-    ptx::tmem_alloc(tmem_holder, 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  pdl_wait();  // everything above touches only shared memory / TMEM / kernel parameters
-  const uint32_t tmem = *tmem_holder;
-  const uint32_t t_row = tmem + (static_cast<uint32_t>((warp & 3) * 32) << 16);
+  pdl_wait();  // everything above touches only shared memory / kernel parameters
   const int ntiles = ceil_div(p.Sq, BWD_BN);
-  const int kvrow = kv0 + r;
   const bool kv_ok = r < rows_here;  // rows past the tile's share belong to the next CTA (or lie past the sequence)
   const float sl2 = p.scale * kLog2e;
   const long long stat_base = (static_cast<long long>(b) * p.nh + h) * p.Sq;
 
-  auto n16_of = [&](int i) { return (min(BWD_BN, p.Sq - i * BWD_BN) + 15) & ~15; };
-  auto issue_scores = [&](int i) {  // thread 0: S^T = K Q_i^T, dP^T = V dO_i^T
-    uint8_t* sQ = sQO + (i % 3) * 16384;
-    const uint32_t idesc = ptx::make_idesc_bf16(128, n16_of(i), 0, 0);
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks)
-      ptx::umma_f16(tmem, desc_kmajor(ptx::smem_u32(sK), ks), desc_kmajor(ptx::smem_u32(sQ), ks), idesc, ks > 0);
-#pragma unroll
-    for (int ks = 0; ks < HD / 16; ++ks)
-      ptx::umma_f16(tmem + 64, desc_kmajor(ptx::smem_u32(sV), ks), desc_kmajor(ptx::smem_u32(sQ + 8192), ks), idesc, ks > 0);
-    ptx::umma_commit(bar_s);
-  };
   auto load_q = [&](int i) {
     uint8_t* sQ = sQO + (i % 3) * 16384;
     tma_load_3d(sQ, &tmQ, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
     tma_load_3d(sQ + 8192, &tmdO, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
   };
-
-  // ---- warp 8: control thread (TMA + MMA issue) --------------------------------------------------------------------
-  if (warp == 8) {
-    if (lane == 0) {
-      ptx::mbar_expect_tx(&bar_ld[0], 16384 * 2 + 8192 * 2);
-      tma_load_3d(sK, &tmK, &bar_ld[0], h * HD, kv0, b);
-      tma_load_3d(sV, &tmV, &bar_ld[0], h * HD, kv0, b);
-      load_q(0);
-      if (ntiles > 1) {
-        ptx::mbar_expect_tx(&bar_ld[1], 8192 * 2);
-        load_q(1);
-      }
-      ptx::mbar_wait(&bar_ld[0], 0);
-      ptx::tc_fence_after();
-      issue_scores(0);
-      for (int i = 0; i < ntiles; ++i) {
-        ptx::mbar_wait(bar_free, i & 1);
-        ptx::tc_fence_after();
-        if (i + 1 < ntiles) {
-          if (i + 2 < ntiles) {
-            if (i >= 1) ptx::mbar_wait(bar_o, (i - 1) & 1);  // stage (i+2)%3 was last read by the dV/dK MMAs of step i-1
-            ptx::mbar_expect_tx(&bar_ld[(i + 2) % 3], 8192 * 2);
-            load_q(i + 2);
-          }
-          ptx::mbar_wait(&bar_ld[(i + 1) % 3], ((i + 1) / 3) & 1);
-          ptx::tc_fence_after();
-          issue_scores(i + 1);
-        }
-        ptx::mbar_wait(bar_ps, i & 1);  // P^T and dS^T of this step are in shared memory
-        uint8_t* sQ = sQO + (i % 3) * 16384;
-        const uint32_t idesc = ptx::make_idesc_bf16(128, HD, 0, 1);
-        const int ksteps = n16_of(i) >> 4;
-        for (int ks = 0; ks < ksteps; ++ks)  // dV += P^T dO_i
-          ptx::umma_f16(tmem + 192, desc_kmajor(ptx::smem_u32(sPT), ks), desc_mnmajor(ptx::smem_u32(sQ + 8192), ks), idesc,
-                        (i > 0 || ks > 0) ? 1u : 0u);
-        for (int ks = 0; ks < ksteps; ++ks)  // dK += dS^T Q_i
-          ptx::umma_f16(tmem + 128, desc_kmajor(ptx::smem_u32(sdST), ks), desc_mnmajor(ptx::smem_u32(sQ), ks), idesc,
-                        (i > 0 || ks > 0) ? 1u : 0u);
-        ptx::umma_commit(bar_o);
-      }
+  if (tid == 0) {
+    ptx::mbar_expect_tx(&bar_ld[0], 16384 * 2 + 8192 * 2);
+    tma_load_3d(sK, &tmK, &bar_ld[0], h * HD, kv0, b);
+    tma_load_3d(sV, &tmV, &bar_ld[0], h * HD, kv0, b);
+    load_q(0);
+    if (ntiles > 1) {
+      ptx::mbar_expect_tx(&bar_ld[1], 8192 * 2);
+      load_q(1);
     }
-  } else {
-  // ---- warps 0-7: math threads ------------------------------------------------------------------------------------
+  }
+  float dk[HD / 2], dv[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
   for (int i = 0; i < ntiles; ++i) {
     const int q0 = i * BWD_BN;
     const int nvalid = min(BWD_BN, p.Sq - q0);
     const int n16 = (nvalid + 15) & ~15;
-    float* sL = sLD;  // (the trailing math_sync of the previous step fenced its readers)
+    float* sL = sLD;
     float* sD = sL + 64;
     if (tid < BWD_BN) {
       const int qr = q0 + tid;
       sL[tid] = (qr < p.Sq) ? p.lse[stat_base + qr] * kLog2e : 0.f;
       sD[tid] = (qr < p.Sq) ? p.dvec[stat_base + qr] * p.scale : 0.f;  // pre-scaled: dS = P (dP*scale - D*scale)
     }
-    ptx::mbar_wait(bar_s, i & 1);
-    ptx::tc_fence_after();
-    uint32_t s_reg[32], d_reg[32];
+    if (tid == 0 && i + 2 < ntiles) {  // ring stage (i+2)%3 was last read in step i-1, which every thread has left
+      ptx::mbar_expect_tx(&bar_ld[(i + 2) % 3], 8192 * 2);
+      load_q(i + 2);
+    }
+    ptx::mbar_wait(&bar_ld[i % 3], (i / 3) & 1);
+    uint8_t* sQ = sQO + (i % 3) * 16384;
+    scores_to_smem(ptx::smem_u32(sK) + g * 8192, ptx::smem_u32(sQ), n16, HD / 16, sS, g * 64);
+    scores_to_smem(ptx::smem_u32(sV) + g * 8192, ptx::smem_u32(sQ) + 8192, n16, HD / 16, sdP, g * 64);
+    math_sync();  // S^T, dP^T and this step's lse / D are visible to all threads
+    float s_reg[32], d_reg[32];
     if (warp_active) {
 #pragma unroll
-    for (int cc = 0; cc < 32; cc += 16) {
-      const int c = half * 32 + cc;
-      if (c < n16) {
-        uint32_t a16[16], b16[16];
-        tmem_ld_32x32b_x16(t_row + c, a16);
-        tmem_ld_32x32b_x16(t_row + 64 + c, b16);
-#pragma unroll
-        for (int k = 0; k < 16; ++k) { s_reg[cc + k] = a16[k]; d_reg[cc + k] = b16[k]; }
+      for (int cc = 0; cc < 32; cc += 4) {
+        const int c = half * 32 + cc;
+        if (c < n16) {
+          const float4 a4 = *reinterpret_cast<const float4*>(sS + r * SP + c);
+          const float4 b4 = *reinterpret_cast<const float4*>(sdP + r * SP + c);
+          s_reg[cc] = a4.x; s_reg[cc + 1] = a4.y; s_reg[cc + 2] = a4.z; s_reg[cc + 3] = a4.w;
+          d_reg[cc] = b4.x; d_reg[cc + 1] = b4.y; d_reg[cc + 2] = b4.z; d_reg[cc + 3] = b4.w;
+        }
       }
     }
-    ptx::tmem_ld_wait();
-    }
-    ptx::tc_fence_before();
-    ptx::mbar_arrive(bar_free);  // (A) scores are in registers
-    math_sync();                 // sL / sD of this step are visible to all math threads
-    if (i >= 1) ptx::mbar_wait(bar_o, (i - 1) & 1);  // P^T / dS^T buffers were read by the MMAs of step i-1
 #pragma unroll
     for (int cc = 0; cc < 32; cc += 16) {
       const int c = half * 32 + cc;
@@ -755,13 +530,13 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
             dq_[k] = e.x; dq_[k + 1] = e.y; dq_[k + 2] = e.z; dq_[k + 3] = e.w;
           }
 #pragma unroll
-          for (int k = 0; k < 8; ++k) pt[k] = ex2(fmaf(__uint_as_float(s_reg[cc + k8 + k]), sl2, -lq[k]));
+          for (int k = 0; k < 8; ++k) pt[k] = ex2(fmaf(s_reg[cc + k8 + k], sl2, -lq[k]));
           if (nvalid < BWD_BN || !kv_ok) {  // ragged q tile / kv rows past the end of the sequence
 #pragma unroll
             for (int k = 0; k < 8; ++k) pt[k] = (kv_ok && c + k8 + k < nvalid) ? pt[k] : 0.f;
           }
 #pragma unroll
-          for (int k = 0; k < 8; ++k) ds[k] = pt[k] * fmaf(__uint_as_float(d_reg[cc + k8 + k]), p.scale, -dq_[k]);
+          for (int k = 0; k < 8; ++k) ds[k] = pt[k] * fmaf(d_reg[cc + k8 + k], p.scale, -dq_[k]);
           uint4 x, y;
           x.x = pack_bf16(pt[0], pt[1]); x.y = pack_bf16(pt[2], pt[3]);
           x.z = pack_bf16(pt[4], pt[5]); x.w = pack_bf16(pt[6], pt[7]);
@@ -773,48 +548,14 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
       }
     }
     ptx::fence_proxy_async();
-    ptx::mbar_arrive(bar_ps);  // (B) this thread's part of P^T / dS^T is visible to the tensor core
-    math_sync();               // all reads of sL / sD are done before the next step overwrites them
+    math_sync();  // P^T / dS^T are visible to the tensor core
+    mma_tile<HD, 1>(dv, ptx::smem_u32(sPT) + g * 8192, ptx::smem_u32(sQ) + 8192, n16 >> 4, i > 0);  // dV += P^T dO_i
+    mma_tile<HD, 1>(dk, ptx::smem_u32(sdST) + g * 8192, ptx::smem_u32(sQ), n16 >> 4, i > 0);         // dK += dS^T Q_i
+    math_sync();  // end of step: the score tiles, P^T / dS^T, lse / D and the ring stage are free again
   }
-  ptx::mbar_wait(bar_o, (ntiles - 1) & 1);
-  ptx::tc_fence_after();
-  bf16* krow = p.out0 + (static_cast<long long>(b) * p.Skv + kvrow) * p.out0_rs + h * HD + half * 32;
-  bf16* vrow = p.out1 + (static_cast<long long>(b) * p.Skv + kvrow) * p.out1_rs + h * HD + half * 32;
-#pragma unroll
-  for (int which = 0; which < 2; ++which) {
-    uint32_t rr[32];
-    if (HD == 64 || half == 0) {
-      ptx::tmem_ld_32x32b_x32(t_row + 128 + which * 64 + half * 32, rr);
-      ptx::tmem_ld_wait();
-    } else {
-      uint32_t r16[16];
-      tmem_ld_32x32b_x16(t_row + 128 + which * 64 + 32, r16);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int k = 0; k < 16; ++k) rr[k] = r16[k];
-    }
-    const int ncol = (HD == 64 || half == 0) ? 32 : HD - 32;
-    if (kv_ok) {
-      bf16* dst = which == 0 ? krow : vrow;
-#pragma unroll
-      for (int k = 0; k < 32; k += 8) {
-        if (k >= ncol) break;
-        uint4 v;
-        v.x = pack_bf16(__uint_as_float(rr[k]), __uint_as_float(rr[k + 1]));
-        v.y = pack_bf16(__uint_as_float(rr[k + 2]), __uint_as_float(rr[k + 3]));
-        v.z = pack_bf16(__uint_as_float(rr[k + 4]), __uint_as_float(rr[k + 5]));
-        v.w = pack_bf16(__uint_as_float(rr[k + 6]), __uint_as_float(rr[k + 7]));
-        *reinterpret_cast<uint4*>(dst + k) = v;
-      }
-    }
-  }
-  }  // math threads
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem, 256);
-  }
+  const long long base = static_cast<long long>(b) * p.Skv + kv0;
+  store_acc<HD>(dk, p.out0 + base * p.out0_rs + h * HD, p.out0_rs, g * 64, rows_here, nullptr);
+  store_acc<HD>(dv, p.out1 + base * p.out1_rs + h * HD, p.out1_rs, g * 64, rows_here, nullptr);
 }
 
 template <typename K>
@@ -881,7 +622,7 @@ static int attn_bwd_dq_tc_impl(const void* q, const void* k, const void* v, cons
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale;
   p.out0 = reinterpret_cast<bf16*>(dq); p.out0_rs = dq_rs; p.lse = const_cast<float*>(lse); p.dvec = dvec;
   p.tile_rows = tile_rows;
-  pdl_launch(dim3(ntile, nh, B), 288, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD>, tq, tdo, tk, tv, p);
+  pdl_launch(dim3(ntile, nh, B), 256, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD>, tq, tdo, tk, tv, p);
   *rows_done = Sq;
   return check_launch("attn_bwd_dq_tc");
 }
@@ -912,7 +653,7 @@ static int attn_bwd_dkdv_tc_impl(const void* q, const void* k, const void* v, co
   p.out0 = reinterpret_cast<bf16*>(dk); p.out0_rs = dk_rs; p.out1 = reinterpret_cast<bf16*>(dv); p.out1_rs = dv_rs;
   p.lse = const_cast<float*>(lse); p.dvec = const_cast<float*>(dvec);
   p.tile_rows = tile_rows;
-  pdl_launch(dim3(ntile, nh, B), 288, DKDV_SMEM, s)(attn_bwd_dkdv_tc_kernel<HD>, tk, tv, tq, tdo, p);
+  pdl_launch(dim3(ntile, nh, B), 256, DKDV_SMEM, s)(attn_bwd_dkdv_tc_kernel<HD>, tk, tv, tq, tdo, p);
   *rows_done = Skv;
   return check_launch("attn_bwd_dkdv_tc");
 }

@@ -38,7 +38,7 @@ int check_launch(const char* what) {
 }
 
 // kernels (defined in the other translation units)
-int gemm_tcgen05(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, cudaStream_t, void*, long long);
+int gemm_tc(const void*, const void*, void*, const float*, int, int, int, int, int, int, int, int, int, cudaStream_t, void*, long long);
 long long gemm_splitk_workspace_bytes(int, int, int);
 void set_reserved_sms(int);
 int pack_bf16(const void*, int, long long, cudaStream_t);
@@ -128,13 +128,13 @@ int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int 
                    int ldc, int a_mn, int b_mn, int epilogue, void* stream) {
   if (epilogue == MUSE_EPI_RESADD_F32 && res == nullptr) { set_last_error("gemm: RESADD epilogue needs res"); return MUSE_ERR_INVALID; }
   if (epilogue == MUSE_EPI_SPLITK_F32) { set_last_error("gemm: the deterministic split-K epilogue goes through muse_gemm_bf16_splitk"); return MUSE_ERR_INVALID; }
-  return gemm_tcgen05(A, B, C, res, M, N, K, lda, ldb, ldc, a_mn, b_mn, epilogue, ST(stream), nullptr, 0);
+  return gemm_tc(A, B, C, res, M, N, K, lda, ldb, ldc, a_mn, b_mn, epilogue, ST(stream), nullptr, 0);
 }
 
 long long muse_gemm_splitk_workspace_bytes(int M, int N, int K) { return gemm_splitk_workspace_bytes(M, N, K); }
 int muse_gemm_bf16_splitk(const void* A, const void* B, float* C, int M, int N, int K, int lda, int ldb, int ldc,
                           int a_mn, int b_mn, void* ws, long long ws_bytes, void* stream) {
-  return gemm_tcgen05(A, B, C, nullptr, M, N, K, lda, ldb, ldc, a_mn, b_mn, MUSE_EPI_SPLITK_F32, ST(stream), ws, ws_bytes);
+  return gemm_tc(A, B, C, nullptr, M, N, K, lda, ldb, ldc, a_mn, b_mn, MUSE_EPI_SPLITK_F32, ST(stream), ws, ws_bytes);
 }
 
 int muse_pack_bf16(const void* table_dev, int n_entries, long long total_blocks, void* stream) {

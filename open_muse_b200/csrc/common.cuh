@@ -23,7 +23,7 @@ int check_launch(const char* what);
 // The hot paths are chains of 300 - 900 short kernels on one stream (a train step, a captured generate2 loop); a plain
 // stream edge costs a full drain + launch between two kernels.  Every kernel of this library therefore (i) tells the
 // hardware right away that its successor may be scheduled (griddepcontrol.launch_dependents: the successor's CTAs take
-// the SM slots that free up while the tail of this grid drains, and run their prologue -- barrier init, TMEM allocation,
+// the SM slots that free up while the tail of this grid drains, and run their prologue -- barrier init,
 // tensor-map prefetch), and (ii) blocks in griddepcontrol.wait before its first global-memory access until the
 // predecessor grid has COMPLETED and its writes are visible.  Correctness never depends on the trigger: with wait in
 // front of every global access (reads AND writes, so there is no WAR hazard either) the order of memory effects is the

@@ -1,4 +1,4 @@
-// MaskGitVQGAN convolutions on the 5th-gen tensor cores (muse/modeling_maskgit_vqgan.py:33-45 Conv2dSame, stride 1,
+// MaskGitVQGAN convolutions on the Hopper tensor cores (wgmma) (muse/modeling_maskgit_vqgan.py:33-45 Conv2dSame, stride 1,
 // k = 3 or 1) as an implicit GEMM with fp32-faithful accuracy:
 //
 //     y[m, co] = bias[co] + res[m, co] + sum_{tap, ci} x[pixel(m) + tap, ci] * w[co, tap, ci]
@@ -8,10 +8,10 @@
 // * No im2col buffer: activations stay NHWC and the A tile of one (tap, 64-channel chunk) is ONE 4-D TMA box
 //   {64 ch, tile_w, tile_h, 1 image} fetched at pixel offset (kw - pad, kh - pad); coordinates outside the image are
 //   zero-filled by the TMA unit, which is exactly the 'same' padding.  The box lands in shared memory as 128 rows x 128 B
-//   (128-byte swizzle) = a K-major tcgen05 operand, rows ordered like the output pixels of the tile.
+//   (128-byte swizzle) = a K-major wgmma operand, rows ordered like the output pixels of the tile.
 // * fp32 accuracy from bf16 tensor cores: every fp32 operand is carried as two bf16 planes  v = hi + lo
 //   (hi = bf16(v), lo = bf16(v - hi), representation error 2^-18 |v|) and the product is accumulated as
-//   hi*hi + lo*hi + hi*lo in the fp32 TMEM accumulator (the dropped lo*lo term is ~2^-18 relative).  The token ids of the
+//   hi*hi + lo*hi + hi*lo in the fp32 register accumulator (the dropped lo*lo term is ~2^-18 relative).  The token ids of the
 //   quantiser downstream need this: a single bf16/TF32 pass perturbs z by ~1e-3 and flips near-tie codes (SURVEY H1).
 //   The planes are produced by the preceding GroupNorm+SiLU kernel (same bytes as one fp32 tensor) or by
 //   split_bf16_nhwc (which also folds the nearest x2 upsample of UpsamplingBlock :146 into its gather).
@@ -19,11 +19,12 @@
 //   arithmetic: output pixel (2y+py, 2x+px) only sees a 2x2 window of the low-resolution input, so each of the four
 //   parities (py, px) is a 2x2 convolution with pre-summed weights (K = 4*C_in instead of 9*C_in, 2.25x fewer FLOPs)
 //   whose tile rows scatter to every other output pixel.
-// * Same persistent warp-specialised pipeline as gemm_tcgen05.cu: warp 0 TMA producer, warp 1 MMA issuer
-//   (tcgen05.mma 128 x BN x 16, kind::f16), warp 2 TMEM allocator, warps 4-7 epilogue with double-buffered TMEM
-//   accumulators; epilogue adds bias / residual and writes fp32 NHWC rows through a padded smem staging slab.
+// * Same persistent warp-specialised pipeline as gemm_wgmma.cu: one TMA producer thread, two consumer warpgroups
+//   (wgmma m64 x BN x k16 on their 64-pixel halves of the tile); the epilogue adds bias / residual to the accumulator
+//   registers, writes fp32 NHWC rows and folds the per-channel GroupNorm statistics of the tile.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace muse {
 
@@ -41,12 +42,9 @@ struct Cfg {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;  // a multiple of 1024 for BN in {16, 128, 256}
-  static constexpr int kTmemCols = 2 * BN;               // 32 (the minimum allocation) for BN = 16
   static constexpr int kBarBytes = 256;
-  static constexpr int kStagingRowBytes = 144;
-  static constexpr int kStagingBytes = 4 * 32 * kStagingRowBytes;
-  static constexpr int kStatBytes = 4 * BN * 2 * 4;  // per-epilogue-warp {sum, sumsq} of every tile column
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + kStatBytes + 1024 + kBarBytes;
+  static constexpr int kStatBytes = 8 * BN * 2 * 4;  // per-consumer-warp {sum, sumsq} of every tile column
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStatBytes + 1024 + kBarBytes;
 };
 
 struct ConvParams {
@@ -81,73 +79,41 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// SWAP (used for C_out == 128, the full-resolution layers): the roles of the operands are exchanged so that the MMA
-// is 128 (output channels, A = weights) x 256 (pixels, B = activations) instead of 128 pixels x 128 channels.  A 128-wide
-// N reads 128 B/clk of operands from shared memory per MMA -- the shared-memory bandwidth limit -- while N = 256 needs
-// 96 B/clk (measured: 0.99 vs 1.34 PFLOP/s).  The accumulator then holds one output channel per TMEM lane and one pixel per
-// column; a warp store of one column is 32 consecutive channels = one full 128-byte segment of the NHWC output.
-template <int BN, bool SWAP>
-__global__ void __launch_bounds__(256, 1)
+template <int BN>
+__global__ void __launch_bounds__(384, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const ConvParams p) {
   pdl_trigger();
   using C_ = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* staging = smem + C_::kStages * C_::kStageBytes;
-  float* stat_smem = reinterpret_cast<float*>(staging + C_::kStagingBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + C_::kStagingBytes + C_::kStatBytes);
+  float* stat_smem = reinterpret_cast<float*>(smem + C_::kStages * C_::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::kStages * C_::kStageBytes + C_::kStatBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + C_::kStages;
-  uint64_t* tmem_full = bars + 2 * C_::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmAh);
     ptx::prefetch_tmap(&tmAl);
     ptx::prefetch_tmap(&tmBh);
     ptx::prefetch_tmap(&tmBl);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < C_::kStages; ++i) {
       ptx::mbar_init(&full_bar[i], 1);
-      ptx::mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      ptx::mbar_init(&tmem_full[i], 1);
-      ptx::mbar_init(&tmem_empty[i], 128);
+      ptx::mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
     }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(tmem_holder, C_::kTmemCols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  pdl_wait();  // everything above touches only shared memory / TMEM / kernel parameters
-  const uint32_t tmem_base = *tmem_holder;
+  pdl_wait();  // everything above touches only shared memory / kernel parameters
   const int tiles_mn = p.num_m * p.num_n;
   const int total_tiles = tiles_mn * (p.up ? 4 : 1);
   const int pad = p.ksize / 2;
 
-  if (warp == 0) {
-    if (ptx::elect_one()) {
+  if (wg == 0) {
+    ptx::setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       // ------------------------------------------------------------ TMA producer
       int stage = 0;
       uint32_t phase = 0;
@@ -170,13 +136,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
           const int dy = p.up ? (tap >> 1) + (parity >> 1) - 1 : (p.fwd2x2 ? (tap >> 1) : tap / p.ksize - pad);
           const int dx = p.up ? (tap & 1) + (parity & 1) - 1 : (p.fwd2x2 ? (tap & 1) : tap % p.ksize - pad);
           const int wb = p.wbatch ? img : 0;
-          if (!SWAP) {
-            tma_load_4d(sa, pass == 1 ? &tmAl : &tmAh, &full_bar[stage], cc * BK, x0 + dx, y0 + dy, img);
-            tma_load_3d(sb, pass == 2 ? &tmBl : &tmBh, &full_bar[stage], tap * p.Cin + cc * BK, wrow0 + n0, wb);
-          } else {  // A = 128 weight rows, B = 256 pixels
-            tma_load_3d(sa, pass == 2 ? &tmBl : &tmBh, &full_bar[stage], tap * p.Cin + cc * BK, wrow0 + n_idx * 128, wb);
-            tma_load_4d(sb, pass == 1 ? &tmAl : &tmAh, &full_bar[stage], cc * BK, x0 + dx, y0 + dy, img);
-          }
+          tma_load_4d(sa, pass == 1 ? &tmAl : &tmAh, &full_bar[stage], cc * BK, x0 + dx, y0 + dy, img);
+          tma_load_3d(sb, pass == 2 ? &tmBl : &tmBh, &full_bar[stage], tap * p.Cin + cc * BK, wrow0 + n0, wb);
           if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
           if (++pass == p.passes) {
             pass = 0;
@@ -185,50 +146,40 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (ptx::elect_one()) {
-      // ------------------------------------------------------------ MMA issuer
-      constexpr uint32_t idesc = ptx::make_idesc_bf16(BM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        ptx::mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint32_t a_addr = ptx::smem_u32(smem + stage * C_::kStageBytes);
-          const uint32_t b_addr = a_addr + C_::kABytes;
+  } else {
+    ptx::setmaxnreg_inc<232>();
+    // -------------------------------------------------------------- consumers: y = acc + bias (+ res), fp32 NHWC
+    const int half = wg - 1;
+    const int t = threadIdx.x & 127;
+    const int cw = threadIdx.x / 32 - 4;                         // consumer warp 0..7
+    const int lr = half * 64 + (t >> 5) * 16 + ((t & 31) >> 2);  // tile pixel of d[4j], d[4j+1]; +8 for d[4j+2..3]
+    const int lc = 2 * (t & 3);
+    float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t adesc = ptx::make_smem_desc_sw128(a_addr + k * 32, 16, 1024);
-            const uint64_t bdesc = ptx::make_smem_desc_sw128(b_addr + k * 32, 16, 1024);
-            ptx::umma_f16(d_tmem, adesc, bdesc, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          ptx::umma_commit(&empty_bar[stage]);
-          if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
-        }
-        ptx::umma_commit(&tmem_full[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // -------------------------------------------------------------- epilogue: y = acc + bias (+ res), fp32 NHWC
-    const int ew = warp - 4;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    uint8_t* stg = staging + ew * (32 * C_::kStagingRowBytes);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = ptx::smem_u32(smem + stage * C_::kStageBytes) + half * 8192;
+        const uint32_t b_addr = ptx::smem_u32(smem + stage * C_::kStageBytes + C_::kABytes);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          ptx::Wgmma<BN, 0, 0>::run(acc, ptx::make_smem_desc_sw128(a_addr + k * 32, 16, 1024),
+                                    ptx::make_smem_desc_sw128(b_addr + k * 32, 16, 1024), (kb > 0 || k > 0) ? 1 : 0);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);
+        if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
+      }
       const int parity = tile / tiles_mn, tl = tile % tiles_mn;
       const int n_idx = tl % p.num_n;
       const int m_idx = tl / p.num_n;
       const int img = m_idx / p.tiles_per_img;
-      const int t = m_idx % p.tiles_per_img;
-      const int y0 = (t / p.tiles_x) * p.tile_h, x0 = (t % p.tiles_x) * p.tile_w;
+      const int tt = m_idx % p.tiles_per_img;
+      const int y0 = (tt / p.tiles_x) * p.tile_h, x0 = (tt % p.tiles_x) * p.tile_w;
       const long long row_base0 = (static_cast<long long>(img) * p.H + y0) * p.W + x0;  // tile pixels are contiguous
       // output row (pixel index) of tile-local pixel tr; up: parity (py, px) scatters to every other pixel of the 2H x 2W grid
       auto out_row = [&](int tr) -> long long {
@@ -236,195 +187,70 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         const int ty = tr >> p.tile_w_log2, tx = tr & (p.tile_w - 1);
         return (static_cast<long long>(img) * (2 * p.H) + 2 * (y0 + ty) + (parity >> 1)) * (2 * p.W) + 2 * (x0 + tx) + (parity & 1);
       };
-      const size_t stat_row = p.up ? (static_cast<size_t>(img) * 4 + parity) * p.tiles_per_img + t : static_cast<size_t>(m_idx);
+      const size_t stat_row = p.up ? (static_cast<size_t>(img) * 4 + parity) * p.tiles_per_img + tt : static_cast<size_t>(m_idx);
       const int n0 = n_idx * BN;
-      // (each branch waits for the accumulator only after issuing its first residual fetch)
-      const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + static_cast<uint32_t>(acc * BN);
-      if (SWAP) {
-        // thread = output channel (TMEM lane), columns = the tile's 256 pixels.  Each 32-pixel slab is transposed through
-        // the warp's staging buffer ([pixel][32 channels], padded rows) so that the global stores are 16 bytes per lane and
-        // 8 lanes cover the 128-byte channel segment of one pixel (4x fewer store instructions than storing columns).
-        const int chq = lane & 7;                          // 4-channel chunk handled in the store phase
-        const int gch = n_idx * 128 + ew * 32 + chq * 4;   // first of its 4 output channels
-        float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias != nullptr) b4 = *reinterpret_cast<const float4*>(p.bias + gch);
-        float st_s[4] = {0.f, 0.f, 0.f, 0.f}, st_q[4] = {0.f, 0.f, 0.f, 0.f};
-        // the residual slab is fetched one slab ahead (first one before the accumulator is even ready)
-        float4 res_next[8];
-        auto fetch_res = [&](int c, float4 (&dst)[8]) {
+      const long long orow[2] = {out_row(lr), out_row(lr + 8)};
 #pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            dst[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c < BN)
-              dst[it] = *reinterpret_cast<const float4*>(p.res + static_cast<size_t>(out_row(c + (lane >> 3) + 4 * it)) * p.N + gch);
-          }
-        };
-        if (p.res != nullptr) fetch_res(0, res_next);
-        ptx::mbar_wait(&tmem_full[acc], acc_phase);
-        ptx::tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-          float4 res_cur[8];
-          if (p.res != nullptr) {
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + lc;
+        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+        if (BN == 16) {  // narrow head (C_out <= 16, e.g. the 3-channel pixel output): element-wise, no statistics
 #pragma unroll
-            for (int it = 0; it < 8; ++it) res_cur[it] = res_next[it];
-            fetch_res(c + 32, res_next);
-          }
-          uint32_t r[32];
-          ptx::tmem_ld_32x32b_x32(lane_addr + c, r);
-          ptx::tmem_ld_wait();
+          for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
-          for (int jj = 0; jj < 32; ++jj)
-            *reinterpret_cast<uint32_t*>(stg + jj * C_::kStagingRowBytes + lane * 4) = r[jj];
-          __syncwarp();
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = (lane >> 3) + 4 * it;  // pixel c + rr of the tile
-            const float4 v = *reinterpret_cast<const float4*>(stg + rr * C_::kStagingRowBytes + chq * 16);
-            const size_t off = static_cast<size_t>(out_row(c + rr)) * p.N + gch;
-            float4 o = make_float4(v.x + b4.x, v.y + b4.y, v.z + b4.z, v.w + b4.w);
-            if (p.res != nullptr) {
-              const float4 q4 = res_cur[it];
-              o.x += q4.x; o.y += q4.y; o.z += q4.z; o.w += q4.w;
+            for (int e = 0; e < 2; ++e) {
+              if (col + e < p.N) {
+                const size_t off = static_cast<size_t>(orow[hr]) * p.N + col + e;
+                float v = acc[4 * j + 2 * hr + e];
+                if (p.bias != nullptr) v += p.bias[col + e];
+                if (p.res != nullptr) v += p.res[off];
+                p.y[off] = v;
+              }
             }
-            *reinterpret_cast<float4*>(p.y + off) = o;
-            st_s[0] += o.x; st_s[1] += o.y; st_s[2] += o.z; st_s[3] += o.w;
-            st_q[0] = fmaf(o.x, o.x, st_q[0]); st_q[1] = fmaf(o.y, o.y, st_q[1]);
-            st_q[2] = fmaf(o.z, o.z, st_q[2]); st_q[3] = fmaf(o.w, o.w, st_q[3]);
-          }
-          __syncwarp();
-        }
-        if (p.stats != nullptr) {  // this warp owns its 32 channels: fold the 4 row groups, lanes 0-7 publish
+        } else if (col < p.N) {  // N % 4 == 0
+          float2 b2 = make_float2(0.f, 0.f);
+          if (p.bias != nullptr) b2 = *reinterpret_cast<const float2*>(p.bias + col);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            st_s[k] += __shfl_xor_sync(0xffffffffu, st_s[k], 8);
-            st_s[k] += __shfl_xor_sync(0xffffffffu, st_s[k], 16);
-            st_q[k] += __shfl_xor_sync(0xffffffffu, st_q[k], 8);
-            st_q[k] += __shfl_xor_sync(0xffffffffu, st_q[k], 16);
-          }
-          if (lane < 8) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              *reinterpret_cast<float2*>(p.stats + (stat_row * p.N + gch + k) * 2) = make_float2(st_s[k], st_q[k]);
-          }
-        }
-      } else if (BN == 16) {
-        ptx::mbar_wait(&tmem_full[acc], acc_phase);
-        ptx::tc_fence_after();
-        // narrow head (C_out <= 16, e.g. the 3-channel pixel output): one row per thread, rows of N floats are
-        // contiguous across the warp, so registers go straight to global
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(lane_addr, r);
-        ptx::tmem_ld_wait();
-        const size_t off = static_cast<size_t>(out_row(ew * 32 + lane)) * p.N;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          if (j < p.N) {
-            float v = __uint_as_float(r[j]);
-            if (p.bias != nullptr) v += p.bias[j];
-            if (p.res != nullptr) v += p.res[off + j];
-            p.y[off + j] = v;
-          }
-        }
-      }
-      float4 nres_next[8];
-      auto nfetch_res = [&](int c, float4 (&dst)[8]) {
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int gcol = n0 + c + (lane & 7) * 4;
-          dst[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (c < BN && gcol < p.N)
-            dst[it] = *reinterpret_cast<const float4*>(p.res + static_cast<size_t>(out_row(ew * 32 + (lane >> 3) + 4 * it)) * p.N + gcol);
-        }
-      };
-      if (!SWAP && BN != 16) {
-        if (p.res != nullptr) nfetch_res(0, nres_next);
-        ptx::mbar_wait(&tmem_full[acc], acc_phase);
-        ptx::tc_fence_after();
-      }
-#pragma unroll 1
-      for (int c = 0; c < ((BN == 16 || SWAP) ? 0 : BN); c += 32) {
-        if (n0 + c >= p.N) break;
-        float4 nres_cur[8];
-        if (p.res != nullptr) {
-#pragma unroll
-          for (int it = 0; it < 8; ++it) nres_cur[it] = nres_next[it];
-          nfetch_res(c + 32, nres_next);
-        }
-        uint4* my_row = reinterpret_cast<uint4*>(stg + lane * C_::kStagingRowBytes);
-        uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(lane_addr + c, r);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int q = 0; q < 8; ++q) my_row[q] = make_uint4(r[4 * q], r[4 * q + 1], r[4 * q + 2], r[4 * q + 3]);
-        __syncwarp();
-        const int ch = lane & 7;
-        const int gcol = n0 + c + ch * 4;
-        const bool col_ok = gcol < p.N;  // N % 4 == 0
-        float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias != nullptr && col_ok) b4 = *reinterpret_cast<const float4*>(p.bias + gcol);
-        float st_s[4] = {0.f, 0.f, 0.f, 0.f}, st_q[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int rr = (lane >> 3) + 4 * it;
-          const float4 v = *reinterpret_cast<const float4*>(stg + rr * C_::kStagingRowBytes + ch * 16);
-          if (col_ok) {
-            const size_t off = static_cast<size_t>(out_row(ew * 32 + rr)) * p.N + gcol;
-            float4 o = make_float4(v.x + b4.x, v.y + b4.y, v.z + b4.z, v.w + b4.w);
+          for (int hr = 0; hr < 2; ++hr) {
+            const size_t off = static_cast<size_t>(orow[hr]) * p.N + col;
+            float2 o = make_float2(acc[4 * j + 2 * hr] + b2.x, acc[4 * j + 2 * hr + 1] + b2.y);
             if (p.res != nullptr) {
-              const float4 q4 = nres_cur[it];
-              o.x += q4.x; o.y += q4.y; o.z += q4.z; o.w += q4.w;
+              const float2 r2 = *reinterpret_cast<const float2*>(p.res + off);
+              o.x += r2.x; o.y += r2.y;
             }
-            *reinterpret_cast<float4*>(p.y + off) = o;
-            st_s[0] += o.x; st_s[1] += o.y; st_s[2] += o.z; st_s[3] += o.w;
-            st_q[0] = fmaf(o.x, o.x, st_q[0]); st_q[1] = fmaf(o.y, o.y, st_q[1]);
-            st_q[2] = fmaf(o.z, o.z, st_q[2]); st_q[3] = fmaf(o.w, o.w, st_q[3]);
+            *reinterpret_cast<float2*>(p.y + off) = o;
+            s0 += o.x; s1 += o.y;
+            q0 = fmaf(o.x, o.x, q0); q1 = fmaf(o.y, o.y, q1);
           }
         }
-        if (p.stats != nullptr) {  // fold the 4 row groups of the warp (lane >> 3), lanes 0-7 publish 4 channels each
+        if (BN != 16 && p.stats != nullptr) {  // fold the 8 row groups of the warp (lane >> 2); lanes 0-3 publish
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            st_s[k] += __shfl_xor_sync(0xffffffffu, st_s[k], 8);
-            st_s[k] += __shfl_xor_sync(0xffffffffu, st_s[k], 16);
-            st_q[k] += __shfl_xor_sync(0xffffffffu, st_q[k], 8);
-            st_q[k] += __shfl_xor_sync(0xffffffffu, st_q[k], 16);
+          for (int o = 4; o < 32; o <<= 1) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+            q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+            q1 += __shfl_xor_sync(0xffffffffu, q1, o);
           }
-          if (lane < 8) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              *reinterpret_cast<float2*>(stat_smem + ((ew * BN) + c + lane * 4 + k) * 2) = make_float2(st_s[k], st_q[k]);
-          }
+          if ((t & 31) < 4)
+            *reinterpret_cast<float4*>(stat_smem + (cw * BN + 8 * j + lc) * 2) = make_float4(s0, q0, s1, q1);
         }
-        __syncwarp();
       }
-      if (!SWAP && BN != 16 && p.stats != nullptr) {
-        ptx::tc_fence_before();
-        asm volatile("bar.sync 1, 128;" ::: "memory");  // the four epilogue warps
-        for (int col = threadIdx.x - 128; col < BN; col += 128) {
+      if (BN != 16 && p.stats != nullptr) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");  // the eight consumer warps
+        for (int col = threadIdx.x - 128; col < BN; col += 256) {
           if (n0 + col < p.N) {
             float2 a = make_float2(0.f, 0.f);
 #pragma unroll
-            for (int wq = 0; wq < 4; ++wq) {
+            for (int wq = 0; wq < 8; ++wq) {
               const float2 v = *reinterpret_cast<const float2*>(stat_smem + ((wq * BN) + col) * 2);
               a.x += v.x; a.y += v.y;
             }
             *reinterpret_cast<float2*>(p.stats + (stat_row * p.N + n0 + col) * 2) = a;
           }
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        asm volatile("bar.sync 1, 256;" ::: "memory");
       }
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(&tmem_empty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, C_::kTmemCols);
   }
 }
 
@@ -543,15 +369,15 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sms <= 0) g_sms = 148;
+    if (g_sms <= 0) g_sms = 132;
   }
   return g_sms;
 }
 
-template <int BN, bool SWAP = false>
+template <int BN>
 int launch_conv(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                 const ConvParams& p, cudaStream_t s) {
-  auto kern = conv_tc_kernel<BN, SWAP>;
+  auto kern = conv_tc_kernel<BN>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes);
@@ -560,7 +386,7 @@ int launch_conv(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap&
   }
   const int total = p.num_m * p.num_n;
   const int grid = total < sm_count() ? total : sm_count();
-  pdl_launch(grid, 256, Cfg<BN>::kSmemBytes, s)(kern, ah, al, bh, bl, p);
+  pdl_launch(grid, 384, Cfg<BN>::kSmemBytes, s)(kern, ah, al, bh, bl, p);
   return check_launch("conv_tc");
 }
 
@@ -575,11 +401,6 @@ int conv2d_tc_supported(int H, int W, int Cin, int Cout, int ksize) {
   return H % (128 / W) == 0;
 }
 
-// x_hi/x_lo: bf16 [B,H,W,Cin]; w_hi/w_lo: bf16 [Cout, k*k*Cin] (tap-major, then input channel); y fp32 [B,H,W,Cout].
-static bool use_swap(int H, int W, int Cout) {
-  return Cout == 128 && (W >= 256 ? W % 256 == 0 : (256 % W == 0 && H % (256 / W) == 0));
-}
-
 // Pixel tiles per image of conv2d_tc for this shape (= the leading extent of its stats output), 0 if unsupported.
 // H, W are the OUTPUT dims; with upsample2x the tiling runs on the H/2 x W/2 input grid, four parities each.
 int conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int upsample2x) {
@@ -588,7 +409,7 @@ int conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int up
     H /= 2; W /= 2;
   }
   if (!conv2d_tc_supported(H, W, Cin, Cout, ksize)) return 0;
-  return (upsample2x ? 4 : 1) * (H * W / (use_swap(H, W, Cout) ? 256 : 128));
+  return (upsample2x ? 4 : 1) * (H * W / 128);
 }
 
 // mode & 3 == 1 (upsample2x): x planes are the LOW-resolution input [B,H/2,W/2,Cin] and w planes the four stacked parity
@@ -598,6 +419,7 @@ int conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int up
 // mode & 4: per-image weights, w planes are [B][Cout][K].
 // mode & 8: single-pass bf16 (fast tokenizer mode): only the hi planes are multiplied (x_lo / w_lo may be null): one tensor-core
 //   product per fp32 product instead of three, bf16-operand accuracy (~4e-3 per layer instead of ~2e-5).
+// x_hi/x_lo: bf16 [B,H,W,Cin]; w_hi/w_lo: bf16 [Cout, k*k*Cin] (tap-major, then input channel); y fp32 [B,H,W,Cout].
 int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias, const float* res,
               float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode, cudaStream_t s) {
   if (B <= 0) return MUSE_OK;
@@ -623,9 +445,7 @@ int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* 
   ConvParams p;
   p.y = y; p.bias = bias; p.res = res; p.stats = (Cout > 16) ? stats : nullptr;
   p.N = Cout; p.H = H; p.W = W; p.Cin = Cin; p.ksize = ksize;
-  // C_out == 128: swapped operands, 256-pixel tiles (needs the image to tile into 256-pixel boxes)
-  const bool swap = use_swap(H, W, Cout);
-  const int tile_px = swap ? 256 : 128;
+  const int tile_px = 128;
   p.tile_w = W >= tile_px ? tile_px : W;
   p.tile_h = tile_px / p.tile_w;
   p.tiles_x = W / p.tile_w;
@@ -637,8 +457,8 @@ int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* 
   p.tile_w_log2 = 0;
   while ((1 << p.tile_w_log2) < p.tile_w) ++p.tile_w_log2;
   if (p.up && (1 << p.tile_w_log2) != p.tile_w) { set_last_error("conv2d_tc: upsample needs a power-of-two tile width"); return MUSE_ERR_UNSUPPORTED; }
-  const int BN = (swap || Cout >= 256) ? 256 : (Cout > 16 ? 128 : 16);
-  p.num_n = swap ? 1 : ceil_div(Cout, BN);
+  const int BN = Cout >= 256 ? 256 : (Cout > 16 ? 128 : 16);
+  p.num_n = ceil_div(Cout, BN);
   p.cchunks = Cin / BK;
   const int taps = (p.up || p.fwd2x2) ? 4 : ksize * ksize;
   p.passes = (mode & 8) ? 1 : 3;
@@ -656,10 +476,9 @@ int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* 
   const unsigned long long wrows = (unsigned long long)Cout * (p.up ? 4 : 1);
   const unsigned long long bdims[3] = {K, wrows, (unsigned long long)(p.wbatch ? B : 1)};
   const unsigned long long bstr[2] = {K * 2, K * 2 * wrows};
-  const unsigned bbox[3] = {64, swap ? 128u : (unsigned)BN, 1};
+  const unsigned bbox[3] = {64, (unsigned)BN, 1};
   if ((rc = make_tmap_nd(&bh, w_hi, 3, bdims, bstr, bbox))) return rc;
   if ((rc = make_tmap_nd(&bl, w_lo, 3, bdims, bstr, bbox))) return rc;
-  if (swap) return launch_conv<256, true>(ah, al, bh, bl, p, s);
   if (BN == 256) return launch_conv<256>(ah, al, bh, bl, p, s);
   if (BN == 128) return launch_conv<128>(ah, al, bh, bl, p, s);
   return launch_conv<16>(ah, al, bh, bl, p, s);

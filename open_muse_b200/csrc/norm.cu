@@ -128,8 +128,7 @@ __global__ void __launch_bounds__(1024) colsum_ordered_kernel(const float* __res
 }
 
 // L2 prefetch (a hint: no register, no scoreboard entry).  The persistent row-streaming backward kernels are bound by
-// exposed load latency, not by issue slots or DRAM bandwidth (ncu, profiles/r02_ncu_glu_bwd.txt: 60 % of the warp samples
-// sit on the first use of a loaded value, DRAM at 51 %, issue slots at 59 %).  A warp walks its rows strictly one after the
+// exposed load latency rather than by issue slots or DRAM bandwidth.  A warp walks its rows strictly one after the
 // other, so the lines of the row it will touch NEXT are requested from HBM while the current row is processed and the demand
 // loads become L2 hits.  prefetch_row: the lanes of a warp cover the 128-byte lines of one row of H elements.
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
@@ -138,9 +137,8 @@ __device__ __forceinline__ void prefetch_row(const T* row, int H, int lane) {
   const int bytes = H * static_cast<int>(sizeof(T));
   for (int off = lane * 128; off < bytes; off += 32 * 128) prefetch_l2(reinterpret_cast<const char*>(row) + off);
 }
-// Measured on one box, same call (profiles/r02_ab_row_prefetch.log): LayerNorm backward 87.5 -> 78.0 us and 71.3 -> 62.1 us
-// (next-row prefetch), GLU + LayerNorm backward 384 -> 361 us (two-iterations-ahead prefetch).  The kernels take the switch as
-// an argument so that the A/B needs one binary.
+// Next-row prefetch for the LayerNorm backward, two iterations ahead for GLU + LayerNorm backward.  The kernels take the
+// switch as an argument so that an A/B comparison needs one binary.
 constexpr int kRowPrefetch = 1;
 
 template <typename TDY, typename TX, typename TDX, int CH>
@@ -870,10 +868,10 @@ int fwd_dispatch(const void* x, const float* w, const float* res, void* y, float
 }
 
 int bwd_grid(int rows, int H, int act) {
-  if (act == ACT_GLU) { const int g = ceil_div(rows, kGluWarps); return g > 148 * 3 ? 148 * 3 : g; }
-  if (H <= 1024) { const int g = ceil_div(rows, kBwdWarps); return g > 148 * 4 ? 148 * 4 : g; }
+  if (act == ACT_GLU) { const int g = ceil_div(rows, kGluWarps); return g > 132 * 3 ? 132 * 3 : g; }
+  if (H <= 1024) { const int g = ceil_div(rows, kBwdWarps); return g > 132 * 4 ? 132 * 4 : g; }
   const int g = ceil_div(rows, kWideWarps);
-  return g > 148 * 4 ? 148 * 4 : g;
+  return g > 132 * 4 ? 132 * 4 : g;
 }
 
 int reduce_dw(const float* dw_ws, float* dw, int grid, int H, cudaStream_t s) {

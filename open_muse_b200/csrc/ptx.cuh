@@ -1,7 +1,6 @@
-// sm_100a PTX wrappers used by the tcgen05 GEMM: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05.{alloc,mma,commit,ld,fence}. Hand-written inline PTX (no CUTLASS dependency).
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor"
-// tables (same fields CUTLASS's cute/arch/mma_sm100_desc.hpp documents).
+// sm_90a PTX wrappers of the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma smem descriptors.
+// Hand-written inline PTX (no CUTLASS dependency).  Descriptor bit layouts follow the PTX ISA wgmma
+// "matrix descriptor" table (the same fields CUTLASS's cute/arch/mma_sm90_desc.hpp documents).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -76,85 +75,27 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued tcgen05.mma of this thread arrive on the mbarrier when complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp receives lane (base_lane+i), columns c..c+31.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
+// ---------------------------------------------------------------- warpgroup helpers
+// Register budget of a warpgroup in a warp-specialised kernel: the TMA producer gives registers back, the MMA
+// warpgroups take them (the accumulator fragments live in registers).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(R)); }
 
-// Shared-memory matrix descriptor (64-bit). Fields (PTX ISA, tcgen05 "matrix descriptor"):
+// Shared-memory matrix descriptor of wgmma (64-bit). Fields (PTX ISA, "matrix descriptor format" of wgmma):
 //  [0,14)  start address >> 4      [16,30) leading-dim byte offset >> 4
-//  [32,46) stride-dim byte offset >> 4   [46,48) version = 1 on sm_100
-//  [49,52) base offset (0: tiles are 1024B aligned)   [61,64) swizzle: 2 = 128B
+//  [32,46) stride-dim byte offset >> 4   [49,52) base offset (0: tiles are 1024B aligned)   [62,64) swizzle: 1 = 128B
+// K-major SW128 tiles: SBO = 1024 (8-row groups), LBO unused.  MN-major SW128 tiles: LBO = byte distance of the 64-element
+// MN chunks, SBO = 1024 (8-k-row groups).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
                                                          uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32.
-//  [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt (1 = bf16)
-//  [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn) << 15) |
-         (static_cast<uint32_t>(b_mn) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 }  // namespace ptx

@@ -7,7 +7,7 @@ Same constructor / config keys / parameter names (``encoder.down.{l}.block.{b}.c
 Hot-path status (see DESIGN.md):
   * tokenise search (``VectorQuantizer``: distances + arg-min, :303-316,342-348) and detokenise lookup
     (``get_codebook_entry``, :318-324) run in libmuse_b200 kernels with a bit-exact contract (csrc/vq.cu).
-  * the convolutional encoder / decoder (GroupNorm+SiLU+3x3 conv stacks) run as tcgen05 implicit-GEMM convolutions
+  * the convolutional encoder / decoder (GroupNorm+SiLU+3x3 conv stacks) run as wgmma implicit-GEMM convolutions
     with fp32-level accuracy (operands carried as bf16 hi/lo planes, three products, fp32 accumulation:
     csrc/conv_tc.cu) fed by a fused GroupNorm+SiLU(+split) kernel; the 3-channel stem/head and odd geometries use the
     fp32 SIMT kernel (csrc/conv.cu).  fp32-faithful because token ids must match the fp32 reference (single-pass
@@ -232,7 +232,7 @@ class MaskGitVQGAN(ModelMixin, ConfigMixin):
 
     def _encode_nhwc(self, pixel_values):
         if not pixel_values.is_cuda:
-            raise RuntimeError("open_muse_b200.MaskGitVQGAN runs on CUDA (sm_100a) only; move inputs to the GPU")
+            raise RuntimeError("open_muse_b200.MaskGitVQGAN runs on CUDA (sm_90a) only; move inputs to the GPU")
         with ops.conv_precision(self.conv_precision):
             return self.encoder.run(ops.to_nhwc(pixel_values.float().contiguous()))
 

@@ -288,7 +288,7 @@ class VQGANModel(ModelMixin, ConfigMixin):
 
     def _encode_nhwc(self, pixel_values):
         if not pixel_values.is_cuda:
-            raise RuntimeError("open_muse_b200.VQGANModel runs on CUDA (sm_100a) only; move inputs to the GPU")
+            raise RuntimeError("open_muse_b200.VQGANModel runs on CUDA (sm_90a) only; move inputs to the GPU")
         with ops.conv_precision(self.conv_precision):
             h = self.encoder.run(ops.to_nhwc(pixel_values.float().contiguous()))
             return ops.conv2d(h, self.quant_conv.weight, bias=self.quant_conv.bias)

@@ -1,4 +1,4 @@
-"""``MaskGitTransformer`` with the reference's Python surface and a hand-written sm_100a hot path.
+"""``MaskGitTransformer`` with the reference's Python surface and a hand-written sm_90a hot path.
 
 Boundary (reference: muse/modeling_transformer.py:1083-1456): same constructor arguments, ``config``
 keys, parameter names / shapes / construction order (so ``torch.manual_seed(s); Model(**cfg)`` gives
@@ -8,7 +8,7 @@ the reference's initial weights and ``pytorch_model.bin`` files are interchangea
 Underneath, nothing is torch-eager: the module tree only *holds* the fp32 master parameters.
 ``forward`` runs three kinds of ``torch.autograd.Function`` -- embedding, one per transformer layer
 (so DDP's gradient buckets fire layer by layer during backward), and head+loss -- whose bodies are
-sequences of libmuse_b200 kernels (tcgen05 GEMMs, fused attention, fused norm/GELU/residual, masked
+sequences of libmuse_b200 kernels (wgmma GEMMs, fused attention, fused norm/GELU/residual, masked
 cross-entropy).  Compute precision is the reference's bf16-autocast recipe: bf16 GEMM operands with
 fp32 accumulation, fp32 residual stream, fp32 norm / softmax / loss statistics.
 """
@@ -874,7 +874,7 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
                 "construct the model with hidden_dropout=0.0, attention_dropout=0.0"
             )
         if not input_ids.is_cuda:
-            raise RuntimeError("open_muse_b200.MaskGitTransformer runs on CUDA (sm_100a) only; move inputs to the GPU")
+            raise RuntimeError("open_muse_b200.MaskGitTransformer runs on CUDA (sm_90a) only; move inputs to the GPU")
         B, S = input_ids.shape
         if _CHECK_IDS:  # debug switch (MUSE_B200_CHECK_IDS=1): torch raises a device assert on out-of-range ids / labels,
             # the kernels clamp silently -- this host-side check (one sync) catches class-offset / vocab mix-ups

@@ -5,7 +5,7 @@ MaskGiTUViT_v2(**cfg)`` reproduces the reference's initial weights, including th
 ``forward(input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels=, label_smoothing=, loss_weight=)`` and the
 classifier-free-guidance ``generate2`` (:330-479).
 
-Everything runs on libmuse_b200: tcgen05 GEMMs for every Linear / 1x1 conv, tcgen05 attention, fused prenorm-residual
+Everything runs on libmuse_b200: wgmma GEMMs for every Linear / 1x1 conv, wgmma attention, fused prenorm-residual
 norm + adaLN modulation, depthwise-conv + Norm2D, GELU + GlobalResponseNorm, the fused decode step; training goes through
 one autograd Function for the whole network (``uvit_v2_train.py``: forward with saved activations + hand-written backward).
 The modules below are parameter containers; the inference arithmetic lives in ``_forward_tokens``.
@@ -375,7 +375,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
     def _forward_tokens(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds):
         c = self.config
         if not input_ids.is_cuda:
-            raise RuntimeError("open_muse_b200.MaskGiTUViT_v2 runs on CUDA (sm_100a) only; move inputs to the GPU")
+            raise RuntimeError("open_muse_b200.MaskGiTUViT_v2 runs on CUDA (sm_90a) only; move inputs to the GPU")
         B, S = input_ids.shape
         hw = int(S ** 0.5)
         if hw * hw != S:

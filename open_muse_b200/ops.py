@@ -1,7 +1,7 @@
 """Thin tensor-level wrappers over the C ABI (pointers, sizes, current CUDA stream).
 
 PyTorch here is plumbing only: device memory (``torch.empty``), streams, autograd bookkeeping.
-Every function launches hand-written sm_100a kernels from libmuse_b200.so and raises if the
+Every function launches hand-written sm_90a kernels from libmuse_b200.so and raises if the
 library is missing or the tensors are not CUDA tensors -- there is no fallback path.
 """
 from __future__ import annotations
@@ -600,7 +600,7 @@ def _packed_conv_weight_split(w):
 
 
 def conv_uses_tensor_cores(H, W, Cin, Cout, k):
-    """Route of conv2d(): tcgen05 bf16x3 implicit GEMM unless the geometry is unsupported or MUSE_B200_CONV=simt.
+    """Route of conv2d(): wgmma bf16x3 implicit GEMM unless the geometry is unsupported or MUSE_B200_CONV=simt.
     Stems with k*k*Cin <= 64 go through an im2col to 64 columns and run as a 1x1 convolution."""
     if _conv_state["route"] == "simt":  # private test hook (ops.conv_route): cross-check against the fp32 FMA kernels
         return False

@@ -2,7 +2,7 @@
 
 Host-side Python only: it wires ``MaskGitTransformer.generate2`` (fused decode-step kernel) to
 ``MaskGitVQGAN.decode_code`` (CUDA detokeniser) and converts to PIL.  Class-conditional generation and text
-conditioning with *precomputed* ``prompt_embeds`` run fully on the B200 path; raw ``text=`` needs a third-party
+conditioning with *precomputed* ``prompt_embeds`` run fully on the H100 path; raw ``text=`` needs a third-party
 text encoder / tokenizer object (CLIP / T5 from ``transformers``), which is outside this repository's scope and is
 called as-is when attached -- for ``MaskGiTUViT_v2`` exactly as the reference pipeline calls it (penultimate-layer states,
 projected pooled embedding, encoded negative / empty prompt, ``clip_skip``).

@@ -10,7 +10,7 @@ Reference writer: scripts/pre_encode.py:136-243 -- one webdataset tar per source
 webdataset is not in this image, and the format is plain POSIX tar, so writer and reader are implemented on ``tarfile``
 with webdataset's member conventions (basename split at the FIRST dot into key and extension, all members of a sample
 contiguous, mode 0444, owner "bigdata").  The tokeniser in front is this package's ``VQGANModel`` / ``MaskGitVQGAN``
-``get_code`` (tcgen05 convolutions + bit-exact arg-min); ``pre_encode_images`` overlaps the device->host copy of one
+``get_code`` (wgmma convolutions + bit-exact arg-min); ``pre_encode_images`` overlaps the device->host copy of one
 batch with the encode of the next."""
 from __future__ import annotations
 

@@ -8,8 +8,8 @@ returns the gradients of that block's parameters (reference names, fp32) as soon
 overlap the rest of the backward pass.  ``UViTTrainFn`` (private test hook ``model._single_train_function``) is the same
 computation as ONE Function for the whole network; the tests pin the two against each other.
 
-All arithmetic is in the C-ABI kernels: tcgen05 GEMMs for every Linear / 1x1 / patch convolution (dgrad with an MN-major
-weight operand, deterministic split-K wgrad), tcgen05 attention backward, and the U-ViT kernels of csrc/uvit_bwd.cu.  Things
+All arithmetic is in the C-ABI kernels: wgmma GEMMs for every Linear / 1x1 / patch convolution (dgrad with an MN-major
+weight operand, deterministic split-K wgrad), wgmma attention backward, and the U-ViT kernels of csrc/uvit_bwd.cu.  Things
 that are single tensors consumed by many blocks get ONE accumulator: the text states (fp32, atomic-accumulating dgrad) and
 the stacked adaLN mapper output (each op adds into its own column slice), so no gradient is summed with eager ops.
 """

@@ -4,7 +4,7 @@ optimizer, of the C entry point itself) in plain torch, so everything ABOVE the 
 MaskGitTransformer and MaskGiTUViT_v2, the packed-operand pointer table, the order in which gradients are handed back, the
 generate2 loops, the tokenizers' module wiring, PipelineMuse, FusedAdamW's launch table -- can be run end to end WITHOUT a GPU
 and compared with what the unmodified reference computed (tests/golden/*.pt).  The kernels themselves are checked on the
-B200 (tests/test_kernels_gpu.py, tests/test_model_gpu.py, ...).
+GPU (tests/test_kernels_gpu.py, tests/test_model_gpu.py, ...).
 
 Two modes:
   exact=True   ``torch.bfloat16`` is aliased to ``torch.float32`` while the stand-ins are installed, so every tensor the host

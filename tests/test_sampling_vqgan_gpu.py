@@ -132,7 +132,7 @@ def test_conv_gn_pool_blocks_vs_torch():
     (2, 16, 8, 128, 48, 3, True, True, False, True),       # narrow image: one 16-row tile per image, C_out = 48
 ])
 def test_conv_tensor_core_path_vs_fp64(B, H, W, cin, cout, k, bias, res, up, gn):
-    """bf16x3 tcgen05 implicit GEMM (csrc/conv_tc.cu) against an fp64 convolution: fp32-level accuracy is the contract
+    """bf16x3 wgmma implicit GEMM (csrc/conv_tc.cu) against an fp64 convolution: fp32-level accuracy is the contract
     (a single bf16 pass would sit at ~4e-3)."""
     if not ops.conv_uses_tensor_cores(H, W, cin, cout, k):
         pytest.skip("geometry routed to the SIMT kernel")
@@ -203,7 +203,7 @@ def test_micro_vqgan_vs_reference(golden):
 def test_vqgan_f16_256_vs_reference_fixture(golden):
     """BASELINE config 3 at its own architecture against the UNMODIFIED reference (tests/golden/f16_256_vqgan.pt: default
     init from the seed, codebook ~ N(0, std(z)), two rand images): encoder output, token ids bit-exact on every position
-    whose top-2 distance margin is above 1e-4 relative, quantised latents, reconstruction -- all through the tcgen05
+    whose top-2 distance margin is above 1e-4 relative, quantised latents, reconstruction -- all through the wgmma
     (bf16x3 implicit-GEMM) convolution route."""
     from open_muse_b200.modeling_maskgit_vqgan import MaskGitVQGAN
 
@@ -290,7 +290,7 @@ def test_vqgan_f16_256_roundtrip_properties():
 
 
 def test_vqgan_f16_256_tensor_core_route_matches_fp32_simt_route(monkeypatch):
-    """The tcgen05 bf16x3 convolutions must be interchangeable with the fp32 SIMT kernels: encoder output and decoded
+    """The wgmma bf16x3 convolutions must be interchangeable with the fp32 SIMT kernels: encoder output and decoded
     pixels agree to fp32-level tolerance and the token ids are identical wherever the arg-min margin is not tiny."""
     from open_muse_b200.modeling_maskgit_vqgan import MaskGitVQGAN
 

@@ -1,6 +1,6 @@
 """GPU twin of tests/test_train_script_cpu.py: the UNMODIFIED reference training script (taken from oracle/_ref/training, the
 git-ignored snapshot __graft_entry__.build() makes, or /root/reference when present) trains the drop-in MaskGitTransformer
-on a B200 through the real kernels: frozen MaskGitVQGAN tokeniser (tcgen05 / SIMT convolutions + bit-exact arg-min) ->
+on the GPU through the real kernels: frozen MaskGitVQGAN tokeniser (wgmma / SIMT convolutions + bit-exact arg-min) ->
 masking -> bf16-autocast forward + fused CE -> backward -> clip -> AdamW -> checkpoints."""
 import json
 import math

@@ -368,7 +368,7 @@ def test_micro_uvit_v2_training_gradients_vs_oracle(golden):
 
 def test_uvit_v2_default_widths_training_gradients_vs_oracle():
     """Training backward at the U-ViT widths (hidden 1024 / 16 heads, blocks 768 / 12 heads + kv_mapper, 256 tokens, 77 text
-    states): exercises the tcgen05 attention backward, the 4-chunk norm kernels and the wide GRN against fp32 autograd."""
+    states): exercises the wgmma attention backward, the 4-chunk norm kernels and the wide GRN against fp32 autograd."""
     cfg = dict(num_hidden_layers=2, num_res_blocks=1, vocab_size=1032, codebook_size=1024, intermediate_size=2816)
     torch.manual_seed(0)
     m = MaskGiTUViT_v2(**cfg)

@@ -8,7 +8,7 @@ fp32 results to ~1e-4 -- a gradient routed to the wrong parameter, a missing res
 hide under bf16 noise as it could in the GPU tests' 1e-2 / 6e-2 tolerances.
 recipe mode (bf16 where the kernels write bf16): the precision recipe of the hot path itself stays within the GPU tests'
 tolerances on the same fixtures.
-The kernels are NOT exercised here (tests/test_kernels_gpu.py, tests/test_model_gpu.py do that on the B200)."""
+The kernels are NOT exercised here (tests/test_kernels_gpu.py, tests/test_model_gpu.py do that on the GPU)."""
 import pytest
 import torch
 

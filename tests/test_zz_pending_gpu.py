@@ -1,16 +1,13 @@
-"""GPU tests written AFTER this round's GPU budget was spent: none of them has run on a B200 yet.
+"""GPU tests of compositions whose parts are validated elsewhere:
 
   * ``use_conv_in_out=True`` (ConvEmbed / ConvMlmLayer, reference muse/modeling_transformer.py:988-1080) against the unmodified
     reference's fp32 outputs in tests/golden/micro_conv_transformer.pt;
   * the UNMODIFIED training/train_muse.py through the real kernels;
   * MaskGiTUViT_v2 at head_dim 48 (the attention kernels are validated at that width through MaskGitTransformer).
 
-Their host side is checked numerically on the CPU (tests/test_v1_numeric_cpu.py::test_conv_in_out_*: logits 1e-7, every
+Their host side is also checked numerically on the CPU (tests/test_v1_numeric_cpu.py::test_conv_in_out_*: logits 1e-7, every
 gradient < 2e-4 of the reference; tests/test_train_muse_script_cpu.py: the script trains on the kernels' torch restatements)
-and every kernel they launch is covered by tests/test_kernels_gpu.py / test_uvit_v2_gpu.py, but these particular
-compositions are new.  They are therefore marked ``xfail(strict=False)``: XPASS when the composition holds the usual
-tolerances, xfailed otherwise, without turning an unvalidated addition into a red suite.  The file name sorts last on
-purpose."""
+and every kernel they launch is covered by tests/test_kernels_gpu.py / test_uvit_v2_gpu.py."""
 import pytest
 import torch
 
@@ -24,7 +21,6 @@ def _rel(a, b):
     return float((a - b).norm() / b.norm().clamp_min(1e-20))
 
 
-@pytest.mark.xfail(strict=False, reason="use_conv_in_out: first GPU run pending (host wiring validated on the CPU only)")
 def test_conv_in_out_vs_reference(golden):
     from open_muse_b200.modeling_transformer import MaskGitTransformer
 
@@ -47,7 +43,7 @@ def test_conv_in_out_vs_reference(golden):
     # same rule as tests/test_model_gpu.py: only the ~1e-6 query / key gradients may sit above 6e-2 (bf16 noise of the recipe)
     bad = {n: e for n, e in errs.items() if e >= 6e-2 and not ("attention.query" in n or "attention.key" in n)}
     assert not bad and max(errs.values()) < 0.5, (bad, max(errs.values()))
-    print("conv in/out on the B200: logits", _rel(logits, g["logits"]), "worst gradient", max(errs.values()))
+    print("conv in/out on the GPU: logits", _rel(logits, g["logits"]), "worst gradient", max(errs.values()))
     m.eval()
     with torch.no_grad():
         ids = m.generate2(encoder_hidden_states=g["encoder_hidden_states"].to(DEV), timesteps=4, guidance_scale=2.0,
@@ -55,7 +51,6 @@ def test_conv_in_out_vs_reference(golden):
     assert ids.shape == (2, 64) and int(ids.min()) >= 0 and int(ids.max()) < g["config"]["codebook_size"]
 
 
-@pytest.mark.xfail(strict=False, reason="train_muse.py on the B200: first GPU run pending (CPU twin: tests/test_train_muse_script_cpu.py)")
 def test_reference_train_muse_script_trains_on_gpu(tmp_path, monkeypatch):
     """GPU twin of tests/test_train_muse_script_cpu.py: the UNMODIFIED training/train_muse.py through the real kernels (CLIP
     text encoder with projection, taming VQGAN tokenizer, MaskGiTUViT_v2 with pooled + micro conditioning, bf16 autocast,
@@ -85,7 +80,6 @@ def test_reference_train_muse_script_trains_on_gpu(tmp_path, monkeypatch):
     assert len(cks) == 1 and json.load(open(os.path.join(out, cks[0], "metadata.json")))["global_step"] == steps
 
 
-@pytest.mark.xfail(strict=False, reason="MaskGiTUViT_v2 at head_dim 48: first GPU run pending (CPU twin: tests/test_uvit_numeric_cpu.py)")
 def test_uvit_head_dim_48_vs_oracle():
     """MaskGiTUViT_v2 with head_dim 48 in the transformer layers and the block attentions (96 / 2, 48 / 1) against the oracle's
     fp32 forward / autograd: the attention kernels are validated at head_dim 48 through MaskGitTransformer, this composition

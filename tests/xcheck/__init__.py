@@ -1,6 +1,6 @@
 """TEST-ONLY cross-check library binding (tests/xcheck/libmuse_b200_xcheck.so): first-generation mma.sync GEMM and
 attention kernels with the product's argument conventions, used by the GPU tests as an independent on-device reference
-for the tcgen05 kernels.  Not part of the product."""
+for the wgmma kernels.  Not part of the product."""
 import ctypes
 from ctypes import c_char_p, c_float, c_int, c_void_p
 from pathlib import Path

@@ -8,7 +8,7 @@
 // Used for self-attention (kv_len = S = 257/256/1024) and cross-attention (kv_len = 77, :886-899).
 //
 // TEST-ONLY: the first-generation mma.sync.m16n8k16 implementation, kept as an independent on-device cross-check of the
-// product's tcgen05 kernels (open_muse_b200/csrc/attention_tc.cu).  Built into tests/xcheck/libmuse_b200_xcheck.so,
+// product's wgmma kernels (open_muse_b200/csrc/attention_tc.cu).  Built into tests/xcheck/libmuse_b200_xcheck.so,
 // never into libmuse_b200.so.
 #include <stdlib.h>
 #include <string.h>

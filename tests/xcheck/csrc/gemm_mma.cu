@@ -1,5 +1,5 @@
-// Legacy-tensor-core (mma.sync m16n8k16) bf16 GEMM with the same contract as gemm_tcgen05().
-// TEST-ONLY: an independent on-device cross-check for the product's tcgen05 kernel (tests compare the two).  Built into
+// Legacy-tensor-core (mma.sync m16n8k16) bf16 GEMM with the same contract as gemm_tc() (csrc/gemm_wgmma.cu).
+// TEST-ONLY: an independent on-device cross-check for the product's wgmma kernel (tests compare the two).  Built into
 // tests/xcheck/libmuse_b200_xcheck.so, never into libmuse_b200.so.
 #include "common.cuh"
 
