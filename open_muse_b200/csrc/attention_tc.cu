@@ -17,16 +17,13 @@
 // three tiles of 86 rows; S = 256 -> two of 128; the 77 text states of cross-attention -> one of 77): a tile starts at row
 // i * R, its CTA still loads a 128-row box (rows past R belong to the next tile or are zero-filled past the sequence), the
 // MMAs run on all 128 rows, but only rows < R are kept, and warps whose 32 rows all lie past R skip the softmax math.
-// No row is ever handed to another kernel.  The looped dimension handles ragged tails by shrinking the MMA N/K to a
-// multiple of 16.
+// The looped dimension handles ragged tails by shrinking the MMA N/K to a multiple of 16.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "tc_host.cuh"
 #include "wgmma.cuh"
 
 namespace muse {
-
-int make_tmap3(CUtensorMap* map, const void* base, long long cols, long long rows, long long batches,
-               long long row_pitch_elems, int box_rows);  // gemm_wgmma.cu
 
 namespace {
 
@@ -38,13 +35,6 @@ namespace {
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(
-          ptx::smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 // exp2 on the SFU without the denormal/range fix-ups of exp2f (inputs here are <= 0 or bounded scores)
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -54,16 +44,6 @@ __device__ __forceinline__ float ex2(float x) {
 
 // named barrier over the 256 math threads (barrier 0 stays __syncthreads for the whole CTA)
 __device__ __forceinline__ void math_sync() { asm volatile("bar.sync 1, 256;\n" ::: "memory"); }
-
-// Operand descriptors for [rows x 64] bf16 tiles laid out by TMA with the 128-byte swizzle (rows of 128 B).
-//  K-major view : row = M/N index, the 64 columns are K.  k-step ks (16 K) -> +32 B.
-//  MN-major view: row = K index, the 64 columns are M/N.  k-step ks (16 rows) -> +2048 B.
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile_addr, int ks) {
-  return ptx::make_smem_desc_sw128(tile_addr + ks * 32, 16, 1024);
-}
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile_addr, int ks) {
-  return ptx::make_smem_desc_sw128(tile_addr + ks * 2048, 8192, 1024);
-}
 
 // Store 8 consecutive bf16 (one 16-byte chunk) of row r, columns [k0, k0+8) of a [128 x K] K-major SW128 operand
 // made of 64-column atoms (16 KB each).
@@ -92,20 +72,17 @@ template <int N, int TB>
 __device__ __forceinline__ void mma_tile(float (&d)[N / 2], uint32_t a, uint32_t b, int ksteps, int accumulate) {
   ptx::wgmma_fence();
   for (int ks = 0; ks < ksteps; ++ks)
-    ptx::Wgmma<N, 0, TB>::run(d, desc_kmajor(a, ks), TB ? desc_mnmajor(b, ks) : desc_kmajor(b, ks), (accumulate || ks > 0) ? 1 : 0);
+    ptx::Wgmma<N, 0, TB>::run(d, ptx::desc_kmajor(a, ks), TB ? ptx::desc_mnmajor(b, ks) : ptx::desc_kmajor(b, ks),
+                              (accumulate || ks > 0) ? 1 : 0);
   ptx::wgmma_commit();
   ptx::wgmma_wait<0>();
 }
-
-// the fragment row / column of d[4j] for the calling thread of its warpgroup (d[4j + 2] is 8 rows further down)
-__device__ __forceinline__ int frag_row() { return ((threadIdx.x & 127) >> 5) * 16 + ((threadIdx.x & 31) >> 2); }
-__device__ __forceinline__ int frag_col() { return 2 * (threadIdx.x & 3); }
 
 template <int N>
 __device__ __forceinline__ void scores_n(uint32_t a, uint32_t b, int ksteps, float* dst, int row0) {
   float d[N / 2];
   mma_tile<N, 0>(d, a, b, ksteps, 0);
-  const int r = row0 + frag_row(), c = frag_col();
+  const int r = row0 + ptx::frag_row(), c = ptx::frag_col();
 #pragma unroll
   for (int j = 0; j < N / 8; ++j) {
     *reinterpret_cast<float2*>(dst + r * SP + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
@@ -126,7 +103,7 @@ __device__ __forceinline__ void scores_to_smem(uint32_t a, uint32_t b, int n16, 
 template <int HD>
 __device__ __forceinline__ void store_acc(const float (&d)[HD / 2], bf16* base, long long rs, int row0, int rows_ok,
                                           const float* row_scale) {
-  const int r = row0 + frag_row(), c = frag_col();
+  const int r = row0 + ptx::frag_row(), c = ptx::frag_col();
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int rr = r + 8 * hr;
@@ -179,10 +156,10 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   if (tid == 0) {
     ptx::mbar_expect_tx(bar_kv, 16384 + 8192);
-    tma_load_3d(sQ, &tmQ, bar_kv, h * HD, q0, b);
-    tma_load_3d(sK, &tmK, bar_kv, h * HD, 0, b);
+    ptx::tma_load_3d(sQ, &tmQ, bar_kv, h * HD, q0, b);
+    ptx::tma_load_3d(sK, &tmK, bar_kv, h * HD, 0, b);
     ptx::mbar_expect_tx(bar_v, 8192);
-    tma_load_3d(sV, &tmV, bar_v, h * HD, 0, b);
+    ptx::tma_load_3d(sV, &tmV, bar_v, h * HD, 0, b);
   }
   const float sl2 = p.scale * kLog2e;
   float m = -INFINITY, l = 0.f;
@@ -200,7 +177,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     __syncthreads();  // S_j is in shared memory and K_j has been consumed
     if (tid == 0 && j + 1 < ntiles) {  // fetch K_{j+1} under the softmax math
       ptx::mbar_expect_tx(bar_kv, 8192);
-      tma_load_3d(sK, &tmK, bar_kv, h * HD, (j + 1) * FWD_BN, b);
+      ptx::tma_load_3d(sK, &tmK, bar_kv, h * HD, (j + 1) * FWD_BN, b);
     }
     float alpha = 1.f;
     if (warp_active) {
@@ -254,7 +231,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     if (j > 0) {  // rescale the running output
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const float a0 = sRow[hh * 64 + frag_row()], a1 = sRow[hh * 64 + frag_row() + 8];
+        const float a0 = sRow[hh * 64 + ptx::frag_row()], a1 = sRow[hh * 64 + ptx::frag_row() + 8];
 #pragma unroll
         for (int i = 0; i < HD / 2; i += 4) {
           o[hh][i] *= a0; o[hh][i + 1] *= a0; o[hh][i + 2] *= a1; o[hh][i + 3] *= a1;
@@ -267,7 +244,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     __syncthreads();  // P_j and V_j have been consumed
     if (tid == 0 && j + 1 < ntiles) {
       ptx::mbar_expect_tx(bar_v, 8192);
-      tma_load_3d(sV, &tmV, bar_v, h * HD, (j + 1) * FWD_BN, b);
+      ptx::tma_load_3d(sV, &tmV, bar_v, h * HD, (j + 1) * FWD_BN, b);
     }
   }
   // epilogue: O / l -> bf16 rows, LSE
@@ -331,13 +308,13 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   auto load_kv = [&](int step) {       // thread 0: TMA of the K/V tile of `step` into its ring stage
     uint8_t* sK = sKV + (step % 3) * 16384;
     const int jn = step % ntiles;
-    tma_load_3d(sK, &tmK, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
-    tma_load_3d(sK + 8192, &tmV, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
+    ptx::tma_load_3d(sK, &tmK, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
+    ptx::tma_load_3d(sK + 8192, &tmV, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
   };
   if (tid == 0) {
     ptx::mbar_expect_tx(&bar_kv[0], 16384 * 2 + 8192 * 2);
-    tma_load_3d(sQ, &tmQ, &bar_kv[0], h * HD, q0, b);
-    tma_load_3d(sdO, &tmdO, &bar_kv[0], h * HD, q0, b);
+    ptx::tma_load_3d(sQ, &tmQ, &bar_kv[0], h * HD, q0, b);
+    ptx::tma_load_3d(sdO, &tmdO, &bar_kv[0], h * HD, q0, b);
     load_kv(0);
     if (nsteps > 1) {
       ptx::mbar_expect_tx(&bar_kv[1], 8192 * 2);
@@ -466,13 +443,13 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
 
   auto load_q = [&](int i) {
     uint8_t* sQ = sQO + (i % 3) * 16384;
-    tma_load_3d(sQ, &tmQ, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
-    tma_load_3d(sQ + 8192, &tmdO, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
+    ptx::tma_load_3d(sQ, &tmQ, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
+    ptx::tma_load_3d(sQ + 8192, &tmdO, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
   };
   if (tid == 0) {
     ptx::mbar_expect_tx(&bar_ld[0], 16384 * 2 + 8192 * 2);
-    tma_load_3d(sK, &tmK, &bar_ld[0], h * HD, kv0, b);
-    tma_load_3d(sV, &tmV, &bar_ld[0], h * HD, kv0, b);
+    ptx::tma_load_3d(sK, &tmK, &bar_ld[0], h * HD, kv0, b);
+    ptx::tma_load_3d(sV, &tmV, &bar_ld[0], h * HD, kv0, b);
     load_q(0);
     if (ntiles > 1) {
       ptx::mbar_expect_tx(&bar_ld[1], 8192 * 2);
@@ -558,110 +535,110 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
   store_acc<HD>(dv, p.out1 + base * p.out1_rs + h * HD, p.out1_rs, g * 64, rows_here, nullptr);
 }
 
-template <typename K>
-int set_smem(K kern, int bytes, bool* done) {
-  if (*done) return MUSE_OK;
-  cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);  // all of L1/smem as shared memory
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(attention smem=%d): %s", bytes, cudaGetErrorString(e)); return MUSE_ERR_CUDA; }
-  *done = true;
-  return MUSE_OK;
+// Raises kernel K's dynamic shared-memory limit and asks for all of L1 as shared memory, once per kernel.
+template <auto K>
+int set_smem(int bytes) {
+  static bool carveout = false;
+  if (!carveout) {
+    cudaFuncSetAttribute(K, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    carveout = true;
+  }
+  return set_max_dynamic_smem<K>(bytes);
 }
 
-}  // namespace
-
 // Balanced tiling of an owned dimension of S rows: ceil(S / 128) tiles of R = ceil(S / tiles) rows each.
-static inline void balanced_tiles(int S, int* ntile, int* rows) {
+void balanced_tiles(int S, int* ntile, int* rows) {
   *ntile = ceil_div(S, 128);
   *rows = ceil_div(S, *ntile);
 }
 
-// Forward pass over all q rows (rows_done = Sq on return).
+// 3-D map {cols, S rows, B} of a [B * S, rs] row-major operand, box {64 columns, box_rows rows, 1}: rows past S inside a
+// batch are out of bounds and read as zeros.
+int qkv_tmap(CUtensorMap* map, const void* base, int cols, int S, int B, int rs, int box_rows) {
+  return make_tmap_bf16(map, "attention", base, {cols, S, B}, {2LL * rs, 2LL * rs * S}, {64, box_rows, 1});
+}
+
 template <int HD>
-static int attn_fwd_tc_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv,
-                            int q_rs, int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s, int* rows_done) {
-  *rows_done = 0;
+int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int q_rs,
+                  int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
   int ntile, tile_rows;
   balanced_tiles(Sq, &ntile, &tile_rows);
   CUtensorMap tq, tk, tv;
   int rc;
-  if ((rc = make_tmap3(&tq, q, nh * HD, Sq, B, q_rs, 128))) return rc;
-  if ((rc = make_tmap3(&tk, k, nh * HD, Skv, B, k_rs, FWD_BN))) return rc;
-  if ((rc = make_tmap3(&tv, v, nh * HD, Skv, B, v_rs, FWD_BN))) return rc;
-  static bool attr = false;
-  if ((rc = set_smem(attn_fwd_tc_kernel<HD>, FWD_SMEM, &attr))) return rc;
+  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs, 128))) return rc;
+  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs, FWD_BN))) return rc;
+  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs, FWD_BN))) return rc;
+  if ((rc = set_smem<attn_fwd_tc_kernel<HD>>(FWD_SMEM))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale; p.tile_rows = tile_rows;
   p.out0 = reinterpret_cast<bf16*>(o); p.out0_rs = o_rs; p.lse = lse;
   pdl_launch(dim3(ntile, nh, B), 128, FWD_SMEM, s)(attn_fwd_tc_kernel<HD>, tq, tk, tv, p);
-  *rows_done = Sq;
   return check_launch("attn_fwd_tc");
 }
-int attn_fwd_tc(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
-                int q_rs, int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s, int* rows_done) {
-  return hd == 64 ? attn_fwd_tc_impl<64>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, s, rows_done)
-                  : attn_fwd_tc_impl<48>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, s, rows_done);
-}
 
+// dQ (and D, into dvec) over q row tiles, then dK / dV over kv row tiles
 template <int HD>
-static int attn_bwd_dq_tc_impl(const void* q, const void* k, const void* v, const void* d_o, const float* lse, float* dvec,
-                               void* dq, int B, int nh, int Sq, int Skv, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs,
-                               float scale, cudaStream_t s, int* rows_done) {
-  *rows_done = 0;
+int attn_bwd_impl(const void* q, const void* k, const void* v, const void* d_o, const float* lse, float* dvec, void* dq,
+                  void* dk, void* dv, int B, int nh, int Sq, int Skv, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs,
+                  int dk_rs, int dv_rs, float scale, cudaStream_t s) {
   int ntile, tile_rows;
   balanced_tiles(Sq, &ntile, &tile_rows);
   CUtensorMap tq, tdo, tk, tv;
   int rc;
-  if ((rc = make_tmap3(&tq, q, nh * HD, Sq, B, q_rs, 128))) return rc;
-  if ((rc = make_tmap3(&tdo, d_o, nh * HD, Sq, B, do_rs, 128))) return rc;
-  if ((rc = make_tmap3(&tk, k, nh * HD, Skv, B, k_rs, BWD_BN))) return rc;
-  if ((rc = make_tmap3(&tv, v, nh * HD, Skv, B, v_rs, BWD_BN))) return rc;
-  static bool attr = false;
-  if ((rc = set_smem(attn_bwd_dq_tc_kernel<HD>, DQ_SMEM, &attr))) return rc;
+  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs, 128))) return rc;
+  if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs, 128))) return rc;
+  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs, BWD_BN))) return rc;
+  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs, BWD_BN))) return rc;
+  if ((rc = set_smem<attn_bwd_dq_tc_kernel<HD>>(DQ_SMEM))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale;
   p.out0 = reinterpret_cast<bf16*>(dq); p.out0_rs = dq_rs; p.lse = const_cast<float*>(lse); p.dvec = dvec;
   p.tile_rows = tile_rows;
   pdl_launch(dim3(ntile, nh, B), 256, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD>, tq, tdo, tk, tv, p);
-  *rows_done = Sq;
-  return check_launch("attn_bwd_dq_tc");
-}
-int attn_bwd_dq_tc(const void* q, const void* k, const void* v, const void* d_o, const float* lse, float* dvec,
-                   void* dq, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs,
-                   float scale, cudaStream_t s, int* rows_done) {
-  return hd == 64 ? attn_bwd_dq_tc_impl<64>(q, k, v, d_o, lse, dvec, dq, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs, scale, s, rows_done)
-                  : attn_bwd_dq_tc_impl<48>(q, k, v, d_o, lse, dvec, dq, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs, scale, s, rows_done);
-}
+  if ((rc = check_launch("attn_bwd_dq_tc"))) return rc;
 
-template <int HD>
-static int attn_bwd_dkdv_tc_impl(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
-                                 const float* dvec, void* dk, void* dv, int B, int nh, int Sq, int Skv, int q_rs, int k_rs,
-                                 int v_rs, int do_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s, int* rows_done) {
-  *rows_done = 0;
-  int ntile, tile_rows;
   balanced_tiles(Skv, &ntile, &tile_rows);
-  CUtensorMap tq, tdo, tk, tv;
-  int rc;
-  if ((rc = make_tmap3(&tk, k, nh * HD, Skv, B, k_rs, 128))) return rc;
-  if ((rc = make_tmap3(&tv, v, nh * HD, Skv, B, v_rs, 128))) return rc;
-  if ((rc = make_tmap3(&tq, q, nh * HD, Sq, B, q_rs, BWD_BN))) return rc;
-  if ((rc = make_tmap3(&tdo, d_o, nh * HD, Sq, B, do_rs, BWD_BN))) return rc;
-  static bool attr = false;
-  if ((rc = set_smem(attn_bwd_dkdv_tc_kernel<HD>, DKDV_SMEM, &attr))) return rc;
-  TcParams p{};
-  p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale;
+  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs, 128))) return rc;
+  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs, 128))) return rc;
+  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs, BWD_BN))) return rc;
+  if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs, BWD_BN))) return rc;
+  if ((rc = set_smem<attn_bwd_dkdv_tc_kernel<HD>>(DKDV_SMEM))) return rc;
   p.out0 = reinterpret_cast<bf16*>(dk); p.out0_rs = dk_rs; p.out1 = reinterpret_cast<bf16*>(dv); p.out1_rs = dv_rs;
-  p.lse = const_cast<float*>(lse); p.dvec = const_cast<float*>(dvec);
   p.tile_rows = tile_rows;
   pdl_launch(dim3(ntile, nh, B), 256, DKDV_SMEM, s)(attn_bwd_dkdv_tc_kernel<HD>, tk, tv, tq, tdo, p);
-  *rows_done = Skv;
   return check_launch("attn_bwd_dkdv_tc");
 }
-int attn_bwd_dkdv_tc(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
-                     const float* dvec, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs,
-                     int v_rs, int do_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s, int* rows_done) {
-  return hd == 64 ? attn_bwd_dkdv_tc_impl<64>(q, k, v, d_o, lse, dvec, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dk_rs, dv_rs, scale, s, rows_done)
-                  : attn_bwd_dkdv_tc_impl<48>(q, k, v, d_o, lse, dvec, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dk_rs, dv_rs, scale, s, rows_done);
+
+int check_args(const char* who, int hd, int a, int b, int c) {
+  if (hd != 64 && hd != 48) { set_last_error("%s: head_dim %d unsupported (64 and 48 are built)", who, hd); return MUSE_ERR_UNSUPPORTED; }
+  if (((a | b | c) & 7) != 0) { set_last_error("%s: row strides must be multiples of 8 elements", who); return MUSE_ERR_INVALID; }
+  return MUSE_OK;
+}
+
+}  // namespace
+
+// Entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its autograd
+// backward, head_dim 64 or 48, no mask, no dropout.
+int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
+             int q_rs, int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
+  if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
+  int rc = check_args("attn_fwd", hd, q_rs | o_rs, k_rs, v_rs);
+  if (rc) return rc;
+  return hd == 64 ? attn_fwd_impl<64>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, s)
+                  : attn_fwd_impl<48>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, s);
+}
+
+int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+             float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs,
+             int v_rs, int o_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s) {
+  if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
+  int rc = check_args("attn_bwd", hd, q_rs | o_rs | do_rs | dq_rs, k_rs | dk_rs, v_rs | dv_rs);
+  if (rc) return rc;
+  (void)o;  // D is recomputed from (P, dP) inside the dQ kernel; O is not needed by backward
+  return hd == 64 ? attn_bwd_impl<64>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs,
+                                      dk_rs, dv_rs, scale, s)
+                  : attn_bwd_impl<48>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs,
+                                      dk_rs, dv_rs, scale, s);
 }
 
 }  // namespace muse

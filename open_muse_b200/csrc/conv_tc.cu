@@ -19,33 +19,23 @@
 //   arithmetic: output pixel (2y+py, 2x+px) only sees a 2x2 window of the low-resolution input, so each of the four
 //   parities (py, px) is a 2x2 convolution with pre-summed weights (K = 4*C_in instead of 9*C_in, 2.25x fewer FLOPs)
 //   whose tile rows scatter to every other output pixel.
-// * Same persistent warp-specialised pipeline as gemm_wgmma.cu: one TMA producer thread, two consumer warpgroups
-//   (wgmma m64 x BN x k16 on their 64-pixel halves of the tile); the epilogue adds bias / residual to the accumulator
-//   registers, writes fp32 NHWC rows and folds the per-channel GroupNorm statistics of the tile.
+// * The persistent warp-specialised pipeline of tc_pipeline.cuh (wgmma m64 x BN x k16 on the two 64-pixel halves of the
+//   tile); the epilogue adds bias / residual to the accumulator registers, writes fp32 NHWC rows and folds the
+//   per-channel GroupNorm statistics of the tile.
 #include "common.cuh"
-#include "ptx.cuh"
-#include "wgmma.cuh"
+#include "tc_host.cuh"
+#include "tc_pipeline.cuh"
 
 namespace muse {
 
-int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const unsigned long long* dims,
-                 const unsigned long long* strides_bytes, const unsigned* box);
-
 namespace {
 
-constexpr int BM = 128;
-constexpr int BK = 64;
+using tc::BK;
 
+// Stages of the ring: a multiple of 1024 B for BN in {16, 128, 256}.  Behind them, per consumer warp, {sum, sumsq} of
+// every tile column.
 template <int BN>
-struct Cfg {
-  static constexpr int kStages = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int kABytes = BM * BK * 2;
-  static constexpr int kBBytes = BN * BK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;  // a multiple of 1024 for BN in {16, 128, 256}
-  static constexpr int kBarBytes = 256;
-  static constexpr int kStatBytes = 8 * BN * 2 * 4;  // per-consumer-warp {sum, sumsq} of every tile column
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStatBytes + 1024 + kBarBytes;
-};
+using Ring = tc::Ring<BN, (BN == 256) ? 4 : (BN == 128 ? 6 : 8), 8 * BN * 2 * 4>;
 
 struct ConvParams {
   float* y;
@@ -62,35 +52,14 @@ struct ConvParams {
   int passes;           // 3: bf16x3 (hi*hi + lo*hi + hi*lo, fp32-faithful); 1: hi*hi only (plain bf16 operands, fast mode)
 };
 
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                            int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];\n" ::
-          "r"(ptx::smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n" ::
-          "r"(ptx::smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-
 template <int BN>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(tc::kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const ConvParams p) {
   pdl_trigger();
-  using C_ = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  float* stat_smem = reinterpret_cast<float*>(smem + C_::kStages * C_::kStageBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::kStages * C_::kStageBytes + C_::kStatBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + C_::kStages;
+  Ring<BN> ring(smem_raw);
+  float* stat_smem = reinterpret_cast<float*>(ring.extra());
 
   const int wg = threadIdx.x >> 7;
 
@@ -99,11 +68,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
     ptx::prefetch_tmap(&tmAl);
     ptx::prefetch_tmap(&tmBh);
     ptx::prefetch_tmap(&tmBl);
-    for (int i = 0; i < C_::kStages; ++i) {
-      ptx::mbar_init(&full_bar[i], 1);
-      ptx::mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
-    }
-    ptx::fence_barrier_init();
+    ring.init();
   }
   __syncthreads();
   pdl_wait();  // everything above touches only shared memory / kernel parameters
@@ -112,11 +77,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
   const int pad = p.ksize / 2;
 
   if (wg == 0) {
-    ptx::setmaxnreg_dec<40>();
+    ptx::setmaxnreg_dec<tc::kProducerRegs>();
     if (threadIdx.x == 0) {
       // ------------------------------------------------------------ TMA producer
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int parity = tile / tiles_mn, tl = tile % tiles_mn;
         const int n_idx = tl % p.num_n;
@@ -128,17 +91,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         const int wrow0 = parity * p.N;  // up: the four parity weight matrices are stacked along the rows
         int pass = 0, cc = 0, tap = 0;  // kb = (tap * cchunks + cc) * passes + pass
         for (int kb = 0; kb < p.num_kb; ++kb) {
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          ptx::mbar_expect_tx(&full_bar[stage], C_::kStageBytes);
-          uint8_t* sa = smem + stage * C_::kStageBytes;
-          uint8_t* sb = sa + C_::kABytes;
+          const auto s = ring.produce();
           // passes: 0 = hi*hi, 1 = lo(A)*hi(B), 2 = hi(A)*lo(B)
           const int dy = p.up ? (tap >> 1) + (parity >> 1) - 1 : (p.fwd2x2 ? (tap >> 1) : tap / p.ksize - pad);
           const int dx = p.up ? (tap & 1) + (parity & 1) - 1 : (p.fwd2x2 ? (tap & 1) : tap % p.ksize - pad);
           const int wb = p.wbatch ? img : 0;
-          tma_load_4d(sa, pass == 1 ? &tmAl : &tmAh, &full_bar[stage], cc * BK, x0 + dx, y0 + dy, img);
-          tma_load_3d(sb, pass == 2 ? &tmBl : &tmBh, &full_bar[stage], tap * p.Cin + cc * BK, wrow0 + n0, wb);
-          if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
+          ptx::tma_load_4d(s.a, pass == 1 ? &tmAl : &tmAh, s.bar, cc * BK, x0 + dx, y0 + dy, img);
+          ptx::tma_load_3d(s.b, pass == 2 ? &tmBl : &tmBh, s.bar, tap * p.Cin + cc * BK, wrow0 + n0, wb);
           if (++pass == p.passes) {
             pass = 0;
             if (++cc == p.cchunks) { cc = 0; ++tap; }
@@ -147,33 +106,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
       }
     }
   } else {
-    ptx::setmaxnreg_inc<232>();
+    ptx::setmaxnreg_inc<tc::kConsumerRegs>();
     // -------------------------------------------------------------- consumers: y = acc + bias (+ res), fp32 NHWC
     const int half = wg - 1;
     const int t = threadIdx.x & 127;
-    const int cw = threadIdx.x / 32 - 4;                         // consumer warp 0..7
-    const int lr = half * 64 + (t >> 5) * 16 + ((t & 31) >> 2);  // tile pixel of d[4j], d[4j+1]; +8 for d[4j+2..3]
-    const int lc = 2 * (t & 3);
+    const int cw = threadIdx.x / 32 - 4;          // consumer warp 0..7
+    const int lr = half * 64 + ptx::frag_row();  // tile pixel of d[4j], d[4j+1]; +8 for d[4j+2..3]
+    const int lc = ptx::frag_col();
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      for (int kb = 0; kb < p.num_kb; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_addr = ptx::smem_u32(smem + stage * C_::kStageBytes) + half * 8192;
-        const uint32_t b_addr = ptx::smem_u32(smem + stage * C_::kStageBytes + C_::kABytes);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          ptx::Wgmma<BN, 0, 0>::run(acc, ptx::make_smem_desc_sw128(a_addr + k * 32, 16, 1024),
-                                    ptx::make_smem_desc_sw128(b_addr + k * 32, 16, 1024), (kb > 0 || k > 0) ? 1 : 0);
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);
-        if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
-      }
+      ring.template consume<false, false>(acc, 0, p.num_kb, half);
       const int parity = tile / tiles_mn, tl = tile % tiles_mn;
       const int n_idx = tl % p.num_n;
       const int m_idx = tl / p.num_n;
@@ -363,30 +307,14 @@ softmax_split_kernel(const float* __restrict__ x, bf16* __restrict__ hi, bf16* _
   }
 }
 
-int g_sms = 0;
-int sm_count() {
-  if (g_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sms <= 0) g_sms = 132;
-  }
-  return g_sms;
-}
-
 template <int BN>
 int launch_conv(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                 const ConvParams& p, cudaStream_t s) {
-  auto kern = conv_tc_kernel<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes);
-    if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(conv_tc): %s", cudaGetErrorString(e)); return MUSE_ERR_CUDA; }
-    attr_set = true;
-  }
+  constexpr auto kern = conv_tc_kernel<BN>;
+  if (int rc = set_max_dynamic_smem<kern>(Ring<BN>::kSmemBytes)) return rc;
   const int total = p.num_m * p.num_n;
   const int grid = total < sm_count() ? total : sm_count();
-  pdl_launch(grid, 384, Cfg<BN>::kSmemBytes, s)(kern, ah, al, bh, bl, p);
+  pdl_launch(grid, tc::kThreads, Ring<BN>::kSmemBytes, s)(kern, ah, al, bh, bl, p);
   return check_launch("conv_tc");
 }
 
@@ -466,19 +394,20 @@ int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* 
   if (p.passes == 1) { x_lo = x_hi; w_lo = w_hi; }  // the lo maps are never dereferenced; keep the encodes valid
 
   CUtensorMap ah, al, bh, bl;
-  const unsigned long long adims[4] = {(unsigned long long)Cin, (unsigned long long)W, (unsigned long long)H, (unsigned long long)B};
-  const unsigned long long astr[3] = {(unsigned long long)Cin * 2, (unsigned long long)W * Cin * 2, (unsigned long long)H * W * Cin * 2};
-  const unsigned abox[4] = {64, (unsigned)p.tile_w, (unsigned)p.tile_h, 1};
+  const long long px = 2LL * Cin;  // bytes per pixel
+  const long long K = static_cast<long long>(taps) * Cin;
+  const long long wrows = static_cast<long long>(Cout) * (p.up ? 4 : 1);
   int rc;
-  if ((rc = make_tmap_nd(&ah, x_hi, 4, adims, astr, abox))) return rc;
-  if ((rc = make_tmap_nd(&al, x_lo, 4, adims, astr, abox))) return rc;
-  const unsigned long long K = static_cast<unsigned long long>(taps) * Cin;
-  const unsigned long long wrows = (unsigned long long)Cout * (p.up ? 4 : 1);
-  const unsigned long long bdims[3] = {K, wrows, (unsigned long long)(p.wbatch ? B : 1)};
-  const unsigned long long bstr[2] = {K * 2, K * 2 * wrows};
-  const unsigned bbox[3] = {64, (unsigned)BN, 1};
-  if ((rc = make_tmap_nd(&bh, w_hi, 3, bdims, bstr, bbox))) return rc;
-  if ((rc = make_tmap_nd(&bl, w_lo, 3, bdims, bstr, bbox))) return rc;
+  if ((rc = make_tmap_bf16(&ah, "conv2d_tc", x_hi, {Cin, W, H, B}, {px, px * W, px * W * H},
+                           {64, p.tile_w, p.tile_h, 1})))
+    return rc;
+  if ((rc = make_tmap_bf16(&al, "conv2d_tc", x_lo, {Cin, W, H, B}, {px, px * W, px * W * H},
+                           {64, p.tile_w, p.tile_h, 1})))
+    return rc;
+  if ((rc = make_tmap_bf16(&bh, "conv2d_tc", w_hi, {K, wrows, p.wbatch ? B : 1}, {2 * K, 2 * K * wrows}, {64, BN, 1})))
+    return rc;
+  if ((rc = make_tmap_bf16(&bl, "conv2d_tc", w_lo, {K, wrows, p.wbatch ? B : 1}, {2 * K, 2 * K * wrows}, {64, BN, 1})))
+    return rc;
   if (BN == 256) return launch_conv<256>(ah, al, bh, bl, p, s);
   if (BN == 128) return launch_conv<128>(ah, al, bh, bl, p, s);
   return launch_conv<16>(ah, al, bh, bl, p, s);

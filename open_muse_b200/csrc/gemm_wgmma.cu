@@ -4,11 +4,10 @@
 // (muse/modeling_transformer.py:198-200,218 q/k/v/out; :789-798 wi_0/wi_1/wo; :980,984 mlm head)
 // and, with transposed operand views, their dgrad / wgrad in backward.
 //
-// Structure (persistent, warp-specialised, one CTA per SM, 384 threads):
-//   warpgroup 0  : TMA producer  - one thread issues cp.async.bulk.tensor 2D tiles (128B swizzle) into a smem ring
-//   warpgroups 1-2: consumers    - each issues wgmma m64 x BN x k16 on its 64-row half of the 128-row tile, then runs
-//                                  the epilogue straight from its accumulator registers (bf16 / fp32 / atomic / +residual)
-// The producer runs up to kStages k-blocks ahead, so it keeps loading the next tile while the consumers store this one.
+// Structure: the persistent warp-specialised pipeline of tc_pipeline.cuh.  The producer thread loads 2-D TMA tiles of A
+// and B; the two consumer warpgroups run the epilogue straight from their accumulator registers (bf16 / fp32 / atomic /
+// +residual / split-K partial).  The producer runs up to a ring's worth of k-blocks ahead, so it keeps loading the next
+// tile while the consumers store this one.
 //
 // Operand "major-ness": an operand is K-major when the reduction dim is contiguous in memory
 // (activations X[T,K], weights W[N,K] in forward) and MN-major when the M/N dim is contiguous
@@ -17,15 +16,15 @@
 // smem (matrix) descriptors and the wgmma transpose flags tell the tensor core which layout it is looking at, so no
 // transposes are materialised anywhere in the training step.
 #include "common.cuh"
-#include "ptx.cuh"
-#include "wgmma.cuh"
+#include "tc_host.cuh"
+#include "tc_pipeline.cuh"
 
 namespace muse {
 
 namespace {
 
-constexpr int BM = 128;
-constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
+using tc::BK;
+using tc::BM;
 
 // EPI_SPLITK_F32: deterministic split-K.  Every split stores its fp32 partial tile into a workspace and a second, fully
 // parallel kernel sums the partials in split order and STORES the result, so the output needs no zero fill and is
@@ -33,14 +32,7 @@ constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle row
 enum Epi { EPI_BF16 = 0, EPI_F32 = 1, EPI_ATOMIC_F32 = 2, EPI_RESADD_F32 = 3, EPI_SPLITK_F32 = 4 };
 
 template <int BN>
-struct Cfg {
-  static constexpr int kStages = (BN == 256) ? 4 : 6;
-  static constexpr int kABytes = BM * BK * 2;
-  static constexpr int kBBytes = BN * BK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kBarBytes = 256;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kBarBytes;
-};
+using Ring = tc::Ring<BN, (BN == 256) ? 4 : 6>;
 
 struct GemmParams {
   void* C;
@@ -52,28 +44,19 @@ struct GemmParams {
 };
 
 template <int BN, bool A_MN, bool B_MN, int EPI>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(tc::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmParams p) {
   pdl_trigger();
-  using C_ = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::kStages * C_::kStageBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + C_::kStages;
+  Ring<BN> ring(smem_raw);
 
   const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
-    for (int i = 0; i < C_::kStages; ++i) {
-      ptx::mbar_init(&full_bar[i], 1);
-      ptx::mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
-    }
-    ptx::fence_barrier_init();
+    ring.init();
   }
   __syncthreads();
   pdl_wait();  // everything above touches only shared memory / kernel parameters
@@ -82,11 +65,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int total_tiles = tiles_mn * p.splits;
 
   if (wg == 0) {
-    ptx::setmaxnreg_dec<40>();
+    ptx::setmaxnreg_dec<tc::kProducerRegs>();
     if (threadIdx.x == 0) {
       // ------------------------------------------------------------ TMA producer
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int n_idx = tile % p.num_n;
         const int m_idx = (tile / p.num_n) % p.num_m;
@@ -95,67 +76,40 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
         const int m0 = m_idx * BM, n0 = n_idx * BN;
         for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          ptx::mbar_expect_tx(&full_bar[stage], C_::kStageBytes);
-          uint8_t* sa = smem + stage * C_::kStageBytes;
-          uint8_t* sb = sa + C_::kABytes;
+          const auto s = ring.produce();
           if (!A_MN) {
-            ptx::tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m0);
+            ptx::tma_load_2d(s.a, &tmA, s.bar, kb * BK, m0);
           } else {
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i)
-              ptx::tma_load_2d(sa + i * (BK * 128), &tmA, &full_bar[stage], m0 + i * 64, kb * BK);
+              ptx::tma_load_2d(s.a + i * (BK * 128), &tmA, s.bar, m0 + i * 64, kb * BK);
           }
           if (!B_MN) {
-            ptx::tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, n0);
+            ptx::tma_load_2d(s.b, &tmB, s.bar, kb * BK, n0);
           } else {
 #pragma unroll
             for (int i = 0; i < BN / 64; ++i)
-              ptx::tma_load_2d(sb + i * (BK * 128), &tmB, &full_bar[stage], n0 + i * 64, kb * BK);
+              ptx::tma_load_2d(s.b + i * (BK * 128), &tmB, s.bar, n0 + i * 64, kb * BK);
           }
-          if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
   } else {
-    ptx::setmaxnreg_inc<232>();
+    ptx::setmaxnreg_inc<tc::kConsumerRegs>();
     // -------------------------------------------------------------- consumers: rows [64 * half, 64 * half + 64) of a tile
     const int half = wg - 1;
-    const int t = threadIdx.x & 127;
-    const int lr = half * 64 + (t >> 5) * 16 + ((t & 31) >> 2);  // tile-local row of d[4j], d[4j+1]; +8 for d[4j+2..3]
-    const int lc = 2 * (t & 3);                                  // tile-local column of d[4j] within its 8-column group
+    const int lr = half * 64 + ptx::frag_row();  // tile-local row of d[4j], d[4j+1]; +8 for d[4j+2..3]
+    const int lc = ptx::frag_col();              // tile-local column of d[4j] within its 8-column group
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int n_idx = tile % p.num_n;
       const int m_idx = (tile / p.num_n) % p.num_m;
       const int split = tile / tiles_mn;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_addr = ptx::smem_u32(smem + stage * C_::kStageBytes) + half * 8192;
-        const uint32_t b_addr = ptx::smem_u32(smem + stage * C_::kStageBytes + C_::kABytes);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // K-major  : 8-row groups 1024 B apart (SBO); a 16-element K step is +32 B inside the row.
-          // MN-major : 64-element MN chunks BK*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO);
-          //            a 16-row K step is +2048 B.  The 64 rows of this half are one such chunk for A.
-          const uint64_t adesc = A_MN ? ptx::make_smem_desc_sw128(a_addr + k * 2048, BK * 128, 1024)
-                                      : ptx::make_smem_desc_sw128(a_addr + k * 32, 16, 1024);
-          const uint64_t bdesc = B_MN ? ptx::make_smem_desc_sw128(b_addr + k * 2048, BK * 128, 1024)
-                                      : ptx::make_smem_desc_sw128(b_addr + k * 32, 16, 1024);
-          ptx::Wgmma<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>::run(acc, adesc, bdesc, (kb > kb0 || k > 0) ? 1 : 0);
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        if (t == 0) ptx::mbar_arrive(&empty_bar[stage]);  // smem slot free: this warpgroup's MMAs have read it
-        if (++stage == C_::kStages) { stage = 0; phase ^= 1; }
-      }
+      ring.template consume<A_MN, B_MN>(acc, kb0, kb1, half);
       // ------------------------------------------------------------ epilogue from the accumulator registers
       const bool partial = (EPI == EPI_SPLITK_F32) && p.splits > 1;
       float* ws_tile = nullptr;
@@ -226,128 +180,19 @@ splitk_reduce_kernel(const float* __restrict__ ws, float* __restrict__ C, int M,
 }
 
 // ------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* ptr = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres);
-  if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || ptr == nullptr) {
-    set_last_error("cudaGetDriverEntryPoint(cuTensorMapEncodeTiled) failed: %s", cudaGetErrorString(e));
-    return nullptr;
-  }
-  fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  return fn;
-}
-
-// 2D bf16 tensor map: inner (contiguous) extent `inner`, outer extent `outer`, row pitch `ld` elements.
-int make_tmap(CUtensorMap* map, const void* base, long long inner, long long outer, long long ld, int box_inner,
-              int box_outer) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return MUSE_ERR_CUDA;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * 2) % 16 != 0) {
-    set_last_error("gemm: operand base must be 16B aligned and leading dim a multiple of 8 elements");
-    return MUSE_ERR_INVALID;
-  }
-  cuuint64_t dims[2] = {static_cast<cuuint64_t>(inner), static_cast<cuuint64_t>(outer)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_inner), static_cast<cuuint32_t>(box_outer)};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed with CUresult %d (inner=%lld outer=%lld ld=%lld)", (int)r, inner,
-                   outer, ld);
-    return MUSE_ERR_CUDA;
-  }
-  return MUSE_OK;
-}
-
-}  // namespace
-
-// 3-D bf16 tensor map {cols, rows, batches} over a [batches*rows, pitch] row-major buffer: box {64 cols, box_rows, 1},
-// 128-byte swizzle.  Rows past `rows` inside a batch are out of bounds -> zero-filled by the TMA unit.
-int make_tmap3(CUtensorMap* map, const void* base, long long cols, long long rows, long long batches,
-               long long row_pitch_elems, int box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return MUSE_ERR_CUDA;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (row_pitch_elems * 2) % 16 != 0) {
-    set_last_error("attention: operand base must be 16B aligned and the row stride a multiple of 8 elements");
-    return MUSE_ERR_INVALID;
-  }
-  cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(batches)};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(row_pitch_elems) * 2,
-                           static_cast<cuuint64_t>(rows) * static_cast<cuuint64_t>(row_pitch_elems) * 2};
-  cuuint32_t box[3] = {64, static_cast<cuuint32_t>(box_rows), 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled(3D) failed with CUresult %d (cols=%lld rows=%lld batches=%lld pitch=%lld)",
-                   (int)r, cols, rows, batches, row_pitch_elems);
-    return MUSE_ERR_CUDA;
-  }
-  return MUSE_OK;
-}
-
-// Generic bf16 tensor map (rank <= 5), 128-byte swizzle, zero fill out of bounds.  dims[0] is the contiguous dimension;
-// strides_bytes[i] is the byte stride of dims[i + 1].
-int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const unsigned long long* dims,
-                 const unsigned long long* strides_bytes, const unsigned* box) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return MUSE_ERR_CUDA;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) { set_last_error("tensor map: base must be 16B aligned"); return MUSE_ERR_INVALID; }
-  cuuint64_t d[5], st[4];
-  cuuint32_t bx[5], estr[5];
-  for (int i = 0; i < rank; ++i) { d[i] = dims[i]; bx[i] = box[i]; estr[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) {
-    st[i] = strides_bytes[i];
-    if (st[i] % 16 != 0) { set_last_error("tensor map: stride %d (%llu B) must be a multiple of 16 B", i, strides_bytes[i]); return MUSE_ERR_INVALID; }
-  }
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), d, st, bx, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error("cuTensorMapEncodeTiled(rank %d) failed with CUresult %d", rank, (int)r); return MUSE_ERR_CUDA; }
-  return MUSE_OK;
-}
-
-namespace {
-
-int g_num_sms = 0;
 int g_reserved_sms = 0;  // SMs left free for concurrently running collective kernels (set_reserved_sms)
 int num_sms() {
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 132;
-  }
-  const int n = g_num_sms - g_reserved_sms;
+  const int n = sm_count() - g_reserved_sms;
   return n > 16 ? n : 16;
 }
 
 template <int BN, bool A_MN, bool B_MN, int EPI>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes);
-    if (e != cudaSuccess) {
-      set_last_error("cudaFuncSetAttribute(gemm smem=%d): %s", Cfg<BN>::kSmemBytes, cudaGetErrorString(e));
-      return MUSE_ERR_CUDA;
-    }
-    attr_set = true;
-  }
+  constexpr auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI>;
+  if (int rc = set_max_dynamic_smem<kern>(Ring<BN>::kSmemBytes)) return rc;
   const int total = p.num_m * p.num_n * p.splits;
   const int grid = total < num_sms() ? total : num_sms();
-  pdl_launch(grid, 384, Cfg<BN>::kSmemBytes, stream)(kern, ta, tb, p);
+  pdl_launch(grid, tc::kThreads, Ring<BN>::kSmemBytes, stream)(kern, ta, tb, p);
   return check_launch("gemm_wgmma");
 }
 
@@ -417,11 +262,14 @@ int gemm_tc(const void* A, const void* B, void* C, const float* res, int M, int 
     return MUSE_ERR_INVALID;
   }
   const int BN = (N >= 256) ? 256 : 128;
+  // K-major operands: boxes of BK columns x the tile's rows; MN-major: 64-column chunks x BK rows
   CUtensorMap ta, tb;
   int rc;
-  rc = a_mn ? make_tmap(&ta, A, M, K, lda, 64, BK) : make_tmap(&ta, A, K, M, lda, BK, BM);
+  rc = a_mn ? make_tmap_bf16(&ta, "gemm", A, {M, K}, {2LL * lda}, {64, BK})
+            : make_tmap_bf16(&ta, "gemm", A, {K, M}, {2LL * lda}, {BK, BM});
   if (rc) return rc;
-  rc = b_mn ? make_tmap(&tb, B, N, K, ldb, 64, BK) : make_tmap(&tb, B, K, N, ldb, BK, BN);
+  rc = b_mn ? make_tmap_bf16(&tb, "gemm", B, {N, K}, {2LL * ldb}, {64, BK})
+            : make_tmap_bf16(&tb, "gemm", B, {K, N}, {2LL * ldb}, {BK, BN});
   if (rc) return rc;
 
   GemmParams p;

@@ -74,6 +74,22 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1,
+                                            int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1,
+                                            int32_t c2, int32_t c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2];\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 
 // ---------------------------------------------------------------- warpgroup helpers
 // Register budget of a warpgroup in a warp-specialised kernel: the TMA producer gives registers back, the MMA
@@ -96,6 +112,17 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
   d |= static_cast<uint64_t>(1) << 62;
   return d;
+}
+
+// Descriptors of k-step ks (16 elements of K) of a bf16 tile that TMA wrote with the 128-byte swizzle, rows of 64 elements.
+//  K-major : a row is one M/N index and holds 64 K elements; the k-step is +32 B inside the rows.
+//  MN-major: a row is one K index and holds 64 M/N elements; the k-step is 16 rows = +2048 B, and the next 64 M/N
+//            elements start 64 rows (8192 B) further on.
+__device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile_addr, int ks) {
+  return make_smem_desc_sw128(tile_addr + ks * 32, 16, 1024);
+}
+__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile_addr, int ks) {
+  return make_smem_desc_sw128(tile_addr + ks * 2048, 8192, 1024);
 }
 
 }  // namespace ptx

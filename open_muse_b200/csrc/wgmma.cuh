@@ -13,6 +13,11 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
 
+// row / column of d[4j] in the m64 tile of the calling thread's warpgroup (d[4j + 2] is 8 rows further down; add 8 j
+// to the column)
+__device__ __forceinline__ int frag_row() { return ((threadIdx.x & 127) >> 5) * 16 + ((threadIdx.x & 31) >> 2); }
+__device__ __forceinline__ int frag_col() { return 2 * (threadIdx.x & 3); }
+
 template <int N, int TA, int TB>
 struct Wgmma;
 
