@@ -1,23 +1,24 @@
 // wgmma / TMA attention for head_dim 64 and 48 (sm_90a): forward, dQ and dK/dV kernels.
 // Replaces the reference's materialised attention (muse/modeling_transformer.py:221-241) and its autograd backward.
 //
-// One CTA = one (batch, head) x one 128-row tile of the "owned" sequence dimension.  Every warpgroup of the CTA issues
-// wgmma on 64-row halves of the tile.  Score-like products (S, dP) land in an fp32 [128 x 64] shared-memory tile from
-// which the softmax math reads whole rows (one row per thread, as written below); the accumulating products (O, dQ, dK,
-// dV) stay in the wgmma accumulator registers for the whole loop and are stored once at the end.
+// One CTA = one (batch, head) x one 64-row tile of the "owned" sequence dimension: a consumer warpgroup that issues the
+// wgmma and does the softmax math, and a producer warp that streams the looped 64-row tiles through a ring of
+// shared-memory stages with TMA (`full` / `empty` mbarriers per stage).  Score-like products (S, dP) stay in the wgmma
+// accumulator registers; the softmax math runs on the fragment (row statistics with quad shuffles), and P / dS are
+// packed to bf16 in registers and fed straight back as the register A operand of the accumulating products, whose
+// accumulators (O, dQ, dK, dV) stay in registers for the whole loop and are stored once at the end.
 //
-//   forward  : owned = q rows.   S = Q K_j^T -> online softmax (fp32) -> P (bf16, smem) -> O += P V_j
+//   forward  : owned = q rows.   S = Q K_j^T -> online softmax (fp32) -> P (bf16 regs) -> O += P V_j
 //   dQ       : owned = q rows.   S, dP = dO V_j^T -> sweep 1: D = sum P*dP ; sweep 2: dS -> dQ += dS K_j
 //   dK/dV    : owned = kv rows.  S^T = K Q_i^T, dP^T = V dO_i^T -> P^T, dS^T -> dV += P^T dO_i, dK += dS^T Q_i
 // Operands are read straight from the strided [tokens, 3H] QKV projection through 3-D TMA tensor maps
 // {64 head columns, S rows, B} (rows past the end of a sequence are zero-filled by the TMA unit), with the same
-// 128-byte-swizzled tiles serving as K-major or MN-major MMA operands depending on the product.  The looped tiles sit in
-// a TMA ring that is refilled while the current tile is being processed.
-// The owned dimension is cut into ceil(S / 128) tiles of EQUAL height R = ceil(S / tiles) (S = 257 with the class token ->
-// three tiles of 86 rows; S = 256 -> two of 128; the 77 text states of cross-attention -> one of 77): a tile starts at row
-// i * R, its CTA still loads a 128-row box (rows past R belong to the next tile or are zero-filled past the sequence), the
-// MMAs run on all 128 rows, but only rows < R are kept, and warps whose 32 rows all lie past R skip the softmax math.
-// The looped dimension handles ragged tails by shrinking the MMA N/K to a multiple of 16.
+// 128-byte-swizzled tiles serving as K-major or MN-major MMA operands depending on the product.
+// The owned dimension is cut into ceil(S / 64) tiles of EQUAL height R = ceil(S / tiles) (S = 257 with the class token ->
+// five tiles of 52 rows; S = 256 -> four of 64; the 77 text states of cross-attention -> two of 39): a tile starts at row
+// i * R, its CTA loads a 64-row box (rows past R belong to the next tile or are zero-filled past the sequence), the MMAs
+// run on all 64 rows, but only rows < R are kept.  The looped dimension's ragged tail is zero-filled by TMA and masked.
+// Several CTAs share an SM, so one CTA's softmax math runs under another's MMAs and loads.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "tc_host.cuh"
@@ -42,19 +43,16 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
-// named barrier over the 256 math threads (barrier 0 stays __syncthreads for the whole CTA)
-__device__ __forceinline__ void math_sync() { asm volatile("bar.sync 1, 256;\n" ::: "memory"); }
-
-// Store 8 consecutive bf16 (one 16-byte chunk) of row r, columns [k0, k0+8) of a [128 x K] K-major SW128 operand
-// made of 64-column atoms (16 KB each).
-__device__ __forceinline__ void st_operand_chunk(uint8_t* base, int r, int k0, uint4 v) {
-  const int atom = k0 >> 6, c8 = (k0 & 63) >> 3;
-  *reinterpret_cast<uint4*>(base + atom * 16384 + r * 128 + ((c8 ^ (r & 7)) << 4)) = v;
-}
+constexpr int kBM = 64;                 // owned rows per CTA (one consumer warpgroup)
+constexpr int kBN = 64;                 // rows of a looped tile
+constexpr int kConsumers = 128;         // threads of the consumer warpgroup; the producer warp follows
+constexpr int kThreads = kConsumers + 32;
+constexpr int kStages = 2;              // ring stages of looped tiles
+constexpr int kTile = 64 * 64 * 2;      // one 64-row x 64-column bf16 TMA box, 8 KB
 
 struct TcParams {
   int Sq, Skv, nh;
-  int tile_rows;  // R: owned rows per CTA (<= 128)
+  int tile_rows;  // R: owned rows per CTA (<= 64)
   float scale;
   // outputs / side inputs (plain global pointers; rows addressed as b*S + s)
   bf16* out0;  long long out0_rs;   // fwd: O ; dq: dQ ; dkdv: dK
@@ -63,476 +61,393 @@ struct TcParams {
   float* dvec;                       // [B, nh, Sq]
 };
 
+// Barriers behind the tiles: own (the CTA's owned tiles, loaded once), full[kStages], empty[kStages].  Step st of the loop
+// uses stage st % kStages in phase (st / kStages) & 1.  `empty` gets one arrival from the consumer warpgroup once the
+// MMAs that read the stage have completed.
+struct Bars {
+  uint64_t* own;
+  uint64_t* full;
+  uint64_t* empty;
+  __device__ explicit Bars(uint8_t* p)
+      : own(reinterpret_cast<uint64_t*>(p)), full(own + 1), empty(own + 1 + kStages) {}
+  __device__ void init() const {  // one thread, before the __syncthreads that publishes the barriers
+    ptx::mbar_init(own, 1);
+    for (int i = 0; i < kStages; ++i) {
+      ptx::mbar_init(&full[i], 1);
+      ptx::mbar_init(&empty[i], 1);
+    }
+    ptx::fence_barrier_init();
+  }
+  // producer: the consumers have released the stage of step st (i.e. finished step st - kStages)
+  __device__ void wait_empty(int st) const { ptx::mbar_wait(&empty[st % kStages], ((st / kStages) & 1) ^ 1); }
+  __device__ void wait_full(int st) const { ptx::mbar_wait(&full[st % kStages], (st / kStages) & 1); }
+  // consumer thread 0, once the MMAs of step st have completed
+  __device__ void release(int st) const { ptx::mbar_arrive(&empty[st % kStages]); }
+};
+constexpr int kBarBytes = 64;
+
 // ------------------------------------------------------------------------------------------------ wgmma helpers
-constexpr int SP = 68;  // row pitch (floats) of the fp32 score tiles: float4 row reads by 8 consecutive rows hit 32 banks
-constexpr int SCORE_BYTES = 128 * SP * 4;
-
-// d (+)= A[64 rows x 16*ksteps] * B, A a K-major tile, B K-major (TB = 0, N rows) or MN-major (TB = 1, N columns).
-template <int N, int TB>
-__device__ __forceinline__ void mma_tile(float (&d)[N / 2], uint32_t a, uint32_t b, int ksteps, int accumulate) {
-  ptx::wgmma_fence();
-  for (int ks = 0; ks < ksteps; ++ks)
-    ptx::Wgmma<N, 0, TB>::run(d, ptx::desc_kmajor(a, ks), TB ? ptx::desc_mnmajor(b, ks) : ptx::desc_kmajor(b, ks),
-                              (accumulate || ks > 0) ? 1 : 0);
-  ptx::wgmma_commit();
-  ptx::wgmma_wait<0>();
-}
-
-template <int N>
-__device__ __forceinline__ void scores_n(uint32_t a, uint32_t b, int ksteps, float* dst, int row0) {
-  float d[N / 2];
-  mma_tile<N, 0>(d, a, b, ksteps, 0);
-  const int r = row0 + ptx::frag_row(), c = ptx::frag_col();
+// The MMAs always run the full 64-row looped tile: rows past the sequence are zero-filled by TMA and their score columns
+// are masked, so a ragged tail costs MMA work but no code path.  (Shrinking the MMA to the tail puts wgmma on a
+// data-dependent branch, and ptxas then serialises every wgmma of the kernel.)  Each step's MMAs are retired before
+// the next step's are issued, for the same reason: ptxas serialises a pipeline stage across which the next step's
+// fragments are defined.
+// d = A B^T for the 64 rows of A and of B, both K-major with 16 KS columns
+template <int KS>
+__device__ __forceinline__ void issue_scores(float (&d)[32], uint32_t a, uint32_t b) {
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    *reinterpret_cast<float2*>(dst + r * SP + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
-    *reinterpret_cast<float2*>(dst + (r + 8) * SP + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-  }
-}
-// rows [row0, row0 + 64) of A B^T (both K-major, N = n16 <= 64 rows of B) -> the fp32 score tile
-__device__ __forceinline__ void scores_to_smem(uint32_t a, uint32_t b, int n16, int ksteps, float* dst, int row0) {
-  switch (n16) {
-    case 16: scores_n<16>(a, b, ksteps, dst, row0); break;
-    case 32: scores_n<32>(a, b, ksteps, dst, row0); break;
-    case 48: scores_n<48>(a, b, ksteps, dst, row0); break;
-    default: scores_n<64>(a, b, ksteps, dst, row0); break;
-  }
+  for (int ks = 0; ks < KS; ++ks) ptx::Wgmma<64, 0, 0>::run(d, ptx::desc_kmajor(a, ks), ptx::desc_kmajor(b, ks), ks > 0);
 }
 
-// bf16 store of an [64 x HD] accumulator fragment: rows row0 + (fragment row) of `base` (row stride rs), if < rows_ok
+// d += A B: A the bf16 register fragment of a 64 x 64 product (wgmma.cuh), B MN-major with HD columns
 template <int HD>
-__device__ __forceinline__ void store_acc(const float (&d)[HD / 2], bf16* base, long long rs, int row0, int rows_ok,
-                                          const float* row_scale) {
-  const int r = row0 + ptx::frag_row(), c = ptx::frag_col();
+__device__ __forceinline__ void issue_acc(float (&d)[HD / 2], const uint32_t (&a)[16], uint32_t b) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) ptx::WgmmaRs<HD, 1>::run(d, a + 4 * ks, ptx::desc_mnmajor(b, ks), 1);
+}
+
+// reductions over the four threads that hold one fragment row
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+__device__ __forceinline__ float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+
+// bf16 store of an [64 x HD] accumulator fragment to rows (fragment row) of `base` (row stride rs) that are < rows_ok,
+// row r scaled by sc[0], row r + 8 by sc[1]
+template <int HD>
+__device__ __forceinline__ void store_acc(const float (&d)[HD / 2], bf16* base, long long rs, int rows_ok,
+                                          const float (&sc)[2]) {
+  const int r = ptx::frag_row(), c = ptx::frag_col();
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int rr = r + 8 * hr;
     if (rr >= rows_ok) continue;
-    const float sc = row_scale ? row_scale[rr] : 1.f;
     bf16* dst = base + rr * rs;
 #pragma unroll
     for (int j = 0; j < HD / 8; ++j)
-      *reinterpret_cast<uint32_t*>(dst + 8 * j + c) = pack_bf16(d[4 * j + 2 * hr] * sc, d[4 * j + 2 * hr + 1] * sc);
+      *reinterpret_cast<uint32_t*>(dst + 8 * j + c) = pack_bf16(d[4 * j + 2 * hr] * sc[hr], d[4 * j + 2 * hr + 1] * sc[hr]);
   }
 }
 
+// column (within the 64-column tile) of fragment element i
+__device__ __forceinline__ int frag_col_of(int i) { return 8 * (i >> 2) + ptx::frag_col() + (i & 1); }
+
 // ------------------------------------------------------------------------------------------------ forward
-// 128 threads = one warpgroup, which issues the MMAs of both 64-row halves (O of both halves in registers).
-// smem: Q 16K | K 8K | V 8K | P 16K | S fp32 | per-row scale | barriers -> two co-resident CTAs per SM overlap each other's
-// TMA / MMA / softmax phases.
-constexpr int FWD_BN = 64;
-constexpr int FWD_SMEM = 16384 /*Q*/ + 8192 /*K*/ + 8192 /*V*/ + 16384 /*P*/ + SCORE_BYTES + 512 + 64;
+// smem: Q 8K | kStages x {K 8K, V 8K} | barriers
+constexpr int FWD_SMEM = kTile + kStages * 2 * kTile + kBarBytes;
 
 template <int HD>
-__global__ void __launch_bounds__(128, 2)
+__global__ void __launch_bounds__(kThreads, 3)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const TcParams p) {
   pdl_trigger();
-  extern __shared__ __align__(1024) uint8_t smem_raw[];  // 128B-swizzled tiles need 1024 B alignment
-  uint8_t* smem = smem_raw;
+  extern __shared__ __align__(1024) uint8_t smem[];  // 128B-swizzled tiles need 1024 B alignment
   if ((ptx::smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sQ = smem;
-  uint8_t* sK = smem + 16384;
-  uint8_t* sV = smem + 24576;
-  uint8_t* sP = smem + 32768;
-  float* sS = reinterpret_cast<float*>(smem + 49152);
-  float* sRow = reinterpret_cast<float*>(smem + 49152 + SCORE_BYTES);  // per-row alpha, then 1 / l
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 49152 + SCORE_BYTES + 512);
-  uint64_t* bar_kv = bars;      // Q (first use) + K tile landed
-  uint64_t* bar_v = bars + 1;   // V tile landed
+  uint8_t* sKV = smem + kTile;
+  const Bars bars(sKV + kStages * 2 * kTile);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int q0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
   const int rows_here = min(p.tile_rows, p.Sq - q0);
-  const bool warp_active = warp * 32 < rows_here;  // warps whose rows all belong to the next tile skip the softmax math
-  if (tid == 0) {
-    ptx::mbar_init(bar_kv, 1);
-    ptx::mbar_init(bar_v, 1);
-    ptx::fence_barrier_init();
-  }
+  if (tid == 0) bars.init();
   __syncthreads();
   pdl_wait();  // everything above touches only shared memory / kernel parameters
-  const int ntiles = ceil_div(p.Skv, FWD_BN);
+  const int ntiles = ceil_div(p.Skv, kBN);
 
-  if (tid == 0) {
-    ptx::mbar_expect_tx(bar_kv, 16384 + 8192);
-    ptx::tma_load_3d(sQ, &tmQ, bar_kv, h * HD, q0, b);
-    ptx::tma_load_3d(sK, &tmK, bar_kv, h * HD, 0, b);
-    ptx::mbar_expect_tx(bar_v, 8192);
-    ptx::tma_load_3d(sV, &tmV, bar_v, h * HD, 0, b);
+  if (tid >= kConsumers) {  // producer warp: Q once, then K_j / V_j through the ring
+    if (tid == kConsumers) {
+      ptx::mbar_expect_tx(bars.own, kTile);
+      ptx::tma_load_3d(sQ, &tmQ, bars.own, h * HD, q0, b);
+      for (int j = 0; j < ntiles; ++j) {
+        bars.wait_empty(j);
+        uint64_t* full = &bars.full[j % kStages];
+        uint8_t* sK = sKV + (j % kStages) * 2 * kTile;
+        ptx::mbar_expect_tx(full, 2 * kTile);
+        ptx::tma_load_3d(sK, &tmK, full, h * HD, j * kBN, b);
+        ptx::tma_load_3d(sK + kTile, &tmV, full, h * HD, j * kBN, b);
+      }
+    }
+    return;
   }
-  const float sl2 = p.scale * kLog2e;
-  float m = -INFINITY, l = 0.f;
-  float o[2][HD / 2];
-#pragma unroll
-  for (int i = 0; i < HD / 2; ++i) { o[0][i] = 0.f; o[1][i] = 0.f; }
 
+  const float sl2 = p.scale * kLog2e;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // per fragment row r, r + 8; l is this thread's partial sum
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  ptx::mbar_wait(bars.own, 0);
   for (int j = 0; j < ntiles; ++j) {
-    const uint32_t par = j & 1;
-    const int nvalid = min(FWD_BN, p.Skv - j * FWD_BN);
-    const int n16 = (nvalid + 15) & ~15;
-    ptx::mbar_wait(bar_kv, par);
-    scores_to_smem(ptx::smem_u32(sQ), ptx::smem_u32(sK), n16, HD / 16, sS, 0);
-    scores_to_smem(ptx::smem_u32(sQ) + 8192, ptx::smem_u32(sK), n16, HD / 16, sS, 64);
-    __syncthreads();  // S_j is in shared memory and K_j has been consumed
-    if (tid == 0 && j + 1 < ntiles) {  // fetch K_{j+1} under the softmax math
-      ptx::mbar_expect_tx(bar_kv, 8192);
-      ptx::tma_load_3d(sK, &tmK, bar_kv, h * HD, (j + 1) * FWD_BN, b);
-    }
-    float alpha = 1.f;
-    if (warp_active) {
-    // the whole score row (<= 64 columns) fits in registers.  The instruction count per score element is what bounds
-    // this loop, so the ragged-tail masking is kept out of the full-tile path and the softmax scale is folded into one
-    // FFMA per element.
-    float sc[64];
+    const int nvalid = min(kBN, p.Skv - j * kBN);
+    const uint32_t sK = ptx::smem_u32(sKV + (j % kStages) * 2 * kTile);
+    float s[32];
+    bars.wait_full(j);
+    ptx::wgmma_fence();
+    issue_scores<HD / 16>(s, ptx::smem_u32(sQ), sK);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(s);
+    if (nvalid < kBN) {  // ragged last tile only
 #pragma unroll
-    for (int c = 0; c < 64; c += 4) {
-      if (c < n16) {
-        const float4 v = *reinterpret_cast<const float4*>(sS + tid * SP + c);
-        sc[c] = v.x; sc[c + 1] = v.y; sc[c + 2] = v.z; sc[c + 3] = v.w;
-      } else {
-        sc[c] = sc[c + 1] = sc[c + 2] = sc[c + 3] = -INFINITY;
-      }
+      for (int i = 0; i < 32; ++i) s[i] = frag_col_of(i) < nvalid ? s[i] : -INFINITY;
     }
-    if (nvalid < FWD_BN) {
+    float alpha[2];
 #pragma unroll
-      for (int i = 0; i < 64; ++i) sc[i] = (i < nvalid) ? sc[i] : -INFINITY;
+    for (int hr = 0; hr < 2; ++hr) {
+      float raw = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) raw = fmaxf(raw, fmaxf(s[4 * jj + 2 * hr], s[4 * jj + 2 * hr + 1]));
+      // Lazy running maximum: the reference point m only moves when the tile's maximum exceeds it by more than 8 (log2
+      // units), i.e. P entries stay below 2^8 -- harmless in bf16 / fp32 -- and the final 1 / l normalisation and the
+      // LSE (m + log2 l) are exact for any reference point.  Most tiles then leave m alone and alpha is exactly 1.
+      const float cand = quad_max(raw) * sl2;
+      const float mx = (cand > m[hr] + 8.0f) ? cand : m[hr];
+      alpha[hr] = ex2(m[hr] - mx);  // 0 on the first tile (m = -inf), 1 when the reference point stays
+      m[hr] = mx;
     }
-    float raw = -INFINITY;
+    uint32_t pa[16];
+    float ls[2] = {0.f, 0.f};
 #pragma unroll
-    for (int i = 0; i < 64; ++i) raw = fmaxf(raw, sc[i]);
-    // Lazy running maximum: the reference point m only moves when the tile's maximum exceeds it by more than 8 (log2
-    // units), i.e. P entries stay below 2^8 -- harmless in bf16 / fp32 -- and the final 1 / l normalisation and the LSE
-    // (m + log2 l) are exact for any reference point.  Most tiles then leave m alone and alpha is exactly 1.
-    const float cand = raw * sl2;
-    const float mx = (cand > m + 8.0f) ? cand : m;
-    alpha = ex2(m - mx);  // 0 on the first tile (m = -inf), 1 when the reference point stays
-    m = mx;
-    float l4[4] = {0.f, 0.f, 0.f, 0.f};  // four independent chains instead of one 64-long dependent add chain
-#pragma unroll
-    for (int i = 0; i < 64; ++i) {
-      sc[i] = ex2(fmaf(sc[i], sl2, -m));
-      l4[i & 3] += sc[i];
+    for (int i = 0; i < 16; ++i) {  // s[2 i], s[2 i + 1] lie in row r + 8 (i & 1)
+      const float p0 = ex2(fmaf(s[2 * i], sl2, -m[i & 1])), p1 = ex2(fmaf(s[2 * i + 1], sl2, -m[i & 1]));
+      ls[i & 1] += p0 + p1;
+      pa[i] = pack_bf16(p0, p1);
     }
-    l = fmaf(l, alpha, (l4[0] + l4[1]) + (l4[2] + l4[3]));
 #pragma unroll
-    for (int i = 0; i < 64; i += 8) {
-      if (i < n16) {
-        uint4 u;
-        u.x = pack_bf16(sc[i], sc[i + 1]); u.y = pack_bf16(sc[i + 2], sc[i + 3]);
-        u.z = pack_bf16(sc[i + 4], sc[i + 5]); u.w = pack_bf16(sc[i + 6], sc[i + 7]);
-        st_operand_chunk(sP, tid, i, u);
-      }
-    }
-    }  // warp_active
-    sRow[tid] = alpha;
-    ptx::fence_proxy_async();
-    __syncthreads();  // P_j is visible to the tensor core, every row's alpha to every thread
-    if (j > 0) {  // rescale the running output
+    for (int hr = 0; hr < 2; ++hr) l[hr] = fmaf(l[hr], alpha[hr], ls[hr]);
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const float a0 = sRow[hh * 64 + ptx::frag_row()], a1 = sRow[hh * 64 + ptx::frag_row() + 8];
-#pragma unroll
-        for (int i = 0; i < HD / 2; i += 4) {
-          o[hh][i] *= a0; o[hh][i + 1] *= a0; o[hh][i + 2] *= a1; o[hh][i + 3] *= a1;
-        }
-      }
-    }
-    ptx::mbar_wait(bar_v, par);
-    mma_tile<HD, 1>(o[0], ptx::smem_u32(sP), ptx::smem_u32(sV), n16 >> 4, j > 0);
-    mma_tile<HD, 1>(o[1], ptx::smem_u32(sP) + 8192, ptx::smem_u32(sV), n16 >> 4, j > 0);
-    __syncthreads();  // P_j and V_j have been consumed
-    if (tid == 0 && j + 1 < ntiles) {
-      ptx::mbar_expect_tx(bar_v, 8192);
-      ptx::tma_load_3d(sV, &tmV, bar_v, h * HD, (j + 1) * FWD_BN, b);
-    }
+    for (int i = 0; i < HD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    ptx::wgmma_fence();
+    issue_acc<HD>(o, pa, sK + kTile);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(o);
+    if (tid == 0) bars.release(j);
   }
   // epilogue: O / l -> bf16 rows, LSE
-  const int row = q0 + tid;
-  sRow[tid] = 1.f / l;
-  if (tid < rows_here) p.lse[(static_cast<long long>(b) * p.nh + h) * p.Sq + row] = (m + log2f(l)) * kLn2;
-  __syncthreads();
-  bf16* obase = p.out0 + (static_cast<long long>(b) * p.Sq + q0) * p.out0_rs + h * HD;
-  store_acc<HD>(o[0], obase, p.out0_rs, 0, rows_here, sRow);
-  store_acc<HD>(o[1], obase, p.out0_rs, 64, rows_here, sRow);
+  const int r = ptx::frag_row();
+  float inv[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const float lsum = quad_sum(l[hr]);
+    inv[hr] = 1.f / lsum;
+    if ((tid & 3) == 0 && r + 8 * hr < rows_here)
+      p.lse[(static_cast<long long>(b) * p.nh + h) * p.Sq + q0 + r + 8 * hr] = (m[hr] + log2f(lsum)) * kLn2;
+  }
+  store_acc<HD>(o, p.out0 + (static_cast<long long>(b) * p.Sq + q0) * p.out0_rs + h * HD, p.out0_rs, rows_here, inv);
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dQ
-// 256 threads = two warpgroups; warpgroup g issues the MMAs of rows [64 g, 64 g + 64) and keeps that half of dQ in
-// registers.  In the softmax math, warps w and w+4 share rows 32*(w%4).. and split the 64 score columns in two halves.
-// K/V tiles sit in a 3-stage TMA ring with prefetch distance 2.
-// smem: Q 16K | dO 16K | 3 x {K_j 8K, V_j 8K} | dS 16K (the partial-D exchange buffer aliases it) | S, dP fp32
-constexpr int BWD_BN = 64;
-constexpr int DQ_SMEM = 16384 * 2 + 3 * 16384 + 16384 + 2 * SCORE_BYTES + 64;
+// The ring streams the K/V tiles twice: sweep 1 accumulates D = sum_j P dP per row, sweep 2 forms dS and dQ.
+// smem: Q 8K | dO 8K | kStages x {K_j 8K, V_j 8K} | barriers
+constexpr int DQ_SMEM = 2 * kTile + kStages * 2 * kTile + kBarBytes;
 
 template <int HD>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(kThreads, 3)
 attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const TcParams p) {
   pdl_trigger();
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
+  extern __shared__ __align__(1024) uint8_t smem[];
   if ((ptx::smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sQ = smem;
-  uint8_t* sdO = smem + 16384;
-  uint8_t* sKV = smem + 32768;             // 3 stages x {K 8 KB, V 8 KB}
-  uint8_t* sdS = smem + 32768 + 49152;
-  float* sDp = reinterpret_cast<float*>(sdS);  // [2][128] partial D (only used between the two sweeps)
-  float* sS = reinterpret_cast<float*>(sdS + 16384);
-  float* sdP = sS + 128 * SP;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + 16384 + 2 * SCORE_BYTES);
-  uint64_t* bar_kv = bars;       // [3] TMA landed
+  uint8_t* sdO = smem + kTile;
+  uint8_t* sKV = smem + 2 * kTile;
+  const Bars bars(sKV + kStages * 2 * kTile);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int g = tid >> 7;                     // warpgroup: MMA rows [64 g, 64 g + 64)
-  const int half = warp >> 2;                 // column half handled by this thread
-  const int r = (warp & 3) * 32 + lane;       // row handled by this thread
+  const int tid = threadIdx.x;
   const int q0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
   const int rows_here = min(p.tile_rows, p.Sq - q0);
-  const bool warp_active = (warp & 3) * 32 < rows_here;  // other warps keep the barrier protocol but skip the math
-  const bool row_ok = r < rows_here;
-  if (tid == 0) {
-    for (int i = 0; i < 3; ++i) ptx::mbar_init(&bar_kv[i], 1);
-    ptx::fence_barrier_init();
-  }
+  if (tid == 0) bars.init();
   __syncthreads();
   pdl_wait();  // everything above touches only shared memory / kernel parameters
-  const int ntiles = ceil_div(p.Skv, BWD_BN);
+  const int ntiles = ceil_div(p.Skv, kBN);
   const int nsteps = 2 * ntiles;
-  const int row = q0 + r;
-  const long long stat_idx = (static_cast<long long>(b) * p.nh + h) * p.Sq + row;
-  const float lse2 = row_ok ? p.lse[stat_idx] * kLog2e : 0.f;
-  const float sl2 = p.scale * kLog2e;
 
-  auto load_kv = [&](int step) {       // thread 0: TMA of the K/V tile of `step` into its ring stage
-    uint8_t* sK = sKV + (step % 3) * 16384;
-    const int jn = step % ntiles;
-    ptx::tma_load_3d(sK, &tmK, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
-    ptx::tma_load_3d(sK + 8192, &tmV, &bar_kv[step % 3], h * HD, jn * BWD_BN, b);
-  };
-  if (tid == 0) {
-    ptx::mbar_expect_tx(&bar_kv[0], 16384 * 2 + 8192 * 2);
-    ptx::tma_load_3d(sQ, &tmQ, &bar_kv[0], h * HD, q0, b);
-    ptx::tma_load_3d(sdO, &tmdO, &bar_kv[0], h * HD, q0, b);
-    load_kv(0);
-    if (nsteps > 1) {
-      ptx::mbar_expect_tx(&bar_kv[1], 8192 * 2);
-      load_kv(1);
+  if (tid >= kConsumers) {  // producer warp: Q, dO once, then K_j / V_j twice through the ring
+    if (tid == kConsumers) {
+      ptx::mbar_expect_tx(bars.own, 2 * kTile);
+      ptx::tma_load_3d(sQ, &tmQ, bars.own, h * HD, q0, b);
+      ptx::tma_load_3d(sdO, &tmdO, bars.own, h * HD, q0, b);
+      for (int st = 0; st < nsteps; ++st) {
+        bars.wait_empty(st);
+        uint64_t* full = &bars.full[st % kStages];
+        uint8_t* sK = sKV + (st % kStages) * 2 * kTile;
+        const int j = st % ntiles;
+        ptx::mbar_expect_tx(full, 2 * kTile);
+        ptx::tma_load_3d(sK, &tmK, full, h * HD, j * kBN, b);
+        ptx::tma_load_3d(sK + kTile, &tmV, full, h * HD, j * kBN, b);
+      }
     }
+    return;
   }
+
+  const int r = ptx::frag_row();
+  const long long stat_base = (static_cast<long long>(b) * p.nh + h) * p.Sq + q0;
+  const float sl2 = p.scale * kLog2e;
+  float lse2[2], dsum[2] = {0.f, 0.f};
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) lse2[hr] = (r + 8 * hr < rows_here) ? p.lse[stat_base + r + 8 * hr] * kLog2e : 0.f;
   float dq[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) dq[i] = 0.f;
-  float dsum = 0.f;
+  ptx::mbar_wait(bars.own, 0);
   for (int st = 0; st < nsteps; ++st) {
     const int j = st % ntiles;
-    const bool sweep2 = st >= ntiles;
-    const int u = st - ntiles;  // index among the sweep-2 steps
-    const int nvalid = min(BWD_BN, p.Skv - j * BWD_BN);
-    const int n16 = (nvalid + 15) & ~15;
-    if (tid == 0 && st + 2 < nsteps) {  // ring stage (st+2)%3 was last read in step st-1, which every thread has left
-      ptx::mbar_expect_tx(&bar_kv[(st + 2) % 3], 8192 * 2);
-      load_kv(st + 2);
-    }
-    ptx::mbar_wait(&bar_kv[st % 3], (st / 3) & 1);
-    uint8_t* sK = sKV + (st % 3) * 16384;
-    scores_to_smem(ptx::smem_u32(sQ) + g * 8192, ptx::smem_u32(sK), n16, HD / 16, sS, g * 64);
-    scores_to_smem(ptx::smem_u32(sdO) + g * 8192, ptx::smem_u32(sK) + 8192, n16, HD / 16, sdP, g * 64);
-    math_sync();  // S and dP of this step are in shared memory
-    float s_reg[32], d_reg[32];
-    if (warp_active) {
+    const int nvalid = min(kBN, p.Skv - j * kBN);
+    const uint32_t sK = ptx::smem_u32(sKV + (st % kStages) * 2 * kTile);
+    float s[32], dp[32];
+    bars.wait_full(st);
+    ptx::wgmma_fence();
+    issue_scores<HD / 16>(s, ptx::smem_u32(sQ), sK);
+    issue_scores<HD / 16>(dp, ptx::smem_u32(sdO), sK + kTile);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(s);
+    ptx::fence_operand(dp);
 #pragma unroll
-      for (int cc = 0; cc < 32; cc += 4) {
-        const int c = half * 32 + cc;
-        if (c < n16) {
-          const float4 a4 = *reinterpret_cast<const float4*>(sS + r * SP + c);
-          const float4 b4 = *reinterpret_cast<const float4*>(sdP + r * SP + c);
-          s_reg[cc] = a4.x; s_reg[cc + 1] = a4.y; s_reg[cc + 2] = a4.z; s_reg[cc + 3] = a4.w;
-          d_reg[cc] = b4.x; d_reg[cc + 1] = b4.y; d_reg[cc + 2] = b4.z; d_reg[cc + 3] = b4.w;
+    for (int i = 0; i < 32; ++i) s[i] = ex2(fmaf(s[i], sl2, -lse2[(i >> 1) & 1]));  // P
+    if (nvalid < kBN) {  // ragged last tile only
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = frag_col_of(i) < nvalid ? s[i] : 0.f;
+    }
+    if (st < ntiles) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dsum[(i >> 1) & 1] = fmaf(s[i], dp[i], dsum[(i >> 1) & 1]);
+      if (st == ntiles - 1) {  // D of the row, for sweep 2 and for the dK/dV kernel
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          dsum[hr] = quad_sum(dsum[hr]);
+          if ((tid & 3) == 0 && r + 8 * hr < rows_here) p.dvec[stat_base + r + 8 * hr] = dsum[hr];
         }
       }
+    } else {
+      const float nd[2] = {-dsum[0] * p.scale, -dsum[1] * p.scale};
+      uint32_t da[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+        da[i] = pack_bf16(s[2 * i] * fmaf(dp[2 * i], p.scale, nd[i & 1]), s[2 * i + 1] * fmaf(dp[2 * i + 1], p.scale, nd[i & 1]));
+      ptx::wgmma_fence();
+      issue_acc<HD>(dq, da, sK);  // dQ += dS K_j
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::fence_operand(dq);
     }
-    const float neg_d_scaled = -dsum * p.scale;
-#pragma unroll
-    for (int cc = 0; cc < 32; cc += 16) {
-      const int c = half * 32 + cc;
-      if (warp_active && c < n16) {
-#pragma unroll
-        for (int i8 = 0; i8 < 16; i8 += 8) {
-          float pr[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) pr[i] = ex2(fmaf(s_reg[cc + i8 + i], sl2, -lse2));
-          if (nvalid < BWD_BN) {  // ragged last tile only
-#pragma unroll
-            for (int i = 0; i < 8; ++i) pr[i] = (c + i8 + i < nvalid) ? pr[i] : 0.f;
-          }
-          if (!sweep2) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) dsum = fmaf(pr[i], d_reg[cc + i8 + i], dsum);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) pr[i] *= fmaf(d_reg[cc + i8 + i], p.scale, neg_d_scaled);
-            uint4 v;
-            v.x = pack_bf16(pr[0], pr[1]); v.y = pack_bf16(pr[2], pr[3]);
-            v.z = pack_bf16(pr[4], pr[5]); v.w = pack_bf16(pr[6], pr[7]);
-            st_operand_chunk(sdS, r, c + i8, v);
-          }
-        }
-      }
-    }
-    if (sweep2) {
-      ptx::fence_proxy_async();
-      math_sync();  // dS is visible to the tensor core
-      mma_tile<HD, 1>(dq, ptx::smem_u32(sdS) + g * 8192, ptx::smem_u32(sK), n16 >> 4, u > 0);  // dQ += dS K_j
-    }
-    if (st == ntiles - 1) {  // D = sum over both column halves, identical in both threads of the row
-      sDp[half * 128 + r] = dsum;
-      math_sync();
-      dsum = sDp[r] + sDp[128 + r];
-      if (half == 0 && row_ok) p.dvec[stat_idx] = dsum;  // for the dK/dV kernels
-    }
-    math_sync();  // end of step: score tiles, dS and the ring stage are free again
+    if (tid == 0) bars.release(st);
   }
-  store_acc<HD>(dq, p.out0 + (static_cast<long long>(b) * p.Sq + q0) * p.out0_rs + h * HD, p.out0_rs, g * 64, rows_here,
-                nullptr);
+  const float one[2] = {1.f, 1.f};
+  store_acc<HD>(dq, p.out0 + (static_cast<long long>(b) * p.Sq + q0) * p.out0_rs + h * HD, p.out0_rs, rows_here, one);
 }
 
 // ------------------------------------------------------------------------------------------------ backward: dK, dV
-// Same structure as the dQ kernel, looping over 64-row q tiles; dK and dV of the warpgroup's 64 kv rows in registers.
-// smem: K_j 16K | V_j 16K | 3 x {Q_i 8K, dO_i 8K} | P^T 16K | dS^T 16K | lse/D 512 B | S^T, dP^T fp32
-constexpr int DKDV_SMEM = 16384 * 2 + 3 * 16384 + 16384 * 2 + 512 + 2 * SCORE_BYTES + 64;
+// Same structure as the dQ kernel, looping over 64-row q tiles; dK and dV of the CTA's kv rows in registers.  The producer
+// warp also stages each q tile's lse (x log2 e) and D (x scale) as 64-float vectors next to the ring, read per column.
+// smem: K 8K | V 8K | kStages x {Q_i 8K, dO_i 8K} | kStages x {lse 64, D 64} floats | barriers
+constexpr int DKDV_SMEM = 2 * kTile + kStages * 2 * kTile + kStages * 2 * kBN * 4 + kBarBytes;
 
 template <int HD>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(kThreads, 2)
 attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                         const TcParams p) {
   pdl_trigger();
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
+  extern __shared__ __align__(1024) uint8_t smem[];
   if ((ptx::smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sK = smem;
-  uint8_t* sV = smem + 16384;
-  uint8_t* sQO = smem + 32768;             // 3 stages x {Q_i 8 KB, dO_i 8 KB}
-  uint8_t* sPT = smem + 32768 + 49152;
-  uint8_t* sdST = sPT + 16384;
-  float* sLD = reinterpret_cast<float*>(sdST + 16384);  // [lse 64 | D 64] of the current q tile
-  float* sS = sLD + 128;
-  float* sdP = sS + 128 * SP;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sdST + 16384 + 512 + 2 * SCORE_BYTES);
-  uint64_t* bar_ld = bars;       // [3] TMA landed
+  uint8_t* sV = smem + kTile;
+  uint8_t* sQO = smem + 2 * kTile;
+  float* sLD = reinterpret_cast<float*>(sQO + kStages * 2 * kTile);
+  const Bars bars(reinterpret_cast<uint8_t*>(sLD + kStages * 2 * kBN));
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int g = tid >> 7;
-  const int half = warp >> 2;
-  const int r = (warp & 3) * 32 + lane;
+  const int tid = threadIdx.x;
   const int kv0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
   const int rows_here = min(p.tile_rows, p.Skv - kv0);
-  const bool warp_active = (warp & 3) * 32 < rows_here;
-  if (tid == 0) {
-    for (int i = 0; i < 3; ++i) ptx::mbar_init(&bar_ld[i], 1);
-    ptx::fence_barrier_init();
-  }
+  if (tid == 0) bars.init();
   __syncthreads();
   pdl_wait();  // everything above touches only shared memory / kernel parameters
-  const int ntiles = ceil_div(p.Sq, BWD_BN);
-  const bool kv_ok = r < rows_here;  // rows past the tile's share belong to the next CTA (or lie past the sequence)
-  const float sl2 = p.scale * kLog2e;
+  const int ntiles = ceil_div(p.Sq, kBN);
   const long long stat_base = (static_cast<long long>(b) * p.nh + h) * p.Sq;
 
-  auto load_q = [&](int i) {
-    uint8_t* sQ = sQO + (i % 3) * 16384;
-    ptx::tma_load_3d(sQ, &tmQ, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
-    ptx::tma_load_3d(sQ + 8192, &tmdO, &bar_ld[i % 3], h * HD, i * BWD_BN, b);
-  };
-  if (tid == 0) {
-    ptx::mbar_expect_tx(&bar_ld[0], 16384 * 2 + 8192 * 2);
-    ptx::tma_load_3d(sK, &tmK, &bar_ld[0], h * HD, kv0, b);
-    ptx::tma_load_3d(sV, &tmV, &bar_ld[0], h * HD, kv0, b);
-    load_q(0);
-    if (ntiles > 1) {
-      ptx::mbar_expect_tx(&bar_ld[1], 8192 * 2);
-      load_q(1);
+  if (tid >= kConsumers) {  // producer warp: K, V once, then {Q_i, dO_i, lse_i, D_i} through the ring
+    const int lane = tid & 31;
+    if (lane == 0) {
+      ptx::mbar_expect_tx(bars.own, 2 * kTile);
+      ptx::tma_load_3d(sK, &tmK, bars.own, h * HD, kv0, b);
+      ptx::tma_load_3d(sV, &tmV, bars.own, h * HD, kv0, b);
     }
+    for (int i = 0; i < ntiles; ++i) {
+      bars.wait_empty(i);
+      float* ld = sLD + (i % kStages) * 2 * kBN;
+      for (int k = lane; k < kBN; k += 32) {
+        const int qr = i * kBN + k;
+        ld[k] = (qr < p.Sq) ? p.lse[stat_base + qr] * kLog2e : 0.f;
+        ld[kBN + k] = (qr < p.Sq) ? p.dvec[stat_base + qr] * p.scale : 0.f;  // pre-scaled: dS = P (dP*scale - D*scale)
+      }
+      __syncwarp();  // the vectors are written before lane 0's arrival publishes the stage
+      if (lane == 0) {
+        uint64_t* full = &bars.full[i % kStages];
+        uint8_t* sQ = sQO + (i % kStages) * 2 * kTile;
+        ptx::mbar_expect_tx(full, 2 * kTile);
+        ptx::tma_load_3d(sQ, &tmQ, full, h * HD, i * kBN, b);
+        ptx::tma_load_3d(sQ + kTile, &tmdO, full, h * HD, i * kBN, b);
+      }
+    }
+    return;
   }
+
+  const int r = ptx::frag_row(), c = ptx::frag_col();
+  const bool kv_ok = r + 8 < rows_here;  // both fragment rows are kept (rows past R belong to the next CTA)
+  const float sl2 = p.scale * kLog2e;
   float dk[HD / 2], dv[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
+  ptx::mbar_wait(bars.own, 0);
   for (int i = 0; i < ntiles; ++i) {
-    const int q0 = i * BWD_BN;
-    const int nvalid = min(BWD_BN, p.Sq - q0);
-    const int n16 = (nvalid + 15) & ~15;
-    float* sL = sLD;
-    float* sD = sL + 64;
-    if (tid < BWD_BN) {
-      const int qr = q0 + tid;
-      sL[tid] = (qr < p.Sq) ? p.lse[stat_base + qr] * kLog2e : 0.f;
-      sD[tid] = (qr < p.Sq) ? p.dvec[stat_base + qr] * p.scale : 0.f;  // pre-scaled: dS = P (dP*scale - D*scale)
-    }
-    if (tid == 0 && i + 2 < ntiles) {  // ring stage (i+2)%3 was last read in step i-1, which every thread has left
-      ptx::mbar_expect_tx(&bar_ld[(i + 2) % 3], 8192 * 2);
-      load_q(i + 2);
-    }
-    ptx::mbar_wait(&bar_ld[i % 3], (i / 3) & 1);
-    uint8_t* sQ = sQO + (i % 3) * 16384;
-    scores_to_smem(ptx::smem_u32(sK) + g * 8192, ptx::smem_u32(sQ), n16, HD / 16, sS, g * 64);
-    scores_to_smem(ptx::smem_u32(sV) + g * 8192, ptx::smem_u32(sQ) + 8192, n16, HD / 16, sdP, g * 64);
-    math_sync();  // S^T, dP^T and this step's lse / D are visible to all threads
-    float s_reg[32], d_reg[32];
-    if (warp_active) {
+    const int nvalid = min(kBN, p.Sq - i * kBN);
+    const uint32_t sQ = ptx::smem_u32(sQO + (i % kStages) * 2 * kTile);
+    const float* sL = sLD + (i % kStages) * 2 * kBN;
+    const float* sD = sL + kBN;
+    float s[32], dp[32];
+    bars.wait_full(i);
+    ptx::wgmma_fence();
+    issue_scores<HD / 16>(s, ptx::smem_u32(sK), sQ);
+    issue_scores<HD / 16>(dp, ptx::smem_u32(sV), sQ + kTile);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(s);
+    ptx::fence_operand(dp);
+    uint32_t pa[16], da[16];
 #pragma unroll
-      for (int cc = 0; cc < 32; cc += 4) {
-        const int c = half * 32 + cc;
-        if (c < n16) {
-          const float4 a4 = *reinterpret_cast<const float4*>(sS + r * SP + c);
-          const float4 b4 = *reinterpret_cast<const float4*>(sdP + r * SP + c);
-          s_reg[cc] = a4.x; s_reg[cc + 1] = a4.y; s_reg[cc + 2] = a4.z; s_reg[cc + 3] = a4.w;
-          d_reg[cc] = b4.x; d_reg[cc + 1] = b4.y; d_reg[cc + 2] = b4.z; d_reg[cc + 3] = b4.w;
-        }
+    for (int k = 0; k < 16; ++k) {  // s[2 k], s[2 k + 1]: row r + 8 (k & 1), q columns col, col + 1
+      const int col = 8 * (k >> 1) + c;
+      const float2 lq = *reinterpret_cast<const float2*>(sL + col);
+      const float2 dd = *reinterpret_cast<const float2*>(sD + col);
+      float p0 = ex2(fmaf(s[2 * k], sl2, -lq.x)), p1 = ex2(fmaf(s[2 * k + 1], sl2, -lq.y));
+      if (nvalid < kBN || !kv_ok) {  // ragged q tile / kv rows that are not kept
+        const bool row_ok = r + 8 * (k & 1) < rows_here;
+        p0 = (row_ok && col < nvalid) ? p0 : 0.f;
+        p1 = (row_ok && col + 1 < nvalid) ? p1 : 0.f;
       }
+      pa[k] = pack_bf16(p0, p1);
+      da[k] = pack_bf16(p0 * fmaf(dp[2 * k], p.scale, -dd.x), p1 * fmaf(dp[2 * k + 1], p.scale, -dd.y));
     }
-#pragma unroll
-    for (int cc = 0; cc < 32; cc += 16) {
-      const int c = half * 32 + cc;
-      if (warp_active && c < n16) {
-#pragma unroll
-        for (int k8 = 0; k8 < 16; k8 += 8) {
-          float pt[8], ds[8], lq[8], dq_[8];
-#pragma unroll
-          for (int k = 0; k < 8; k += 4) {  // per-column lse / D: 16-byte broadcast reads
-            const float4 a = *reinterpret_cast<const float4*>(sL + c + k8 + k);
-            const float4 e = *reinterpret_cast<const float4*>(sD + c + k8 + k);
-            lq[k] = a.x; lq[k + 1] = a.y; lq[k + 2] = a.z; lq[k + 3] = a.w;
-            dq_[k] = e.x; dq_[k + 1] = e.y; dq_[k + 2] = e.z; dq_[k + 3] = e.w;
-          }
-#pragma unroll
-          for (int k = 0; k < 8; ++k) pt[k] = ex2(fmaf(s_reg[cc + k8 + k], sl2, -lq[k]));
-          if (nvalid < BWD_BN || !kv_ok) {  // ragged q tile / kv rows past the end of the sequence
-#pragma unroll
-            for (int k = 0; k < 8; ++k) pt[k] = (kv_ok && c + k8 + k < nvalid) ? pt[k] : 0.f;
-          }
-#pragma unroll
-          for (int k = 0; k < 8; ++k) ds[k] = pt[k] * fmaf(d_reg[cc + k8 + k], p.scale, -dq_[k]);
-          uint4 x, y;
-          x.x = pack_bf16(pt[0], pt[1]); x.y = pack_bf16(pt[2], pt[3]);
-          x.z = pack_bf16(pt[4], pt[5]); x.w = pack_bf16(pt[6], pt[7]);
-          y.x = pack_bf16(ds[0], ds[1]); y.y = pack_bf16(ds[2], ds[3]);
-          y.z = pack_bf16(ds[4], ds[5]); y.w = pack_bf16(ds[6], ds[7]);
-          st_operand_chunk(sPT, r, c + k8, x);
-          st_operand_chunk(sdST, r, c + k8, y);
-        }
-      }
-    }
-    ptx::fence_proxy_async();
-    math_sync();  // P^T / dS^T are visible to the tensor core
-    mma_tile<HD, 1>(dv, ptx::smem_u32(sPT) + g * 8192, ptx::smem_u32(sQ) + 8192, n16 >> 4, i > 0);  // dV += P^T dO_i
-    mma_tile<HD, 1>(dk, ptx::smem_u32(sdST) + g * 8192, ptx::smem_u32(sQ), n16 >> 4, i > 0);         // dK += dS^T Q_i
-    math_sync();  // end of step: the score tiles, P^T / dS^T, lse / D and the ring stage are free again
+    ptx::wgmma_fence();
+    issue_acc<HD>(dv, pa, sQ + kTile);  // dV += P^T dO_i
+    issue_acc<HD>(dk, da, sQ);          // dK += dS^T Q_i
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(dk);
+    ptx::fence_operand(dv);
+    if (tid == 0) bars.release(i);
   }
   const long long base = static_cast<long long>(b) * p.Skv + kv0;
-  store_acc<HD>(dk, p.out0 + base * p.out0_rs + h * HD, p.out0_rs, g * 64, rows_here, nullptr);
-  store_acc<HD>(dv, p.out1 + base * p.out1_rs + h * HD, p.out1_rs, g * 64, rows_here, nullptr);
+  const float one[2] = {1.f, 1.f};
+  store_acc<HD>(dk, p.out0 + base * p.out0_rs + h * HD, p.out0_rs, rows_here, one);
+  store_acc<HD>(dv, p.out1 + base * p.out1_rs + h * HD, p.out1_rs, rows_here, one);
 }
 
 // Raises kernel K's dynamic shared-memory limit and asks for all of L1 as shared memory, once per kernel.
@@ -546,16 +461,16 @@ int set_smem(int bytes) {
   return set_max_dynamic_smem<K>(bytes);
 }
 
-// Balanced tiling of an owned dimension of S rows: ceil(S / 128) tiles of R = ceil(S / tiles) rows each.
+// Balanced tiling of an owned dimension of S rows: ceil(S / 64) tiles of R = ceil(S / tiles) rows each.
 void balanced_tiles(int S, int* ntile, int* rows) {
-  *ntile = ceil_div(S, 128);
+  *ntile = ceil_div(S, kBM);
   *rows = ceil_div(S, *ntile);
 }
 
-// 3-D map {cols, S rows, B} of a [B * S, rs] row-major operand, box {64 columns, box_rows rows, 1}: rows past S inside a
+// 3-D map {cols, S rows, B} of a [B * S, rs] row-major operand, box {64 columns, 64 rows, 1}: rows past S inside a
 // batch are out of bounds and read as zeros.
-int qkv_tmap(CUtensorMap* map, const void* base, int cols, int S, int B, int rs, int box_rows) {
-  return make_tmap_bf16(map, "attention", base, {cols, S, B}, {2LL * rs, 2LL * rs * S}, {64, box_rows, 1});
+int qkv_tmap(CUtensorMap* map, const void* base, int cols, int S, int B, int rs) {
+  return make_tmap_bf16(map, "attention", base, {cols, S, B}, {2LL * rs, 2LL * rs * S}, {64, 64, 1});
 }
 
 template <int HD>
@@ -565,14 +480,14 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   balanced_tiles(Sq, &ntile, &tile_rows);
   CUtensorMap tq, tk, tv;
   int rc;
-  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs, 128))) return rc;
-  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs, FWD_BN))) return rc;
-  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs, FWD_BN))) return rc;
+  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs))) return rc;
+  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs))) return rc;
+  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs))) return rc;
   if ((rc = set_smem<attn_fwd_tc_kernel<HD>>(FWD_SMEM))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale; p.tile_rows = tile_rows;
   p.out0 = reinterpret_cast<bf16*>(o); p.out0_rs = o_rs; p.lse = lse;
-  pdl_launch(dim3(ntile, nh, B), 128, FWD_SMEM, s)(attn_fwd_tc_kernel<HD>, tq, tk, tv, p);
+  pdl_launch(dim3(ntile, nh, B), kThreads, FWD_SMEM, s)(attn_fwd_tc_kernel<HD>, tq, tk, tv, p);
   return check_launch("attn_fwd_tc");
 }
 
@@ -585,27 +500,23 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* d_o, 
   balanced_tiles(Sq, &ntile, &tile_rows);
   CUtensorMap tq, tdo, tk, tv;
   int rc;
-  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs, 128))) return rc;
-  if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs, 128))) return rc;
-  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs, BWD_BN))) return rc;
-  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs, BWD_BN))) return rc;
+  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs))) return rc;
+  if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs))) return rc;
+  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs))) return rc;
+  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs))) return rc;
   if ((rc = set_smem<attn_bwd_dq_tc_kernel<HD>>(DQ_SMEM))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale;
   p.out0 = reinterpret_cast<bf16*>(dq); p.out0_rs = dq_rs; p.lse = const_cast<float*>(lse); p.dvec = dvec;
   p.tile_rows = tile_rows;
-  pdl_launch(dim3(ntile, nh, B), 256, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD>, tq, tdo, tk, tv, p);
+  pdl_launch(dim3(ntile, nh, B), kThreads, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD>, tq, tdo, tk, tv, p);
   if ((rc = check_launch("attn_bwd_dq_tc"))) return rc;
 
   balanced_tiles(Skv, &ntile, &tile_rows);
-  if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs, 128))) return rc;
-  if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs, 128))) return rc;
-  if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs, BWD_BN))) return rc;
-  if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs, BWD_BN))) return rc;
   if ((rc = set_smem<attn_bwd_dkdv_tc_kernel<HD>>(DKDV_SMEM))) return rc;
   p.out0 = reinterpret_cast<bf16*>(dk); p.out0_rs = dk_rs; p.out1 = reinterpret_cast<bf16*>(dv); p.out1_rs = dv_rs;
   p.tile_rows = tile_rows;
-  pdl_launch(dim3(ntile, nh, B), 256, DKDV_SMEM, s)(attn_bwd_dkdv_tc_kernel<HD>, tk, tv, tq, tdo, p);
+  pdl_launch(dim3(ntile, nh, B), kThreads, DKDV_SMEM, s)(attn_bwd_dkdv_tc_kernel<HD>, tk, tv, tq, tdo, p);
   return check_launch("attn_bwd_dkdv_tc");
 }
 
