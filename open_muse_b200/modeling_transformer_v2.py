@@ -6,9 +6,10 @@ MaskGiTUViT_v2(**cfg)`` reproduces the reference's initial weights, including th
 classifier-free-guidance ``generate2`` (:330-479).
 
 Everything runs on libmuse_b200: wgmma GEMMs for every Linear / 1x1 conv, wgmma attention, fused prenorm-residual
-norm + adaLN modulation, depthwise-conv + Norm2D, GELU + GlobalResponseNorm, the fused decode step; training goes through
-one autograd Function for the whole network (``uvit_v2_train.py``: forward with saved activations + hand-written backward).
-The modules below are parameter containers; the inference arithmetic lives in ``_forward_tokens``.
+norm + adaLN modulation, depthwise-conv + Norm2D, GELU + GlobalResponseNorm, the fused decode step.  The block forwards
+(ResBlock, AttentionBlock2D, TransformerLayer, the force_down_up_sample resampling) are defined once in ``uvit_v2_train.py``
+next to their hand-written backwards; inference (``_forward_tokens``) calls them without keeping their saved state, training
+runs them inside one autograd Function per block.  The modules below are parameter containers.
 Activations are token-major ``[B*h*w, C]`` throughout -- the NCHW <-> NHWC permutes of the reference disappear.
 """
 from __future__ import annotations
@@ -21,6 +22,7 @@ import torch
 from torch import nn
 
 from . import ops
+from . import uvit_v2_train as T
 from .modeling_utils import ConfigMixin, ModelMixin
 from .sampling import cosine_schedule
 
@@ -332,46 +334,6 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         return W
 
     # ------------------------------------------------------------------------------------------- forward
-    def _res_block(self, h, w, mod_all, B, hw):
-        c = self.config
-        rms = 0 if c.norm_type == "layernorm" else 1
-        d = ops.dwconv3x3_norm(h, w["dw"], w["dw_norm"], B, hw, hw, c.layer_norm_eps, rms)
-        g = ops.grn(ops.linear_fwd(d, w["cw0"]), w["gamma"], w["beta"], B, hw * hw)
-        h = ops.linear_fwd(g, w["cw4"], res=h)  # + block input (fused residual epilogue)
-        o, n = w["mod"]
-        return ops.adaln_apply_(h, mod_all[:, o:o + n], B, hw * hw)
-
-    def _cross_attn(self, y, enc, a, B, S, Skv, res=None):
-        Hc = a["o"].shape[0]
-        q = ops.linear_fwd(y, a["q"])
-        kv = ops.linear_fwd(enc, a["kv"])
-        ctx, _ = ops.attn_fwd(q, kv[:, :Hc], kv[:, Hc:], B, a["nh"], S, Skv, a["sc"], head_dim=a["hd"])
-        return ops.linear_fwd(ctx, a["o"], res=res)
-
-    def _attention_block(self, h, enc_h, w, B, S, Skv):
-        c = self.config
-        rms = 0 if c.norm_type == "layernorm" else 1
-        enc = enc_h if w["kvm"] is None else ops.linear_fwd(ops.silu_bf16(enc_h), w["kvm"])
-        _, y = ops.add_norm_mod(h, w["ln1"], c.layer_norm_eps, rms, want_residual=False)
-        a1 = self._cross_attn(y, enc, w["a1"], B, S, Skv)
-        r2, y2 = ops.add_norm_mod(a1, w["ln2"], c.layer_norm_eps, rms, residual=h)
-        return self._cross_attn(y2, enc, w["a2"], B, S, Skv, res=r2)  # + prenorm residual (fused epilogue)
-
-    def _layer(self, x, r, enc, w, mod_all, B, S, Skv):
-        c = self.config
-        H, rms, eps = c.hidden_size, (0 if c.norm_type == "layernorm" else 1), c.layer_norm_eps
-        m = lambda k: mod_all[:, w[k][0]:w[k][0] + w[k][1]]
-        r1, y = ops.add_norm_mod(x, w["ln1"], eps, rms, residual=r, mod=m("mod1"), rows_per_sample=S)
-        qkv = ops.linear_fwd(y, w["sa"]["qkv"])
-        ctx, _ = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, w["sa"]["nh"], S, S, w["sa"]["sc"],
-                              head_dim=w["sa"]["hd"])
-        a = ops.linear_fwd(ctx, w["sa"]["o"])
-        r2, y = ops.add_norm_mod(a, w["ln2"], eps, rms, residual=r1, mod=m("mod2"), rows_per_sample=S)
-        cc = self._cross_attn(y, enc, w["ca"], B, S, Skv)
-        r3, y = ops.add_norm_mod(cc, w["ln3"], eps, 0, residual=r2, mod=m("mod3"), rows_per_sample=S)
-        f = ops.linear_fwd(ops.glu_fwd(ops.linear_fwd(y, w["wi"])), w["wo"])
-        return f, r3
-
     def _forward_tokens(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds):
         c = self.config
         if not input_ids.is_cuda:
@@ -396,19 +358,14 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         dbg = self._debug_stages
         if dbg is not None:
             dbg.update(enc=enc.float().view(B, Skv, -1), cond=cond.float(), embed=h.view(B, S, -1).clone())
-        if "ds" in W:  # force_down_up_sample (:509-513): Norm2D, then the k2s2 conv as one GEMM over [B*S/4, (dy, dx, ci)] patches
-            if hw % 2:
-                raise ValueError(f"force_down_up_sample needs an even token grid, got {hw}x{hw}")
-            C = h.shape[1]
-            _, y = ops.add_norm_mod(h, W["ds_norm"], eps, rms, want_residual=False)
-            y = y.view(B, hw // 2, 2, hw // 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(B * S // 4, 4 * C)
-            h = ops.linear_fwd(y, W["ds"], out_dtype=torch.float32)
+        if "ds" in W:  # force_down_up_sample (:509-513)
+            h, _ = T._resample_fwd(h, W, "ds", B, hw, eps, rms)
             hw, S = hw // 2, S // 4
             if dbg is not None:
-                dbg["downsample"] = h.view(B, hw, hw, C).permute(0, 3, 1, 2).clone()
+                dbg["downsample"] = h.view(B, hw, hw, -1).permute(0, 3, 1, 2).clone()
         for w in W["down"]:
-            h = self._res_block(h, w, mod_all, B, hw)
-            h = self._attention_block(h, enc, w, B, S, Skv)
+            h, _ = T._res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=False)
+            h, _ = T._attn_block_fwd(h, enc, w, B, S, Skv, eps, rms)
         if dbg is not None:
             dbg["down"] = h.view(B, S, -1).clone()
         _, y = ops.add_norm_mod(h, W["pth_norm"], eps, rms, want_residual=False)
@@ -416,7 +373,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         if dbg is not None:
             dbg["hidden0"] = x.float().view(B, S, -1)
         for i, w in enumerate(W["layers"]):
-            x, r = self._layer(x, r, enc, w, mod_all, B, S, Skv)
+            x, r, _ = T._layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms)
             if dbg is not None:
                 dbg[f"layer{i}"] = (x.float() + r).view(B, S, -1)
         _, y = ops.add_norm_mod(x, W["pfh_norm"], eps, rms, residual=r, want_residual=False)  # (x + residual) -> norm (:289-291)
@@ -424,18 +381,15 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         if dbg is not None:
             dbg["from_hidden"] = h.view(B, S, -1).clone()
         for w in W["up"]:
-            h = self._res_block(h, w, mod_all, B, hw)
-            h = self._attention_block(h, enc, w, B, S, Skv)
+            h, _ = T._res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=False)
+            h, _ = T._attn_block_fwd(h, enc, w, B, S, Skv, eps, rms)
         if dbg is not None:
             dbg["up"] = h.view(B, S, -1).clone()
-        if "us" in W:  # (:555-559): Norm2D, then ConvTranspose2d(2, 2) as one GEMM to [B*S, (dy, dx, co)] + depth-to-space
-            C = h.shape[1]
-            _, y = ops.add_norm_mod(h, W["us_norm"], eps, rms, want_residual=False)
-            t = ops.linear_fwd(y, W["us"], out_dtype=torch.float32)
-            h = t.view(B, hw, hw, 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(B * S * 4, C)
+        if "us" in W:  # (:555-559)
+            h, _ = T._resample_fwd(h, W, "us", B, hw, eps, rms)
             hw, S = hw * 2, S * 4
             if dbg is not None:
-                dbg["upsample"] = h.view(B, hw, hw, C).permute(0, 3, 1, 2).clone()
+                dbg["upsample"] = h.view(B, hw, hw, -1).permute(0, 3, 1, 2).clone()
         # ConvMlmLayer: 1x1 conv -> Norm2D -> 1x1 conv
         y1 = ops.linear_fwd(ops.cast_bf16(h), W["mlm1"])
         _, y2 = ops.add_norm_mod(y1, W["mlm_norm"], eps, rms, want_residual=False)
@@ -446,20 +400,11 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         c = self.config
         B, S = input_ids.shape
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            # training: one autograd Function for the whole network (uvit_v2_train.py)
+            # training: one autograd Function per block, so parameter gradients appear during backward (DDP overlap)
             if self.training and (c.hidden_dropout > 0.0 or c.attention_dropout > 0.0):
                 raise NotImplementedError("open_muse_b200.MaskGiTUViT_v2: dropout > 0 in training mode is not implemented")
-            from . import uvit_v2_train as T
-
-            if getattr(self, "_single_train_function", False):  # private test hook: one Function for the whole network
-                if c.force_down_up_sample:
-                    raise NotImplementedError("open_muse_b200.MaskGiTUViT_v2: force_down_up_sample=True trains through the "
-                                              "per-block Functions only (the default path)")
-                padded, loss = T.UViTTrainFn.apply(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels,
-                                                   label_smoothing, loss_weight, *self.parameters())
-            else:  # default: one Function per block, so parameter gradients appear during backward (DDP overlap)
-                padded, loss = T.train_forward(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels,
-                                               label_smoothing, loss_weight)
+            padded, loss = T.train_forward(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels,
+                                           label_smoothing, loss_weight)
             logits = padded.view(B, S, -1)[:, :, : c.codebook_size]
             if not (_raw_bf16 or torch.is_autocast_enabled()):
                 logits = logits.float()

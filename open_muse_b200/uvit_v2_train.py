@@ -1,17 +1,18 @@
-"""Training step (forward with saved activations + hand-written backward) of ``MaskGiTUViT_v2`` on libmuse_b200.
+"""Block forwards of ``MaskGiTUViT_v2`` and its training step (forward with saved activations + hand-written backward) on
+libmuse_b200.
 
-Default path (``train_forward``): one ``torch.autograd.Function`` per block -- conditioning MLP, text-state projection, token
-embedding, optional down-sampling convolution (``ResampleFn``), every ResBlock + AttentionBlock2D pair, the two projections,
-every transformer layer, optional up-sampling transposed convolution, ConvMlmLayer + cross-entropy.  Each forward is the
-inference path of ``modeling_transformer_v2.py`` with the activations its backward kernels need kept alive; each backward
-returns the gradients of that block's parameters (reference names, fp32) as soon as it has run, so DDP's bucket all-reduces
-overlap the rest of the backward pass.  ``UViTTrainFn`` (private test hook ``model._single_train_function``) is the same
-computation as ONE Function for the whole network; the tests pin the two against each other.
+``_res_block_fwd``, ``_attn_block_fwd``, ``_layer_fwd`` and ``_resample_fwd`` are the ONE definition of those blocks:
+inference (``MaskGiTUViT_v2._forward_tokens``) calls them and drops the state they return, training keeps it for the
+matching ``*_bwd``, which unpacks the same tuple.  ``train_forward`` runs one ``torch.autograd.Function`` per block --
+conditioning MLP, text-state projection, token embedding, optional down-sampling convolution (``ResampleFn``), every
+ResBlock + AttentionBlock2D pair, the two projections, every transformer layer, optional up-sampling transposed convolution,
+ConvMlmLayer + cross-entropy.  Each backward returns the gradients of that block's parameters (reference names, fp32) as
+soon as it has run, so DDP's bucket all-reduces overlap the rest of the backward pass.
 
 All arithmetic is in the C-ABI kernels: wgmma GEMMs for every Linear / 1x1 / patch convolution (dgrad with an MN-major
-weight operand, deterministic split-K wgrad), wgmma attention backward, and the U-ViT kernels of csrc/uvit_bwd.cu.  Things
-that are single tensors consumed by many blocks get ONE accumulator: the text states (fp32, atomic-accumulating dgrad) and
-the stacked adaLN mapper output (each op adds into its own column slice), so no gradient is summed with eager ops.
+weight operand, split-K wgrad accumulating with fp32 atomics), wgmma attention backward, and the U-ViT kernels of csrc/uvit_bwd.cu.  Inside
+a block, tensors consumed by several ops get ONE accumulator: the text states (fp32, atomic-accumulating dgrad) and the
+block's adaLN (scale | shift) rows (each op adds into its own column slice); autograd sums these across the blocks.
 """
 from __future__ import annotations
 
@@ -49,16 +50,11 @@ class _G(dict):
         return self[key]
 
 
-def _sub(G, W, key, idx=None):
-    """gradient dict for a nested block of W (W[key] is a dict, or a list of dicts when idx is given)."""
-    holder = G.setdefault(key, {} if idx is None else {})
-    if idx is None:
-        if not isinstance(holder, _G):
-            holder = G[key] = _G(W[key])
-        return holder
-    if idx not in holder:
-        holder[idx] = _G(W[key][idx])
-    return holder[idx]
+def _sub(G, W, key):
+    """gradient dict for a nested block of W (W[key] is a dict)."""
+    if key not in G:
+        G[key] = _G(W[key])
+    return G[key]
 
 
 # ------------------------------------------------------------------------------------------------ attention helper
@@ -97,12 +93,16 @@ def _attn_bwd(do, y, ctx_in, a, ga, st, B, S, Skv, fused, d_ctx_acc=None):
 
 
 # ------------------------------------------------------------------------------------------------ blocks
-def _res_block_fwd(h, w, mod_all, B, hw, eps, rms):
-    d, conv = ops.dwconv3x3_norm(h, w["dw"], w["dw_norm"], B, hw, hw, eps, rms, save_conv=True)
+def _res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=True):
+    """save=False (inference): no conv output is written and adaLN modulates in place (no copy), so no state is returned."""
+    out = ops.dwconv3x3_norm(h, w["dw"], w["dw_norm"], B, hw, hw, eps, rms, save_conv=save)
+    d, conv = out if save else (out, None)
     g1 = ops.linear_fwd(d, w["cw0"])
     g2, stats = ops.grn(g1, w["gamma"], w["beta"], B, hw * hw, save_stats=True)
-    h2 = ops.linear_fwd(g2, w["cw4"], res=h)
+    h2 = ops.linear_fwd(g2, w["cw4"], res=h)  # + block input (fused residual epilogue)
     o, n = w["mod"]
+    if not save:
+        return ops.adaln_apply_(h2, mod_all[:, o:o + n], B, hw * hw), None
     h3 = ops.adaln_apply(h2, mod_all[:, o:o + n], B, hw * hw)
     return h3, (h, d, conv, g1, g2, stats, h2)
 
@@ -148,7 +148,7 @@ def _attn_block_bwd(dout, st, w, g, enc, d_enc, B, S, Skv, eps, rms):
     return dh
 
 
-def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, H, eps, rms):
+def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms):
     m = lambda k: mod_all[:, w[k][0]:w[k][0] + w[k][1]]
     r1, y1 = ops.add_norm_mod(x, w["ln1"], eps, rms, residual=r, mod=m("mod1"), rows_per_sample=S)
     c, s_sa = _attn_fwd(y1, None, w["sa"], B, S, S, True)
@@ -182,225 +182,25 @@ def _layer_bwd(df, dr3, st, w, g, enc, d_enc, mod_all, d_mod_all, B, S, Skv, eps
     return dx, dr
 
 
-# ------------------------------------------------------------------------------------------------ whole network
-def forward(model, W, input_ids, encoder_hidden_states, cond_embeds, micro_conds):
-    """Inference-identical forward that also returns the saved state for ``backward``."""
-    from .modeling_transformer_v2 import sinusoidal_encode
-
-    c = model.config
-    B, S = input_ids.shape
-    hw = int(S ** 0.5)
-    rms, eps, H = (0 if c.norm_type == "layernorm" else 1), c.layer_norm_eps, c.hidden_size
-    Skv = encoder_hidden_states.shape[1]
-    ehs = encoder_hidden_states.reshape(B * Skv, -1).to(BF16).contiguous()
-    r_enc, enc = ops.add_norm_mod(ops.linear_fwd(ehs, W["encoder_proj"]), W["enc_norm"], eps, rms)
-    mc = sinusoidal_encode(micro_conds.flatten(), c.micro_cond_encode_dim).reshape(B, -1)
-    cond_in = torch.cat([cond_embeds.float(), mc], dim=1).to(BF16).contiguous()
-    c1 = ops.linear_fwd(cond_in, W["cond0"])
-    c1s = ops.silu_bf16(c1)
-    cond = ops.linear_fwd(c1s, W["cond2"])
-    sc = ops.silu_bf16(cond)
-    mod_all = ops.linear_fwd(sc, W["mappers"], out_dtype=F32)
-    ids = input_ids.contiguous().to(torch.int64)
-    e = ops.embed_fwd(ids, W["emb"], None)
-    _, en = ops.add_norm_mod(e, W["emb_norm"], eps, rms, want_residual=False)
-    h = ops.linear_fwd(en, W["emb_conv"], out_dtype=F32)
-    blocks = {"down": [], "up": []}
-    for w in W["down"]:
-        h, s_r = _res_block_fwd(h, w, mod_all, B, hw, eps, rms)
-        h, s_a = _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms)
-        blocks["down"].append((s_r, s_a))
-    h_down = h
-    _, y_pth = ops.add_norm_mod(h, W["pth_norm"], eps, rms, want_residual=False)
-    x, r, layers = ops.linear_fwd(y_pth, W["pth"]), None, []
-    for w in W["layers"]:
-        x, r, s_l = _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, H, eps, rms)
-        layers.append(s_l)
-    r_f, y_f = ops.add_norm_mod(x, W["pfh_norm"], eps, rms, residual=r)
-    h = ops.linear_fwd(y_f, W["pfh"], out_dtype=F32)
-    for w in W["up"]:
-        h, s_r = _res_block_fwd(h, w, mod_all, B, hw, eps, rms)
-        h, s_a = _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms)
-        blocks["up"].append((s_r, s_a))
-    hb = ops.cast_bf16(h)
-    y1 = ops.linear_fwd(hb, W["mlm1"])
-    r_m, y2 = ops.add_norm_mod(y1, W["mlm_norm"], eps, rms)
-    logits = ops.linear_fwd(y2, W["mlm2"])
-    saved = dict(B=B, S=S, hw=hw, Skv=Skv, ehs=ehs, r_enc=r_enc, enc=enc, cond_in=cond_in, c1=c1, c1s=c1s, cond=cond, sc=sc,
-                 mod_all=mod_all, ids=ids, e=e, en=en, blocks=blocks, h_down=h_down, y_pth=y_pth, layers=layers, r_f=r_f,
-                 y_f=y_f, hb=hb, y1=y1, r_m=r_m, y2=y2)
-    return logits, saved
-
-
-def backward(model, W, saved, d_logits):
-    """d_logits: bf16 [B*S, vpad].  Returns the nested fp32 gradient dict G mirroring W."""
-    c = model.config
-    s = saved
-    B, S, hw, Skv = s["B"], s["S"], s["hw"], s["Skv"]
-    rms, eps = (0 if c.norm_type == "layernorm" else 1), c.layer_norm_eps
-    enc, mod_all = s["enc"], s["mod_all"]
-    G = _G(W)
-    d_enc = _z(enc)          # fp32 accumulator: the text states feed every cross attention
-    d_mod = _z(mod_all)      # every adaLN op adds into its own column slice
-    # ConvMlmLayer
-    dy2 = _lin_bwd(d_logits, s["y2"], W["mlm2"], G.of("mlm2"))
-    dy1, _ = ops.add_norm_mod_bwd(dy2, None, s["r_m"], W["mlm_norm"], eps, rms, BF16, dw=G.of("mlm_norm"), want_dr=False)
-    dh = _lin_bwd(dy1, s["hb"], W["mlm1"], G.of("mlm1"), dx_dtype=F32)
-    for i in reversed(range(len(W["up"]))):
-        w, g = W["up"][i], _sub(G, W, "up", i)
-        s_r, s_a = s["blocks"]["up"][i]
-        dh = _attn_block_bwd(dh, s_a, w, g, enc, d_enc, B, S, Skv, eps, rms)
-        dh = _res_block_bwd(dh, s_r, w, g, mod_all, d_mod, B, hw, eps, rms)
-    dy_f = _lin_bwd(ops.cast_bf16(dh), s["y_f"], W["pfh"], G.of("pfh"))
-    dx, dr = ops.add_norm_mod_bwd(dy_f, None, s["r_f"], W["pfh_norm"], eps, rms, BF16, dw=G.of("pfh_norm"))
-    for i in reversed(range(len(W["layers"]))):
-        dx, dr = _layer_bwd(dx, dr, s["layers"][i], W["layers"][i], _sub(G, W, "layers", i), enc, d_enc, mod_all, d_mod, B, S,
-                            Skv, eps, rms)
-    dy_pth = _lin_bwd(dx, s["y_pth"], W["pth"], G.of("pth"))
-    dh, _ = ops.add_norm_mod_bwd(dy_pth, None, s["h_down"], W["pth_norm"], eps, rms, F32, dw=G.of("pth_norm"), want_dr=False)
-    for i in reversed(range(len(W["down"]))):
-        w, g = W["down"][i], _sub(G, W, "down", i)
-        s_r, s_a = s["blocks"]["down"][i]
-        dh = _attn_block_bwd(dh, s_a, w, g, enc, d_enc, B, S, Skv, eps, rms)
-        dh = _res_block_bwd(dh, s_r, w, g, mod_all, d_mod, B, hw, eps, rms)
-    # ConvEmbed
-    d_en = _lin_bwd(ops.cast_bf16(dh), s["en"], W["emb_conv"], G.of("emb_conv"))
-    d_e, _ = ops.add_norm_mod_bwd(d_en, None, s["e"], W["emb_norm"], eps, rms, F32, dw=G.of("emb_norm"), want_dr=False)
-    ops.embed_bwd(s["ids"], d_e, G.of("emb"), None)
-    # conditioning: stacked adaLN mappers <- SiLU <- cond_embed MLP
-    d_sc = _lin_bwd(ops.cast_bf16(d_mod), s["sc"], W["mappers"], G.of("mappers"))
-    d_cond = ops.silu_bwd(d_sc, s["cond"])
-    d_c1s = _lin_bwd(d_cond, s["c1s"], W["cond2"], G.of("cond2"))
-    d_c1 = ops.silu_bwd(d_c1s, s["c1"])
-    _lin_bwd(d_c1, s["cond_in"], W["cond0"], G.of("cond0"), need_dx=False)
-    # text states: encoder_proj + norm
-    d_y0, _ = ops.add_norm_mod_bwd(d_enc, None, s["r_enc"], W["enc_norm"], eps, rms, BF16, dw=G.of("enc_norm"), want_dr=False)
-    _lin_bwd(d_y0, s["ehs"], W["encoder_proj"], G.of("encoder_proj"), need_dx=False)
-    return G
-
-
-def param_grads(model, G):
-    """Maps the packed gradient buffers back onto the parameters (reference names), in ``model.parameters()`` order."""
-    c = model.config
-    out = {}
-
-    def put(p, g):
-        if p is not None and g is not None:
-            out[p] = g.reshape(p.shape)
-
-    def rows(g, *ps):
-        o = 0
-        for p in ps:
-            put(p, g[o:o + p.shape[0]])
-            o += p.shape[0]
-
-    def attn(a, g, fused):
-        if fused:
-            rows(g["qkv"], a.query.weight, a.key.weight, a.value.weight)
-        else:
-            put(a.query.weight, g["q"])
-            rows(g["kv"], a.key.weight, a.value.weight)
-        put(a.out.weight, g["o"])
-
-    mappers = []
-
-    def block(blk, gl):
-        for i, (rb, ab) in enumerate(zip(blk.res_blocks, blk.attention_blocks)):
-            g = gl[i]
-            put(rb.depthwise.weight, g["dw"].t().contiguous())
-            put(rb.norm.norm.weight, g.get("dw_norm"))
-            put(rb.channelwise[0].weight, g["cw0"])
-            put(rb.channelwise[2].gamma, g["gamma"])
-            put(rb.channelwise[2].beta, g["beta"])
-            put(rb.channelwise[4].weight, g["cw4"])
-            mappers.append(rb.adaLN_modulation.mapper.weight)
-            if ab.kv_mapper is not None:
-                put(ab.kv_mapper.weight, g["kvm"])
-            put(ab.attn_layer_norm.weight, g.get("ln1"))
-            attn(ab.attention, g["a1"], False)
-            put(ab.crossattn_layer_norm.weight, g.get("ln2"))
-            attn(ab.crossattention, g["a2"], False)
-
-    put(model.encoder_proj.weight, G["encoder_proj"])
-    put(model.encoder_proj_layer_norm.weight, G.get("enc_norm"))
-    put(model.cond_embed[0].weight, G["cond0"])
-    put(model.cond_embed[2].weight, G["cond2"])
-    put(model.embed.embeddings.weight, G["emb"])
-    put(model.embed.layer_norm.weight, G.get("emb_norm"))
-    put(model.embed.conv.weight, G["emb_conv"])
-    put(model.project_to_hidden_norm.weight, G.get("pth_norm"))
-    put(model.project_to_hidden.weight, G["pth"])
-    put(model.project_from_hidden_norm.weight, G.get("pfh_norm"))
-    put(model.project_from_hidden.weight, G["pfh"])
-    put(model.mlm_layer.conv1.weight, G["mlm1"])
-    put(model.mlm_layer.layer_norm.norm.weight, G.get("mlm_norm"))
-    put(model.mlm_layer.conv2.weight, G["mlm2"][: c.codebook_size])
-    block(model.down_blocks[0], G["down"])  # mapper order must match _weights(): down, layers, up
-    for i, l in enumerate(model.transformer_layers):
-        g = G["layers"][i]
-        put(l.attn_layer_norm.weight, g.get("ln1"))
-        mappers.append(l.self_attn_adaLN_modulation.mapper.weight)
-        attn(l.attention, g["sa"], True)
-        put(l.crossattn_layer_norm.weight, g.get("ln2"))
-        attn(l.crossattention, g["ca"], False)
-        mappers.append(l.cross_attn_adaLN_modulation.mapper.weight)
-        put(l.ffn.pre_mlp_layer_norm.weight, g.get("ln3"))
-        mappers.append(l.ffn.adaLN_modulation.mapper.weight)
-        rows(g["wi"], l.ffn.wi_0.weight, l.ffn.wi_1.weight)
-        put(l.ffn.wo.weight, g["wo"])
-    block(model.up_blocks[0], G["up"])
-    rows(G["mappers"], *mappers)
-    return [out.get(p) for p in model.parameters()]
-
-
-class UViTTrainFn(torch.autograd.Function):
-    """(logits_padded, loss) = f(params...): the whole MaskGiTUViT_v2 training forward; backward returns every gradient."""
-
-    @staticmethod
-    def forward(ctx, model, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels, label_smoothing,
-                loss_weight, *params):
-        W = model._weights()
-        logits, saved = forward(model, W, input_ids, encoder_hidden_states, cond_embeds, micro_conds)
-        V = model.config.codebook_size
-        ctx.model, ctx.W, ctx.saved, ctx.V, ctx.ls = model, W, saved, V, label_smoothing
-        ctx.set_materialize_grads(False)
-        if labels is None:
-            ctx.ce = None
-            return logits, None
-        labels = labels.reshape(-1).contiguous().to(torch.int64)
-        out, ws = ops.ce_fwd(logits, labels, V, label_smoothing)
-        row_scale, loss = None, out[0]
-        if loss_weight is not None:  # (sum_r w_r loss_r) / sum_r w_r on the unreduced loss (:305-317)
-            lw = loss_weight.reshape(-1).float()
-            row_scale = (lw / lw.sum()).contiguous()
-            loss = (ws[1] * row_scale).sum()
-        ctx.ce = (labels, ws, out, row_scale)
-        ctx.save_for_backward(logits)  # an OUTPUT of this Function: as a plain ctx attribute it would form a reference cycle
-        return logits, loss
-
-    @staticmethod
-    def backward(ctx, d_logits, d_loss):
-        dl = None
-        if d_loss is not None and ctx.ce is not None:
-            labels, ws, out, row_scale = ctx.ce
-            dl = ops.ce_bwd(ctx.saved_tensors[0], labels, ws, d_loss.to(F32).reshape(1).contiguous(), out, ctx.V, ctx.ls,
-                            row_scale=row_scale)
-        if d_logits is not None:
-            extra = d_logits.to(BF16).contiguous()
-            dl = extra if dl is None else dl + extra
-        if dl is None:
-            raise RuntimeError("MaskGiTUViT_v2: backward called without any gradient")
-        G = backward(ctx.model, ctx.W, ctx.saved, dl)
-        grads = param_grads(ctx.model, G)
-        ctx.saved = None
-        return (None,) * 8 + tuple(grads)
+def _resample_fwd(h, W, key, B, hw, eps, rms):
+    """force_down_up_sample (reference :509-513, :555-559) on the hw x hw grid it reads: Norm2D, then ``ds`` = the k2s2
+    conv as one GEMM over 2x2 patches ``[B*hw*hw/4, (dy, dx, ci)]``, or ``us`` = the ConvTranspose2d(2, 2) as one GEMM to
+    ``[B*hw*hw, (dy, dx, co)]`` followed by depth-to-space.  Returns the fp32 tokens and the GEMM operand (for its wgrad)."""
+    if key == "ds" and hw % 2:
+        raise ValueError(f"force_down_up_sample needs an even token grid, got {hw}x{hw}")
+    C = h.shape[1]
+    _, y = ops.add_norm_mod(h, W[key + "_norm"], eps, rms, want_residual=False)
+    if key == "ds":
+        a = y.view(B, hw // 2, 2, hw // 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(B * hw * hw // 4, 4 * C)
+        return ops.linear_fwd(a, W["ds"], out_dtype=F32), a
+    t = ops.linear_fwd(y, W["us"], out_dtype=F32)
+    return t.view(B, hw, hw, 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(B * hw * hw * 4, C), y
 
 
 # =================================================================================================================
-# Per-block autograd Functions: the same forward / backward helpers as above, cut at the block boundaries so that the
-# gradients of a block's parameters exist as soon as its backward has run and DDP's bucket all-reduces overlap the rest
-# of the backward pass (the whole-network Function above releases everything at the very end).  Tensors consumed by
-# every block enter each Function as fp32 inputs -- the normalised text states ``enc32`` and the SiLU'd conditioning
+# Per-block autograd Functions: the forward / backward helpers above, cut at the block boundaries so that the gradients
+# of a block's parameters exist as soon as its backward has run and DDP's bucket all-reduces overlap the rest of the
+# backward pass.  Tensors consumed by every block enter each Function as fp32 inputs -- the normalised text states ``enc32`` and the SiLU'd conditioning
 # vector ``sc32`` -- and autograd sums their per-block gradients; each block computes its own adaLN (scale | shift) rows
 # from ``sc`` with its slice of the stacked mapper matrix.
 class _Shared:
@@ -569,7 +369,7 @@ class ULayerFn(torch.autograd.Function):
         w = sh.W["layers"][idx]
         wl, w_map = _local_mods(sh, w, ["mod1", "mod2", "mod3"])
         mod = ops.linear_fwd(sh.sc, w_map, out_dtype=F32)
-        f, r3, s_l = _layer_fwd(x, r, sh.enc, wl, mod, sh.B, sh.S, sh.Skv, sh.H, sh.eps, sh.rms)
+        f, r3, s_l = _layer_fwd(x, r, sh.enc, wl, mod, sh.B, sh.S, sh.Skv, sh.eps, sh.rms)
         s_l = list(s_l)
         assert s_l[9] is r3
         s_l[9] = None  # r3 is an OUTPUT of this Function: held through save_for_backward, a ctx attribute would be a cycle
@@ -625,27 +425,17 @@ class ProjFn(torch.autograd.Function):
 
 
 class ResampleFn(torch.autograd.Function):
-    """force_down_up_sample (reference :509-513, :555-559): ``ds`` = Norm2D + Conv2d(k=2, s=2) in front of the down stage,
-    ``us`` = Norm2D + ConvTranspose2d(k=2, s=2) behind the up stage.  Both are ONE GEMM on the token-major layout: the
-    strided conv reads 2x2 patches ``[B*S/4, (dy, dx, ci)]``, the transposed conv writes ``[B*S, (dy, dx, co)]`` followed
-    by depth-to-space; the backward is the same GEMM's dgrad / wgrad with the inverse token permutation around it.
-    ``sh`` describes the grid this op READS (hw x hw tokens per sample)."""
+    """``_resample_fwd``: ``ds`` in front of the down stage, ``us`` behind the up stage; the backward is the same GEMM's
+    dgrad / wgrad with the inverse token permutation around it.  ``sh`` describes the grid this op READS (hw x hw tokens
+    per sample)."""
 
     @staticmethod
     def forward(ctx, sh, key, h, w_norm, w_conv):
-        W, B, hw = sh.W, sh.B, sh.hw
-        C = h.shape[1]
+        B, hw = sh.B, sh.hw
         if h.dtype != F32 or h.shape[0] != B * hw * hw:
             raise ValueError(f"ResampleFn: expected fp32 [{B * hw * hw}, C] tokens, got {h.dtype} {tuple(h.shape)}")
         h = h.contiguous()
-        _, y = ops.add_norm_mod(h, W[key + "_norm"], sh.eps, sh.rms, want_residual=False)
-        if key == "ds":
-            a = y.view(B, hw // 2, 2, hw // 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(B * hw * hw // 4, 4 * C)
-            out = ops.linear_fwd(a, W["ds"], out_dtype=F32)
-        else:
-            a = y
-            t = ops.linear_fwd(y, W["us"], out_dtype=F32)
-            out = t.view(B, hw, hw, 2, 2, C).permute(0, 1, 3, 2, 4, 5).reshape(B * hw * hw * 4, C)
+        out, a = _resample_fwd(h, sh.W, key, B, hw, sh.eps, sh.rms)
         ctx.sh, ctx.sv, ctx.key = sh, (h, a), key
         ctx.has_norm, ctx.conv_shape = w_norm is not None, w_conv.shape
         ctx.set_materialize_grads(False)
@@ -741,8 +531,6 @@ def train_forward(model, input_ids, encoder_hidden_states, cond_embeds, micro_co
     down, up = model.down_blocks[0], model.up_blocks[0]
     sh_full = sh
     if c.force_down_up_sample:  # the stages and the transformer layers run on the (hw/2)^2 grid (reference :509-513)
-        if sh.hw % 2:
-            raise ValueError(f"force_down_up_sample needs an even token grid, got {sh.hw}x{sh.hw}")
         h = ResampleFn.apply(sh_full, "ds", h, down.downsample[0].norm.weight, down.downsample[1].weight)
         sh = copy.copy(sh_full)  # same operand caches (W, enc, sc), coarse grid
         sh.S, sh.hw = S // 4, sh_full.hw // 2

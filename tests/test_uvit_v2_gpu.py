@@ -167,9 +167,6 @@ def test_micro_uvit_v2_force_down_up_sample_training_gradients_vs_oracle(golden)
     print("worst grad rel-L2:", ", ".join(f"{k}={v:.2e}" for k, v in worst))
     bad = {k: v for k, v in errs.items() if v > 8e-2 and not (".query." in k or ".key." in k)}
     assert not bad, bad
-    m._single_train_function = True  # the whole-network Function (test hook) does not cover the resampling ops
-    with pytest.raises(NotImplementedError):
-        m(*args, labels=g["labels"].to(DEV))
 
 
 def test_uvit_v2_default_widths_vs_oracle():
@@ -417,25 +414,3 @@ def test_micro_uvit_v2_loss_weight_training(golden):
     assert abs(float(loss) - float(g["loss_weighted"])) / float(g["loss_weighted"]) < 2e-3
     for n in ("mlm_layer.conv2.weight", "transformer_layers.1.ffn.wo.weight", "embed.embeddings.weight", "encoder_proj.weight"):
         assert _rel(dict(m.named_parameters())[n].grad, q[n].grad) < 5e-2, n
-
-
-def test_uvit_v2_block_functions_match_whole_network_function(golden, monkeypatch):
-    """The per-block autograd Functions (default: gradients appear during backward, DDP overlap) and the single
-    whole-network Function (private ``_single_train_function`` test hook) run the same kernels: loss identical, gradients equal up to the
-    summation order of the shared accumulators."""
-    g = golden("micro_uvit_v2.pt")
-    args = [g[k].to(DEV) for k in ("input_ids", "encoder_hidden_states", "cond_embeds", "micro_conds")]
-    grads, losses = {}, {}
-    for mode in ("blocks", "mono"):
-        m = MaskGiTUViT_v2(**g["config"])
-        m.load_state_dict(g["state_dict"])
-        m.to(DEV).train()
-        m._single_train_function = mode == "mono"
-        with torch.autocast("cuda", dtype=torch.bfloat16):
-            _, loss = m(*args, labels=g["labels"].to(DEV), label_smoothing=0.1)
-        loss.backward()
-        losses[mode] = float(loss)
-        grads[mode] = {n: p.grad.clone() for n, p in m.named_parameters()}
-    assert losses["blocks"] == losses["mono"]
-    worst = max(_rel(grads["blocks"][n], grads["mono"][n]) for n in grads["mono"])
-    assert worst < 2e-2, worst
