@@ -470,7 +470,7 @@ void balanced_tiles(int S, int* ntile, int* rows) {
 // 3-D map {cols, S rows, B} of a [B * S, rs] row-major operand, box {64 columns, 64 rows, 1}: rows past S inside a
 // batch are out of bounds and read as zeros.
 int qkv_tmap(CUtensorMap* map, const void* base, int cols, int S, int B, int rs) {
-  return make_tmap_bf16(map, "attention", base, {cols, S, B}, {2LL * rs, 2LL * rs * S}, {64, 64, 1});
+  return make_tmap(map, "attention", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, {cols, S, B}, {2LL * rs, 2LL * rs * S}, {64, 64, 1});
 }
 
 template <int HD>

@@ -398,15 +398,15 @@ int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* 
   const long long K = static_cast<long long>(taps) * Cin;
   const long long wrows = static_cast<long long>(Cout) * (p.up ? 4 : 1);
   int rc;
-  if ((rc = make_tmap_bf16(&ah, "conv2d_tc", x_hi, {Cin, W, H, B}, {px, px * W, px * W * H},
+  if ((rc = make_tmap(&ah, "conv2d_tc", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, x_hi, {Cin, W, H, B}, {px, px * W, px * W * H},
                            {64, p.tile_w, p.tile_h, 1})))
     return rc;
-  if ((rc = make_tmap_bf16(&al, "conv2d_tc", x_lo, {Cin, W, H, B}, {px, px * W, px * W * H},
+  if ((rc = make_tmap(&al, "conv2d_tc", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, x_lo, {Cin, W, H, B}, {px, px * W, px * W * H},
                            {64, p.tile_w, p.tile_h, 1})))
     return rc;
-  if ((rc = make_tmap_bf16(&bh, "conv2d_tc", w_hi, {K, wrows, p.wbatch ? B : 1}, {2 * K, 2 * K * wrows}, {64, BN, 1})))
+  if ((rc = make_tmap(&bh, "conv2d_tc", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, w_hi, {K, wrows, p.wbatch ? B : 1}, {2 * K, 2 * K * wrows}, {64, BN, 1})))
     return rc;
-  if ((rc = make_tmap_bf16(&bl, "conv2d_tc", w_lo, {K, wrows, p.wbatch ? B : 1}, {2 * K, 2 * K * wrows}, {64, BN, 1})))
+  if ((rc = make_tmap(&bl, "conv2d_tc", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, w_lo, {K, wrows, p.wbatch ? B : 1}, {2 * K, 2 * K * wrows}, {64, BN, 1})))
     return rc;
   if (BN == 256) return launch_conv<256>(ah, al, bh, bl, p, s);
   if (BN == 128) return launch_conv<128>(ah, al, bh, bl, p, s);

@@ -5,9 +5,11 @@
 // and, with transposed operand views, their dgrad / wgrad in backward.
 //
 // Structure: the persistent warp-specialised pipeline of tc_pipeline.cuh.  The producer thread loads 2-D TMA tiles of A
-// and B; the two consumer warpgroups run the epilogue straight from their accumulator registers (bf16 / fp32 / atomic /
-// +residual / split-K partial).  The producer runs up to a ring's worth of k-blocks ahead, so it keeps loading the next
-// tile while the consumers store this one.
+// and B; each consumer warpgroup converts its 64-row half of the accumulator in 128-byte column chunks into two
+// double-buffered shared-memory staging buffers and stores them with TMA (bf16 / fp32 / +residual / split-K partial; the
+// fp32 residual arrives by TMA into the same buffers ahead of use).  The stores are asynchronous, so they drain while the
+// warpgroup's next tile runs its MMAs; the producer runs up to a ring's worth of k-blocks ahead, so it keeps loading the
+// next tile meanwhile.  The atomic epilogue adds straight from the accumulator registers.
 //
 // Operand "major-ness": an operand is K-major when the reduction dim is contiguous in memory
 // (activations X[T,K], weights W[N,K] in forward) and MN-major when the M/N dim is contiguous
@@ -31,22 +33,27 @@ using tc::BM;
 // bit-identical from run to run (the atomic variant is order-dependent).
 enum Epi { EPI_BF16 = 0, EPI_F32 = 1, EPI_ATOMIC_F32 = 2, EPI_RESADD_F32 = 3, EPI_SPLITK_F32 = 4 };
 
+// Epilogue staging buffer: 64 rows x 128 B (a chunk of 64 bf16 or 32 fp32 columns of a warpgroup's half tile), laid out
+// with the 128-byte swizzle of the output tensor map.  Two per consumer warpgroup, then one mbarrier per buffer for the
+// residual loads of EPI_RESADD_F32.
+constexpr int kEpiBuf = 64 * 128;
+
 template <int BN>
-using Ring = tc::Ring<BN, (BN == 256) ? 4 : 6>;
+using Ring = tc::Ring<BN, (BN == 256) ? 4 : 6, 4 * kEpiBuf + 4 * 8>;
 
 struct GemmParams {
-  void* C;
-  const float* res;
+  void* C;  // EPI_ATOMIC_F32 only; the other epilogues store through the output tensor map
   int M, N, K;
   int ldc;
   int num_m, num_n, num_kb, kb_per_split, splits;
-  float* ws;      // EPI_SPLITK_F32: [splits][num_m * num_n][BM * BN] fp32 partial tiles
 };
 
+// tmC: the output, box {128 B of columns, 64 rows}: C [M, N] (pitch ldc), or for split-K partial tiles the workspace
+// [splits * num_m * num_n * BM, BN] fp32.  tmR: the fp32 residual [M, N] (pitch ldc) of EPI_RESADD_F32, same box.
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(tc::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const GemmParams p) {
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   Ring<BN> ring(smem_raw);
@@ -56,7 +63,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
-    ring.init();
+    if (EPI != EPI_ATOMIC_F32) ptx::prefetch_tmap(&tmC);
+    if (EPI == EPI_RESADD_F32) {
+      ptx::prefetch_tmap(&tmR);
+      uint64_t* rbar = reinterpret_cast<uint64_t*>(ring.extra() + 4 * kEpiBuf);
+      for (int i = 0; i < 4; ++i) ptx::mbar_init(&rbar[i], 1);
+    }
+    ring.init();  // ends with the barrier-init fence
   }
   __syncthreads();
   pdl_wait();  // everything above touches only shared memory / kernel parameters
@@ -98,8 +111,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     ptx::setmaxnreg_inc<tc::kConsumerRegs>();
     // -------------------------------------------------------------- consumers: rows [64 * half, 64 * half + 64) of a tile
     const int half = wg - 1;
-    const int lr = half * 64 + ptx::frag_row();  // tile-local row of d[4j], d[4j+1]; +8 for d[4j+2..3]
-    const int lc = ptx::frag_col();              // tile-local column of d[4j] within its 8-column group
+    const bool leader = (threadIdx.x & 127) == 0;  // issues the warpgroup's bulk copies
+    const int fr = ptx::frag_row();                 // half-local row of d[4j], d[4j+1]; +8 for d[4j+2..3]
+    const int lc = ptx::frag_col();                 // tile-local column of d[4j] within its 8-column group
+    uint8_t* ebuf = ring.extra() + half * 2 * kEpiBuf;  // this warpgroup's two staging buffers
+    uint64_t* rbar = reinterpret_cast<uint64_t*>(ring.extra() + 4 * kEpiBuf) + 2 * half;
+    // A chunk is 128 B of each of the 64 rows; chunk q goes through buffer q & 1.  Every epilogue has an even number of
+    // chunks per tile, so each tile starts on buffer 0 and the residual barriers on phase 0.
+    constexpr bool kF32 = EPI != EPI_BF16;
+    constexpr int kCols = kF32 ? 32 : 64;
+    constexpr int kChunks = BN / kCols;
+    constexpr int kJ = kCols / 8;  // 8-column fragment groups per chunk
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -109,51 +131,82 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int split = tile / tiles_mn;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+      // output coordinates of this warpgroup's half; the split-K partial of `tile` is workspace rows [BM tile, BM tile + BM)
+      const bool partial = EPI == EPI_SPLITK_F32 && p.splits > 1;
+      const int orow = (partial ? tile * BM : m_idx * BM) + half * 64;
+      const int ocol = partial ? 0 : n_idx * BN;
+      if (EPI == EPI_RESADD_F32 && leader) {
+        // the first two residual chunks load during the mainloop, once the previous tile's stores have read the buffers
+        ptx::bulk_wait_read<0>();
+        for (int b = 0; b < 2; ++b) {
+          ptx::mbar_expect_tx(&rbar[b], kEpiBuf);
+          ptx::tma_load_2d(ebuf + b * kEpiBuf, &tmR, &rbar[b], ocol + b * kCols, orow);
+        }
+      }
       ring.template consume<A_MN, B_MN>(acc, kb0, kb1, half);
-      // ------------------------------------------------------------ epilogue from the accumulator registers
-      const bool partial = (EPI == EPI_SPLITK_F32) && p.splits > 1;
-      float* ws_tile = nullptr;
-      if (EPI == EPI_SPLITK_F32 && partial)
-        ws_tile = p.ws + (static_cast<size_t>(split) * tiles_mn + tile % tiles_mn) * (BM * BN);
+      if constexpr (EPI == EPI_ATOMIC_F32) {
+        // ---------------------------------------------------------- fp32 atomics straight from the accumulator registers
+        const int lr = half * 64 + fr;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          const float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
-          const int r = lr + 8 * hr, c = 8 * j + lc;
-          if (EPI == EPI_SPLITK_F32 && partial) {
-            *reinterpret_cast<float2*>(ws_tile + static_cast<size_t>(r) * BN + c) = make_float2(v0, v1);
-            continue;
+          for (int hr = 0; hr < 2; ++hr) {
+            const float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+            const int grow = m_idx * BM + lr + 8 * hr, gcol = n_idx * BN + 8 * j + lc;
+            if (grow >= p.M || gcol >= p.N) continue;
+            float* dst = reinterpret_cast<float*>(p.C) + static_cast<size_t>(grow) * p.ldc + gcol;
+            if (gcol + 1 < p.N) atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
+            else atomicAdd(dst, v0);
           }
-          const int grow = m_idx * BM + r, gcol = n_idx * BN + c;
-          if (grow >= p.M || gcol >= p.N) continue;
-          const size_t off = static_cast<size_t>(grow) * p.ldc + gcol;
-          const bool pair = gcol + 1 < p.N;
-          if (EPI == EPI_BF16) {
-            bf16* dst = reinterpret_cast<bf16*>(p.C) + off;
-            if (pair) *reinterpret_cast<uint32_t*>(dst) = pack_bf16(v0, v1);
-            else dst[0] = __float2bfloat16_rn(v0);
+        }
+      } else {
+        // ---------------------------------------------------------- chunks through shared memory, TMA stores
+#pragma unroll
+        for (int q = 0; q < kChunks; ++q) {
+          uint8_t* buf = ebuf + (q & 1) * kEpiBuf;
+          if (EPI == EPI_RESADD_F32) {
+            ptx::mbar_wait(&rbar[q & 1], (q >> 1) & 1);  // residual chunk q has landed (so the store of q - 2 has read buf)
           } else {
-            float* dst = reinterpret_cast<float*>(p.C) + off;
-            if (EPI == EPI_F32 || EPI == EPI_SPLITK_F32) {
-              if (pair) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
-              else dst[0] = v0;
-            } else if (EPI == EPI_ATOMIC_F32) {
-              if (pair) atomicAdd(reinterpret_cast<float2*>(dst), make_float2(v0, v1));
-              else atomicAdd(dst, v0);
-            } else {  // EPI_RESADD_F32: out = residual + bf16(acc)  (Linear output is bf16 under autocast)
-              const float* rs = p.res + off;
-              if (pair) {
-                const float2 q2 = *reinterpret_cast<const float2*>(rs);
-                *reinterpret_cast<float2*>(dst) = make_float2(q2.x + bf16_round(v0), q2.y + bf16_round(v1));
+            if (leader) ptx::bulk_wait_read<1>();  // the store of chunk q - 2 has read buf
+            ptx::named_barrier_sync(1 + half, 128);
+          }
+#pragma unroll
+          for (int jj = 0; jj < kJ; ++jj) {
+            const int j = q * kJ + jj;
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+              const int r = fr + 8 * hr;
+              // 16-byte unit u of row r sits at unit u ^ (r & 7): the 128-byte swizzle, so the 8 rows of a warp's store
+              // fall into different banks
+              if (!kF32) {
+                *reinterpret_cast<uint32_t*>(buf + r * 128 + ((jj ^ (r & 7)) << 4) + 2 * lc) = pack_bf16(v0, v1);
               } else {
-                dst[0] = rs[0] + bf16_round(v0);
+                float2* dst = reinterpret_cast<float2*>(buf + r * 128 + (((2 * jj + (lc >> 2)) ^ (r & 7)) << 4) + 4 * (lc & 3));
+                if (EPI == EPI_RESADD_F32) {  // out = residual + bf16(acc)  (Linear output is bf16 under autocast)
+                  const float2 rs = *dst;
+                  *dst = make_float2(rs.x + bf16_round(v0), rs.y + bf16_round(v1));
+                } else {
+                  *dst = make_float2(v0, v1);
+                }
               }
+            }
+          }
+          ptx::fence_proxy_async();  // the chunk is visible to the TMA unit
+          ptx::named_barrier_sync(1 + half, 128);
+          if (leader) {
+            ptx::tma_store_2d(&tmC, buf, ocol + q * kCols, orow);
+            ptx::bulk_commit();
+            if (EPI == EPI_RESADD_F32 && q + 2 < kChunks) {
+              ptx::bulk_wait_read<0>();
+              ptx::mbar_expect_tx(&rbar[q & 1], kEpiBuf);
+              ptx::tma_load_2d(buf, &tmR, &rbar[q & 1], ocol + (q + 2) * kCols, orow);
             }
           }
         }
       }
     }
+    if (leader) ptx::bulk_wait<0>();  // shared memory must outlive the last stores
   }
 }
 
@@ -186,36 +239,40 @@ int num_sms() {
   return n > 16 ? n : 16;
 }
 
+// A, B, the output and the residual (EPI_RESADD_F32; a copy of the output map otherwise)
+struct GemmMaps {
+  CUtensorMap a, b, c, r;
+};
+
 template <int BN, bool A_MN, bool B_MN, int EPI>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+int launch(const GemmMaps& m, const GemmParams& p, cudaStream_t stream) {
   constexpr auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI>;
   if (int rc = set_max_dynamic_smem<kern>(Ring<BN>::kSmemBytes)) return rc;
   const int total = p.num_m * p.num_n * p.splits;
   const int grid = total < num_sms() ? total : num_sms();
-  pdl_launch(grid, tc::kThreads, Ring<BN>::kSmemBytes, stream)(kern, ta, tb, p);
+  pdl_launch(grid, tc::kThreads, Ring<BN>::kSmemBytes, stream)(kern, m.a, m.b, m.c, m.r, p);
   return check_launch("gemm_wgmma");
 }
 
 template <int BN, bool A_MN, bool B_MN>
-int launch_epi(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t s) {
+int launch_epi(int epi, const GemmMaps& m, const GemmParams& p, cudaStream_t s) {
   switch (epi) {
-    case EPI_BF16: return launch<BN, A_MN, B_MN, EPI_BF16>(ta, tb, p, s);
-    case EPI_F32: return launch<BN, A_MN, B_MN, EPI_F32>(ta, tb, p, s);
-    case EPI_ATOMIC_F32: return launch<BN, A_MN, B_MN, EPI_ATOMIC_F32>(ta, tb, p, s);
-    case EPI_RESADD_F32: return launch<BN, A_MN, B_MN, EPI_RESADD_F32>(ta, tb, p, s);
-    case EPI_SPLITK_F32: return launch<BN, A_MN, B_MN, EPI_SPLITK_F32>(ta, tb, p, s);
+    case EPI_BF16: return launch<BN, A_MN, B_MN, EPI_BF16>(m, p, s);
+    case EPI_F32: return launch<BN, A_MN, B_MN, EPI_F32>(m, p, s);
+    case EPI_ATOMIC_F32: return launch<BN, A_MN, B_MN, EPI_ATOMIC_F32>(m, p, s);
+    case EPI_RESADD_F32: return launch<BN, A_MN, B_MN, EPI_RESADD_F32>(m, p, s);
+    case EPI_SPLITK_F32: return launch<BN, A_MN, B_MN, EPI_SPLITK_F32>(m, p, s);
   }
   set_last_error("gemm: unknown epilogue %d", epi);
   return MUSE_ERR_INVALID;
 }
 
 template <int BN>
-int launch_major(int a_mn, int b_mn, int epi, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
-                 cudaStream_t s) {
-  if (!a_mn && !b_mn) return launch_epi<BN, false, false>(epi, ta, tb, p, s);
-  if (!a_mn && b_mn) return launch_epi<BN, false, true>(epi, ta, tb, p, s);
-  if (a_mn && b_mn) return launch_epi<BN, true, true>(epi, ta, tb, p, s);
-  return launch_epi<BN, true, false>(epi, ta, tb, p, s);
+int launch_major(int a_mn, int b_mn, int epi, const GemmMaps& m, const GemmParams& p, cudaStream_t s) {
+  if (!a_mn && !b_mn) return launch_epi<BN, false, false>(epi, m, p, s);
+  if (!a_mn && b_mn) return launch_epi<BN, false, true>(epi, m, p, s);
+  if (a_mn && b_mn) return launch_epi<BN, true, true>(epi, m, p, s);
+  return launch_epi<BN, true, false>(epi, m, p, s);
 }
 
 }  // namespace
@@ -261,27 +318,30 @@ int gemm_tc(const void* A, const void* B, void* C, const float* res, int M, int 
     set_last_error("gemm: C must be 16B aligned");
     return MUSE_ERR_INVALID;
   }
+  if (epi == EPI_RESADD_F32 && (res == nullptr || (reinterpret_cast<uintptr_t>(res) & 15) != 0)) {
+    set_last_error("gemm: the residual epilogue needs a 16B-aligned residual");
+    return MUSE_ERR_INVALID;
+  }
   const int BN = (N >= 256) ? 256 : 128;
+  constexpr CUtensorMapDataType kBf16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kF32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   // K-major operands: boxes of BK columns x the tile's rows; MN-major: 64-column chunks x BK rows
-  CUtensorMap ta, tb;
+  GemmMaps m;
   int rc;
-  rc = a_mn ? make_tmap_bf16(&ta, "gemm", A, {M, K}, {2LL * lda}, {64, BK})
-            : make_tmap_bf16(&ta, "gemm", A, {K, M}, {2LL * lda}, {BK, BM});
+  rc = a_mn ? make_tmap(&m.a, "gemm", kBf16, A, {M, K}, {2LL * lda}, {64, BK})
+            : make_tmap(&m.a, "gemm", kBf16, A, {K, M}, {2LL * lda}, {BK, BM});
   if (rc) return rc;
-  rc = b_mn ? make_tmap_bf16(&tb, "gemm", B, {N, K}, {2LL * ldb}, {64, BK})
-            : make_tmap_bf16(&tb, "gemm", B, {K, N}, {2LL * ldb}, {BK, BN});
+  rc = b_mn ? make_tmap(&m.b, "gemm", kBf16, B, {N, K}, {2LL * ldb}, {64, BK})
+            : make_tmap(&m.b, "gemm", kBf16, B, {K, N}, {2LL * ldb}, {BK, BN});
   if (rc) return rc;
 
   GemmParams p;
   p.C = C;
-  p.res = res;
   p.M = M; p.N = N; p.K = K; p.ldc = ldc;
   p.num_m = ceil_div(M, BM);
   p.num_n = ceil_div(N, BN);
   p.num_kb = ceil_div(K, BK);
   p.splits = 1;
   p.kb_per_split = p.num_kb;
-  p.ws = reinterpret_cast<float*>(ws);
   if (epi == EPI_ATOMIC_F32 || epi == EPI_SPLITK_F32) {
     int num_m, num_n, num_kb, bn;
     split_plan(M, N, K, &num_m, &num_n, &num_kb, &p.kb_per_split, &p.splits, &bn);
@@ -293,11 +353,22 @@ int gemm_tc(const void* A, const void* B, void* C, const float* res, int M, int 
       }
     }
   }
-  rc = (BN == 256) ? launch_major<256>(a_mn, b_mn, epi, ta, tb, p, stream) : launch_major<128>(a_mn, b_mn, epi, ta, tb, p, stream);
+  // The output map clips at M and N, so rows past M, pad columns (ldc > N) and the neighbours of a column slice of a
+  // wider tensor are never written.  Boxes are 128 B of columns x the 64 rows of a consumer warpgroup.
+  if (epi == EPI_SPLITK_F32 && p.splits > 1)
+    rc = make_tmap(&m.c, "gemm", kF32, ws, {BN, 1LL * p.splits * p.num_m * p.num_n * BM}, {4LL * BN}, {32, 64});
+  else if (epi == EPI_BF16)
+    rc = make_tmap(&m.c, "gemm", kBf16, C, {N, M}, {2LL * ldc}, {64, 64});
+  else
+    rc = make_tmap(&m.c, "gemm", kF32, C, {N, M}, {4LL * ldc}, {32, 64});
+  if (rc) return rc;
+  m.r = m.c;
+  if (epi == EPI_RESADD_F32 && (rc = make_tmap(&m.r, "gemm", kF32, res, {N, M}, {4LL * ldc}, {32, 64}))) return rc;
+  rc = (BN == 256) ? launch_major<256>(a_mn, b_mn, epi, m, p, stream) : launch_major<128>(a_mn, b_mn, epi, m, p, stream);
   if (rc || epi != EPI_SPLITK_F32 || p.splits <= 1) return rc;
   const long long n_out4 = static_cast<long long>(M) * ((N + 3) / 4);
   pdl_launch(static_cast<unsigned>(ceil_div_ll(n_out4, 256)), 256, 0, stream)(splitk_reduce_kernel,
-      p.ws, reinterpret_cast<float*>(C), M, N, ldc, p.num_n, p.num_m * p.num_n, BN, p.splits);
+      reinterpret_cast<const float*>(ws), reinterpret_cast<float*>(C), M, N, ldc, p.num_n, p.num_m * p.num_n, BN, p.splits);
   return check_launch("gemm splitk reduce");
 }
 

@@ -65,7 +65,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
-// 2D tiled load global -> shared, completion signalled on an mbarrier (complete_tx::bytes).
+// 2D tiled load global -> shared, completion signalled on an mbarrier (complete_tx::bytes).  The element type (bf16
+// operand tiles, fp32 residual tiles) is the tensor map's.
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
                                             int32_t c0, int32_t c1) {
   asm volatile(
@@ -90,8 +91,33 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// 2D tiled store shared -> global.  Elements of the box outside the tensor map's extents are not written.  The source
+// must be visible to the async proxy (fence_proxy_async after the generic-proxy writes) and stay untouched until
+// bulk_wait_read has covered the store's bulk group.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+// at most N of this thread's bulk groups still reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
+}
+// at most N of this thread's bulk groups not yet complete (their global writes performed)
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;\n" ::"n"(N) : "memory");
+}
 
 // ---------------------------------------------------------------- warpgroup helpers
+// Named barrier `id` (1..15; 0 is __syncthreads) over `threads` threads, a multiple of 32.
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
+}
+
 // Register budget of a warpgroup in a warp-specialised kernel: the TMA producer gives registers back, the MMA
 // warpgroups take them (the accumulator fragments live in registers).
 template <int R>

@@ -26,8 +26,9 @@ EncodeTiledFn get_encode_fn() {
 
 }  // namespace
 
-int make_tmap_bf16(CUtensorMap* map, const char* who, const void* base, std::initializer_list<long long> dims,
-                   std::initializer_list<long long> byte_strides, std::initializer_list<long long> box) {
+int make_tmap(CUtensorMap* map, const char* who, CUtensorMapDataType dtype, const void* base,
+              std::initializer_list<long long> dims, std::initializer_list<long long> byte_strides,
+              std::initializer_list<long long> box) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return MUSE_ERR_CUDA;
   const int rank = static_cast<int>(dims.size());
@@ -44,10 +45,10 @@ int make_tmap_bf16(CUtensorMap* map, const char* who, const void* base, std::ini
     aligned = aligned && st[i] % 16 == 0;
   }
   if (!aligned) {
-    set_last_error("%s: operand base must be 16B aligned and its row strides multiples of 8 elements", who);
+    set_last_error("%s: operand base must be 16B aligned and its row strides multiples of 16 bytes", who);
     return MUSE_ERR_INVALID;
   }
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), d, st, bx, estr,
+  CUresult r = fn(map, dtype, rank, const_cast<void*>(base), d, st, bx, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

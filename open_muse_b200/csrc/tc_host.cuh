@@ -8,11 +8,13 @@
 
 namespace muse {
 
-// bf16 TMA tensor map with the 128-byte swizzle, zero-filled out of bounds, rank = dims.size() <= 5.  dims[0] is the
-// contiguous dimension, byte_strides[i] the stride of dims[i + 1], box[i] the box extent along dims[i].  The base must be
-// 16-byte aligned and every stride a multiple of 16 bytes (MUSE_ERR_INVALID otherwise); `who` prefixes the error message.
-int make_tmap_bf16(CUtensorMap* map, const char* who, const void* base, std::initializer_list<long long> dims,
-                   std::initializer_list<long long> byte_strides, std::initializer_list<long long> box);
+// TMA tensor map of bf16 or fp32 elements (dtype) with the 128-byte swizzle, zero-filled out of bounds, rank =
+// dims.size() <= 5.  dims[0] is the contiguous dimension, byte_strides[i] the stride of dims[i + 1], box[i] the box extent
+// along dims[i] (box[0] at most 128 bytes).  The base must be 16-byte aligned and every stride a multiple of 16 bytes
+// (MUSE_ERR_INVALID otherwise); `who` prefixes the error message.
+int make_tmap(CUtensorMap* map, const char* who, CUtensorMapDataType dtype, const void* base,
+              std::initializer_list<long long> dims, std::initializer_list<long long> byte_strides,
+              std::initializer_list<long long> box);
 
 // multiprocessor count of the current device, queried once
 int sm_count();

@@ -73,23 +73,33 @@ struct Ring {
 
   // Consumer warpgroup `half`: acc = (rows [64 half, 64 half + 64) of A) x B^T over the next kb1 - kb0 stages, which hold
   // k-blocks [kb0, kb1); the first k-step overwrites acc.  A_MN / B_MN: the operand's M/N dimension is the contiguous one.
+  // One wgmma group stays in flight: k-block kb is issued before the group of kb - 1 is waited for and its stage released,
+  // so the tensor pipe does not drain between k-blocks.  acc is complete on return.
   template <bool A_MN, bool B_MN>
   __device__ __forceinline__ void consume(float (&acc)[BN / 2], int kb0, int kb1, int half) {
+    const bool leader = (threadIdx.x & 127) == 0;
+    int prev = -1;  // stage of the group still in flight
     for (int kb = kb0; kb < kb1; ++kb) {
       ptx::mbar_wait(&full[stage], phase);
       // 64 rows of A are 8 KB in both layouts: 64 K-major rows, or one 64-element MN chunk
       const uint32_t a = ptx::smem_u32(smem + stage * kStageBytes) + half * 8192;
       const uint32_t b = ptx::smem_u32(smem + stage * kStageBytes + kABytes);
+      ptx::fence_operand(acc);
       ptx::wgmma_fence();
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k)
         ptx::Wgmma<BN, A_MN, B_MN>::run(acc, A_MN ? ptx::desc_mnmajor(a, k) : ptx::desc_kmajor(a, k),
                                         B_MN ? ptx::desc_mnmajor(b, k) : ptx::desc_kmajor(b, k), (kb > kb0 || k > 0) ? 1 : 0);
       ptx::wgmma_commit();
-      ptx::wgmma_wait<0>();
-      if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty[stage]);  // the MMAs have read the stage
+      ptx::wgmma_wait<1>();
+      ptx::fence_operand(acc);
+      if (leader && prev >= 0) ptx::mbar_arrive(&empty[prev]);  // the MMAs of k-block kb - 1 have read its stage
+      prev = stage;
       advance();
     }
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(acc);
+    if (leader && prev >= 0) ptx::mbar_arrive(&empty[prev]);
   }
 };
 
