@@ -21,7 +21,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 3
+#define MUSE_B200_ABI_VERSION 4
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -151,6 +151,45 @@ int muse_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
                   float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int head_dim, int q_rs,
                   int k_rs, int v_rs, int o_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale,
                   void* stream);
+
+/* Dropout (nn.Dropout(p) in training mode).  Keep masks come from Philox4x32-10 keyed by the 64-bit seed at *seed (device
+ * memory, so a captured graph draws a fresh seed per replay) with a per-forward unique site id; the mapping from
+ * (seed, site, coordinates) to bits and the rate (p_eff = round(p * 65536) / 65536, kept values scaled by 1 / (1 - p_eff))
+ * are documented in csrc/philox.cuh.  Masks are stored as uint32 words, rows padded to 32 bits, bit k % 32 of word
+ * k / 32 set = element k kept.
+ * Attention on the probabilities (:236-237): as muse_attn_fwd, plus bits [B, nh, Sq, ceil(Skv / 32)] written; the lse is
+ * that of the undropped probabilities.  muse_attn_bwd_dropout reads the bits (no seed). */
+int muse_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
+                          const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int head_dim,
+                          int q_rs, int k_rs, int v_rs, int o_rs, float scale, void* stream);
+int muse_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
+                          const unsigned int* bits, float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh,
+                          int Sq, int Skv, int head_dim, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs,
+                          int dv_rs, float scale, void* stream);
+/* Elementwise (the embedding output, :956): y = x * keep / (1 - p_eff) over contiguous
+ * [rows, cols] (cols % 8 == 0, dtype 0 fp32 / 1 bf16, y may alias x), bits [rows, ceil(cols / 32)] written;
+ * backward dx = dy * keep / (1 - p_eff) (dx may alias dy). */
+int muse_dropout_fwd(const void* x, void* y, int dtype, unsigned int* bits, const unsigned long long* seed, int site,
+                     float p, long long rows, int cols, void* stream);
+int muse_dropout_bwd(const void* dy, void* dx, int dtype, const unsigned int* bits, float p, long long rows, int cols,
+                     void* stream);
+
+/* FeedForward.dropout (:797) fused into the passes that produce / consume the wo operand (same masks, layout and rate as
+ * muse_dropout_fwd, bits [rows, ceil(I / 32)]):
+ *   muse_norm_fwd_glu_dropout / muse_norm_bwd_glu_dropout: muse_norm_fwd / muse_norm_bwd with act 2, bf16 x / y / dy / dx;
+ *   the forward writes the dropped output and the bits, the backward scales dy by the bits as it reads it and recomputes the
+ *   GLU product from [a | b] (dw / dw_ws as in muse_norm_bwd);
+ *   muse_glu_fwd_dropout / muse_glu_bwd_dropout: muse_glu_fwd / muse_glu_bwd likewise (no mid norm). */
+int muse_norm_fwd_glu_dropout(const void* x, const float* w, void* y, float* mean, float* rstd, unsigned int* bits,
+                              const unsigned long long* seed, int site, float p, int rows, int H, float eps, int rms,
+                              void* stream);
+int muse_norm_bwd_glu_dropout(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,
+                              const unsigned int* bits, float p, void* dx, float* dw, float* dw_ws, int rows, int H, int rms,
+                              void* stream);
+int muse_glu_fwd_dropout(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
+                         long long rows, int I, void* stream);
+int muse_glu_bwd_dropout(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
+                         void* stream);
 
 /* F.cross_entropy(logits.view(-1,V), labels.view(-1), ignore_index=-100, label_smoothing) (:1276-1280).
  * logits bf16 [rows, ld] (ld >= V, multiple of 8). lse/row_loss: fp32 [rows] scratch (lse kept for bwd).

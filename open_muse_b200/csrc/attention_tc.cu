@@ -19,7 +19,15 @@
 // i * R, its CTA loads a 64-row box (rows past R belong to the next tile or are zero-filled past the sequence), the MMAs
 // run on all 64 rows, but only rows < R are kept.  The looped dimension's ragged tail is zero-filled by TMA and masked.
 // Several CTAs share an SM, so one CTA's softmax math runs under another's MMAs and loads.
+//
+// Dropout on the probabilities (DROP = true instantiations; the DROP = false ones are the kernels without it): the forward
+// draws the keep bits of its fragment with philox.cuh's attention mapping (four Philox calls per thread and 64 x 64 tile),
+// stores them, and scales the bf16 P operand of O += P V by Z = keep / (1 - p) -- l and the LSE stay those of the
+// undropped P.  The dQ kernel reads the bits of its rows and applies Z to dP (dP = Z (dO V^T); D = rowsum(P dP) as
+// before); the dK/dV kernel, which walks S^T, has its producer warp stage each q tile's 64 x 64 bits (funnel-shifted to
+// the CTA's first kv row) next to lse / D and applies Z to P^T (dV) and to dP^T (dS).
 #include "common.cuh"
+#include "philox.cuh"
 #include "ptx.cuh"
 #include "tc_host.cuh"
 #include "wgmma.cuh"
@@ -59,6 +67,13 @@ struct TcParams {
   bf16* out1;  long long out1_rs;   // dkdv: dV
   float* lse;                        // [B, nh, Sq]
   float* dvec;                       // [B, nh, Sq]
+  // dropout on the probabilities (DROP instantiations only): keep bits [B, nh, Sq, bwords] (philox.cuh), written by the
+  // forward from (seed, site), read by both backward kernels
+  uint32_t* bits;
+  const unsigned long long* seed;
+  uint32_t site, thresh;
+  int bwords;   // ceil(Skv / 32)
+  float dscale; // 1 / (1 - p_eff)
 };
 
 // Barriers behind the tiles: own (the CTA's owned tiles, loaded once), full[kStages], empty[kStages].  Step st of the loop
@@ -136,11 +151,23 @@ __device__ __forceinline__ void store_acc(const float (&d)[HD / 2], bf16* base, 
 // column (within the 64-column tile) of fragment element i
 __device__ __forceinline__ int frag_col_of(int i) { return 8 * (i >> 2) + ptx::frag_col() + (i & 1); }
 
+// ------------------------------------------------------------------------------------------------ dropout helpers
+// The keep bits a thread owns in one 32-column half G of a tile row are the 8 lanes of one Philox call (philox.cuh):
+// lane 2 (g % 4) + e is column 8 g + c + e (g = 4 G .. 4 G + 3, e = 0, 1).  As a stored word they sit at bit
+// 8 (g % 4) + c + e, so a word shifted right by c and a call's lanes are read the same way: lane l <-> bit 8 (l >> 1) + (l & 1).
+__device__ __forceinline__ uint32_t lanes_to_word(uint32_t kb, int c) {
+  return ((kb & 3u) | ((kb & 0xCu) << 6) | ((kb & 0x30u) << 12) | ((kb & 0xC0u) << 18)) << c;
+}
+// keep bit of accumulator element i, from the shifted words w[hr][G] of its rows
+__device__ __forceinline__ bool kept(const uint32_t (&w)[2][2], int i) {
+  return (w[(i >> 1) & 1][i >> 4] >> (8 * ((i >> 2) & 3) + (i & 1))) & 1u;
+}
+
 // ------------------------------------------------------------------------------------------------ forward
 // smem: Q 8K | kStages x {K 8K, V 8K} | barriers
 constexpr int FWD_SMEM = kTile + kStages * 2 * kTile + kBarBytes;
 
-template <int HD>
+template <int HD, bool DROP>
 __global__ void __launch_bounds__(kThreads, 3)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const TcParams p) {
@@ -176,6 +203,9 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
 
   const float sl2 = p.scale * kLog2e;
+  const uint32_t bh = static_cast<uint32_t>(b * p.nh + h);
+  unsigned long long seed = 0;
+  if constexpr (DROP) seed = *p.seed;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // per fragment row r, r + 8; l is this thread's partial sum
   float o[HD / 2];
 #pragma unroll
@@ -211,10 +241,33 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
     uint32_t pa[16];
     float ls[2] = {0.f, 0.f};
+    uint32_t kw[2][2];  // keep bits of rows r, r + 8 x column halves, as (unshifted) words
+    if constexpr (DROP) {
+      const int c = ptx::frag_col();
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const uint32_t q = q0 + ptx::frag_row() + 8 * hr;
+#pragma unroll
+        for (int G = 0; G < 2; ++G) {
+          kw[hr][G] = lanes_to_word(philox::attn_keep8(seed, p.site, bh, q, 8 * j + 4 * G + c / 2, p.thresh), 0);
+          // the quad's four threads hold the four column pairs of the word: OR them, thread 2 hr + G stores it
+          uint32_t w = kw[hr][G] << c;
+          w |= __shfl_xor_sync(0xffffffffu, w, 1);
+          w |= __shfl_xor_sync(0xffffffffu, w, 2);
+          const int word = 2 * j + G, nv = p.Skv - 32 * word;
+          if ((tid & 3) == 2 * hr + G && ptx::frag_row() + 8 * hr < rows_here && word < p.bwords)
+            p.bits[(static_cast<long long>(bh) * p.Sq + q) * p.bwords + word] = nv >= 32 ? w : w & ((1u << nv) - 1u);
+        }
+      }
+    }
 #pragma unroll
     for (int i = 0; i < 16; ++i) {  // s[2 i], s[2 i + 1] lie in row r + 8 (i & 1)
-      const float p0 = ex2(fmaf(s[2 * i], sl2, -m[i & 1])), p1 = ex2(fmaf(s[2 * i + 1], sl2, -m[i & 1]));
+      float p0 = ex2(fmaf(s[2 * i], sl2, -m[i & 1])), p1 = ex2(fmaf(s[2 * i + 1], sl2, -m[i & 1]));
       ls[i & 1] += p0 + p1;
+      if constexpr (DROP) {  // l keeps the undropped sum; only the P V operand is dropped and rescaled
+        p0 = kept(kw, 2 * i) ? p0 * p.dscale : 0.f;
+        p1 = kept(kw, 2 * i + 1) ? p1 * p.dscale : 0.f;
+      }
       pa[i] = pack_bf16(p0, p1);
     }
 #pragma unroll
@@ -246,7 +299,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // smem: Q 8K | dO 8K | kStages x {K_j 8K, V_j 8K} | barriers
 constexpr int DQ_SMEM = 2 * kTile + kStages * 2 * kTile + kBarBytes;
 
-template <int HD>
+template <int HD, bool DROP>
 __global__ void __launch_bounds__(kThreads, 3)
 attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -286,7 +339,7 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     return;
   }
 
-  const int r = ptx::frag_row();
+  const int r = ptx::frag_row(), c = ptx::frag_col();
   const long long stat_base = (static_cast<long long>(b) * p.nh + h) * p.Sq + q0;
   const float sl2 = p.scale * kLog2e;
   float lse2[2], dsum[2] = {0.f, 0.f};
@@ -301,6 +354,16 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const int nvalid = min(kBN, p.Skv - j * kBN);
     const uint32_t sK = ptx::smem_u32(sKV + (st % kStages) * 2 * kTile);
     float s[32], dp[32];
+    uint32_t kw[2][2];  // keep bits of rows r, r + 8 x column halves of tile j, shifted to this thread's column pairs
+    if constexpr (DROP) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+        for (int G = 0; G < 2; ++G) {
+          const int word = 2 * j + G;
+          kw[hr][G] = (r + 8 * hr < rows_here && word < p.bwords) ? p.bits[(stat_base + r + 8 * hr) * p.bwords + word] >> c : 0u;
+        }
+    }
     bars.wait_full(st);
     ptx::wgmma_fence();
     issue_scores<HD / 16>(s, ptx::smem_u32(sQ), sK);
@@ -309,6 +372,10 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     ptx::wgmma_wait<0>();
     ptx::fence_operand(s);
     ptx::fence_operand(dp);
+    if constexpr (DROP) {  // dP = Z (dO V^T)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dp[i] = kept(kw, i) ? dp[i] * p.dscale : 0.f;
+    }
 #pragma unroll
     for (int i = 0; i < 32; ++i) s[i] = ex2(fmaf(s[i], sl2, -lse2[(i >> 1) & 1]));  // P
     if (nvalid < kBN) {  // ragged last tile only
@@ -346,10 +413,12 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 // ------------------------------------------------------------------------------------------------ backward: dK, dV
 // Same structure as the dQ kernel, looping over 64-row q tiles; dK and dV of the CTA's kv rows in registers.  The producer
 // warp also stages each q tile's lse (x log2 e) and D (x scale) as 64-float vectors next to the ring, read per column.
-// smem: K 8K | V 8K | kStages x {Q_i 8K, dO_i 8K} | kStages x {lse 64, D 64} floats | barriers
+// With dropout the producer also stages the q tile's keep bits: 64 q rows x 2 words (the CTA's 64 kv rows).
+// smem: K 8K | V 8K | kStages x {Q_i 8K, dO_i 8K} | kStages x {lse 64, D 64} floats | [kStages x 128 bit words] | barriers
 constexpr int DKDV_SMEM = 2 * kTile + kStages * 2 * kTile + kStages * 2 * kBN * 4 + kBarBytes;
+constexpr int DKDV_DROP_SMEM = DKDV_SMEM + kStages * 2 * kBN * 4;
 
-template <int HD>
+template <int HD, bool DROP>
 __global__ void __launch_bounds__(kThreads, 2)
 attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -361,7 +430,8 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
   uint8_t* sV = smem + kTile;
   uint8_t* sQO = smem + 2 * kTile;
   float* sLD = reinterpret_cast<float*>(sQO + kStages * 2 * kTile);
-  const Bars bars(reinterpret_cast<uint8_t*>(sLD + kStages * 2 * kBN));
+  uint32_t* sBits = reinterpret_cast<uint32_t*>(sLD + kStages * 2 * kBN);  // DROP only: [stage][q 64][2 words]
+  const Bars bars(reinterpret_cast<uint8_t*>(sLD + kStages * 2 * kBN) + (DROP ? kStages * 2 * kBN * 4 : 0));
 
   const int tid = threadIdx.x;
   const int kv0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
@@ -386,6 +456,18 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
         const int qr = i * kBN + k;
         ld[k] = (qr < p.Sq) ? p.lse[stat_base + qr] * kLog2e : 0.f;
         ld[kBN + k] = (qr < p.Sq) ? p.dvec[stat_base + qr] * p.scale : 0.f;  // pre-scaled: dS = P (dP*scale - D*scale)
+        if constexpr (DROP) {  // bits kv0 .. kv0 + 63 of row qr: three stored words, funnel-shifted to kv0
+          uint32_t w[3] = {0u, 0u, 0u};
+          const int w0 = kv0 >> 5;
+          if (qr < p.Sq) {
+            const uint32_t* row = p.bits + (stat_base + qr) * p.bwords;
+#pragma unroll
+            for (int t = 0; t < 3; ++t) w[t] = (w0 + t < p.bwords) ? row[w0 + t] : 0u;
+          }
+          uint32_t* bt = sBits + (i % kStages) * 2 * kBN + 2 * k;
+          bt[0] = __funnelshift_r(w[0], w[1], kv0 & 31);
+          bt[1] = __funnelshift_r(w[1], w[2], kv0 & 31);
+        }
       }
       __syncwarp();  // the vectors are written before lane 0's arrival publishes the stage
       if (lane == 0) {
@@ -432,8 +514,17 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
         p0 = (row_ok && col < nvalid) ? p0 : 0.f;
         p1 = (row_ok && col + 1 < nvalid) ? p1 : 0.f;
       }
-      pa[k] = pack_bf16(p0, p1);
-      da[k] = pack_bf16(p0 * fmaf(dp[2 * k], p.scale, -dd.x), p1 * fmaf(dp[2 * k + 1], p.scale, -dd.y));
+      if constexpr (DROP) {  // dV += (P Z)^T dO_i ; dS = P (Z dP - D)
+        const uint32_t* bt = sBits + (i % kStages) * 2 * kBN + (r >> 5);
+        const int sh = (r & 31) + 8 * (k & 1);
+        const bool z0 = (bt[2 * col] >> sh) & 1u, z1 = (bt[2 * col + 2] >> sh) & 1u;
+        const float dp0 = z0 ? dp[2 * k] * p.dscale : 0.f, dp1 = z1 ? dp[2 * k + 1] * p.dscale : 0.f;
+        pa[k] = pack_bf16(z0 ? p0 * p.dscale : 0.f, z1 ? p1 * p.dscale : 0.f);
+        da[k] = pack_bf16(p0 * fmaf(dp0, p.scale, -dd.x), p1 * fmaf(dp1, p.scale, -dd.y));
+      } else {
+        pa[k] = pack_bf16(p0, p1);
+        da[k] = pack_bf16(p0 * fmaf(dp[2 * k], p.scale, -dd.x), p1 * fmaf(dp[2 * k + 1], p.scale, -dd.y));
+      }
     }
     ptx::wgmma_fence();
     issue_acc<HD>(dv, pa, sQ + kTile);  // dV += P^T dO_i
@@ -473,9 +564,24 @@ int qkv_tmap(CUtensorMap* map, const void* base, int cols, int S, int B, int rs)
   return make_tmap(map, "attention", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, {cols, S, B}, {2LL * rs, 2LL * rs * S}, {64, 64, 1});
 }
 
-template <int HD>
+// Dropout arguments of one attention call: bits == nullptr means no dropout (the DROP = false kernels)
+struct Drop {
+  uint32_t* bits;                  // [B, nh, Sq, ceil(Skv / 32)] keep bits (written by the forward, read by the backward)
+  const unsigned long long* seed;  // forward only: device pointer to the 64-bit Philox key
+  int site;
+  float p;
+};
+
+void set_drop(TcParams& p, const Drop& d, int Skv) {
+  p.bits = d.bits; p.seed = d.seed; p.site = static_cast<uint32_t>(d.site);
+  p.thresh = philox::threshold(d.p);
+  p.dscale = philox::keep_scale(p.thresh);
+  p.bwords = ceil_div(Skv, 32);
+}
+
+template <int HD, bool DROP>
 int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int q_rs,
-                  int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
+                  int k_rs, int v_rs, int o_rs, float scale, const Drop& drop, cudaStream_t s) {
   int ntile, tile_rows;
   balanced_tiles(Sq, &ntile, &tile_rows);
   CUtensorMap tq, tk, tv;
@@ -483,19 +589,20 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs))) return rc;
   if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs))) return rc;
   if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs))) return rc;
-  if ((rc = set_smem<attn_fwd_tc_kernel<HD>>(FWD_SMEM))) return rc;
+  if ((rc = set_smem<attn_fwd_tc_kernel<HD, DROP>>(FWD_SMEM))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale; p.tile_rows = tile_rows;
   p.out0 = reinterpret_cast<bf16*>(o); p.out0_rs = o_rs; p.lse = lse;
-  pdl_launch(dim3(ntile, nh, B), kThreads, FWD_SMEM, s)(attn_fwd_tc_kernel<HD>, tq, tk, tv, p);
+  if (DROP) set_drop(p, drop, Skv);
+  pdl_launch(dim3(ntile, nh, B), kThreads, FWD_SMEM, s)(attn_fwd_tc_kernel<HD, DROP>, tq, tk, tv, p);
   return check_launch("attn_fwd_tc");
 }
 
 // dQ (and D, into dvec) over q row tiles, then dK / dV over kv row tiles
-template <int HD>
+template <int HD, bool DROP>
 int attn_bwd_impl(const void* q, const void* k, const void* v, const void* d_o, const float* lse, float* dvec, void* dq,
                   void* dk, void* dv, int B, int nh, int Sq, int Skv, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs,
-                  int dk_rs, int dv_rs, float scale, cudaStream_t s) {
+                  int dk_rs, int dv_rs, float scale, const Drop& drop, cudaStream_t s) {
   int ntile, tile_rows;
   balanced_tiles(Sq, &ntile, &tile_rows);
   CUtensorMap tq, tdo, tk, tv;
@@ -504,19 +611,21 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* d_o, 
   if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs))) return rc;
   if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs))) return rc;
   if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs))) return rc;
-  if ((rc = set_smem<attn_bwd_dq_tc_kernel<HD>>(DQ_SMEM))) return rc;
+  if ((rc = set_smem<attn_bwd_dq_tc_kernel<HD, DROP>>(DQ_SMEM))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale;
   p.out0 = reinterpret_cast<bf16*>(dq); p.out0_rs = dq_rs; p.lse = const_cast<float*>(lse); p.dvec = dvec;
   p.tile_rows = tile_rows;
-  pdl_launch(dim3(ntile, nh, B), kThreads, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD>, tq, tdo, tk, tv, p);
+  if (DROP) set_drop(p, drop, Skv);
+  pdl_launch(dim3(ntile, nh, B), kThreads, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD, DROP>, tq, tdo, tk, tv, p);
   if ((rc = check_launch("attn_bwd_dq_tc"))) return rc;
 
   balanced_tiles(Skv, &ntile, &tile_rows);
-  if ((rc = set_smem<attn_bwd_dkdv_tc_kernel<HD>>(DKDV_SMEM))) return rc;
+  constexpr int smem = DROP ? DKDV_DROP_SMEM : DKDV_SMEM;
+  if ((rc = set_smem<attn_bwd_dkdv_tc_kernel<HD, DROP>>(smem))) return rc;
   p.out0 = reinterpret_cast<bf16*>(dk); p.out0_rs = dk_rs; p.out1 = reinterpret_cast<bf16*>(dv); p.out1_rs = dv_rs;
   p.tile_rows = tile_rows;
-  pdl_launch(dim3(ntile, nh, B), kThreads, DKDV_SMEM, s)(attn_bwd_dkdv_tc_kernel<HD>, tk, tv, tq, tdo, p);
+  pdl_launch(dim3(ntile, nh, B), kThreads, smem, s)(attn_bwd_dkdv_tc_kernel<HD, DROP>, tk, tv, tq, tdo, p);
   return check_launch("attn_bwd_dkdv_tc");
 }
 
@@ -526,30 +635,62 @@ int check_args(const char* who, int hd, int a, int b, int c) {
   return MUSE_OK;
 }
 
-}  // namespace
-
-// Entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its autograd
-// backward, head_dim 64 or 48, no mask, no dropout.
-int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
-             int q_rs, int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
+int fwd_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
+                 int q_rs, int k_rs, int v_rs, int o_rs, float scale, const Drop& d, cudaStream_t s) {
   if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
   int rc = check_args("attn_fwd", hd, q_rs | o_rs, k_rs, v_rs);
   if (rc) return rc;
-  return hd == 64 ? attn_fwd_impl<64>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, s)
-                  : attn_fwd_impl<48>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, s);
+  if (d.bits == nullptr)
+    return hd == 64 ? attn_fwd_impl<64, false>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
+                    : attn_fwd_impl<48, false>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s);
+  return hd == 64 ? attn_fwd_impl<64, true>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
+                  : attn_fwd_impl<48, true>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s);
+}
+
+int bwd_dispatch(const void* q, const void* k, const void* v, const void* d_o, const float* lse, float* dvec, void* dq,
+                 void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs, int v_rs, int o_rs,
+                 int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, const Drop& d, cudaStream_t s) {
+  if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
+  int rc = check_args("attn_bwd", hd, q_rs | o_rs | do_rs | dq_rs, k_rs | dk_rs, v_rs | dv_rs);
+  if (rc) return rc;
+#define MUSE_ATTN_BWD(HD, DROP) \
+  attn_bwd_impl<HD, DROP>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs, dk_rs, dv_rs, scale, d, s)
+  if (d.bits == nullptr) return hd == 64 ? MUSE_ATTN_BWD(64, false) : MUSE_ATTN_BWD(48, false);
+  return hd == 64 ? MUSE_ATTN_BWD(64, true) : MUSE_ATTN_BWD(48, true);
+#undef MUSE_ATTN_BWD
+}
+
+}  // namespace
+
+// Entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its autograd
+// backward, head_dim 64 or 48, no mask; the _dropout variants apply nn.Dropout(p) to the probabilities (:236-237) with
+// the keep bits of philox.cuh.
+int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
+             int q_rs, int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
+  return fwd_dispatch(q, k, v, o, lse, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, o_rs, scale, Drop{}, s);
+}
+
+int attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, uint32_t* bits,
+                     const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int hd, int q_rs,
+                     int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
+  if (bits == nullptr || seed == nullptr) { set_last_error("attn_fwd_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
+  return fwd_dispatch(q, k, v, o, lse, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, o_rs, scale, Drop{bits, seed, site, p}, s);
 }
 
 int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
              float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs,
              int v_rs, int o_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s) {
-  if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
-  int rc = check_args("attn_bwd", hd, q_rs | o_rs | do_rs | dq_rs, k_rs | dk_rs, v_rs | dv_rs);
-  if (rc) return rc;
   (void)o;  // D is recomputed from (P, dP) inside the dQ kernel; O is not needed by backward
-  return hd == 64 ? attn_bwd_impl<64>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs,
-                                      dk_rs, dv_rs, scale, s)
-                  : attn_bwd_impl<48>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs,
-                                      dk_rs, dv_rs, scale, s);
+  return bwd_dispatch(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs,
+                      dv_rs, scale, Drop{}, s);
+}
+
+int attn_bwd_dropout(const void* q, const void* k, const void* v, const void* d_o, const float* lse, const uint32_t* bits,
+                     float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs,
+                     int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s) {
+  if (bits == nullptr) { set_last_error("attn_bwd_dropout: bits are required"); return MUSE_ERR_INVALID; }
+  return bwd_dispatch(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, q_rs, do_rs, dq_rs, dk_rs,
+                      dv_rs, scale, Drop{const_cast<uint32_t*>(bits), nullptr, 0, p}, s);
 }
 
 }  // namespace muse

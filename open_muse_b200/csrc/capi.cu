@@ -57,6 +57,14 @@ int glu_fwd(const void*, void*, long long, int, cudaStream_t);
 int glu_bwd(const void*, const void*, void*, long long, int, cudaStream_t);
 int attn_fwd(const void*, const void*, const void*, void*, float*, int, int, int, int, int, int, int, int, int, float, cudaStream_t);
 int attn_bwd(const void*, const void*, const void*, const void*, const void*, const float*, float*, void*, void*, void*, int, int, int, int, int, int, int, int, int, int, int, int, int, float, cudaStream_t);
+int attn_fwd_dropout(const void*, const void*, const void*, void*, float*, uint32_t*, const unsigned long long*, int, float, int, int, int, int, int, int, int, int, int, float, cudaStream_t);
+int attn_bwd_dropout(const void*, const void*, const void*, const void*, const float*, const uint32_t*, float, float*, void*, void*, void*, int, int, int, int, int, int, int, int, int, int, int, int, float, cudaStream_t);
+int dropout_fwd(const void*, void*, int, uint32_t*, const unsigned long long*, int, float, long long, int, cudaStream_t);
+int dropout_bwd(const void*, void*, int, const uint32_t*, float, long long, int, cudaStream_t);
+int norm_fwd_glu_dropout(const void*, const float*, void*, float*, float*, void*, const unsigned long long*, int, float, int, int, float, int, cudaStream_t);
+int norm_bwd_glu_dropout(const void*, const void*, const float*, const float*, const float*, const void*, float, void*, float*, float*, int, int, int, cudaStream_t);
+int glu_fwd_dropout(const void*, void*, void*, const unsigned long long*, int, float, long long, int, cudaStream_t);
+int glu_bwd_dropout(const void*, const void*, const void*, float, void*, long long, int, cudaStream_t);
 int ce_fwd(const void*, const long long*, float*, float*, float*, int, int, int, float, cudaStream_t);
 int ce_bwd(const void*, const long long*, const float*, const float*, const float*, const float*, void*, int, int, int, float, cudaStream_t);
 int vq_argmin(const float*, const float*, float*, long long*, float*, int, int, int, cudaStream_t);
@@ -199,6 +207,47 @@ int muse_attn_bwd(const void* q, const void* k, const void* v, const void* o, co
                   void* stream) {
   return attn_bwd(q, k, v, o, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, head_dim, q_rs, k_rs, v_rs, o_rs, do_rs,
                   dq_rs, dk_rs, dv_rs, scale, ST(stream));
+}
+
+int muse_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
+                          const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int head_dim,
+                          int q_rs, int k_rs, int v_rs, int o_rs, float scale, void* stream) {
+  return attn_fwd_dropout(q, k, v, o, lse, bits, seed, site, p, B, nh, Sq, Skv, head_dim, q_rs, k_rs, v_rs, o_rs, scale,
+                          ST(stream));
+}
+int muse_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
+                          const unsigned int* bits, float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh,
+                          int Sq, int Skv, int head_dim, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs,
+                          int dv_rs, float scale, void* stream) {
+  return attn_bwd_dropout(q, k, v, d_o, lse, bits, p, dvec, dq, dk, dv, B, nh, Sq, Skv, head_dim, q_rs, k_rs, v_rs, do_rs,
+                          dq_rs, dk_rs, dv_rs, scale, ST(stream));
+}
+int muse_dropout_fwd(const void* x, void* y, int dtype, unsigned int* bits, const unsigned long long* seed, int site,
+                     float p, long long rows, int cols, void* stream) {
+  return dropout_fwd(x, y, dtype, bits, seed, site, p, rows, cols, ST(stream));
+}
+int muse_dropout_bwd(const void* dy, void* dx, int dtype, const unsigned int* bits, float p, long long rows, int cols,
+                     void* stream) {
+  return dropout_bwd(dy, dx, dtype, bits, p, rows, cols, ST(stream));
+}
+
+int muse_norm_fwd_glu_dropout(const void* x, const float* w, void* y, float* mean, float* rstd, unsigned int* bits,
+                              const unsigned long long* seed, int site, float p, int rows, int H, float eps, int rms,
+                              void* stream) {
+  return norm_fwd_glu_dropout(x, w, y, mean, rstd, bits, seed, site, p, rows, H, eps, rms, ST(stream));
+}
+int muse_norm_bwd_glu_dropout(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,
+                              const unsigned int* bits, float p, void* dx, float* dw, float* dw_ws, int rows, int H, int rms,
+                              void* stream) {
+  return norm_bwd_glu_dropout(dy, x, w, mean, rstd, bits, p, dx, dw, dw_ws, rows, H, rms, ST(stream));
+}
+int muse_glu_fwd_dropout(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
+                         long long rows, int I, void* stream) {
+  return glu_fwd_dropout(ab, out, bits, seed, site, p, rows, I, ST(stream));
+}
+int muse_glu_bwd_dropout(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
+                         void* stream) {
+  return glu_bwd_dropout(ab, dout, bits, p, dab, rows, I, ST(stream));
 }
 
 int muse_ce_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* loss_out, int rows,

@@ -3,7 +3,9 @@
 //   * token + position embedding gather (muse/modeling_transformer.py:942-957) and its backward
 //   * GLU: gelu(a) * b (muse/modeling_transformer.py:789-792) forward / backward
 //   * plain fp32 -> bf16 cast (gradient of the residual stream entering a dgrad GEMM)
+//   * nn.Dropout of the embedding output and of the FFN hidden state (keep bits of philox.cuh) and its backward
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace muse {
 namespace {
@@ -254,8 +256,12 @@ __global__ void __launch_bounds__(512) embed_seg_final_kernel(const int* __restr
 // ---------------------------------------------------------------- GLU
 // ab: [rows, 2*I] bf16 (a = cols [0,I), b = cols [I,2I)); out [rows, I] bf16.
 // Rounding points follow the reference under bf16 autocast: gelu(a) is rounded to bf16 before the product.
+// DROP: FeedForward.dropout (:797) fused -- the forward draws the chunk's keep byte (philox.cuh elementwise mapping), writes
+// the dropped product and the byte (the last chunk of a row also zeroes the pad bytes of the row's last word); the
+// backward scales dout by the stored byte as it reads it.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
-glu_fwd_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, long long rows, int I) {
+glu_fwd_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, long long rows, int I, const philox::ElemDrop dr) {
   pdl_enter();
   const int chunks = I / 8;
   const long long idx = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
@@ -267,11 +273,22 @@ glu_fwd_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, long long ro
   load8(ab + r * 2 * I + I + c, b);
 #pragma unroll
   for (int j = 0; j < 8; ++j) o[j] = bf16_round(gelu_f(a[j])) * b[j];
+  if constexpr (DROP) {
+    const uint32_t kb = philox::elem_keep8(*dr.seed, dr.site, static_cast<uint32_t>(r), c / 8, dr.thresh);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] *= philox::keep_z(kb, j, dr.scale);
+    uint8_t* br = dr.bits + r * dr.row_bytes;
+    br[c / 8] = static_cast<uint8_t>(kb);
+    if (c / 8 == chunks - 1)
+      for (int k = chunks; k < dr.row_bytes; ++k) br[k] = 0;
+  }
   store8(out + r * I + c, o);
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
-glu_bwd_kernel(const bf16* __restrict__ ab, const bf16* __restrict__ dout, bf16* __restrict__ dab, long long rows, int I) {
+glu_bwd_kernel(const bf16* __restrict__ ab, const bf16* __restrict__ dout, bf16* __restrict__ dab, long long rows, int I,
+               const philox::ElemDrop dr) {
   pdl_enter();
   const int chunks = I / 8;
   const long long idx = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
@@ -282,6 +299,11 @@ glu_bwd_kernel(const bf16* __restrict__ ab, const bf16* __restrict__ dout, bf16*
   load8(ab + r * 2 * I + c, a);
   load8(ab + r * 2 * I + I + c, b);
   load8(dout + r * I + c, d);
+  if constexpr (DROP) {
+    const uint32_t kb = dr.bits[r * dr.row_bytes + c / 8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) d[j] *= philox::keep_z(kb, j, dr.scale);
+  }
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     float gv, gg;
@@ -293,7 +315,89 @@ glu_bwd_kernel(const bf16* __restrict__ ab, const bf16* __restrict__ dout, bf16*
   store8(dab + r * 2 * I + I + c, db);
 }
 
+// ---------------------------------------------------------------- dropout (elementwise sites)
+// One thread per 8 columns of a row = one Philox call = one byte of the row's keep-bit words (little-endian: byte k of
+// the row is bits 8 (k % 4) .. of word k / 4, i.e. columns 8 k .. 8 k + 7).  Threads past the last column zero the pad
+// bytes of the row's last word.  y may alias x.
+template <typename T>
+__global__ void __launch_bounds__(256)
+dropout_fwd_kernel(const T* x, T* y, uint8_t* __restrict__ bits, const unsigned long long* __restrict__ seed,
+                   uint32_t site, uint32_t t, float scale, long long rows, int cols, int row_bytes) {
+  pdl_enter();
+  const long long idx = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (idx >= rows * row_bytes) return;
+  const long long r = idx / row_bytes;
+  const int k = static_cast<int>(idx % row_bytes);
+  if (8 * k >= cols) {
+    bits[idx] = 0;
+    return;
+  }
+  const uint32_t kb = philox::elem_keep8(*seed, site, static_cast<uint32_t>(r), static_cast<uint32_t>(k), t);
+  float v[8];
+  load8(x + r * cols + 8 * k, v);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] = ((kb >> j) & 1u) ? v[j] * scale : 0.f;
+  store8(y + r * cols + 8 * k, v);
+  bits[idx] = static_cast<uint8_t>(kb);
+}
+
+// dx = dy * keep * scale; dx may alias dy
+template <typename T>
+__global__ void __launch_bounds__(256)
+dropout_bwd_kernel(const T* dy, T* dx, const uint8_t* __restrict__ bits, float scale, long long rows, int cols,
+                   int row_bytes) {
+  pdl_enter();
+  const int chunks = cols / 8;
+  const long long idx = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (idx >= rows * chunks) return;
+  const long long r = idx / chunks;
+  const int k = static_cast<int>(idx % chunks);
+  const uint32_t kb = bits[r * row_bytes + k];
+  float v[8];
+  load8(dy + r * cols + 8 * k, v);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] = ((kb >> j) & 1u) ? v[j] * scale : 0.f;
+  store8(dx + r * cols + 8 * k, v);
+}
+
 }  // namespace
+
+int dropout_fwd(const void* x, void* y, int dtype, uint32_t* bits, const unsigned long long* seed, int site, float p,
+                long long rows, int cols, cudaStream_t s) {
+  if (cols % 8 != 0) { set_last_error("dropout_fwd: cols=%d must be a multiple of 8", cols); return MUSE_ERR_INVALID; }
+  if (bits == nullptr || seed == nullptr) { set_last_error("dropout_fwd: bits and seed are required"); return MUSE_ERR_INVALID; }
+  const int row_bytes = 4 * ceil_div(cols, 32);
+  const long long n = rows * row_bytes;
+  if (n <= 0) return MUSE_OK;
+  const uint32_t t = philox::threshold(p);
+  const float scale = philox::keep_scale(t);
+  uint8_t* b = reinterpret_cast<uint8_t*>(bits);
+  const unsigned grid = static_cast<unsigned>(ceil_div_ll(n, 256));
+  if (dtype == 0)
+    pdl_launch(grid, 256, 0, s)(dropout_fwd_kernel<float>, reinterpret_cast<const float*>(x), reinterpret_cast<float*>(y), b,
+                                seed, static_cast<uint32_t>(site), t, scale, rows, cols, row_bytes);
+  else
+    pdl_launch(grid, 256, 0, s)(dropout_fwd_kernel<bf16>, reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), b,
+                                seed, static_cast<uint32_t>(site), t, scale, rows, cols, row_bytes);
+  return check_launch("dropout_fwd");
+}
+
+int dropout_bwd(const void* dy, void* dx, int dtype, const uint32_t* bits, float p, long long rows, int cols, cudaStream_t s) {
+  if (cols % 8 != 0) { set_last_error("dropout_bwd: cols=%d must be a multiple of 8", cols); return MUSE_ERR_INVALID; }
+  const long long n = rows * (cols / 8);
+  if (n <= 0) return MUSE_OK;
+  const int row_bytes = 4 * ceil_div(cols, 32);
+  const float scale = philox::keep_scale(philox::threshold(p));
+  const uint8_t* b = reinterpret_cast<const uint8_t*>(bits);
+  const unsigned grid = static_cast<unsigned>(ceil_div_ll(n, 256));
+  if (dtype == 0)
+    pdl_launch(grid, 256, 0, s)(dropout_bwd_kernel<float>, reinterpret_cast<const float*>(dy), reinterpret_cast<float*>(dx), b,
+                                scale, rows, cols, row_bytes);
+  else
+    pdl_launch(grid, 256, 0, s)(dropout_bwd_kernel<bf16>, reinterpret_cast<const bf16*>(dy), reinterpret_cast<bf16*>(dx), b,
+                                scale, rows, cols, row_bytes);
+  return check_launch("dropout_bwd");
+}
 
 int pack_bf16(const void* table_dev, int n_entries, long long total_blocks, cudaStream_t s) {
   if (n_entries <= 0 || total_blocks <= 0) return MUSE_OK;
@@ -368,15 +472,38 @@ int glu_fwd(const void* ab, void* out, long long rows, int I, cudaStream_t s) {
   if (I % 8 != 0) { set_last_error("glu_fwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
   const long long n = rows * (I / 8);
   if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_fwd_kernel, reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I);
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_fwd_kernel<false>, reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, philox::ElemDrop{});
   return check_launch("glu_fwd");
+}
+
+int glu_fwd_dropout(const void* ab, void* out, void* bits, const unsigned long long* seed, int site, float p, long long rows,
+                    int I, cudaStream_t s) {
+  if (I % 8 != 0) { set_last_error("glu_fwd_dropout: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
+  if (bits == nullptr || seed == nullptr) { set_last_error("glu_fwd_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
+  const long long n = rows * (I / 8);
+  if (n <= 0) return MUSE_OK;
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_fwd_kernel<true>, reinterpret_cast<const bf16*>(ab),
+      reinterpret_cast<bf16*>(out), rows, I, philox::elem_drop(bits, seed, site, p, I));
+  return check_launch("glu_fwd_dropout");
+}
+
+int glu_bwd_dropout(const void* ab, const void* dout, const void* bits, float p, void* dab, long long rows, int I,
+                    cudaStream_t s) {
+  if (I % 8 != 0) { set_last_error("glu_bwd_dropout: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
+  if (bits == nullptr) { set_last_error("glu_bwd_dropout: bits are required"); return MUSE_ERR_INVALID; }
+  const long long n = rows * (I / 8);
+  if (n <= 0) return MUSE_OK;
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_bwd_kernel<true>, reinterpret_cast<const bf16*>(ab),
+      reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I,
+      philox::elem_drop(const_cast<void*>(bits), nullptr, 0, p, I));
+  return check_launch("glu_bwd_dropout");
 }
 
 int glu_bwd(const void* ab, const void* dout, void* dab, long long rows, int I, cudaStream_t s) {
   if (I % 8 != 0) { set_last_error("glu_bwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
   const long long n = rows * (I / 8);
   if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_bwd_kernel, reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I);
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_bwd_kernel<false>, reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I, philox::ElemDrop{});
   return check_launch("glu_bwd");
 }
 

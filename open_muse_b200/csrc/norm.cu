@@ -9,7 +9,10 @@
 //              backward recomputes it and emits d[a | b] directly (LN backward + GLU backward in one pass)
 //   * residual: y = residual + norm(x) (normformer post-attention norm + residual add, :882-884)
 //   * backward: dx = norm_bwd(dy) (+ dres), so the residual-stream gradient add is free.
+//   * act=2 with dropout: FeedForward.dropout (:797) on the normalised output -- the forward draws the keep bits
+//              (philox.cuh) and writes the dropped bf16 output and the bits, the backward scales dy by them as it reads it
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace muse {
 namespace {
@@ -621,10 +624,11 @@ __device__ __forceinline__ uint32_t bf16x2_mul(uint32_t a, uint32_t b) {  // bf1
 // per SM): with the loads interleaved chunk by chunk only ~24 KB per SM were in flight, which by Little's law capped the
 // kernel at ~3.7 TB/s whatever the instruction count (same-box A/B: 219 -> 193 us at [65 792, 2 x 2048]).  The backward
 // got nothing from the same treatment (362 -> 360 us): it is bound by instruction issue, and keeps three CTAs per SM.
-template <int CH>
+template <int CH, bool DROP>
 __global__ void __launch_bounds__(kGluWarps * 32, (CH <= 8) ? 2 : 1)
 glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf16* __restrict__ y,
-                    float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows, int H, float eps, int rms) {
+                    float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows, int H, float eps, int rms,
+                    const philox::ElemDrop drop) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kGluWarps + (threadIdx.x >> 5);
@@ -688,21 +692,32 @@ glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf
     if (rstd_out) rstd_out[row] = rstd;
   }
   bf16* yr = y + static_cast<size_t>(row) * H;
+  unsigned long long seed = 0;
+  if constexpr (DROP) seed = *drop.seed;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
     const int col = (c * 32 + lane) * 8;
     if (col < H) {
       float wv[8];
       if (w) load8(w + col, wv);
+      uint32_t kb = 0xFFu;
+      if constexpr (DROP) kb = philox::elem_keep8(seed, drop.site, static_cast<uint32_t>(row), col / 8, drop.thresh);
       uint4 ou;
       uint32_t* op = reinterpret_cast<uint32_t*>(&ou);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 p = unpack_bf16(vp[c][j]);
-        const float r0 = w ? rstd * wv[2 * j] : rstd, r1 = w ? rstd * wv[2 * j + 1] : rstd;
+        float r0 = w ? rstd * wv[2 * j] : rstd, r1 = w ? rstd * wv[2 * j + 1] : rstd;
+        if constexpr (DROP) {  // the dropped output is the wo operand (and what the wo weight gradient reads)
+          r0 *= philox::keep_z(kb, 2 * j, drop.scale);
+          r1 *= philox::keep_z(kb, 2 * j + 1, drop.scale);
+        }
         op[j] = pack_bf16((p.x - mean) * r0, (p.y - mean) * r1);
       }
       *reinterpret_cast<uint4*>(yr + col) = ou;
+      if constexpr (DROP) drop.bits[static_cast<size_t>(row) * drop.row_bytes + col / 8] = static_cast<uint8_t>(kb);
+    } else if (DROP && col / 8 < drop.row_bytes) {
+      drop.bits[static_cast<size_t>(row) * drop.row_bytes + col / 8] = 0;  // pad bytes of the row's last word
     }
   }
 }
@@ -712,12 +727,15 @@ glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf
 // HAVE_Y: the saved forward output y = bf16(xhat * w) is available, so the first pass gets its two row reductions from
 // (dy, y) alone -- s1 = mean(dy * w), s2 = mean(dy * w * xhat) = mean(dy * y) -- without reading [a | b] or evaluating the
 // GELU, and the weight-gradient accumulation moves into the second pass.
-template <bool HAVE_Y>
+// DROP (never with HAVE_Y: the saved output is the dropped one): dy is the gradient of the dropped output and is scaled
+// by the stored keep bits as it is read, in both passes.
+template <bool HAVE_Y, bool DROP>
 __global__ void __launch_bounds__(kGluWarps * 32, 3)
 glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, const float* __restrict__ w,
                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in, bf16* __restrict__ dab,
                     float* __restrict__ dw, float* __restrict__ dw_ws, const bf16* __restrict__ yf, int rows, int H,
-                    int rms, int pf) {
+                    int rms, int pf, const philox::ElemDrop drop) {
+  static_assert(!(HAVE_Y && DROP), "the dropout backward recomputes the GLU product");
   pdl_enter();
   extern __shared__ __align__(16) float s_dw[];  // [kGluWarps][H] private rows
   const int lane = threadIdx.x & 31;
@@ -765,6 +783,8 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
       const uint32_t aw[4] = {au.x, au.y, au.z, au.w}, bw[4] = {bu.x, bu.y, bu.z, bu.w}, dd[4] = {du.x, du.y, du.z, du.w};
       float wv[8], pr[8];
       if (w) load8(w + col, wv);
+      uint32_t kb = 0xFFu;
+      if constexpr (DROP) kb = drop.bits[static_cast<size_t>(row) * drop.row_bytes + col / 8];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float2 a2 = unpack_bf16(aw[j]);
@@ -772,7 +792,11 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
         gelu_eval(a2.x, g0, t0);
         gelu_eval(a2.y, g1, t1);
         const float2 v2 = unpack_bf16(bf16x2_mul(pack_bf16(g0, g1), bw[j]));
-        const float2 d2 = unpack_bf16(dd[j]);
+        float2 d2 = unpack_bf16(dd[j]);
+        if constexpr (DROP) {
+          d2.x *= philox::keep_z(kb, 2 * j, drop.scale);
+          d2.y *= philox::keep_z(kb, 2 * j + 1, drop.scale);
+        }
         const float xh0 = (v2.x - mean) * rstd, xh1 = (v2.y - mean) * rstd;
         const float q0 = w ? d2.x * wv[2 * j] : d2.x, q1 = w ? d2.y * wv[2 * j + 1] : d2.y;
         s1 += q0 + q1;
@@ -808,6 +832,8 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
       const uint32_t aw[4] = {au.x, au.y, au.z, au.w}, bw[4] = {bu.x, bu.y, bu.z, bu.w}, dd[4] = {du.x, du.y, du.z, du.w};
       float wv[8];
       if (w) load8(w + col, wv);
+      uint32_t kb = 0xFFu;
+      if constexpr (DROP) kb = drop.bits[static_cast<size_t>(row) * drop.row_bytes + col / 8];
       uint4 oa, ob;
       float pr2[8];
       uint32_t* pa = reinterpret_cast<uint32_t*>(&oa);
@@ -822,7 +848,11 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
         const float2 gr = unpack_bf16(gp);  // bf16(gelu(a))
         const float2 v2 = unpack_bf16(bf16x2_mul(gp, bw[j]));
         const float2 b2 = unpack_bf16(bw[j]);
-        const float2 d2 = unpack_bf16(dd[j]);
+        float2 d2 = unpack_bf16(dd[j]);
+        if constexpr (DROP) {
+          d2.x *= philox::keep_z(kb, 2 * j, drop.scale);
+          d2.y *= philox::keep_z(kb, 2 * j + 1, drop.scale);
+        }
         const float xh0 = (v2.x - mean) * rstd, xh1 = (v2.y - mean) * rstd;
         const float q0 = w ? d2.x * wv[2 * j] : d2.x, q1 = w ? d2.y * wv[2 * j + 1] : d2.y;
         const float o0 = rstd * (q0 - s1 - xh0 * s2), o1 = rstd * (q1 - s1 - xh1 * s2);
@@ -912,6 +942,16 @@ int bwd_dispatch(const void* dy, const void* x, const float* w, const float* mea
   return reduce_dw(dw_ws, dw, grid, H, s);
 }
 
+void glu_bwd_smem_attr() {
+  static bool attr = false;
+  if (!attr) {
+    cudaFuncSetAttribute(glu_norm_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
+    cudaFuncSetAttribute(glu_norm_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
+    cudaFuncSetAttribute(glu_norm_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
+    attr = true;
+  }
+}
+
 int check_args(const char* who, int H, int act, const void* res_or_dres) {
   if (H % 8 != 0 || H > 4096 || H < 8) {
     set_last_error("%s: H=%d must be a multiple of 8 in [8, 4096]", who, H);
@@ -933,7 +973,7 @@ int norm_fwd(const void* x, int x_dt, const float* w, const float* res, void* y,
   if (act == ACT_GLU && x_dt == 1 && y_dt == 1 && H <= 4096) {
     const int grid = ceil_div(rows, kGluWarps);
     const int ch = ceil_div(H, 256);
-#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(glu_norm_fwd_kernel<CH>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms)
+#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(glu_norm_fwd_kernel<CH, false>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, philox::ElemDrop{})
     if (ch <= 1) MUSE_GF(1); else if (ch <= 2) MUSE_GF(2); else if (ch <= 4) MUSE_GF(4); else if (ch <= 8) MUSE_GF(8); else MUSE_GF(16);
 #undef MUSE_GF
     return check_launch("glu_norm_fwd");
@@ -1002,20 +1042,15 @@ int norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* w,
   if (act == ACT_GLU && dy_dt == 1 && x_dt == 1 && dx_dt == 1 && H <= 4096) {
     const int grid = bwd_grid(rows, H, act);
     const size_t smem = dw ? static_cast<size_t>(kGluWarps) * H * sizeof(float) : 0;
-    static bool attr = false;
-    if (!attr) {
-      cudaFuncSetAttribute(glu_norm_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
-      cudaFuncSetAttribute(glu_norm_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
-      attr = true;
-    }
+    glu_bwd_smem_attr();
     if (y_fwd != nullptr)
-      pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<true>,
+      pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<true, false>,
           reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-          dw_ws, reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, kRowPrefetch);
+          dw_ws, reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, kRowPrefetch, philox::ElemDrop{});
     else
-      pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<false>,
+      pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<false, false>,
           reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-          dw_ws, nullptr, rows, H, rms, 0);
+          dw_ws, nullptr, rows, H, rms, 0, philox::ElemDrop{});
     rc = check_launch("glu_norm_bwd");
     if (rc || !dw || !dw_ws) return rc;
     return reduce_dw(dw_ws, dw, grid, H, s);
@@ -1033,6 +1068,45 @@ int norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* w,
   }
   set_last_error("norm_bwd: bad dtype codes");
   return MUSE_ERR_INVALID;
+}
+
+// act = 2 (GLU + mid norm, bf16 in and out) with FeedForward.dropout fused: y is the dropped output, bits [rows,
+// ceil(H / 32)] uint32 words written (philox.cuh elementwise mapping, seed read from *seed).
+int norm_fwd_glu_dropout(const void* x, const float* w, void* y, float* mean, float* rstd, void* bits,
+                         const unsigned long long* seed, int site, float p, int rows, int H, float eps, int rms,
+                         cudaStream_t s) {
+  if (rows <= 0) return MUSE_OK;
+  int rc = check_args("norm_fwd_glu_dropout", H, ACT_GLU, nullptr);
+  if (rc) return rc;
+  if (bits == nullptr || seed == nullptr) { set_last_error("norm_fwd_glu_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
+  const philox::ElemDrop drop = philox::elem_drop(bits, seed, site, p, H);
+  const int grid = ceil_div(rows, kGluWarps);
+  const int ch = ceil_div(H, 256);
+#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(glu_norm_fwd_kernel<CH, true>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop)
+  if (ch <= 1) MUSE_GF(1); else if (ch <= 2) MUSE_GF(2); else if (ch <= 4) MUSE_GF(4); else if (ch <= 8) MUSE_GF(8); else MUSE_GF(16);
+#undef MUSE_GF
+  return check_launch("glu_norm_fwd_dropout");
+}
+
+// its backward: dy (gradient of the dropped output) is scaled by the bits as it is read; the GLU product is recomputed
+// from [a | b].  dw / dw_ws as in norm_bwd.
+int norm_bwd_glu_dropout(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,
+                         const void* bits, float p, void* dx, float* dw, float* dw_ws, int rows, int H, int rms,
+                         cudaStream_t s) {
+  if (rows <= 0) return MUSE_OK;
+  int rc = check_args("norm_bwd_glu_dropout", H, ACT_GLU, nullptr);
+  if (rc) return rc;
+  if (bits == nullptr) { set_last_error("norm_bwd_glu_dropout: bits are required"); return MUSE_ERR_INVALID; }
+  const philox::ElemDrop drop = philox::elem_drop(const_cast<void*>(bits), nullptr, 0, p, H);
+  const int grid = bwd_grid(rows, H, ACT_GLU);
+  const size_t smem = dw ? static_cast<size_t>(kGluWarps) * H * sizeof(float) : 0;
+  glu_bwd_smem_attr();
+  pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<false, true>,
+      reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
+      dw_ws, nullptr, rows, H, rms, 0, drop);
+  rc = check_launch("glu_norm_bwd_dropout");
+  if (rc || !dw || !dw_ws) return rc;
+  return reduce_dw(dw_ws, dw, grid, H, s);
 }
 
 }  // namespace muse

@@ -256,18 +256,28 @@ def _f32(p):
 
 
 class _EmbedFn(torch.autograd.Function):
+    """word[ids] + pos (reference Embed.forward :942-957); drop = (p, seed, site) applies its dropout (:956)."""
+
     @staticmethod
-    def forward(ctx, ids, word, pos):
+    def forward(ctx, ids, word, pos, drop=None):
         ctx.save_for_backward(ids)
         ctx.shapes = (word.shape, pos.shape)
-        return ops.embed_fwd(ids, _f32(word), _f32(pos))
+        x = ops.embed_fwd(ids, _f32(word), _f32(pos))
+        ctx.drop = None
+        if drop is not None:
+            x, bits = ops.dropout_fwd(x, *drop)
+            ctx.drop = (drop[0], bits)
+        return x
 
     @staticmethod
     def backward(ctx, dx):
         (ids,) = ctx.saved_tensors
         wshape, pshape = ctx.shapes
-        dword, dpos = ops.embed_bwd_det(ids, dx.contiguous(), wshape[0], pshape[0])
-        return None, dword, dpos
+        dx = dx.contiguous()
+        if ctx.drop is not None:
+            dx = ops.dropout_bwd(dx, ctx.drop[1], ctx.drop[0])
+        dword, dpos = ops.embed_bwd_det(ids, dx, wshape[0], pshape[0])
+        return None, dword, dpos, None
 
 
 class _ConvSpec:
@@ -410,8 +420,11 @@ class _ConvHeadFn(torch.autograd.Function):
 class _LayerSpec:
     """Static description of one transformer layer handed to the layer Function."""
 
-    def __init__(self, B, S, H, I, nh, eps, rms, normformer, cross, Skv, E, w, enc_op=None):
+    def __init__(self, B, S, H, I, nh, eps, rms, normformer, cross, Skv, E, w, enc_op=None, drop=None):
         self.B, self.S, self.H, self.I, self.nh = B, S, H, I, nh
+        # dropout of this layer in training mode: (attention p, hidden p, seed tensor, first site id) -- self-attention
+        # uses site, cross-attention site + 1, the FFN site + 2; a rate of 0 leaves its site out
+        self.p_attn, self.p_hidden, self.seed, self.site = drop if drop is not None else (0.0, 0.0, None, 0)
         self.eps, self.rms, self.normformer, self.cross = eps, rms, normformer, cross
         self.Skv, self.E = Skv, E
         self.enc_op = enc_op  # bf16 copy of the (projected, fp32) encoder states used as the K/V GEMM operand
@@ -466,7 +479,12 @@ class _LayerFn(torch.autograd.Function):
         # ---- self attention
         h1, st1 = ops.norm_fwd(x, _f32(w_attn_ln), s.eps, torch.bfloat16, rms=s.rms, save_stats=grad)
         qkv = ops.linear_fwd(h1, s.w["qkv"])
-        ctxt, lse = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh)
+        if s.p_attn:
+            ctxt, lse, abits = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh,
+                                            dropout=(s.p_attn, s.seed, s.site))
+            sv["abits"] = abits
+        else:
+            ctxt, lse = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh)
         fused_norms = s.normformer and not s.cross and H <= 1024  # post-attention norm + FFN pre-norm in one pass
         h2 = st3 = None
         if fused_norms:
@@ -486,7 +504,12 @@ class _LayerFn(torch.autograd.Function):
             qc = ops.linear_fwd(hc, s.w["cq"])
             enc_op = s.enc_op if s.enc_op is not None else enc  # bf16 GEMM operand (enc itself may be the fp32 projection)
             kvc = ops.linear_fwd(enc_op, s.w["ckv"])
-            cctx, clse = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh)
+            if s.p_attn:
+                cctx, clse, cbits = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh,
+                                                 dropout=(s.p_attn, s.seed, s.site + 1))
+                sv["cbits"] = cbits
+            else:
+                cctx, clse = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh)
             if s.normformer:
                 cao = ops.linear_fwd(cctx, s.w["co"])
                 x2b, stcp = ops.norm_fwd(cao, _f32(w_cpost), s.eps, torch.float32, res=x2, rms=s.rms, save_stats=grad)
@@ -502,8 +525,16 @@ class _LayerFn(torch.autograd.Function):
         if h2 is None:
             h2, st3 = ops.norm_fwd(x2, _f32(w_pre), s.eps, torch.bfloat16, rms=0, save_stats=grad)
         ab = ops.linear_fwd(h2, s.w["wi"])
-        if s.normformer:  # GLU product + mid_mlp_layer_norm in one pass; gelu(a)*b is never written to HBM
+        # FeedForward.dropout (:797) is fused into the pass that writes ml: ml is then the dropped wo operand (which is
+        # also what the wo weight gradient reads), and the keep bits are saved for the backward
+        ffn_drop = (s.p_hidden, s.seed, s.site + 2)
+        if s.normformer and s.p_hidden:
+            ml, st4, sv["fbits"] = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms,
+                                                save_stats=grad, dropout=ffn_drop)
+        elif s.normformer:  # GLU product + mid_mlp_layer_norm in one pass; gelu(a)*b is never written to HBM
             ml, st4 = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms, save_stats=grad)
+        elif s.p_hidden:
+            (ml, sv["fbits"]), st4 = ops.glu_fwd(ab, dropout=ffn_drop), None
         else:
             ml, st4 = ops.glu_fwd(ab), None
         x3 = ops.linear_fwd(ml, s.w["wo"], res=x2)
@@ -536,9 +567,15 @@ class _LayerFn(torch.autograd.Function):
             dy = ops.cast_bf16(dx3)
         d_ml = ops.linear_dgrad(dy, s.w["wo"])
         g_wo = ops.linear_wgrad_det(dy, sv["ml"])
-        if s.normformer:  # LN backward + GLU backward fused: reads d_ml and [a|b], writes d[a|b]
+        if s.normformer and s.p_hidden:  # d_ml is scaled by the keep bits as it is read; the saved ml is the dropped
+            # output, so the kernel recomputes the GLU product from [a | b] instead of reading it
+            d_ab, g_mid = ops.norm_bwd(d_ml, sv["ab"], _f32(w_mid), sv["st4"], torch.bfloat16, act=2, rms=s.rms,
+                                       want_dw=True, dropout=(s.p_hidden, sv["fbits"]))
+        elif s.normformer:  # LN backward + GLU backward fused: reads d_ml and [a|b], writes d[a|b]
             d_ab, g_mid = ops.norm_bwd(d_ml, sv["ab"], _f32(w_mid), sv["st4"], torch.bfloat16, act=2, rms=s.rms,
                                        y_fwd=sv["ml"], want_dw=True)
+        elif s.p_hidden:
+            g_mid, d_ab = None, ops.glu_bwd(sv["ab"], d_ml, dropout=(s.p_hidden, sv["fbits"]))
         else:
             g_mid = None
             d_ab = ops.glu_bwd(sv["ab"], d_ml)
@@ -564,7 +601,8 @@ class _LayerFn(torch.autograd.Function):
             d_kvc = torch.empty_like(sv["kvc"])
             kvc = sv["kvc"]
             ops.attn_bwd(sv["qc"], kvc[:, :H], kvc[:, H:], sv["cctx"], d_cctx, sv["clse"], d_qc, d_kvc[:, :H],
-                         d_kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh)
+                         d_kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh,
+                         **({"dropout": (s.p_attn, sv["cbits"])} if s.p_attn else {}))
             g_ckv = ops.linear_wgrad_det(d_kvc, sv["enc"])
             if ctx.needs_input_grad[1]:  # projected encoder states: d enc = d[k|v] @ [Wk;Wv], fp32, summed over layers by autograd
                 d_enc = ops.linear_dgrad(d_kvc, s.w["ckv"], out_dtype=torch.float32)
@@ -585,7 +623,8 @@ class _LayerFn(torch.autograd.Function):
         qkv = sv["qkv"]
         d_qkv = torch.empty_like(qkv)
         ops.attn_bwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], sv["ctxt"], d_ctx, sv["lse"], d_qkv[:, :H],
-                     d_qkv[:, H:2 * H], d_qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh)
+                     d_qkv[:, H:2 * H], d_qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh,
+                     **({"dropout": (s.p_attn, sv["abits"])} if s.p_attn else {}))
         d_h1 = ops.linear_dgrad(d_qkv, s.w["qkv"])
         g_qkv = ops.linear_wgrad_det(d_qkv, sv["h1"])
         dx1, g_attn_ln = ops.norm_bwd(d_h1, sv["x"], _f32(w_attn_ln), sv["st1"], torch.float32, dres=dx2, rms=s.rms,
@@ -868,11 +907,6 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
             raise ValueError("If `add_cross_attention` is True, `encoder_hidden_states` should be provided.")
         if encoder_attention_mask is not None:
             raise TypeError("encoder_attention_mask is not supported (it raises in the reference too: quirk Q2)")
-        if self.training and (self.hidden_dropout > 0.0 or self.attention_dropout > 0.0):
-            raise NotImplementedError(
-                "open_muse_b200: dropout > 0 in training mode is not implemented (all reference configs use 0.0); "
-                "construct the model with hidden_dropout=0.0, attention_dropout=0.0"
-            )
         if not input_ids.is_cuda:
             raise RuntimeError("open_muse_b200.MaskGitTransformer runs on CUDA (sm_90a) only; move inputs to the GPU")
         B, S = input_ids.shape
@@ -899,12 +933,20 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
             raise IndexError(f"sequence length {S} exceeds max_position_embeddings {self.max_position_embeddings}")
         packed = self._packed.refresh()
         ids = input_ids.contiguous().to(torch.int64)
+        # nn.Dropout is active iff the module is in training mode (also under no_grad).  One seed per forward, drawn on the
+        # device from torch's default generator: torch.manual_seed reproduces the masks, and a captured CUDA graph draws
+        # a fresh seed on every replay without a host sync.  Site ids: 0 the embedding, 1 + 3 i .. 3 + 3 i layer i.
+        p_hidden, p_attn, seed = 0.0, 0.0, None
+        if self.training and (self.hidden_dropout > 0.0 or self.attention_dropout > 0.0):
+            p_hidden, p_attn = float(self.hidden_dropout), float(self.attention_dropout)
+            seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=input_ids.device)
         if c.use_conv_in_out:
             conv = _ConvSpec(B, n, p, self.embedding_size, H, c.layer_norm_eps, rms, packed.head)
             x = _ConvEmbedFn.apply(ids, conv, self.embed.embeddings.weight, self.embed.layer_norm.weight,
                                    self.embed.conv.weight, self.embed.position_embeddings.weight)
         else:
-            x = _EmbedFn.apply(ids, self.embed.word_embeddings.weight, self.embed.position_embeddings.weight)
+            x = _EmbedFn.apply(ids, self.embed.word_embeddings.weight, self.embed.position_embeddings.weight,
+                               (p_hidden, seed, 0) if p_hidden else None)
 
         enc = None
         Skv = E = 0
@@ -927,7 +969,8 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
             enc_op = ops.cast_bf16(enc.detach())
         for i, layer in enumerate(self.transformer_layers):
             spec = _LayerSpec(B, S, H, self.intermediate_size, self.num_attention_heads, c.layer_norm_eps, rms,
-                              c.use_normformer, enc is not None, Skv, E, packed.layers[i], enc_op)
+                              c.use_normformer, enc is not None, Skv, E, packed.layers[i], enc_op,
+                              drop=(p_attn, p_hidden, seed, 1 + 3 * i) if seed is not None else None)
             x = _LayerFn.apply(x, enc, spec, *self._layer_params(layer))
 
         flat_labels = labels.reshape(-1).contiguous().to(torch.int64) if labels is not None else None
@@ -986,6 +1029,10 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
         ``_noise`` = per-step (q_exp, u) tensors, ``_trace`` = list collecting per-step state) run the same kernels launched
         one by one."""
         c = self.config
+        if self.training and (self.hidden_dropout > 0.0 or self.attention_dropout > 0.0):
+            # the reference would sample with dropout applied to every forward of the decode loop
+            raise RuntimeError("generate2 on a MaskGitTransformer in training mode would sample with dropout > 0 active; "
+                               "call model.eval() first")
         mask_id, seq_len, n_codes = c.mask_token_id, c.num_vq_tokens, c.codebook_size
         batch = len(class_ids) if class_ids is not None else encoder_hidden_states.shape[0]
         if class_ids is not None:

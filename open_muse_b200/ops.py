@@ -63,7 +63,7 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
-_KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
+_KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_attn_bwd_dropout": 2, "muse_norm_bwd_glu_dropout": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
                      "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3,
                      "muse_dwconv3x3_norm_bwd": 2}
 _prof = {"on": False, "events": []}
@@ -220,8 +220,10 @@ def embed_bwd_det(ids, dx, vocab, n_pos):
 
 
 # ------------------------------------------------------------------------------------------ norms
-def norm_fwd(x, w, eps, out_dtype, res=None, act=0, rms=0, save_stats=True):
-    """act: 0 none, 1 GELU(x) first, 2 GLU (x is [rows, 2H] = [a | b], the normalised value is gelu(a) * b)."""
+def norm_fwd(x, w, eps, out_dtype, res=None, act=0, rms=0, save_stats=True, dropout=None):
+    """act: 0 none, 1 GELU(x) first, 2 GLU (x is [rows, 2H] = [a | b], the normalised value is gelu(a) * b).
+    dropout = (p, seed, site), act 2 with bf16 x and y only: FeedForward.dropout fused into the pass (the output is the
+    dropped one); then returns (y, stats, bits) with bits int32 [rows, ceil(H / 32)] for norm_bwd (see dropout_fwd)."""
     st = _prep(x)
     rows = x.shape[0]
     H = x.shape[1] // 2 if act == 2 else x.shape[1]
@@ -231,6 +233,14 @@ def norm_fwd(x, w, eps, out_dtype, res=None, act=0, rms=0, save_stats=True):
         mean, rstd = stats[0], stats[1]
     else:
         stats = mean = rstd = None
+    if dropout is not None:
+        assert act == 2 and x.dtype == torch.bfloat16 and out_dtype == torch.bfloat16 and res is None
+        p, seed, site = dropout
+        bits = torch.empty(rows, (H + 31) // 32, dtype=torch.int32, device=x.device)
+        _call("muse_norm_fwd_glu_dropout", _p(x), _p(w), _p(y), _p(mean), _p(rstd), _p(bits), _p(seed), int(site), float(p),
+              rows, H, float(eps), rms, st)
+        _drop_record(site, bits)
+        return y, stats, bits
     _call("muse_norm_fwd", _p(x), _dt(x), _p(w), _p(res), _p(y), _dt(y), _p(mean), _p(rstd), rows, H, float(eps),
           act, rms, st)
     return y, stats
@@ -247,14 +257,29 @@ def take_bf16_copy(t):
     return None
 
 
-def norm_bwd(dy, x, w, stats, dx_dtype, dw=None, dres=None, act=0, rms=0, y_fwd=None, want_dw=False, bf16_copy=False):
+def norm_bwd(dy, x, w, stats, dx_dtype, dw=None, dres=None, act=0, rms=0, y_fwd=None, want_dw=False, bf16_copy=False,
+             dropout=None):
     """y_fwd: the saved forward output (act=2, bf16 only) -- lets the kernel skip one GELU pass over [a | b].
     dw: fp32 [H] buffer the weight gradient is ADDED to (atomics; caller zero-fills).  want_dw=True instead returns
-    (dx, dw) with a freshly stored dw reduced in a fixed order (run-to-run bit-identical)."""
+    (dx, dw) with a freshly stored dw reduced in a fixed order (run-to-run bit-identical).
+    dropout = (p, bits) from norm_fwd(..., dropout=...): dy (the gradient of the dropped output) is scaled by the bits as
+    the kernel reads it; y_fwd is then ignored (the saved output is the dropped one, the GLU product is recomputed)."""
     st = _prep(x)
     rows = x.shape[0]
     H = x.shape[1] // 2 if act == 2 else x.shape[1]
     dx = torch.empty(x.shape, dtype=dx_dtype, device=x.device)
+    if dropout is not None:
+        assert act == 2 and dy.dtype == x.dtype == dx_dtype == torch.bfloat16 and dres is None and not bf16_copy
+        p, bits = dropout
+        ws = None
+        if want_dw:
+            dw = torch.empty(H, dtype=torch.float32, device=x.device)
+            ws = torch.empty(max(1, _lib.load().muse_norm_bwd_workspace_floats(rows, H, act)), dtype=torch.float32,
+                             device=x.device)
+            _state["launches"] += 1  # the ordered column sum
+        _call("muse_norm_bwd_glu_dropout", _p(dy), _p(x), _p(w), _p(stats[0]), _p(stats[1]), _p(bits), float(p), _p(dx),
+              _p(dw), _p(ws), rows, H, rms, st)
+        return (dx, dw) if want_dw else dx
     if y_fwd is not None and not (act == 2 and y_fwd.dtype == torch.bfloat16 and y_fwd.is_contiguous()):
         y_fwd = None
     copy = None
@@ -302,41 +327,121 @@ def norm2_bwd(d_h2, x2, w2, dres, a, w1, stats, rms1=0, rms2=0):
 
 
 # ------------------------------------------------------------------------------------------ GLU
-def glu_fwd(ab):
+def glu_fwd(ab, dropout=None):
+    """dropout = (p, seed, site): FeedForward.dropout fused into the pass; then returns (out, bits) (see dropout_fwd)."""
     st = _prep(ab)
     rows, two_i = ab.shape
     out = torch.empty(rows, two_i // 2, dtype=torch.bfloat16, device=ab.device)
+    if dropout is not None:
+        p, seed, site = dropout
+        bits = torch.empty(rows, (two_i // 2 + 31) // 32, dtype=torch.int32, device=ab.device)
+        _call("muse_glu_fwd_dropout", _p(ab), _p(out), _p(bits), _p(seed), int(site), float(p), rows, two_i // 2, st)
+        _drop_record(site, bits)
+        return out, bits
     _call("muse_glu_fwd", _p(ab), _p(out), rows, two_i // 2, st)
     return out
 
 
-def glu_bwd(ab, dout):
+def glu_bwd(ab, dout, dropout=None):
+    """dropout = (p, bits) from glu_fwd(..., dropout=...): dout is scaled by the bits as the kernel reads it."""
     st = _prep(ab)
     rows, two_i = ab.shape
     dab = torch.empty_like(ab)
+    if dropout is not None:
+        p, bits = dropout
+        _call("muse_glu_bwd_dropout", _p(ab), _p(dout), _p(bits), float(p), _p(dab), rows, two_i // 2, st)
+        return dab
     _call("muse_glu_bwd", _p(ab), _p(dout), _p(dab), rows, two_i // 2, st)
     return dab
 
 
 # ------------------------------------------------------------------------------------------ attention
-def attn_fwd(q, k, v, B, nh, Sq, Skv, scale, head_dim=64):
+def attn_fwd(q, k, v, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
     """q: [B*Sq, *] view with head h at columns h*head_dim; k, v: [B*Skv, *] views.  Returns ctx [B*Sq, nh*head_dim], lse.
-    head_dim: 64 (default) or 48 (configs/imagenet.yaml: hidden 768 / 16 heads)."""
+    head_dim: 64 (default) or 48 (configs/imagenet.yaml: hidden 768 / 16 heads).
+    dropout = (p, seed, site): nn.Dropout(p) on the probabilities with the keep bits of (seed: int64 [1] device tensor,
+    site) -- see dropout_fwd; then returns (ctx, lse, bits) with bits int32 [B, nh, Sq, ceil(Skv / 32)] for attn_bwd."""
     st = _prep(q)
     hd = int(head_dim)
     o = torch.empty(B * Sq, nh * hd, dtype=torch.bfloat16, device=q.device)
     lse = torch.empty(B, nh, Sq, dtype=torch.float32, device=q.device)
+    if dropout is not None:
+        p, seed, site = dropout
+        bits = torch.empty(B, nh, Sq, (Skv + 31) // 32, dtype=torch.int32, device=q.device)
+        _call("muse_attn_fwd_dropout", _p(q), _p(k), _p(v), _p(o), _p(lse), _p(bits), _p(seed), int(site), float(p), B, nh,
+              Sq, Skv, hd, q.stride(0), k.stride(0), v.stride(0), o.stride(0), float(scale), st)
+        _drop_record(site, bits)
+        return o, lse, bits
     _call("muse_attn_fwd", _p(q), _p(k), _p(v), _p(o), _p(lse), B, nh, Sq, Skv, hd, q.stride(0), k.stride(0),
           v.stride(0), o.stride(0), float(scale), st)
     return o, lse
 
 
-def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, B, nh, Sq, Skv, scale, head_dim=64):
+def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
+    """dropout = (p, bits): the rate and the keep bits attn_fwd(..., dropout=...) returned."""
     st = _prep(q)
     dvec = torch.empty(B, nh, Sq, dtype=torch.float32, device=q.device)
+    if dropout is not None:
+        p, bits = dropout
+        _call("muse_attn_bwd_dropout", _p(q), _p(k), _p(v), _p(do), _p(lse), _p(bits), float(p), _p(dvec), _p(dq), _p(dk),
+              _p(dv), B, nh, Sq, Skv, int(head_dim), q.stride(0), k.stride(0), v.stride(0), do.stride(0), dq.stride(0),
+              dk.stride(0), dv.stride(0), float(scale), st)
+        return
     _call("muse_attn_bwd", _p(q), _p(k), _p(v), _p(o), _p(do), _p(lse), _p(dvec), _p(dq), _p(dk), _p(dv), B, nh, Sq,
           Skv, int(head_dim), q.stride(0), k.stride(0), v.stride(0), o.stride(0), do.stride(0), dq.stride(0), dk.stride(0),
           dv.stride(0), float(scale), st)
+
+
+# ------------------------------------------------------------------------------------------ dropout
+# nn.Dropout(p) in training mode.  The keep masks come from Philox4x32-10 keyed by a 64-bit seed that lives in device memory
+# (an int64 [1] tensor drawn from torch's CUDA generator once per forward, so torch.manual_seed reproduces a run and a
+# captured CUDA graph draws a fresh one per replay) and a site id unique within the forward; csrc/philox.cuh holds the
+# mapping from (seed, site, coordinates) to bits and the rate actually applied, p_eff = round(p * 65536) / 65536.  The
+# forward stores the bits (int32 words, rows padded to 32 bits, bit k % 32 of word k / 32 set = element k kept) and the
+# backward reads them: no seed, no second draw.
+_drop_state = {"log": None}
+
+
+class dropout_record:
+    """Test hook: ``with ops.dropout_record() as log:`` appends (site, bits) for every dropout op launched inside the block
+    (attention and elementwise sites), so that tests can compare the masks with a restatement of the generator or hand
+    them to another implementation.  Not a product switch."""
+
+    def __enter__(self):
+        self.prev = _drop_state["log"]
+        _drop_state["log"] = []
+        return _drop_state["log"]
+
+    def __exit__(self, *exc):
+        _drop_state["log"] = self.prev
+        return False
+
+
+def _drop_record(site, bits):
+    if _drop_state["log"] is not None:
+        _drop_state["log"].append((int(site), bits))
+
+
+def dropout_fwd(x, p, seed, site):
+    """x contiguous fp32 / bf16 [rows, cols] (cols % 8 == 0) is dropped IN PLACE: x * keep / (1 - p_eff).  Returns
+    (x, bits) with bits int32 [rows, ceil(cols / 32)]."""
+    st = _prep(x)
+    rows, cols = x.shape
+    assert x.is_contiguous()
+    bits = torch.empty(rows, (cols + 31) // 32, dtype=torch.int32, device=x.device)
+    _call("muse_dropout_fwd", _p(x), _p(x), _dt(x), _p(bits), _p(seed), int(site), float(p), rows, cols, st)
+    _drop_record(site, bits)
+    return x, bits
+
+
+def dropout_bwd(dy, bits, p, out=None):
+    """dx = dy * keep / (1 - p_eff) with the bits dropout_fwd stored; out (may be dy itself) receives dx."""
+    st = _prep(dy)
+    rows, cols = dy.shape
+    assert dy.is_contiguous()
+    dx = torch.empty_like(dy) if out is None else out
+    _call("muse_dropout_bwd", _p(dy), _p(dx), _dt(dy), _p(bits), float(p), rows, cols, st)
+    return dx
 
 
 # ------------------------------------------------------------------------------------------ loss
