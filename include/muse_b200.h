@@ -21,7 +21,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 4
+#define MUSE_B200_ABI_VERSION 5
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -240,6 +240,16 @@ int muse_dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, co
 /* x = forward input (bf16), dout bf16, nx / sumsq from the forward, s1_ws fp32 [B,C] scratch -> dx bf16; dgamma, dbeta +=. */
 int muse_grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
                  void* dx, float* dgamma, float* dbeta, int B, int HW, int C, void* stream);
+/* The ResBlock's nn.Dropout between GlobalResponseNorm and channelwise[4] (:603-609) fused into the GRN passes (masks,
+ * layout and rate as muse_dropout_fwd; row = token of the B * HW rows, bits [B * HW, ceil(C / 32)]):
+ *   muse_grn_fwd_dropout: muse_grn_fwd, then out = bf16(fp32 GRN output * keep / (1 - p_eff)) and the bits written;
+ *   muse_grn_bwd_dropout: muse_grn_bwd with dout (the gradient of the dropped output) scaled by the bits as it is read. */
+int muse_grn_fwd_dropout(const void* x, const float* gamma, const float* beta, void* out, float* sumsq_ws, float* nx_ws,
+                         unsigned int* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C,
+                         void* stream);
+int muse_grn_bwd_dropout(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma,
+                         float* s1_ws, void* dx, float* dgamma, float* dbeta, const unsigned int* bits, float p, int B,
+                         int HW, int C, void* stream);
 /* y = x * (1 + scale_b) + shift_b: dx = dy * (1 + scale_b); dscale_shift[b] += (sum dy * x | sum dy). */
 int muse_adaln_bwd(const float* dy, const float* x, const float* scale_shift, long long ss_stride, float* dx,
                    float* dscale_shift, int B, int rows_per_sample, int C, void* stream);

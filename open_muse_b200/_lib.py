@@ -60,6 +60,8 @@ SIGNATURES = {
     "muse_add_norm_mod_bwd": (c_int, [_P, _I, _P, _P, _P, _P, _L, _I, _P, _I, _P, _P, _P, _I, _I, _F, _I, _P]),
     "muse_dwconv3x3_norm_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
     "muse_grn_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "muse_grn_fwd_dropout": (c_int, [_P] * 8 + [_I, _F, _I, _I, _I, _P]),
+    "muse_grn_bwd_dropout": (c_int, [_P] * 10 + [_F, _I, _I, _I, _P]),
     "muse_adaln_bwd": (c_int, [_P, _P, _P, _L, _P, _P, _I, _I, _I, _P]),
     "muse_silu_bwd": (c_int, [_P, _P, _I, _P, _I, _L, _I, _P]),
     "muse_adaln_apply": (c_int, [_P, _P, _L, _I, _I, _I, _P]),
@@ -83,7 +85,7 @@ SIGNATURES = {
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 class MuseB200Error(RuntimeError):

@@ -75,6 +75,8 @@ int grn_fwd(const void*, const float*, const float*, void*, float*, float*, int,
 int add_norm_mod_bwd(const void*, int, const float*, const float*, const float*, const float*, long long, int, void*, int, float*, float*, float*, int, int, float, int, cudaStream_t);
 int dwconv3x3_norm_bwd(const void*, const void*, const float*, const float*, const float*, const float*, float*, float*, float*, float*, int, int, int, int, float, int, cudaStream_t);
 int grn_bwd(const void*, const void*, const float*, const float*, const float*, float*, void*, float*, float*, int, int, int, cudaStream_t);
+int grn_fwd_dropout(const void*, const float*, const float*, void*, float*, float*, void*, const unsigned long long*, int, float, int, int, int, cudaStream_t);
+int grn_bwd_dropout(const void*, const void*, const float*, const float*, const float*, float*, void*, float*, float*, const void*, float, int, int, int, cudaStream_t);
 int adaln_bwd(const float*, const float*, const float*, long long, float*, float*, int, int, int, cudaStream_t);
 int silu_bwd(const void*, const void*, int, void*, int, long long, int, cudaStream_t);
 int adaln_apply(float*, const float*, long long, int, int, int, cudaStream_t);
@@ -292,6 +294,16 @@ int muse_dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, co
 int muse_grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
                  void* dx, float* dgamma, float* dbeta, int B, int HW, int C, void* stream) {
   return grn_bwd(x, dout, nx, sumsq, gamma, s1_ws, dx, dgamma, dbeta, B, HW, C, ST(stream));
+}
+int muse_grn_fwd_dropout(const void* x, const float* gamma, const float* beta, void* out, float* sumsq_ws, float* nx_ws,
+                         unsigned int* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C,
+                         void* stream) {
+  return grn_fwd_dropout(x, gamma, beta, out, sumsq_ws, nx_ws, bits, seed, site, p, B, HW, C, ST(stream));
+}
+int muse_grn_bwd_dropout(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma,
+                         float* s1_ws, void* dx, float* dgamma, float* dbeta, const unsigned int* bits, float p, int B,
+                         int HW, int C, void* stream) {
+  return grn_bwd_dropout(x, dout, nx, sumsq, gamma, s1_ws, dx, dgamma, dbeta, bits, p, B, HW, C, ST(stream));
 }
 int muse_adaln_bwd(const float* dy, const float* x, const float* scale_shift, long long ss_stride, float* dx,
                    float* dscale_shift, int B, int rows_per_sample, int C, void* stream) {

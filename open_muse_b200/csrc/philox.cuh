@@ -1,9 +1,15 @@
 // Dropout keep masks: Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011) and the ONE
-// mapping from (seed, site, coordinates) to keep bits.  Every dropout kernel (attention_tc.cu, elementwise.cu) draws its
-// bits through the functions below; the CPU restatement in tests/test_dropout_cpu.py is the only other copy.
+// mapping from (seed, site, coordinates) to keep bits.  Every dropout kernel (attention_tc.cu, elementwise.cu, norm.cu,
+// uvit.cu) draws its bits through the functions below; the CPU restatement in tests/test_dropout_cpu.py is the only
+// other copy.
 //
 //   key     = the 64-bit seed (lo, hi words), read by the kernels from device memory (drawn on the device per forward)
 //   counter = (c0, c1, c2, site): the last word is the site id, unique within one forward (layer x site kind)
+//
+// Site ids.  MaskGitTransformer: 0 the embedding; layer i: 1 + 3 i self-attention, 2 + 3 i cross-attention, 3 + 3 i FFN.
+// MaskGiTUViT_v2: unit j = down pairs 0 .. R-1, then layers R .. R+L-1, then up pairs R+L .. 2R+L-1 (R = num_res_blocks,
+// L = num_hidden_layers) owns 3 j + kind; a ResBlock + AttentionBlock2D pair: 0 the ResBlock's dropout after GRN (an
+// elementwise site over [B*h*w, 4C]), 1 attention, 2 crossattention; a layer: 0 attention, 1 crossattention, 2 FFN.
 //   output  = four 32-bit words = eight 16-bit uniforms u, lane L = bits 16 (L & 1) .. of word L >> 1
 //   keep    = u >= t, with t = round(p * 65536); kept values are scaled by 65536 / (65536 - t)
 // With 16-bit uniforms the effective rate is p_eff = t / 65536 (|p_eff - p| <= 2^-17 = 7.6e-6) and the scale makes the

@@ -6,9 +6,12 @@
 //   * dwconv3x3_norm: ResBlock head (:604-612): depthwise 3x3 conv (bf16-rounded like the autocast conv output) + Norm2D.
 //   * grn           : GELU + GlobalResponseNorm (:741-751): Gx = ||g||_2 over (h, w) per (image, channel),
 //                     Nx = Gx / (mean_c Gx + 1e-6), out = gamma * (g * Nx) + beta + g.
+//                     With dropout: the ResBlock's nn.Dropout between GRN and channelwise[4] (:603-609) fused into the
+//                     apply pass, which draws the keep bits (philox.cuh) and writes the dropped output and the bits.
 //   * adaln_apply   : in-place fp32 x * (1 + scale_b) + shift_b at the end of a ResBlock.
 //   * silu          : SiLU of the conditioning vectors / text states feeding the adaLN and kv mappers.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace muse {
 namespace {
@@ -194,9 +197,14 @@ grn_finalize_kernel(const float* __restrict__ stat, float* __restrict__ nx_out, 
 }
 
 // GRN pass 3: out = gamma * (g * nx) + beta + g, g = bf16(gelu(x)); 8 channels per thread
+// DROP: the thread's 8 channels of one token row are one Philox call of the elementwise mapping (row = token of the
+// B*HW rows, columns = the C channels): the fp32 output is scaled by keep / (1 - p_eff) and rounded once, and the keep
+// byte is stored (the last chunk of a row also zeroes the pad bytes of the row's last word).
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 grn_apply_kernel(const bf16* __restrict__ x, const float* __restrict__ nx, const float* __restrict__ gamma,
-                 const float* __restrict__ beta, bf16* __restrict__ out, long long total8, int HW, int C) {
+                 const float* __restrict__ beta, bf16* __restrict__ out, long long total8, int HW, int C,
+                 const philox::ElemDrop drop) {
   pdl_enter();
   const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= total8) return;
@@ -212,6 +220,17 @@ grn_apply_kernel(const bf16* __restrict__ x, const float* __restrict__ nx, const
   for (int j = 0; j < 8; ++j) {
     const float g = bf16_round(gelu_f(v[j]));
     o[j] = fmaf(g8[j], g * n8[j], b8[j]) + g;
+  }
+  if constexpr (DROP) {
+    const long long row = i / c8;
+    const int k = col / 8;
+    const uint32_t kb = philox::elem_keep8(*drop.seed, drop.site, static_cast<uint32_t>(row), k, drop.thresh);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] *= philox::keep_z(kb, j, drop.scale);
+    uint8_t* br = drop.bits + row * drop.row_bytes;
+    br[k] = static_cast<uint8_t>(kb);
+    if (k == c8 - 1)
+      for (int q = c8; q < drop.row_bytes; ++q) br[q] = 0;
   }
   store8(out + i * 8, o);
 }
@@ -293,9 +312,11 @@ int dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y
   return check_launch("dwconv3x3_norm");
 }
 
-// x bf16 [B, HW, C] -> out bf16 [B, HW, C]; sumsq_ws / nx_ws fp32 [B, C] (kept by the caller for the backward pass)
-int grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws, int B, int HW,
-            int C, cudaStream_t s) {
+namespace {
+
+template <bool DROP>
+int launch_grn(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws, int B, int HW,
+               int C, const philox::ElemDrop& drop, cudaStream_t s) {
   if (B <= 0 || HW <= 0) return MUSE_OK;
   if (C % 8 != 0) { set_last_error("grn: C must be a multiple of 8"); return MUSE_ERR_UNSUPPORTED; }
   const bf16* xp = reinterpret_cast<const bf16*>(x);
@@ -306,9 +327,25 @@ int grn_fwd(const void* x, const float* gamma, const float* beta, void* out, flo
   rc = check_launch("grn_finalize");
   if (rc) return rc;
   const long long total8 = static_cast<long long>(B) * HW * (C / 8);
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(grn_apply_kernel, xp, nx_ws, gamma, beta,
-                                                                                   reinterpret_cast<bf16*>(out), total8, HW, C);
-  return check_launch("grn_apply");
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(grn_apply_kernel<DROP>, xp, nx_ws, gamma, beta,
+                                                                         reinterpret_cast<bf16*>(out), total8, HW, C, drop);
+  return check_launch(DROP ? "grn_apply_dropout" : "grn_apply");
+}
+
+}  // namespace
+
+// x bf16 [B, HW, C] -> out bf16 [B, HW, C]; sumsq_ws / nx_ws fp32 [B, C] (kept by the caller for the backward pass)
+int grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws, int B, int HW,
+            int C, cudaStream_t s) {
+  return launch_grn<false>(x, gamma, beta, out, stat_ws, nx_ws, B, HW, C, philox::ElemDrop{}, s);
+}
+
+// grn_fwd followed by the ResBlock's dropout (:607): out is the dropped output, bits [B * HW, ceil(C / 32)] uint32
+// words written (philox.cuh elementwise mapping, seed read from *seed)
+int grn_fwd_dropout(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws,
+                    void* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C, cudaStream_t s) {
+  if (bits == nullptr || seed == nullptr) { set_last_error("grn_fwd_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
+  return launch_grn<true>(x, gamma, beta, out, stat_ws, nx_ws, B, HW, C, philox::elem_drop(bits, seed, site, p, C), s);
 }
 
 int adaln_apply(float* x, const float* ss, long long ss_stride, int B, int rows_per_sample, int C, cudaStream_t s) {

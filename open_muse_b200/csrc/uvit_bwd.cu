@@ -2,6 +2,7 @@
 // embedding backward are shared with the v1 path).  All HBM-bound; parameter / per-sample reductions are folded in
 // registers and shared memory before touching global atomics.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace muse {
 namespace {
@@ -298,10 +299,14 @@ dwconv_bwd_kernel(const float* __restrict__ dc, const float* __restrict__ x, con
 }
 
 // ---- GELU + GRN backward --------------------------------------------------------------------------------------------
+// DROP (both passes that read dout): dout is the gradient of the dropped output (the ResBlock's dropout after GRN) and
+// is scaled by the stored keep bits as it is read -- 2 bits of one byte per token here, one byte of 8 in pass C.
 // pass A: per (image, channel) S1 = sum_hw dout * g ; dbeta += sum dout ; dgamma += nx * S1
+template <bool DROP>
 __global__ void __launch_bounds__(128)
 grn_bwd_stats_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dout, const float* __restrict__ nx,
-                     float* __restrict__ s1_out, float* __restrict__ dgamma, float* __restrict__ dbeta, int HW, int C) {
+                     float* __restrict__ s1_out, float* __restrict__ dgamma, float* __restrict__ dbeta, int HW, int C,
+                     const philox::ElemDrop drop) {
   pdl_enter();
   const int c = (blockIdx.x * 128 + threadIdx.x) * 2;
   if (c >= C) return;
@@ -310,7 +315,12 @@ grn_bwd_stats_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dout, 
   float a0 = 0.f, a1 = 0.f, d0 = 0.f, d1 = 0.f;
   for (int t = 0; t < HW; ++t) {
     const float2 v = unpack_bf16(*reinterpret_cast<const uint32_t*>(x + off + static_cast<size_t>(t) * C));
-    const float2 d = unpack_bf16(*reinterpret_cast<const uint32_t*>(dout + off + static_cast<size_t>(t) * C));
+    float2 d = unpack_bf16(*reinterpret_cast<const uint32_t*>(dout + off + static_cast<size_t>(t) * C));
+    if constexpr (DROP) {
+      const uint32_t kb = drop.bits[(static_cast<size_t>(b) * HW + t) * drop.row_bytes + c / 8];
+      d.x *= philox::keep_z(kb, c % 8, drop.scale);
+      d.y *= philox::keep_z(kb, c % 8 + 1, drop.scale);
+    }
     a0 = fmaf(d.x, bf16_round(gelu_f(v.x)), a0);
     a1 = fmaf(d.y, bf16_round(gelu_f(v.y)), a1);
     d0 += d.x;
@@ -355,10 +365,11 @@ grn_bwd_finalize_kernel(float* __restrict__ s1, const float* __restrict__ sumsq,
 }
 
 // pass C: dg = dout * (gamma * nx + 1) + coef * g ; dx = dg * gelu'(x)
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 grn_bwd_apply_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dout, const float* __restrict__ nx,
                      const float* __restrict__ coef, const float* __restrict__ gamma, bf16* __restrict__ dx,
-                     long long total8, int HW, int C) {
+                     long long total8, int HW, int C, const philox::ElemDrop drop) {
   pdl_enter();
   const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= total8) return;
@@ -368,6 +379,11 @@ grn_bwd_apply_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dout, 
   float v[8], d[8], n8[8], k8[8], g8[8], o[8];
   load8(x + i * 8, v);
   load8(dout + i * 8, d);
+  if constexpr (DROP) {
+    const uint32_t kb = drop.bits[(i / c8) * drop.row_bytes + col / 8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) d[j] *= philox::keep_z(kb, j, drop.scale);
+  }
   load8(nx + b * C + col, n8);
   load8(coef + b * C + col, k8);
   load8(gamma + col, g8);
@@ -481,24 +497,42 @@ int dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, const f
   return check_launch("dwconv_bwd");
 }
 
-// x bf16 (GEMM output before GELU), dout bf16, nx / sumsq fp32 [B,C] saved by the forward; s1_ws fp32 [B,C] scratch;
-// dx bf16; dgamma / dbeta [C] accumulate.
-int grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws, void* dx,
-            float* dgamma, float* dbeta, int B, int HW, int C, cudaStream_t s) {
+namespace {
+
+template <bool DROP>
+int launch_grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
+                   void* dx, float* dgamma, float* dbeta, int B, int HW, int C, const philox::ElemDrop& drop, cudaStream_t s) {
   if (B <= 0 || HW <= 0) return MUSE_OK;
   if (C % 8 != 0) { set_last_error("grn_bwd: C must be a multiple of 8"); return MUSE_ERR_UNSUPPORTED; }
   const bf16* xp = reinterpret_cast<const bf16*>(x);
   const bf16* dp = reinterpret_cast<const bf16*>(dout);
-  pdl_launch(dim3(ceil_div(C, 256), B), 128, 0, s)(grn_bwd_stats_kernel, xp, dp, nx, s1_ws, dgamma, dbeta, HW, C);
-  int rc = check_launch("grn_bwd_stats");
+  pdl_launch(dim3(ceil_div(C, 256), B), 128, 0, s)(grn_bwd_stats_kernel<DROP>, xp, dp, nx, s1_ws, dgamma, dbeta, HW, C, drop);
+  int rc = check_launch(DROP ? "grn_bwd_stats_dropout" : "grn_bwd_stats");
   if (rc) return rc;
   pdl_launch(B, 256, 0, s)(grn_bwd_finalize_kernel, s1_ws, sumsq, gamma, C);
   rc = check_launch("grn_bwd_finalize");
   if (rc) return rc;
   const long long total8 = static_cast<long long>(B) * HW * (C / 8);
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(grn_bwd_apply_kernel, xp, dp, nx, s1_ws, gamma,
-                                                                                       reinterpret_cast<bf16*>(dx), total8, HW, C);
-  return check_launch("grn_bwd_apply");
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(grn_bwd_apply_kernel<DROP>, xp, dp, nx, s1_ws, gamma,
+                                                                         reinterpret_cast<bf16*>(dx), total8, HW, C, drop);
+  return check_launch(DROP ? "grn_bwd_apply_dropout" : "grn_bwd_apply");
+}
+
+}  // namespace
+
+// x bf16 (GEMM output before GELU), dout bf16, nx / sumsq fp32 [B,C] saved by the forward; s1_ws fp32 [B,C] scratch;
+// dx bf16; dgamma / dbeta [C] accumulate.
+int grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws, void* dx,
+            float* dgamma, float* dbeta, int B, int HW, int C, cudaStream_t s) {
+  return launch_grn_bwd<false>(x, dout, nx, sumsq, gamma, s1_ws, dx, dgamma, dbeta, B, HW, C, philox::ElemDrop{}, s);
+}
+
+// backward of grn_fwd_dropout: dout (the gradient of the dropped output) is scaled by the bits as it is read
+int grn_bwd_dropout(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
+                    void* dx, float* dgamma, float* dbeta, const void* bits, float p, int B, int HW, int C, cudaStream_t s) {
+  if (bits == nullptr) { set_last_error("grn_bwd_dropout: bits are required"); return MUSE_ERR_INVALID; }
+  return launch_grn_bwd<true>(x, dout, nx, sumsq, gamma, s1_ws, dx, dgamma, dbeta, B, HW, C,
+                              philox::elem_drop(const_cast<void*>(bits), nullptr, 0, p, C), s);
 }
 
 int adaln_bwd(const float* dy, const float* x, const float* ss, long long ss_stride, float* dx, float* dss, int B,

@@ -334,7 +334,8 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         return W
 
     # ------------------------------------------------------------------------------------------- forward
-    def _forward_tokens(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds):
+    def _forward_tokens(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, drop=None):
+        """drop: the forward's dropout (p_hidden, p_attn, seed) in training mode, else None (uvit_v2_train.unit_drop)"""
         c = self.config
         if not input_ids.is_cuda:
             raise RuntimeError("open_muse_b200.MaskGiTUViT_v2 runs on CUDA (sm_90a) only; move inputs to the GPU")
@@ -363,9 +364,11 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
             hw, S = hw // 2, S // 4
             if dbg is not None:
                 dbg["downsample"] = h.view(B, hw, hw, -1).permute(0, 3, 1, 2).clone()
-        for w in W["down"]:
-            h, _ = T._res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=False)
-            h, _ = T._attn_block_fwd(h, enc, w, B, S, Skv, eps, rms)
+        R, L = len(W["down"]), len(W["layers"])
+        for j, w in enumerate(W["down"]):
+            dj = T.unit_drop(drop, j)
+            h, _ = T._res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=False, drop=dj)
+            h, _ = T._attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=dj)
         if dbg is not None:
             dbg["down"] = h.view(B, S, -1).clone()
         _, y = ops.add_norm_mod(h, W["pth_norm"], eps, rms, want_residual=False)
@@ -373,16 +376,17 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         if dbg is not None:
             dbg["hidden0"] = x.float().view(B, S, -1)
         for i, w in enumerate(W["layers"]):
-            x, r, _ = T._layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms)
+            x, r, _ = T._layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=T.unit_drop(drop, R + i))
             if dbg is not None:
                 dbg[f"layer{i}"] = (x.float() + r).view(B, S, -1)
         _, y = ops.add_norm_mod(x, W["pfh_norm"], eps, rms, residual=r, want_residual=False)  # (x + residual) -> norm (:289-291)
         h = ops.linear_fwd(y, W["pfh"], out_dtype=torch.float32)
         if dbg is not None:
             dbg["from_hidden"] = h.view(B, S, -1).clone()
-        for w in W["up"]:
-            h, _ = T._res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=False)
-            h, _ = T._attn_block_fwd(h, enc, w, B, S, Skv, eps, rms)
+        for j, w in enumerate(W["up"]):
+            dj = T.unit_drop(drop, R + L + j)
+            h, _ = T._res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=False, drop=dj)
+            h, _ = T._attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=dj)
         if dbg is not None:
             dbg["up"] = h.view(B, S, -1).clone()
         if "us" in W:  # (:555-559)
@@ -399,18 +403,23 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
                 loss_weight=None, _raw_bf16=False):
         c = self.config
         B, S = input_ids.shape
+        # nn.Dropout is active iff the module is in training mode (also under no_grad), each rate gating its own sites.
+        # One seed per forward, drawn on the device from torch's default generator as MaskGitTransformer does:
+        # torch.manual_seed reproduces the masks.  Site ids: uvit_v2_train.unit_drop.
+        drop = None
+        if self.training and (c.hidden_dropout > 0.0 or c.attention_dropout > 0.0):
+            seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=input_ids.device)
+            drop = (float(c.hidden_dropout), float(c.attention_dropout), seed)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             # training: one autograd Function per block, so parameter gradients appear during backward (DDP overlap)
-            if self.training and (c.hidden_dropout > 0.0 or c.attention_dropout > 0.0):
-                raise NotImplementedError("open_muse_b200.MaskGiTUViT_v2: dropout > 0 in training mode is not implemented")
             padded, loss = T.train_forward(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels,
-                                           label_smoothing, loss_weight)
+                                           label_smoothing, loss_weight, drop=drop)
             logits = padded.view(B, S, -1)[:, :, : c.codebook_size]
             if not (_raw_bf16 or torch.is_autocast_enabled()):
                 logits = logits.float()
             return logits if labels is None else (logits, loss)
         with torch.no_grad():
-            padded = self._forward_tokens(input_ids, encoder_hidden_states, cond_embeds, micro_conds)
+            padded = self._forward_tokens(input_ids, encoder_hidden_states, cond_embeds, micro_conds, drop=drop)
             V = c.codebook_size
             logits = padded.view(B, S, -1)[:, :, :V]
             if not (_raw_bf16 or torch.is_autocast_enabled()):
@@ -459,6 +468,10 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         """MaskGIT parallel decoding with classifier-free guidance, semantics of the reference (:330-479); per step one
         doubled-batch forward and ONE fused kernel (guidance mix, categorical sample, confidence, k-th cut, re-mask)."""
         c = self.config
+        if self.training and (c.hidden_dropout > 0.0 or c.attention_dropout > 0.0):
+            # the reference would sample with dropout applied to every forward of the decode loop
+            raise RuntimeError("generate2 on a MaskGiTUViT_v2 in training mode would sample with dropout > 0 active; "
+                               "call model.eval() first")
         B = encoder_hidden_states.shape[0]
         seq_len = 256 if seq_len is None else seq_len
         mask_id, K = c.mask_token_id, c.codebook_size

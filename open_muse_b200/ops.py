@@ -64,7 +64,8 @@ def _p(t):
 
 
 _KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_attn_bwd_dropout": 2, "muse_norm_bwd_glu_dropout": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
-                     "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3,
+                     "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3, "muse_grn_fwd_dropout": 3,
+                     "muse_grn_bwd_dropout": 3,
                      "muse_dwconv3x3_norm_bwd": 2}
 _prof = {"on": False, "events": []}
 
@@ -488,12 +489,21 @@ def dwconv3x3_norm(x, wk, norm_w, B, hh, ww, eps, rms, save_conv=False):
     return (y, conv) if save_conv else y
 
 
-def grn(x, gamma, beta, B, HW, save_stats=False):
-    """bf16 [B*HW, C] -> bf16: GELU + GlobalResponseNorm.  save_stats: also return (sumsq, nx) for grn_bwd."""
+def grn(x, gamma, beta, B, HW, save_stats=False, dropout=None):
+    """bf16 [B*HW, C] -> bf16: GELU + GlobalResponseNorm.  save_stats: also return (sumsq, nx) for grn_bwd.
+    dropout = (p, seed, site): the ResBlock's dropout that follows GRN fused into the pass (the output is the dropped one);
+    then returns (out, stats, bits) with bits int32 [B*HW, ceil(C / 32)] for grn_bwd (see dropout_fwd)."""
     st = _prep(x)
     C = x.shape[1]
     out = torch.empty_like(x)
     ws = torch.empty(2, B, C, dtype=torch.float32, device=x.device)
+    if dropout is not None:
+        p, seed, site = dropout
+        bits = torch.empty(B * HW, (C + 31) // 32, dtype=torch.int32, device=x.device)
+        _call("muse_grn_fwd_dropout", _p(x), _p(gamma), _p(beta), _p(out), _p(ws[0]), _p(ws[1]), _p(bits), _p(seed),
+              int(site), float(p), B, HW, C, st)
+        _drop_record(site, bits)
+        return out, ws, bits
     _call("muse_grn_fwd", _p(x), _p(gamma), _p(beta), _p(out), _p(ws[0]), _p(ws[1]), B, HW, C, st)
     return (out, ws) if save_stats else out
 
@@ -521,11 +531,17 @@ def dwconv3x3_norm_bwd(dy, conv, x, wk, norm_w, dres, dwk, dnw, B, hh, ww, eps, 
     return dx
 
 
-def grn_bwd(x, dout, stats, gamma, dgamma, dbeta, B, HW):
+def grn_bwd(x, dout, stats, gamma, dgamma, dbeta, B, HW, dropout=None):
+    """dropout = (p, bits) from grn(..., dropout=...): dout is scaled by the bits as the kernels read it."""
     st = _prep(x)
     C = x.shape[1]
     dx = torch.empty_like(x)
     ws = torch.empty(B, C, dtype=torch.float32, device=x.device)
+    if dropout is not None:
+        p, bits = dropout
+        _call("muse_grn_bwd_dropout", _p(x), _p(dout), _p(stats[1]), _p(stats[0]), _p(gamma), _p(ws), _p(dx), _p(dgamma),
+              _p(dbeta), _p(bits), float(p), B, HW, C, st)
+        return dx
     _call("muse_grn_bwd", _p(x), _p(dout), _p(stats[1]), _p(stats[0]), _p(gamma), _p(ws), _p(dx), _p(dgamma), _p(dbeta), B, HW,
           C, st)
     return dx

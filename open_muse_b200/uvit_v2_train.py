@@ -57,8 +57,33 @@ def _sub(G, W, key):
     return G[key]
 
 
+# ------------------------------------------------------------------------------------------------ dropout
+# nn.Dropout in training mode (ops.dropout_record documents the masks).  A block forward receives its unit's spec
+# ``drop = (p_hidden, p_attn, seed, first site)`` or None; unit j (down pairs, then layers, then up pairs) owns the site ids
+# 3 j .. 3 j + 2: a ResBlock + AttentionBlock2D pair uses 3 j for the ResBlock, 3 j + 1 for ``attention`` and 3 j + 2 for
+# ``crossattention``; a transformer layer 3 j for ``attention``, 3 j + 1 for ``crossattention`` and 3 j + 2 for the FFN.
+# A rate of 0 leaves its sites out.  The forward keeps (p, bits) of each active site in the state its backward unpacks.
+def unit_drop(drop, j):
+    """the spec of unit j from the forward's (p_hidden, p_attn, seed), or None when dropout is inactive"""
+    return None if drop is None else (*drop, 3 * j)
+
+
+def _site(drop, k, attn):
+    """(p, seed, site) of site k of a unit's spec, or None when that site is inactive"""
+    if drop is None:
+        return None
+    p = drop[1] if attn else drop[0]
+    return (p, drop[2], drop[3] + k) if p else None
+
+
+def _dkw(dr):
+    """the keyword a backward op takes for the (p, bits) a forward saved: none at all when the site was inactive"""
+    return {} if dr is None else {"dropout": dr}
+
+
 # ------------------------------------------------------------------------------------------------ attention helper
-def _attn_fwd(y, ctx_in, a, B, S, Skv, fused):
+def _attn_fwd(y, ctx_in, a, B, S, Skv, fused, drop=None):
+    """drop = (p, seed, site) of this attention's probabilities, or None"""
     Hc = a["o"].shape[0]
     if fused:
         qkv = ops.linear_fwd(y, a["qkv"])
@@ -69,65 +94,76 @@ def _attn_fwd(y, ctx_in, a, B, S, Skv, fused):
         kv = ops.linear_fwd(ctx_in, a["kv"])
         k, v = kv[:, :Hc], kv[:, Hc:]
         saved = (q, kv)
-    o, lse = ops.attn_fwd(q, k, v, B, a["nh"], S, Skv, a["sc"], head_dim=a["hd"])
-    return o, (saved, o, lse)
+    if drop is None:
+        o, lse = ops.attn_fwd(q, k, v, B, a["nh"], S, Skv, a["sc"], head_dim=a["hd"])
+        return o, (saved, o, lse, None)
+    o, lse, bits = ops.attn_fwd(q, k, v, B, a["nh"], S, Skv, a["sc"], head_dim=a["hd"], dropout=drop)
+    return o, (saved, o, lse, (drop[0], bits))
 
 
 def _attn_bwd(do, y, ctx_in, a, ga, st, B, S, Skv, fused, d_ctx_acc=None):
     """returns dy (bf16); the context gradient is accumulated into d_ctx_acc (fp32) for cross attention."""
-    saved, o, lse = st
+    saved, o, lse, dr = st
     Hc = a["o"].shape[0]
     if fused:
         qkv = saved
         dqkv = torch.empty_like(qkv)
         ops.attn_bwd(qkv[:, :Hc], qkv[:, Hc:2 * Hc], qkv[:, 2 * Hc:], o, do, lse, dqkv[:, :Hc], dqkv[:, Hc:2 * Hc],
-                     dqkv[:, 2 * Hc:], B, a["nh"], S, Skv, a["sc"], head_dim=a["hd"])
+                     dqkv[:, 2 * Hc:], B, a["nh"], S, Skv, a["sc"], head_dim=a["hd"], **_dkw(dr))
         return _lin_bwd(dqkv, y, a["qkv"], ga.of("qkv"))
     q, kv = saved
     dq, dkv = torch.empty_like(q), torch.empty_like(kv)
     ops.attn_bwd(q, kv[:, :Hc], kv[:, Hc:], o, do, lse, dq, dkv[:, :Hc], dkv[:, Hc:], B, a["nh"], S, Skv, a["sc"],
-                 head_dim=a["hd"])
+                 head_dim=a["hd"], **_dkw(dr))
     ops.linear_wgrad(dkv, ctx_in, ga.of("kv"))
     ops.linear_dgrad_acc(dkv, a["kv"], d_ctx_acc)
     return _lin_bwd(dq, y, a["q"], ga.of("q"))
 
 
 # ------------------------------------------------------------------------------------------------ blocks
-def _res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=True):
-    """save=False (inference): no conv output is written and adaLN modulates in place (no copy), so no state is returned."""
+def _res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=True, drop=None):
+    """save=False (inference): no conv output is written and adaLN modulates in place (no copy), so no state is returned.
+    drop: the unit's dropout spec -- channelwise[3] is fused into the GRN pass, whose dropped output is the cw4 operand
+    (and what the cw4 weight gradient reads)."""
     out = ops.dwconv3x3_norm(h, w["dw"], w["dw_norm"], B, hw, hw, eps, rms, save_conv=save)
     d, conv = out if save else (out, None)
     g1 = ops.linear_fwd(d, w["cw0"])
-    g2, stats = ops.grn(g1, w["gamma"], w["beta"], B, hw * hw, save_stats=True)
+    gd = _site(drop, 0, attn=False)
+    if gd is None:
+        g2, stats = ops.grn(g1, w["gamma"], w["beta"], B, hw * hw, save_stats=True)
+        gdr = None
+    else:
+        g2, stats, bits = ops.grn(g1, w["gamma"], w["beta"], B, hw * hw, save_stats=True, dropout=gd)
+        gdr = (gd[0], bits)
     h2 = ops.linear_fwd(g2, w["cw4"], res=h)  # + block input (fused residual epilogue)
     o, n = w["mod"]
     if not save:
         return ops.adaln_apply_(h2, mod_all[:, o:o + n], B, hw * hw), None
     h3 = ops.adaln_apply(h2, mod_all[:, o:o + n], B, hw * hw)
-    return h3, (h, d, conv, g1, g2, stats, h2)
+    return h3, (h, d, conv, g1, g2, stats, h2, gdr)
 
 
 def _res_block_bwd(dh3, st, w, g, mod_all, d_mod_all, B, hw, eps, rms):
-    h, d, conv, g1, g2, stats, h2 = st
+    h, d, conv, g1, g2, stats, h2, gdr = st
     o, n = w["mod"]
     dh2 = ops.adaln_bwd(dh3, h2, mod_all[:, o:o + n], d_mod_all[:, o:o + n], B, hw * hw)
     dg2 = _lin_bwd(ops.cast_bf16(dh2), g2, w["cw4"], g.of("cw4"))
-    dg1 = ops.grn_bwd(g1, dg2, stats, w["gamma"], g.of("gamma"), g.of("beta"), B, hw * hw)
+    dg1 = ops.grn_bwd(g1, dg2, stats, w["gamma"], g.of("gamma"), g.of("beta"), B, hw * hw, **_dkw(gdr))
     dd = _lin_bwd(dg1, d, w["cw0"], g.of("cw0"))
     return ops.dwconv3x3_norm_bwd(dd, conv, h, w["dw"], w["dw_norm"], dh2, g.of("dw"), g.of("dw_norm"), B, hw, hw, eps, rms)
 
 
-def _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms):
+def _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=None):
     se = encb = None
     if w["kvm"] is not None:
         se = ops.silu_bf16(enc)
         encb = ops.linear_fwd(se, w["kvm"])
     ctx_in = enc if encb is None else encb
     _, y1 = ops.add_norm_mod(h, w["ln1"], eps, rms, want_residual=False)
-    c1, s1 = _attn_fwd(y1, ctx_in, w["a1"], B, S, Skv, False)
+    c1, s1 = _attn_fwd(y1, ctx_in, w["a1"], B, S, Skv, False, _site(drop, 1, attn=True))
     a1o = ops.linear_fwd(c1, w["a1"]["o"])
     r2, y2 = ops.add_norm_mod(a1o, w["ln2"], eps, rms, residual=h)
-    c2, s2 = _attn_fwd(y2, ctx_in, w["a2"], B, S, Skv, False)
+    c2, s2 = _attn_fwd(y2, ctx_in, w["a2"], B, S, Skv, False, _site(drop, 2, attn=True))
     out = ops.linear_fwd(c2, w["a2"]["o"], res=r2)
     return out, (h, se, ctx_in, y1, c1, s1, r2, y2, c2, s2)
 
@@ -148,27 +184,32 @@ def _attn_block_bwd(dout, st, w, g, enc, d_enc, B, S, Skv, eps, rms):
     return dh
 
 
-def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms):
+def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=None):
     m = lambda k: mod_all[:, w[k][0]:w[k][0] + w[k][1]]
     r1, y1 = ops.add_norm_mod(x, w["ln1"], eps, rms, residual=r, mod=m("mod1"), rows_per_sample=S)
-    c, s_sa = _attn_fwd(y1, None, w["sa"], B, S, S, True)
+    c, s_sa = _attn_fwd(y1, None, w["sa"], B, S, S, True, _site(drop, 0, attn=True))
     a = ops.linear_fwd(c, w["sa"]["o"])
     r2, y2 = ops.add_norm_mod(a, w["ln2"], eps, rms, residual=r1, mod=m("mod2"), rows_per_sample=S)
-    cc, s_ca = _attn_fwd(y2, enc, w["ca"], B, S, Skv, False)
+    cc, s_ca = _attn_fwd(y2, enc, w["ca"], B, S, Skv, False, _site(drop, 1, attn=True))
     co = ops.linear_fwd(cc, w["ca"]["o"])
     r3, y3 = ops.add_norm_mod(co, w["ln3"], eps, 0, residual=r2, mod=m("mod3"), rows_per_sample=S)
     ab = ops.linear_fwd(y3, w["wi"])
-    gl = ops.glu_fwd(ab)
+    fd = _site(drop, 2, attn=False)
+    if fd is None:
+        gl, fdr = ops.glu_fwd(ab), None
+    else:  # GLUFeedForward.dropout fused into the GLU pass: gl is the dropped wo operand
+        gl, bits = ops.glu_fwd(ab, dropout=fd)
+        fdr = (fd[0], bits)
     f = ops.linear_fwd(gl, w["wo"])
-    return f, r3, (r is not None, r1, y1, c, s_sa, r2, y2, cc, s_ca, r3, y3, ab, gl)
+    return f, r3, (r is not None, r1, y1, c, s_sa, r2, y2, cc, s_ca, r3, y3, ab, gl, fdr)
 
 
 def _layer_bwd(df, dr3, st, w, g, enc, d_enc, mod_all, d_mod_all, B, S, Skv, eps, rms):
-    had_r, r1, y1, c, s_sa, r2, y2, cc, s_ca, r3, y3, ab, gl = st
+    had_r, r1, y1, c, s_sa, r2, y2, cc, s_ca, r3, y3, ab, gl, fdr = st
     m = lambda t, k: t[:, w[k][0]:w[k][0] + w[k][1]]
     gsa, gca = _sub(g, w, "sa"), _sub(g, w, "ca")
     dgl = _lin_bwd(df, gl, w["wo"], g.of("wo"))
-    dy3 = _lin_bwd(ops.glu_bwd(ab, dgl), y3, w["wi"], g.of("wi"))
+    dy3 = _lin_bwd(ops.glu_bwd(ab, dgl, **_dkw(fdr)), y3, w["wi"], g.of("wi"))
     dco, dr2 = ops.add_norm_mod_bwd(dy3, dr3, r3, w["ln3"], eps, 0, BF16, mod=m(mod_all, "mod3"), rows_per_sample=S,
                                     dw=g.of("ln3"), dmod=m(d_mod_all, "mod3"))
     dcc = _lin_bwd(dco, cc, w["ca"]["o"], gca.of("o"))
@@ -328,12 +369,12 @@ class UBlockFn(torch.autograd.Function):
     """ResBlock + AttentionBlock2D pair of the down / up stage"""
 
     @staticmethod
-    def forward(ctx, sh, model, which, idx, h, enc32, sc32, *params):
+    def forward(ctx, sh, model, which, idx, drop, h, enc32, sc32, *params):
         w = sh.W[which][idx]
         wl, w_map = _local_mods(sh, w, ["mod"])
         mod = ops.linear_fwd(sh.sc, w_map, out_dtype=F32)
-        h, s_r = _res_block_fwd(h, wl, mod, sh.B, sh.hw, sh.eps, sh.rms)
-        h, s_a = _attn_block_fwd(h, sh.enc, wl, sh.B, sh.S, sh.Skv, sh.eps, sh.rms)
+        h, s_r = _res_block_fwd(h, wl, mod, sh.B, sh.hw, sh.eps, sh.rms, drop=drop)
+        h, s_a = _attn_block_fwd(h, sh.enc, wl, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop)
         ctx.sh, ctx.sv, ctx.key = sh, (wl, w_map, mod, s_r, s_a), (model, which, idx)
         ctx.set_materialize_grads(False)
         return h
@@ -351,7 +392,7 @@ class UBlockFn(torch.autograd.Function):
         grads = [g["dw"].t().contiguous(), g.get("dw_norm"), g["cw0"], g["gamma"], g["beta"], g["cw4"], g_map, g.get("kvm"),
                  g.get("ln1")] + _attn_grads(g["a1"], ab.attention, False) + [g.get("ln2")] + _attn_grads(g["a2"], ab.crossattention, False)
         ctx.sv = None  # release the block's activations now, not when the graph dies
-        return (None, None, None, None, dh, d_enc, d_sc32, *_align(params, grads))
+        return (None, None, None, None, None, dh, d_enc, d_sc32, *_align(params, grads))
 
 
 def layer_params(l):
@@ -365,11 +406,11 @@ class ULayerFn(torch.autograd.Function):
     """one TransformerLayer carrying (hidden, residual)"""
 
     @staticmethod
-    def forward(ctx, sh, model, idx, x, r, enc32, sc32, *params):
+    def forward(ctx, sh, model, idx, drop, x, r, enc32, sc32, *params):
         w = sh.W["layers"][idx]
         wl, w_map = _local_mods(sh, w, ["mod1", "mod2", "mod3"])
         mod = ops.linear_fwd(sh.sc, w_map, out_dtype=F32)
-        f, r3, s_l = _layer_fwd(x, r, sh.enc, wl, mod, sh.B, sh.S, sh.Skv, sh.eps, sh.rms)
+        f, r3, s_l = _layer_fwd(x, r, sh.enc, wl, mod, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop)
         s_l = list(s_l)
         assert s_l[9] is r3
         s_l[9] = None  # r3 is an OUTPUT of this Function: held through save_for_backward, a ctx attribute would be a cycle
@@ -397,7 +438,7 @@ class ULayerFn(torch.autograd.Function):
             _attn_grads(g["ca"], l.crossattention, False) + [g_map[H2:2 * H2], g.get("ln3"), g_map[2 * H2:], g["wi"][:I], g["wi"][I:],
                                                              g["wo"]]
         ctx.sv = None  # release the block's activations now, not when the graph dies
-        return (None, None, None, dx, dr, d_enc, d_sc32, *_align(params, grads))
+        return (None, None, None, None, dx, dr, d_enc, d_sc32, *_align(params, grads))
 
 
 class ProjFn(torch.autograd.Function):
@@ -512,8 +553,10 @@ class TailFn(torch.autograd.Function):
         return None, None, dh, None, None, None, g1.reshape(ctx.shapes[0]), g_n, g2[: ctx.V].reshape(ctx.shapes[1])
 
 
-def train_forward(model, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels, label_smoothing, loss_weight):
-    """(logits_padded, loss) through the per-block Functions."""
+def train_forward(model, input_ids, encoder_hidden_states, cond_embeds, micro_conds, labels, label_smoothing, loss_weight,
+                  drop=None):
+    """(logits_padded, loss) through the per-block Functions.  drop: the forward's dropout (p_hidden, p_attn, seed) or
+    None (see unit_drop)."""
     from .modeling_transformer_v2 import sinusoidal_encode
 
     c = model.config
@@ -534,15 +577,16 @@ def train_forward(model, input_ids, encoder_hidden_states, cond_embeds, micro_co
         h = ResampleFn.apply(sh_full, "ds", h, down.downsample[0].norm.weight, down.downsample[1].weight)
         sh = copy.copy(sh_full)  # same operand caches (W, enc, sc), coarse grid
         sh.S, sh.hw = S // 4, sh_full.hw // 2
+    R, L = len(down.res_blocks), len(model.transformer_layers)
     for i, (rb, ab) in enumerate(zip(down.res_blocks, down.attention_blocks)):
-        h = UBlockFn.apply(sh, model, "down", i, h, enc32, sc32, *_present(block_params(rb, ab)))
+        h = UBlockFn.apply(sh, model, "down", i, unit_drop(drop, i), h, enc32, sc32, *_present(block_params(rb, ab)))
     x = ProjFn.apply(sh, "pth", h, None, model.project_to_hidden_norm.weight, model.project_to_hidden.weight)
     r = None
     for i, l in enumerate(model.transformer_layers):
-        x, r = ULayerFn.apply(sh, model, i, x, r, enc32, sc32, *_present(layer_params(l)))
+        x, r = ULayerFn.apply(sh, model, i, unit_drop(drop, R + i), x, r, enc32, sc32, *_present(layer_params(l)))
     h = ProjFn.apply(sh, "pfh", x, r, model.project_from_hidden_norm.weight, model.project_from_hidden.weight)
     for i, (rb, ab) in enumerate(zip(up.res_blocks, up.attention_blocks)):
-        h = UBlockFn.apply(sh, model, "up", i, h, enc32, sc32, *_present(block_params(rb, ab)))
+        h = UBlockFn.apply(sh, model, "up", i, unit_drop(drop, R + L + i), h, enc32, sc32, *_present(block_params(rb, ab)))
     if c.force_down_up_sample:  # back to the full grid (:555-559); sh still describes the coarse grid this op reads
         h = ResampleFn.apply(sh, "us", h, up.upsample[0].norm.weight, up.upsample[1].weight)
         sh = sh_full
