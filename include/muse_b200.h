@@ -8,6 +8,12 @@
  *   - allocate nothing: scratch and outputs are caller-provided;
  *   - return 0 (MUSE_OK) or a non-zero status; muse_last_error() gives the message (thread-local).
  * Dtype codes: 0 = float32, 1 = bfloat16.  "bf16" pointers are 16-bit bfloat16 arrays.
+ * Dropout (nn.Dropout(p) in training mode) is fused into the ops that take `bits`; bits == NULL means no dropout.  Keep
+ * masks come from Philox4x32-10 keyed by the 64-bit seed at *seed (device memory, so a captured graph draws a fresh seed per
+ * replay) with a per-forward unique site id; the mapping from (seed, site, coordinates) to bits and the rate (p_eff =
+ * round(p * 65536) / 65536, kept values scaled by 1 / (1 - p_eff)) are documented in csrc/philox.cuh.  A forward writes
+ * the bits (and needs seed), its backward reads them (no seed).  Masks are stored as uint32 words, rows padded to 32 bits,
+ * bit k % 32 of word k / 32 set = element k kept.
  */
 #ifndef MUSE_B200_H_
 #define MUSE_B200_H_
@@ -21,7 +27,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 5
+#define MUSE_B200_ABI_VERSION 6
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -109,9 +115,12 @@ int muse_embed_bwd_sorted(const long long* order, const long long* bounds, const
  *   y = (res ? res : 0) + norm(v) * w ; mean/rstd [rows] are saved for backward.  v = x (act 0), gelu(x) (act 1: the
  *   exact-erf GELU of MlmLayer :980-983) or, with act 2, x is [rows, 2H] = [a | b] and v = bf16(gelu(a)) * b: the
  *   FeedForward GLU product (:789-792) feeding mid_mlp_layer_norm (:795-796) without materialising it.
- *   rms = 1 selects RMSNorm. */
+ *   rms = 1 selects RMSNorm.
+ * bits (nullable; act 2, bf16 x / y, no res): FeedForward.dropout (:797) fused into the pass that produces the wo
+ * operand: y is the dropped output, bits [rows, ceil(H / 32)] written. */
 int muse_norm_fwd(const void* x, int x_dtype, const float* w, const float* res, void* y, int y_dtype, float* mean,
-                  float* rstd, int rows, int H, float eps, int act, int rms, void* stream);
+                  float* rstd, unsigned int* bits, const unsigned long long* seed, int site, float p, int rows, int H,
+                  float eps, int act, int rms, void* stream);
 /* dx = norm_bwd(dy) (* gelu'(x) if act 1) (+ dres if given).  Weight gradient dw[H] = sum_rows dy * xhat (nullable):
  *   dx_bf16_copy (nullable; fp32 dx, H <= 1024, no GLU): a bf16 copy of dx written in the same pass (the residual-stream
  *   gradient is the next GEMM operand).
@@ -119,10 +128,13 @@ int muse_norm_fwd(const void* x, int x_dtype, const float* w, const float* res, 
  *   bit-identical, no zero fill needed; dw_ws null: dw += ... with atomics (caller zero-fills; order-dependent).
  * act 2: dx is [rows, 2H] = d[a | b] (LayerNorm backward and GLU backward in one pass; v is recomputed from x).
  * y_fwd (nullable, act 2 with bf16 tensors only): the forward output bf16 [rows, H]; when given, the row reductions of
- * the first pass come from (dy, y_fwd) alone instead of re-evaluating the GELU over [a | b]. */
+ * the first pass come from (dy, y_fwd) alone instead of re-evaluating the GELU over [a | b].
+ * bits (nullable; act 2, bf16 dy / x / dx, no dres, no dx_bf16_copy, no y_fwd): the bits muse_norm_fwd wrote; dy (the
+ * gradient of the dropped output) is scaled by them as it is read and the GLU product is recomputed from [a | b]. */
 int muse_norm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, const float* w, const float* mean,
-                  const float* rstd, const float* dres, const void* y_fwd, void* dx, int dx_dtype, void* dx_bf16_copy,
-                  float* dw, float* dw_ws, int rows, int H, int act, int rms, void* stream);
+                  const float* rstd, const float* dres, const void* y_fwd, const unsigned int* bits, float p, void* dx,
+                  int dx_dtype, void* dx_bf16_copy, float* dw, float* dw_ws, int rows, int H, int act, int rms,
+                  void* stream);
 long long muse_norm_bwd_workspace_floats(int rows, int H, int act);
 
 /* Two chained norms of a normformer layer in one pass (muse/modeling_transformer.py:882-884 then :787):
@@ -136,60 +148,36 @@ int muse_norm2_bwd(const void* d_h2, const float* x2, const float* w2, const flo
                    const float* dres, const void* a, const float* w1, const float* mean1, const float* rstd1, float* dx2,
                    void* d_a, float* dw2, float* dw1, float* ws, int rows, int H, int rms1, int rms2, void* stream);
 
-/* GLU of FeedForward (:789-792): ab bf16 [rows, 2I] = [wi_0(x) | wi_1(x)], out bf16 [rows, I] = gelu(a) * b. */
-int muse_glu_fwd(const void* ab, void* out, long long rows, int I, void* stream);
-int muse_glu_bwd(const void* ab, const void* dout, void* dab, long long rows, int I, void* stream);
+/* GLU of FeedForward (:789-792): ab bf16 [rows, 2I] = [wi_0(x) | wi_1(x)], out bf16 [rows, I] = gelu(a) * b.
+ * bits (nullable): FeedForward.dropout (:797) fused into the pass (the model without the mid norm): out is the dropped
+ * output, bits [rows, ceil(I / 32)] written; the backward scales dout by them as it reads it. */
+int muse_glu_fwd(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
+                 long long rows, int I, void* stream);
+int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
+                 void* stream);
 
 /* Attention.attention (:221-241) fused: O = softmax(Q K^T * scale) V per (batch, head), head_dim 64 or 48
  * (configs/imagenet.yaml: hidden 768 / 16 heads).  Q/K/V/O are bf16 with row strides (elements) q_rs/k_rs/v_rs/o_rs, head h at
  * column offset h*head_dim,
- * batch b at row offset b*Sq (Q,O) or b*Skv (K,V).  lse fp32 [B,nh,Sq] is saved for backward. */
-int muse_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv,
-                  int head_dim, int q_rs, int k_rs, int v_rs, int o_rs, float scale, void* stream);
-/* dvec: fp32 scratch [B,nh,Sq]. */
-int muse_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                  float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int head_dim, int q_rs,
-                  int k_rs, int v_rs, int o_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale,
-                  void* stream);
+ * batch b at row offset b*Sq (Q,O) or b*Skv (K,V).  lse fp32 [B,nh,Sq] is saved for backward.
+ * bits (nullable): dropout on the probabilities (:236-237), bits [B, nh, Sq, ceil(Skv / 32)] written; the lse is that of
+ * the undropped probabilities. */
+int muse_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
+                  const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int head_dim,
+                  int q_rs, int k_rs, int v_rs, int o_rs, float scale, void* stream);
+/* dvec: fp32 scratch [B,nh,Sq].  bits (nullable): the bits muse_attn_fwd wrote. */
+int muse_attn_bwd(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
+                  const unsigned int* bits, float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq,
+                  int Skv, int head_dim, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs,
+                  float scale, void* stream);
 
-/* Dropout (nn.Dropout(p) in training mode).  Keep masks come from Philox4x32-10 keyed by the 64-bit seed at *seed (device
- * memory, so a captured graph draws a fresh seed per replay) with a per-forward unique site id; the mapping from
- * (seed, site, coordinates) to bits and the rate (p_eff = round(p * 65536) / 65536, kept values scaled by 1 / (1 - p_eff))
- * are documented in csrc/philox.cuh.  Masks are stored as uint32 words, rows padded to 32 bits, bit k % 32 of word
- * k / 32 set = element k kept.
- * Attention on the probabilities (:236-237): as muse_attn_fwd, plus bits [B, nh, Sq, ceil(Skv / 32)] written; the lse is
- * that of the undropped probabilities.  muse_attn_bwd_dropout reads the bits (no seed). */
-int muse_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
-                          const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int head_dim,
-                          int q_rs, int k_rs, int v_rs, int o_rs, float scale, void* stream);
-int muse_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
-                          const unsigned int* bits, float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh,
-                          int Sq, int Skv, int head_dim, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs,
-                          int dv_rs, float scale, void* stream);
-/* Elementwise (the embedding output, :956): y = x * keep / (1 - p_eff) over contiguous
- * [rows, cols] (cols % 8 == 0, dtype 0 fp32 / 1 bf16, y may alias x), bits [rows, ceil(cols / 32)] written;
+/* Dropout as a pass of its own (the embedding output, :956): y = x * keep / (1 - p_eff) over contiguous
+ * [rows, cols] (cols % 8 == 0, dtype 0 fp32 / 1 bf16, y may alias x), bits [rows, ceil(cols / 32)] written (required);
  * backward dx = dy * keep / (1 - p_eff) (dx may alias dy). */
 int muse_dropout_fwd(const void* x, void* y, int dtype, unsigned int* bits, const unsigned long long* seed, int site,
                      float p, long long rows, int cols, void* stream);
 int muse_dropout_bwd(const void* dy, void* dx, int dtype, const unsigned int* bits, float p, long long rows, int cols,
                      void* stream);
-
-/* FeedForward.dropout (:797) fused into the passes that produce / consume the wo operand (same masks, layout and rate as
- * muse_dropout_fwd, bits [rows, ceil(I / 32)]):
- *   muse_norm_fwd_glu_dropout / muse_norm_bwd_glu_dropout: muse_norm_fwd / muse_norm_bwd with act 2, bf16 x / y / dy / dx;
- *   the forward writes the dropped output and the bits, the backward scales dy by the bits as it reads it and recomputes the
- *   GLU product from [a | b] (dw / dw_ws as in muse_norm_bwd);
- *   muse_glu_fwd_dropout / muse_glu_bwd_dropout: muse_glu_fwd / muse_glu_bwd likewise (no mid norm). */
-int muse_norm_fwd_glu_dropout(const void* x, const float* w, void* y, float* mean, float* rstd, unsigned int* bits,
-                              const unsigned long long* seed, int site, float p, int rows, int H, float eps, int rms,
-                              void* stream);
-int muse_norm_bwd_glu_dropout(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,
-                              const unsigned int* bits, float p, void* dx, float* dw, float* dw_ws, int rows, int H, int rms,
-                              void* stream);
-int muse_glu_fwd_dropout(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
-                         long long rows, int I, void* stream);
-int muse_glu_bwd_dropout(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
-                         void* stream);
 
 /* F.cross_entropy(logits.view(-1,V), labels.view(-1), ignore_index=-100, label_smoothing) (:1276-1280).
  * logits bf16 [rows, ld] (ld >= V, multiple of 8). lse/row_loss: fp32 [rows] scratch (lse kept for bwd).
@@ -217,9 +205,12 @@ int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* norm_w
                             int w, int C, float eps, int rms, void* stream);  /* conv_out (nullable) bf16: saved for bwd */
 /* nn.GELU + GlobalResponseNorm (:741-751) on x bf16 [B, HW, C]: g = gelu(x), Gx = ||g||_2 over the HW tokens,
  * Nx = Gx / (mean_c Gx + 1e-6), out = gamma * (g * Nx) + beta + g (bf16).  sumsq_ws (Gx^2) and nx_ws: fp32 [B, C],
- * left filled for muse_grn_bwd. */
-int muse_grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* sumsq_ws, float* nx_ws, int B,
-                 int HW, int C, void* stream);
+ * left filled for muse_grn_bwd.  bits (nullable): the ResBlock's nn.Dropout between GlobalResponseNorm and channelwise[4]
+ * (:603-609) fused into the pass: out = bf16(fp32 GRN output * keep / (1 - p_eff)), bits [B * HW, ceil(C / 32)] written
+ * (row = token). */
+int muse_grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* sumsq_ws, float* nx_ws,
+                 unsigned int* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C,
+                 void* stream);
 /* AdaLNModulation at the end of a ResBlock (:617): x fp32 [B*rows_per_sample, C] *= (1 + scale_b), += shift_b, in place. */
 int muse_adaln_apply(float* x, const float* scale_shift, long long ss_stride, int B, int rows_per_sample, int C,
                      void* stream);
@@ -237,19 +228,11 @@ int muse_add_norm_mod_bwd(const void* dy, int dy_dtype, const float* dr_out, con
 int muse_dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, const float* wk, const float* norm_w,
                             const float* dres, float* dc_ws, float* dx, float* dwk, float* dnorm_w, int B, int h, int w,
                             int C, float eps, int rms, void* stream);
-/* x = forward input (bf16), dout bf16, nx / sumsq from the forward, s1_ws fp32 [B,C] scratch -> dx bf16; dgamma, dbeta +=. */
+/* x = forward input (bf16), dout bf16, nx / sumsq from the forward, s1_ws fp32 [B,C] scratch -> dx bf16; dgamma, dbeta +=.
+ * bits (nullable): the bits muse_grn_fwd wrote; dout (the gradient of the dropped output) is scaled by them as it is read. */
 int muse_grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
-                 void* dx, float* dgamma, float* dbeta, int B, int HW, int C, void* stream);
-/* The ResBlock's nn.Dropout between GlobalResponseNorm and channelwise[4] (:603-609) fused into the GRN passes (masks,
- * layout and rate as muse_dropout_fwd; row = token of the B * HW rows, bits [B * HW, ceil(C / 32)]):
- *   muse_grn_fwd_dropout: muse_grn_fwd, then out = bf16(fp32 GRN output * keep / (1 - p_eff)) and the bits written;
- *   muse_grn_bwd_dropout: muse_grn_bwd with dout (the gradient of the dropped output) scaled by the bits as it is read. */
-int muse_grn_fwd_dropout(const void* x, const float* gamma, const float* beta, void* out, float* sumsq_ws, float* nx_ws,
-                         unsigned int* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C,
-                         void* stream);
-int muse_grn_bwd_dropout(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma,
-                         float* s1_ws, void* dx, float* dgamma, float* dbeta, const unsigned int* bits, float p, int B,
-                         int HW, int C, void* stream);
+                 void* dx, float* dgamma, float* dbeta, const unsigned int* bits, float p, int B, int HW, int C,
+                 void* stream);
 /* y = x * (1 + scale_b) + shift_b: dx = dy * (1 + scale_b); dscale_shift[b] += (sum dy * x | sum dy). */
 int muse_adaln_bwd(const float* dy, const float* x, const float* scale_shift, long long ss_stride, float* dx,
                    float* dscale_shift, int B, int rows_per_sample, int C, void* stream);

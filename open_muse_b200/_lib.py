@@ -35,33 +35,25 @@ SIGNATURES = {
     "muse_embed_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "muse_embed_bwd_sorted_workspace_bytes": (c_longlong, [_I, _I, _I]),
     "muse_embed_bwd_sorted": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
-    "muse_norm_fwd": (c_int, [_P, _I, _P, _P, _P, _I, _P, _P, _I, _I, _F, _I, _I, _P]),
-    "muse_norm_bwd": (c_int, [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "muse_norm_fwd": (c_int, [_P, _I, _P, _P, _P, _I, _P, _P, _P, _P, _I, _F, _I, _I, _F, _I, _I, _P]),
+    "muse_norm_bwd": (c_int, [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _F, _P, _I, _P, _P, _P, _I, _I, _I, _I, _P]),
     "muse_norm_bwd_workspace_floats": (c_longlong, [_I, _I, _I]),
     "muse_norm2_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _F, _I, _I, _P]),
     "muse_norm2_bwd": (c_int, [_P] * 15 + [_I, _I, _I, _I, _P]),
-    "muse_glu_fwd": (c_int, [_P, _P, _L, _I, _P]),
-    "muse_glu_bwd": (c_int, [_P, _P, _P, _L, _I, _P]),
-    "muse_attn_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
-    "muse_attn_bwd": (c_int, [_P] * 10 + [_I] * 13 + [_F, _P]),
-    "muse_attn_fwd_dropout": (c_int, [_P] * 7 + [_I, _F] + [_I] * 9 + [_F, _P]),
-    "muse_attn_bwd_dropout": (c_int, [_P] * 6 + [_F] + [_P] * 4 + [_I] * 12 + [_F, _P]),
+    "muse_glu_fwd": (c_int, [_P, _P, _P, _P, _I, _F, _L, _I, _P]),
+    "muse_glu_bwd": (c_int, [_P, _P, _P, _F, _P, _L, _I, _P]),
+    "muse_attn_fwd": (c_int, [_P] * 7 + [_I, _F] + [_I] * 9 + [_F, _P]),
+    "muse_attn_bwd": (c_int, [_P] * 6 + [_F] + [_P] * 4 + [_I] * 12 + [_F, _P]),
     "muse_dropout_fwd": (c_int, [_P, _P, _I, _P, _P, _I, _F, _L, _I, _P]),
     "muse_dropout_bwd": (c_int, [_P, _P, _I, _P, _F, _L, _I, _P]),
-    "muse_norm_fwd_glu_dropout": (c_int, [_P] * 7 + [_I, _F, _I, _I, _F, _I, _P]),
-    "muse_norm_bwd_glu_dropout": (c_int, [_P] * 6 + [_F] + [_P] * 3 + [_I, _I, _I, _P]),
-    "muse_glu_fwd_dropout": (c_int, [_P, _P, _P, _P, _I, _F, _L, _I, _P]),
-    "muse_glu_bwd_dropout": (c_int, [_P, _P, _P, _F, _P, _L, _I, _P]),
     "muse_ce_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),
     "muse_ce_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),
     "muse_add_norm_mod_fwd": (c_int, [_P, _I, _P, _P, _P, _L, _I, _P, _P, _I, _I, _I, _F, _I, _P]),
     "muse_dwconv3x3_norm_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
-    "muse_grn_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "muse_grn_fwd": (c_int, [_P] * 8 + [_I, _F, _I, _I, _I, _P]),
     "muse_add_norm_mod_bwd": (c_int, [_P, _I, _P, _P, _P, _P, _L, _I, _P, _I, _P, _P, _P, _I, _I, _F, _I, _P]),
     "muse_dwconv3x3_norm_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
-    "muse_grn_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
-    "muse_grn_fwd_dropout": (c_int, [_P] * 8 + [_I, _F, _I, _I, _I, _P]),
-    "muse_grn_bwd_dropout": (c_int, [_P] * 10 + [_F, _I, _I, _I, _P]),
+    "muse_grn_bwd": (c_int, [_P] * 10 + [_F, _I, _I, _I, _P]),
     "muse_adaln_bwd": (c_int, [_P, _P, _P, _L, _P, _P, _I, _I, _I, _P]),
     "muse_silu_bwd": (c_int, [_P, _P, _I, _P, _I, _L, _I, _P]),
     "muse_adaln_apply": (c_int, [_P, _P, _L, _I, _I, _I, _P]),
@@ -85,7 +77,7 @@ SIGNATURES = {
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class MuseB200Error(RuntimeError):

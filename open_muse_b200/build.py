@@ -80,7 +80,7 @@ def build_xcheck(verbose: bool = False, force: bool = False) -> Path:
     out_dir = src_dir / "build"
     out_dir.mkdir(parents=True, exist_ok=True)
     sources = sorted(src_dir.glob("*.cu"))
-    headers = [CSRC / "common.cuh"]
+    headers = [CSRC / "common.cuh", PKG_DIR.parent / "include" / "muse_b200.h"]
     objs, jobs = [], []
     for src in sources:
         obj = out_dir / (src.stem + ".o")

@@ -635,62 +635,46 @@ int check_args(const char* who, int hd, int a, int b, int c) {
   return MUSE_OK;
 }
 
-int fwd_dispatch(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
-                 int q_rs, int k_rs, int v_rs, int o_rs, float scale, const Drop& d, cudaStream_t s) {
+}  // namespace
+}  // namespace muse
+
+using namespace muse;
+
+extern "C" {
+
+// Entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its autograd
+// backward, head_dim 64 or 48, no mask; with bits, nn.Dropout(p) is applied to the probabilities (:236-237) with the keep
+// bits of philox.cuh (the DROP = true kernels).
+int muse_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
+                  const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int hd, int q_rs,
+                  int k_rs, int v_rs, int o_rs, float scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (bits != nullptr && seed == nullptr) { set_last_error("attn_fwd: dropout needs a seed"); return MUSE_ERR_INVALID; }
   if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
   int rc = check_args("attn_fwd", hd, q_rs | o_rs, k_rs, v_rs);
   if (rc) return rc;
-  if (d.bits == nullptr)
+  const Drop d{bits, seed, site, p};
+  if (bits == nullptr)
     return hd == 64 ? attn_fwd_impl<64, false>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
                     : attn_fwd_impl<48, false>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s);
   return hd == 64 ? attn_fwd_impl<64, true>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
                   : attn_fwd_impl<48, true>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s);
 }
 
-int bwd_dispatch(const void* q, const void* k, const void* v, const void* d_o, const float* lse, float* dvec, void* dq,
-                 void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs, int v_rs, int o_rs,
-                 int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, const Drop& d, cudaStream_t s) {
+// D is recomputed from (P, dP) inside the dQ kernel, so the backward does not read O.
+int muse_attn_bwd(const void* q, const void* k, const void* v, const void* d_o, const float* lse, const unsigned int* bits,
+                  float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs,
+                  int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (B <= 0 || Sq <= 0 || Skv <= 0) return MUSE_OK;
-  int rc = check_args("attn_bwd", hd, q_rs | o_rs | do_rs | dq_rs, k_rs | dk_rs, v_rs | dv_rs);
+  int rc = check_args("attn_bwd", hd, q_rs | do_rs | dq_rs, k_rs | dk_rs, v_rs | dv_rs);
   if (rc) return rc;
+  const Drop d{const_cast<unsigned int*>(bits), nullptr, 0, p};
 #define MUSE_ATTN_BWD(HD, DROP) \
   attn_bwd_impl<HD, DROP>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs, dk_rs, dv_rs, scale, d, s)
-  if (d.bits == nullptr) return hd == 64 ? MUSE_ATTN_BWD(64, false) : MUSE_ATTN_BWD(48, false);
+  if (bits == nullptr) return hd == 64 ? MUSE_ATTN_BWD(64, false) : MUSE_ATTN_BWD(48, false);
   return hd == 64 ? MUSE_ATTN_BWD(64, true) : MUSE_ATTN_BWD(48, true);
 #undef MUSE_ATTN_BWD
 }
 
-}  // namespace
-
-// Entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its autograd
-// backward, head_dim 64 or 48, no mask; the _dropout variants apply nn.Dropout(p) to the probabilities (:236-237) with
-// the keep bits of philox.cuh.
-int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int nh, int Sq, int Skv, int hd,
-             int q_rs, int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
-  return fwd_dispatch(q, k, v, o, lse, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, o_rs, scale, Drop{}, s);
-}
-
-int attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, uint32_t* bits,
-                     const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int hd, int q_rs,
-                     int k_rs, int v_rs, int o_rs, float scale, cudaStream_t s) {
-  if (bits == nullptr || seed == nullptr) { set_last_error("attn_fwd_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
-  return fwd_dispatch(q, k, v, o, lse, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, o_rs, scale, Drop{bits, seed, site, p}, s);
-}
-
-int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-             float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs, int k_rs,
-             int v_rs, int o_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s) {
-  (void)o;  // D is recomputed from (P, dP) inside the dQ kernel; O is not needed by backward
-  return bwd_dispatch(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs,
-                      dv_rs, scale, Drop{}, s);
-}
-
-int attn_bwd_dropout(const void* q, const void* k, const void* v, const void* d_o, const float* lse, const uint32_t* bits,
-                     float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq, int Skv, int hd, int q_rs,
-                     int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs, float scale, cudaStream_t s) {
-  if (bits == nullptr) { set_last_error("attn_bwd_dropout: bits are required"); return MUSE_ERR_INVALID; }
-  return bwd_dispatch(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, hd, q_rs, k_rs, v_rs, q_rs, do_rs, dq_rs, dk_rs,
-                      dv_rs, scale, Drop{const_cast<uint32_t*>(bits), nullptr, 0, p}, s);
-}
-
-}  // namespace muse
+}  // extern "C"

@@ -5,10 +5,9 @@
 #include <math.h>
 #include <stdint.h>
 
-#define MUSE_OK 0
-#define MUSE_ERR_INVALID 1
-#define MUSE_ERR_CUDA 2
-#define MUSE_ERR_UNSUPPORTED 3
+// Status codes, and the declaration of every entry point: each file defines its muse_* functions at global scope in an
+// extern "C" block, so a definition whose parameter types differ from the header's does not compile.
+#include "../../include/muse_b200.h"
 
 namespace muse {
 

@@ -317,8 +317,41 @@ transpose_cp_kernel(const float* __restrict__ in, float* __restrict__ out, int r
 
 }  // namespace
 
-int conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H, int W,
-                int Cin, int Cout, int ksize, int upsample2x, cudaStream_t s) {
+// Decoder output -> display bytes with the reference's recipe (muse/pipeline_muse.py:245-252, quirk Q10), same fp32 operation
+// order so the bytes are identical: t = 2x - 1; t = clip(t, -1, 1); t = (t + 1) / 2; byte = (uint8)(255 * t)  (truncation).
+// Input is the decoder's native NHWC tensor, output HWC uint8 per image: the NCHW round trip of the reference
+// (decode -> permute(1, 2, 0) -> numpy) and the 4x larger fp32 device->host copy disappear.
+__global__ void __launch_bounds__(256)
+image_to_uint8_kernel(const float* __restrict__ x, unsigned char* __restrict__ y, long long n4) {
+  pdl_enter();
+  const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (i >= n4) return;
+  const float4 v = *reinterpret_cast<const float4*>(x + i * 4);
+  const float f[4] = {v.x, v.y, v.z, v.w};
+  uchar4 o;
+  unsigned char* ob = reinterpret_cast<unsigned char*>(&o);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    float t = __fsub_rn(__fmul_rn(2.0f, f[k]), 1.0f);
+    t = fminf(fmaxf(t, -1.0f), 1.0f);
+    t = __fdiv_rn(__fadd_rn(t, 1.0f), 2.0f);
+    ob[k] = static_cast<unsigned char>(static_cast<int>(__fmul_rn(255.0f, t)));  // truncation toward zero, values in [0, 255]
+  }
+  *reinterpret_cast<uchar4*>(y + i * 4) = o;
+}
+
+// workspace: partials float [nblocks*B*C*2] with nblocks = ceil(HW / rows_per_block) (see muse_groupnorm_workspace_floats)
+static int gn_rows_per_block(int C) { return (256 / (C / 4)) * 64; }
+
+}  // namespace muse
+
+using namespace muse;
+
+extern "C" {
+
+int muse_conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H, int W,
+                     int Cin, int Cout, int ksize, int upsample2x, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (ksize != 1 && ksize != 3) { set_last_error("conv2d: kernel size %d unsupported (1 or 3)", ksize); return MUSE_ERR_UNSUPPORTED; }
   if (upsample2x == 1 && ((H | W) & 1)) { set_last_error("conv2d: upsample2x needs even output dims"); return MUSE_ERR_INVALID; }
   if (upsample2x == 2 && ksize != 3) { set_last_error("conv2d: the stride-2 mode is the 3x3 taming Downsample"); return MUSE_ERR_INVALID; }
@@ -337,18 +370,16 @@ int conv2d_nhwc(const float* x, const float* wk, const float* bias, const float*
   return check_launch("conv2d_nhwc");
 }
 
-// workspace: partials float [nblocks*B*C*2] with nblocks = ceil(HW / rows_per_block) (see gn_workspace_floats)
-static int gn_rows_per_block(int C) { return (256 / (C / 4)) * 64; }
-
-long long gn_workspace_floats(int B, int HW, int C) {
+long long muse_groupnorm_workspace_floats(int B, int HW, int C) {
   if (C % 4 != 0 || C > 1024 || 256 % (C / 4) != 0) return -1;
   return static_cast<long long>(ceil_div(HW, gn_rows_per_block(C))) * B * C * 2;
 }
 
 // y (fp32) or y_hi / y_lo (bf16 split planes) receive the result: exactly one of the two forms must be given.
-int groupnorm_silu_nhwc(const float* x, const float* gamma, const float* beta, float* y, void* y_hi, void* y_lo,
-                        float* partials_ws, float* scale_shift_ws, int B, int HW, int C, int groups, float eps,
-                        int precomputed_tiles, int apply_silu, cudaStream_t s) {
+int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* beta, float* y, void* y_hi, void* y_lo,
+                             float* partials_ws, float* scale_shift_ws, int B, int HW, int C, int groups, float eps,
+                             int precomputed_tiles, int apply_silu, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if ((y != nullptr) == (y_hi != nullptr) || (y_hi == nullptr && y_lo != nullptr)) {
     set_last_error("groupnorm: give either y (fp32) or y_hi (+ y_lo unless the single-pass bf16 mode is used)");
     return MUSE_ERR_INVALID;
@@ -387,37 +418,16 @@ int groupnorm_silu_nhwc(const float* x, const float* gamma, const float* beta, f
   return check_launch("gn_apply_silu");
 }
 
-// Decoder output -> display bytes with the reference's recipe (muse/pipeline_muse.py:245-252, quirk Q10), same fp32 operation
-// order so the bytes are identical: t = 2x - 1; t = clip(t, -1, 1); t = (t + 1) / 2; byte = (uint8)(255 * t)  (truncation).
-// Input is the decoder's native NHWC tensor, output HWC uint8 per image: the NCHW round trip of the reference
-// (decode -> permute(1, 2, 0) -> numpy) and the 4x larger fp32 device->host copy disappear.
-__global__ void __launch_bounds__(256)
-image_to_uint8_kernel(const float* __restrict__ x, unsigned char* __restrict__ y, long long n4) {
-  pdl_enter();
-  const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
-  if (i >= n4) return;
-  const float4 v = *reinterpret_cast<const float4*>(x + i * 4);
-  const float f[4] = {v.x, v.y, v.z, v.w};
-  uchar4 o;
-  unsigned char* ob = reinterpret_cast<unsigned char*>(&o);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    float t = __fsub_rn(__fmul_rn(2.0f, f[k]), 1.0f);
-    t = fminf(fmaxf(t, -1.0f), 1.0f);
-    t = __fdiv_rn(__fadd_rn(t, 1.0f), 2.0f);
-    ob[k] = static_cast<unsigned char>(static_cast<int>(__fmul_rn(255.0f, t)));  // truncation toward zero, values in [0, 255]
-  }
-  *reinterpret_cast<uchar4*>(y + i * 4) = o;
-}
-
-int image_to_uint8(const float* x, unsigned char* y, long long n, cudaStream_t s) {
+int muse_image_to_uint8(const float* x, unsigned char* y, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
   if (n % 4 != 0) { set_last_error("image_to_uint8: element count must be a multiple of 4"); return MUSE_ERR_INVALID; }
   pdl_launch(static_cast<unsigned>(ceil_div_ll(n / 4, 256)), 256, 0, s)(image_to_uint8_kernel, x, y, n / 4);
   return check_launch("image_to_uint8");
 }
 
-int avgpool2_nhwc(const float* x, float* y, int B, int Ho, int Wo, int C, cudaStream_t s) {
+int muse_avgpool2_nhwc(const float* x, float* y, int B, int Ho, int Wo, int C, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (C % 4 != 0) { set_last_error("avgpool: C must be a multiple of 4"); return MUSE_ERR_UNSUPPORTED; }
   const long long total = static_cast<long long>(B) * Ho * Wo * (C / 4);
   if (total <= 0) return MUSE_OK;
@@ -426,10 +436,11 @@ int avgpool2_nhwc(const float* x, float* y, int B, int Ho, int Wo, int C, cudaSt
 }
 
 // in: [B, rows, cols] -> out: [B, cols, rows]
-int transpose_batched(const float* in, float* out, int B, int rows, int cols, cudaStream_t s) {
+int muse_transpose_batched(const float* in, float* out, int B, int rows, int cols, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (B <= 0 || rows <= 0 || cols <= 0) return MUSE_OK;
   pdl_launch(dim3(ceil_div(cols, 32), ceil_div(rows, 32), B), 256, 0, s)(transpose_cp_kernel, in, out, rows, cols);
   return check_launch("transpose_batched");
 }
 
-}  // namespace muse
+}  // extern "C"

@@ -319,24 +319,29 @@ int launch_conv(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap&
 }
 
 }  // namespace
+}  // namespace muse
 
-// 1 if conv2d_tc handles the shape (otherwise the caller uses the fp32 SIMT kernel of conv.cu).
-int conv2d_tc_supported(int H, int W, int Cin, int Cout, int ksize) {
-  if (ksize != 1 && ksize != 3 && ksize != 2) return 0;  // 2: the 2x2 forward-offset window (mode 2 of conv2d_tc)
+using namespace muse;
+
+extern "C" {
+
+// 1 if muse_conv2d_nhwc_tc handles the shape (otherwise the caller uses the fp32 SIMT kernel of conv.cu).
+int muse_conv2d_tc_supported(int H, int W, int Cin, int Cout, int ksize) {
+  if (ksize != 1 && ksize != 3 && ksize != 2) return 0;  // 2: the 2x2 forward-offset window (mode 2 of muse_conv2d_nhwc_tc)
   if (Cin % 64 != 0 || Cout < 1 || (Cout > 16 && Cout % 4 != 0)) return 0;
   if (W >= 128) return W % 128 == 0;
   if (W < 8 || 128 % W != 0) return 0;
   return H % (128 / W) == 0;
 }
 
-// Pixel tiles per image of conv2d_tc for this shape (= the leading extent of its stats output), 0 if unsupported.
+// Pixel tiles per image of muse_conv2d_nhwc_tc for this shape (= the leading extent of its stats output), 0 if unsupported.
 // H, W are the OUTPUT dims; with upsample2x the tiling runs on the H/2 x W/2 input grid, four parities each.
-int conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int upsample2x) {
+int muse_conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int upsample2x) {
   if (upsample2x) {
     if ((H | W) & 1 || ksize != 3 || Cout <= 16) return 0;
     H /= 2; W /= 2;
   }
-  if (!conv2d_tc_supported(H, W, Cin, Cout, ksize)) return 0;
+  if (!muse_conv2d_tc_supported(H, W, Cin, Cout, ksize)) return 0;
   return (upsample2x ? 4 : 1) * (H * W / 128);
 }
 
@@ -348,20 +353,21 @@ int conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int up
 // mode & 8: single-pass bf16 (fast tokenizer mode): only the hi planes are multiplied (x_lo / w_lo may be null): one tensor-core
 //   product per fp32 product instead of three, bf16-operand accuracy (~4e-3 per layer instead of ~2e-5).
 // x_hi/x_lo: bf16 [B,H,W,Cin]; w_hi/w_lo: bf16 [Cout, k*k*Cin] (tap-major, then input channel); y fp32 [B,H,W,Cout].
-int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias, const float* res,
-              float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode, cudaStream_t s) {
+int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias, const float* res,
+                        float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (B <= 0) return MUSE_OK;
   const int upsample2x = (mode & 3) == 1;
   const int fwd2x2 = (mode & 3) == 2;
   if (fwd2x2 != (ksize == 2)) { set_last_error("conv2d_tc: ksize 2 and mode 2 go together"); return MUSE_ERR_INVALID; }
   if (upsample2x) {
-    if (conv2d_tc_tiles_per_image(H, W, Cin, Cout, ksize, 1) == 0) {
+    if (muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, ksize, 1) == 0) {
       set_last_error("conv2d_tc: unsupported upsample shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W, Cin, Cout, ksize);
       return MUSE_ERR_UNSUPPORTED;
     }
     H /= 2; W /= 2;  // the tiling / TMA grid is the input grid
   }
-  if (!conv2d_tc_supported(H, W, Cin, Cout, ksize)) {
+  if (!muse_conv2d_tc_supported(H, W, Cin, Cout, ksize)) {
     set_last_error("conv2d_tc: unsupported shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W, Cin, Cout, ksize);
     return MUSE_ERR_UNSUPPORTED;
   }
@@ -414,7 +420,8 @@ int conv2d_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* 
 }
 
 // x fp32 [B,H,W,Cin] with k*k*Cin <= 64 -> hi, lo bf16 [B,H,W,64]: row = the k*k*Cin taps of the pixel (tap-major), zero padded
-int im2col_split_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int Cin, int ksize, cudaStream_t s) {
+int muse_im2col_split_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int Cin, int ksize, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (ksize * ksize * Cin > 64 || (ksize != 1 && ksize != 3)) {
     set_last_error("im2col_split: k*k*Cin = %d must be <= 64", ksize * ksize * Cin);
     return MUSE_ERR_UNSUPPORTED;
@@ -427,7 +434,8 @@ int im2col_split_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, i
 }
 
 // x fp32 [B,2Ho,2Wo,C] -> hi, lo bf16 [B,Ho,Wo,4C]
-int split_s2d_bf16_nhwc(const float* x, void* hi, void* lo, int B, int Ho, int Wo, int C, cudaStream_t s) {
+int muse_split_s2d_bf16_nhwc(const float* x, void* hi, void* lo, int B, int Ho, int Wo, int C, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (C % 8 != 0) { set_last_error("split_s2d: C must be a multiple of 8"); return MUSE_ERR_UNSUPPORTED; }
   const long long total8 = static_cast<long long>(B) * Ho * Wo * 4 * (C / 8);
   if (total8 <= 0) return MUSE_OK;
@@ -437,7 +445,8 @@ int split_s2d_bf16_nhwc(const float* x, void* hi, void* lo, int B, int Ho, int W
 }
 
 // out_f32 given: plain fp32 softmax (hi / lo unused); else the bf16 hi/lo planes
-int softmax_split_rows(const float* x, void* hi, void* lo, float* out_f32, long long rows, int n, float scale, cudaStream_t s) {
+int muse_softmax_split_rows(const float* x, void* hi, void* lo, float* out_f32, long long rows, int n, float scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0 || n <= 0) return MUSE_OK;
   if (out_f32 == x) { set_last_error("softmax: in-place output is not supported"); return MUSE_ERR_INVALID; }
   pdl_launch(static_cast<unsigned>(ceil_div_ll(rows, 8)), 256, 0, s)(softmax_split_kernel, x, reinterpret_cast<bf16*>(hi),
@@ -446,7 +455,8 @@ int softmax_split_rows(const float* x, void* hi, void* lo, float* out_f32, long 
 }
 
 // x fp32 [B, H/(1+up), W/(1+up), C] -> hi, lo bf16 [B,H,W,C]
-int split_bf16_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int C, int upsample2x, cudaStream_t s) {
+int muse_split_bf16_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int C, int upsample2x, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (C % 8 != 0) { set_last_error("split_bf16: C must be a multiple of 8"); return MUSE_ERR_UNSUPPORTED; }
   if (upsample2x && ((H | W) & 1)) { set_last_error("split_bf16: upsample2x needs even output dims"); return MUSE_ERR_INVALID; }
   const long long total8 = static_cast<long long>(B) * H * W * (C / 8);
@@ -456,4 +466,4 @@ int split_bf16_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int
   return check_launch("split_bf16");
 }
 
-}  // namespace muse
+}  // extern "C"

@@ -361,9 +361,15 @@ dropout_bwd_kernel(const T* dy, T* dx, const uint8_t* __restrict__ bits, float s
 }
 
 }  // namespace
+}  // namespace muse
 
-int dropout_fwd(const void* x, void* y, int dtype, uint32_t* bits, const unsigned long long* seed, int site, float p,
-                long long rows, int cols, cudaStream_t s) {
+using namespace muse;
+
+extern "C" {
+
+int muse_dropout_fwd(const void* x, void* y, int dtype, unsigned int* bits, const unsigned long long* seed, int site,
+                     float p, long long rows, int cols, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (cols % 8 != 0) { set_last_error("dropout_fwd: cols=%d must be a multiple of 8", cols); return MUSE_ERR_INVALID; }
   if (bits == nullptr || seed == nullptr) { set_last_error("dropout_fwd: bits and seed are required"); return MUSE_ERR_INVALID; }
   const int row_bytes = 4 * ceil_div(cols, 32);
@@ -382,7 +388,9 @@ int dropout_fwd(const void* x, void* y, int dtype, uint32_t* bits, const unsigne
   return check_launch("dropout_fwd");
 }
 
-int dropout_bwd(const void* dy, void* dx, int dtype, const uint32_t* bits, float p, long long rows, int cols, cudaStream_t s) {
+int muse_dropout_bwd(const void* dy, void* dx, int dtype, const unsigned int* bits, float p, long long rows, int cols,
+                     void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (cols % 8 != 0) { set_last_error("dropout_bwd: cols=%d must be a multiple of 8", cols); return MUSE_ERR_INVALID; }
   const long long n = rows * (cols / 8);
   if (n <= 0) return MUSE_OK;
@@ -399,13 +407,15 @@ int dropout_bwd(const void* dy, void* dx, int dtype, const uint32_t* bits, float
   return check_launch("dropout_bwd");
 }
 
-int pack_bf16(const void* table_dev, int n_entries, long long total_blocks, cudaStream_t s) {
+int muse_pack_bf16(const void* table_dev, int n_entries, long long total_blocks, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n_entries <= 0 || total_blocks <= 0) return MUSE_OK;
   pdl_launch(static_cast<unsigned>(total_blocks), 256, 0, s)(pack_bf16_kernel, reinterpret_cast<const PackEntry*>(table_dev), n_entries);
   return check_launch("pack_bf16");
 }
 
-int cast_bf16(const float* src, void* dst, long long n, cudaStream_t s) {
+int muse_cast_bf16(const float* src, void* dst, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
   if (n % 8 != 0) { set_last_error("cast_bf16: n=%lld must be a multiple of 8", n); return MUSE_ERR_INVALID; }
   const long long n8 = n / 8;
@@ -413,8 +423,9 @@ int cast_bf16(const float* src, void* dst, long long n, cudaStream_t s) {
   return check_launch("cast_bf16");
 }
 
-int embed_fwd(const long long* ids, const float* word, const float* pos, float* out, int B, int S, int H, int vocab,
-              cudaStream_t s) {
+int muse_embed_fwd(const long long* ids, const float* word, const float* pos, float* out, int B, int S, int H, int vocab,
+                   void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (H % 4 != 0) { set_last_error("embed_fwd: H must be a multiple of 4"); return MUSE_ERR_INVALID; }
   const int tokens = B * S;
   if (tokens <= 0) return MUSE_OK;
@@ -422,8 +433,9 @@ int embed_fwd(const long long* ids, const float* word, const float* pos, float* 
   return check_launch("embed_fwd");
 }
 
-int embed_bwd(const long long* ids, const float* dx, float* dword, float* dpos, int B, int S, int H, int vocab,
-              cudaStream_t s) {
+int muse_embed_bwd(const long long* ids, const float* dx, float* dword, float* dpos, int B, int S, int H, int vocab,
+                   void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (H % 4 != 0) { set_last_error("embed_bwd: H must be a multiple of 4"); return MUSE_ERR_INVALID; }
   const int tokens = B * S;
   if (tokens <= 0) return MUSE_OK;
@@ -442,12 +454,13 @@ int embed_bwd(const long long* ids, const float* dx, float* dword, float* dpos, 
 }
 
 // workspace: (tokens / kSegChunk + vocab) partial rows of H floats, then vocab + 1 ints of chunk offsets
-long long embed_bwd_sorted_workspace_bytes(int tokens, int H, int vocab) {
+long long muse_embed_bwd_sorted_workspace_bytes(int tokens, int H, int vocab) {
   return (static_cast<long long>(tokens) / kSegChunk + vocab) * H * 4 + (static_cast<long long>(vocab) + 1) * 4;
 }
 
-int embed_bwd_sorted(const long long* order, const long long* bounds, const float* dx, float* dword, float* dpos,
-                     void* ws, int B, int S, int H, int vocab, cudaStream_t s) {
+int muse_embed_bwd_sorted(const long long* order, const long long* bounds, const float* dx, float* dword, float* dpos,
+                          void* ws, int B, int S, int H, int vocab, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (H % 4 != 0) { set_last_error("embed_bwd_sorted: H must be a multiple of 4"); return MUSE_ERR_INVALID; }
   const int tokens = B * S;
   if (tokens <= 0 || vocab <= 0) return MUSE_OK;
@@ -468,43 +481,30 @@ int embed_bwd_sorted(const long long* order, const long long* bounds, const floa
   return check_launch("embed_bwd_pos");
 }
 
-int glu_fwd(const void* ab, void* out, long long rows, int I, cudaStream_t s) {
+// bits == nullptr: no dropout; else FeedForward.dropout fused into the pass, bits [rows, ceil(I / 32)] written.
+int muse_glu_fwd(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
+                 long long rows, int I, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (I % 8 != 0) { set_last_error("glu_fwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
+  if (bits != nullptr && seed == nullptr) { set_last_error("glu_fwd: dropout needs a seed"); return MUSE_ERR_INVALID; }
   const long long n = rows * (I / 8);
   if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_fwd_kernel<false>, reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, philox::ElemDrop{});
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? glu_fwd_kernel<true> : glu_fwd_kernel<false>,
+      reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, philox::elem_drop(bits, seed, site, p, I));
   return check_launch("glu_fwd");
 }
 
-int glu_fwd_dropout(const void* ab, void* out, void* bits, const unsigned long long* seed, int site, float p, long long rows,
-                    int I, cudaStream_t s) {
-  if (I % 8 != 0) { set_last_error("glu_fwd_dropout: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
-  if (bits == nullptr || seed == nullptr) { set_last_error("glu_fwd_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
-  const long long n = rows * (I / 8);
-  if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_fwd_kernel<true>, reinterpret_cast<const bf16*>(ab),
-      reinterpret_cast<bf16*>(out), rows, I, philox::elem_drop(bits, seed, site, p, I));
-  return check_launch("glu_fwd_dropout");
-}
-
-int glu_bwd_dropout(const void* ab, const void* dout, const void* bits, float p, void* dab, long long rows, int I,
-                    cudaStream_t s) {
-  if (I % 8 != 0) { set_last_error("glu_bwd_dropout: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
-  if (bits == nullptr) { set_last_error("glu_bwd_dropout: bits are required"); return MUSE_ERR_INVALID; }
-  const long long n = rows * (I / 8);
-  if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_bwd_kernel<true>, reinterpret_cast<const bf16*>(ab),
-      reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I,
-      philox::elem_drop(const_cast<void*>(bits), nullptr, 0, p, I));
-  return check_launch("glu_bwd_dropout");
-}
-
-int glu_bwd(const void* ab, const void* dout, void* dab, long long rows, int I, cudaStream_t s) {
+// bits: those muse_glu_fwd wrote (nullptr: no dropout); dout is scaled by them as it is read.
+int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
+                 void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (I % 8 != 0) { set_last_error("glu_bwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
   const long long n = rows * (I / 8);
   if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(glu_bwd_kernel<false>, reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I, philox::ElemDrop{});
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? glu_bwd_kernel<true> : glu_bwd_kernel<false>,
+      reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I,
+      philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, I));
   return check_launch("glu_bwd");
 }
 
-}  // namespace muse
+}  // extern "C"

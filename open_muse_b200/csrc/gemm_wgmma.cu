@@ -277,11 +277,6 @@ int launch_major(int a_mn, int b_mn, int epi, const GemmMaps& m, const GemmParam
 
 }  // namespace
 
-// The persistent GEMM owns one CTA per SM with a static tile assignment, so a CTA that cannot start (its SM is held by an
-// NCCL all-reduce CTA during data-parallel training) delays the whole kernel by its full duration.  Under DDP the host
-// reserves as many SMs as NCCL has channels: the GEMM grid shrinks by that many CTAs and both kernels fit side by side.
-void set_reserved_sms(int n) { g_reserved_sms = n < 0 ? 0 : n; }
-
 // C[M,N] (ldc) = op(A) * op(B)^T with op selected by a_mn / b_mn:
 //   a_mn == 0: A points at a row-major [M, K] matrix (pitch lda);  a_mn == 1: at a row-major [K, M] matrix.
 //   b_mn == 0: B points at a row-major [N, K] matrix (pitch ldb);  b_mn == 1: at a row-major [K, N] matrix.
@@ -300,15 +295,8 @@ static void split_plan(int M, int N, int K, int* num_m, int* num_n, int* num_kb,
   *splits = ceil_div(*num_kb, *kb_per_split);
 }
 
-long long gemm_splitk_workspace_bytes(int M, int N, int K) {
-  int num_m, num_n, num_kb, kbs, splits, bn;
-  split_plan(M, N, K, &num_m, &num_n, &num_kb, &kbs, &splits, &bn);
-  if (splits <= 1) return 0;
-  return static_cast<long long>(splits) * num_m * num_n * BM * bn * 4;
-}
-
-int gemm_tc(const void* A, const void* B, void* C, const float* res, int M, int N, int K, int lda, int ldb,
-                 int ldc, int a_mn, int b_mn, int epi, cudaStream_t stream, void* ws, long long ws_bytes) {
+static int gemm_tc(const void* A, const void* B, void* C, const float* res, int M, int N, int K, int lda, int ldb,
+                   int ldc, int a_mn, int b_mn, int epi, cudaStream_t stream, void* ws, long long ws_bytes) {
   if (M <= 0 || N <= 0 || K <= 0) return MUSE_OK;
   if (epi == EPI_BF16 ? (ldc % 8 != 0) : (ldc % 4 != 0)) {
     set_last_error("gemm: ldc=%d must be a multiple of %d", ldc, epi == EPI_BF16 ? 8 : 4);
@@ -373,3 +361,37 @@ int gemm_tc(const void* A, const void* B, void* C, const float* res, int M, int 
 }
 
 }  // namespace muse
+
+using namespace muse;
+
+extern "C" {
+
+// The persistent GEMM owns one CTA per SM with a static tile assignment, so a CTA that cannot start (its SM is held by an
+// NCCL all-reduce CTA during data-parallel training) delays the whole kernel by its full duration.  Under DDP the host
+// reserves as many SMs as NCCL has channels: the GEMM grid shrinks by that many CTAs and both kernels fit side by side.
+int muse_reserve_sms(int n) {
+  g_reserved_sms = n < 0 ? 0 : n;
+  return MUSE_OK;
+}
+
+int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int M, int N, int K, int lda, int ldb,
+                   int ldc, int a_mn, int b_mn, int epilogue, void* stream) {
+  if (epilogue == MUSE_EPI_RESADD_F32 && res == nullptr) { set_last_error("gemm: RESADD epilogue needs res"); return MUSE_ERR_INVALID; }
+  if (epilogue == MUSE_EPI_SPLITK_F32) { set_last_error("gemm: the deterministic split-K epilogue goes through muse_gemm_bf16_splitk"); return MUSE_ERR_INVALID; }
+  return gemm_tc(A, B, C, res, M, N, K, lda, ldb, ldc, a_mn, b_mn, epilogue, static_cast<cudaStream_t>(stream), nullptr, 0);
+}
+
+long long muse_gemm_splitk_workspace_bytes(int M, int N, int K) {
+  int num_m, num_n, num_kb, kbs, splits, bn;
+  split_plan(M, N, K, &num_m, &num_n, &num_kb, &kbs, &splits, &bn);
+  if (splits <= 1) return 0;
+  return static_cast<long long>(splits) * num_m * num_n * BM * bn * 4;
+}
+
+int muse_gemm_bf16_splitk(const void* A, const void* B, float* C, int M, int N, int K, int lda, int ldb, int ldc,
+                          int a_mn, int b_mn, void* ws, long long ws_bytes, void* stream) {
+  return gemm_tc(A, B, C, nullptr, M, N, K, lda, ldb, ldc, a_mn, b_mn, MUSE_EPI_SPLITK_F32, static_cast<cudaStream_t>(stream),
+                 ws, ws_bytes);
+}
+
+}  // extern "C"

@@ -132,9 +132,15 @@ ce_bwd_kernel(const bf16* __restrict__ logits, const long long* __restrict__ lab
 }
 
 }  // namespace
+}  // namespace muse
 
-int ce_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* loss_out, int rows, int V,
-           int ld, float ls, cudaStream_t s) {
+using namespace muse;
+
+extern "C" {
+
+int muse_ce_fwd(const void* logits, const long long* labels, float* lse, float* row_loss, float* loss_out, int rows, int V,
+                int ld, float ls, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (ld % 8 != 0 || ld < V) { set_last_error("ce_fwd: ld=%d must be a multiple of 8 and >= V=%d", ld, V); return MUSE_ERR_INVALID; }
   pdl_launch(ceil_div(rows, 4), 128, 0, s)(ce_fwd_kernel, reinterpret_cast<const bf16*>(logits), labels, lse, row_loss, rows, V, ld, ls);
@@ -144,12 +150,13 @@ int ce_fwd(const void* logits, const long long* labels, float* lse, float* row_l
   return check_launch("ce_reduce");
 }
 
-int ce_bwd(const void* logits, const long long* labels, const float* lse, const float* dloss, const float* loss_cnt,
-           const float* row_scale, void* dlogits, int rows, int V, int ld, float ls, cudaStream_t s) {
+int muse_ce_bwd(const void* logits, const long long* labels, const float* lse, const float* dloss, const float* loss_cnt,
+                const float* row_scale, void* dlogits, int rows, int V, int ld, float ls, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (ld % 8 != 0 || ld < V) { set_last_error("ce_bwd: ld=%d must be a multiple of 8 and >= V=%d", ld, V); return MUSE_ERR_INVALID; }
   pdl_launch(ceil_div(rows, 4), 128, 0, s)(ce_bwd_kernel, reinterpret_cast<const bf16*>(logits), labels, lse, dloss, loss_cnt, row_scale, reinterpret_cast<bf16*>(dlogits), rows, V, ld, ls);
   return check_launch("ce_bwd");
 }
 
-}  // namespace muse
+}  // extern "C"

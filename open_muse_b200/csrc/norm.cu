@@ -963,17 +963,31 @@ int check_args(const char* who, int H, int act, const void* res_or_dres) {
 }
 
 }  // namespace
+}  // namespace muse
+
+using namespace muse;
+
+extern "C" {
 
 // dtype codes: 0 = fp32, 1 = bf16.  act: 0 none, 1 GELU(x), 2 GLU (x is [rows, 2H]).
-int norm_fwd(const void* x, int x_dt, const float* w, const float* res, void* y, int y_dt, float* mean, float* rstd,
-             int rows, int H, float eps, int act, int rms, cudaStream_t s) {
+// bits (act 2, bf16 in and out): FeedForward.dropout fused into the GLU + mid norm pass, y is the dropped output and bits
+// [rows, ceil(H / 32)] uint32 words are written (philox.cuh elementwise mapping, seed read from *seed).
+int muse_norm_fwd(const void* x, int x_dt, const float* w, const float* res, void* y, int y_dt, float* mean, float* rstd,
+                  unsigned int* bits, const unsigned long long* seed, int site, float p, int rows, int H, float eps,
+                  int act, int rms, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   int rc = check_args("norm_fwd", H, act, res);
   if (rc) return rc;
+  if (bits != nullptr && (act != ACT_GLU || x_dt != 1 || y_dt != 1 || seed == nullptr)) {
+    set_last_error("norm_fwd: dropout needs act 2, bf16 x and y, and a seed");
+    return MUSE_ERR_INVALID;
+  }
   if (act == ACT_GLU && x_dt == 1 && y_dt == 1 && H <= 4096) {
+    const philox::ElemDrop drop = philox::elem_drop(bits, seed, site, p, H);
     const int grid = ceil_div(rows, kGluWarps);
     const int ch = ceil_div(H, 256);
-#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(glu_norm_fwd_kernel<CH, false>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, philox::ElemDrop{})
+#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(bits ? glu_norm_fwd_kernel<CH, true> : glu_norm_fwd_kernel<CH, false>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop)
     if (ch <= 1) MUSE_GF(1); else if (ch <= 2) MUSE_GF(2); else if (ch <= 4) MUSE_GF(4); else if (ch <= 8) MUSE_GF(8); else MUSE_GF(16);
 #undef MUSE_GF
     return check_launch("glu_norm_fwd");
@@ -987,8 +1001,9 @@ int norm_fwd(const void* x, int x_dt, const float* w, const float* res, void* y,
 }
 
 // x2 = res + norm1(a) * w1 ; h2 = norm2(x2) * w2  (a bf16 [rows,H], res / x2 fp32, h2 bf16; H % 8 == 0, H <= 1024)
-int norm2_fwd(const void* a, const float* res, const float* w1, const float* w2, float* x2, void* h2, float* mean1,
-              float* rstd1, float* mean2, float* rstd2, int rows, int H, float eps, int rms1, int rms2, cudaStream_t s) {
+int muse_norm2_fwd(const void* a, const float* res, const float* w1, const float* w2, float* x2, void* h2, float* mean1,
+                   float* rstd1, float* mean2, float* rstd2, int rows, int H, float eps, int rms1, int rms2, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024 || H < 8) { set_last_error("norm2_fwd: H=%d must be a multiple of 8 in [8, 1024]", H); return MUSE_ERR_UNSUPPORTED; }
   const int grid = ceil_div(rows, kWarpsPerBlock);
@@ -1000,9 +1015,10 @@ int norm2_fwd(const void* a, const float* res, const float* w1, const float* w2,
 }
 
 // ws: 2 * norm_bwd_workspace_floats(rows, H, 0) floats (dw2 partial rows, then dw1 partial rows); dw2 / dw1 are STORED.
-int norm2_bwd(const void* d_h2, const float* x2, const float* w2, const float* mean2, const float* rstd2, const float* dres,
-              const void* a, const float* w1, const float* mean1, const float* rstd1, float* dx2, void* d_a, float* dw2,
-              float* dw1, float* ws, int rows, int H, int rms1, int rms2, cudaStream_t s) {
+int muse_norm2_bwd(const void* d_h2, const float* x2, const float* w2, const float* mean2, const float* rstd2, const float* dres,
+                   const void* a, const float* w1, const float* mean1, const float* rstd1, float* dx2, void* d_a, float* dw2,
+                   float* dw1, float* ws, int rows, int H, int rms1, int rms2, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024 || H < 8) { set_last_error("norm2_bwd: H=%d must be a multiple of 8 in [8, 1024]", H); return MUSE_ERR_UNSUPPORTED; }
   const int grid = bwd_grid(rows, H, 0);
@@ -1027,30 +1043,37 @@ int norm2_bwd(const void* d_h2, const float* x2, const float* w2, const float* m
 }
 
 // floats of workspace a deterministic (dw_ws != nullptr) backward needs: one partial row of H per CTA
-long long norm_bwd_workspace_floats(int rows, int H, int act) {
+long long muse_norm_bwd_workspace_floats(int rows, int H, int act) {
   if (rows <= 0) return 0;
   return static_cast<long long>(bwd_grid(rows, H, act)) * H;
 }
 
-int norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* w, const float* mean, const float* rstd,
-             const float* dres, const void* y_fwd, void* dx, int dx_dt, void* dx_copy, float* dw, float* dw_ws, int rows,
-             int H, int act, int rms, cudaStream_t s) {
+int muse_norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* w, const float* mean, const float* rstd,
+                  const float* dres, const void* y_fwd, const unsigned int* bits, float p, void* dx, int dx_dt,
+                  void* dx_copy, float* dw, float* dw_ws, int rows, int H, int act, int rms, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   int rc = check_args("norm_bwd", H, act, dres);
   if (rc) return rc;
   if (dx_copy && (dx_dt != 0 || act == ACT_GLU)) { set_last_error("norm_bwd: dx_copy needs an fp32 dx and no GLU"); return MUSE_ERR_INVALID; }
+  // with bits, dy is the gradient of the dropped output: scaled by the bits as it is read, the GLU product recomputed
+  if (bits != nullptr && (act != ACT_GLU || dy_dt != 1 || x_dt != 1 || dx_dt != 1 || y_fwd != nullptr)) {
+    set_last_error("norm_bwd: dropout needs act 2, bf16 dy, x and dx, and no y_fwd");
+    return MUSE_ERR_INVALID;
+  }
   if (act == ACT_GLU && dy_dt == 1 && x_dt == 1 && dx_dt == 1 && H <= 4096) {
     const int grid = bwd_grid(rows, H, act);
     const size_t smem = dw ? static_cast<size_t>(kGluWarps) * H * sizeof(float) : 0;
+    const philox::ElemDrop drop = philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, H);
     glu_bwd_smem_attr();
     if (y_fwd != nullptr)
       pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<true, false>,
           reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-          dw_ws, reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, kRowPrefetch, philox::ElemDrop{});
+          dw_ws, reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, kRowPrefetch, drop);
     else
-      pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<false, false>,
+      pdl_launch(grid, kGluWarps * 32, smem, s)(bits ? glu_norm_bwd_kernel<false, true> : glu_norm_bwd_kernel<false, false>,
           reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-          dw_ws, nullptr, rows, H, rms, 0, philox::ElemDrop{});
+          dw_ws, nullptr, rows, H, rms, 0, drop);
     rc = check_launch("glu_norm_bwd");
     if (rc || !dw || !dw_ws) return rc;
     return reduce_dw(dw_ws, dw, grid, H, s);
@@ -1070,43 +1093,4 @@ int norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* w,
   return MUSE_ERR_INVALID;
 }
 
-// act = 2 (GLU + mid norm, bf16 in and out) with FeedForward.dropout fused: y is the dropped output, bits [rows,
-// ceil(H / 32)] uint32 words written (philox.cuh elementwise mapping, seed read from *seed).
-int norm_fwd_glu_dropout(const void* x, const float* w, void* y, float* mean, float* rstd, void* bits,
-                         const unsigned long long* seed, int site, float p, int rows, int H, float eps, int rms,
-                         cudaStream_t s) {
-  if (rows <= 0) return MUSE_OK;
-  int rc = check_args("norm_fwd_glu_dropout", H, ACT_GLU, nullptr);
-  if (rc) return rc;
-  if (bits == nullptr || seed == nullptr) { set_last_error("norm_fwd_glu_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
-  const philox::ElemDrop drop = philox::elem_drop(bits, seed, site, p, H);
-  const int grid = ceil_div(rows, kGluWarps);
-  const int ch = ceil_div(H, 256);
-#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(glu_norm_fwd_kernel<CH, true>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop)
-  if (ch <= 1) MUSE_GF(1); else if (ch <= 2) MUSE_GF(2); else if (ch <= 4) MUSE_GF(4); else if (ch <= 8) MUSE_GF(8); else MUSE_GF(16);
-#undef MUSE_GF
-  return check_launch("glu_norm_fwd_dropout");
-}
-
-// its backward: dy (gradient of the dropped output) is scaled by the bits as it is read; the GLU product is recomputed
-// from [a | b].  dw / dw_ws as in norm_bwd.
-int norm_bwd_glu_dropout(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,
-                         const void* bits, float p, void* dx, float* dw, float* dw_ws, int rows, int H, int rms,
-                         cudaStream_t s) {
-  if (rows <= 0) return MUSE_OK;
-  int rc = check_args("norm_bwd_glu_dropout", H, ACT_GLU, nullptr);
-  if (rc) return rc;
-  if (bits == nullptr) { set_last_error("norm_bwd_glu_dropout: bits are required"); return MUSE_ERR_INVALID; }
-  const philox::ElemDrop drop = philox::elem_drop(const_cast<void*>(bits), nullptr, 0, p, H);
-  const int grid = bwd_grid(rows, H, ACT_GLU);
-  const size_t smem = dw ? static_cast<size_t>(kGluWarps) * H * sizeof(float) : 0;
-  glu_bwd_smem_attr();
-  pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<false, true>,
-      reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-      dw_ws, nullptr, rows, H, rms, 0, drop);
-  rc = check_launch("glu_norm_bwd_dropout");
-  if (rc || !dw || !dw_ws) return rc;
-  return reduce_dw(dw_ws, dw, grid, H, s);
-}
-
-}  // namespace muse
+}  // extern "C"

@@ -116,14 +116,20 @@ adamw_ema_pack_kernel(const __grid_constant__ OptChunk chunk, const float* __res
 }
 
 }  // namespace
+}  // namespace muse
+
+using namespace muse;
+
+extern "C" {
 
 // entries_host: HOST array of n_entries {p, g, m, v, ema, packed, numel, unused} (8 x int64 each; device pointers inside);
 // scal_dev: 8 floats; step_dev: one int64 (number of optimizer steps taken so far); lr_dev: nullable device float
 // (graph-capturable learning-rate schedule) else lr_host is used.
-int adamw_ema_step(const void* entries_host, int n_entries, float* scal_dev, long long* step_dev,
-                   const float* lr_dev, float lr_host, float beta1, float beta2, float eps, float weight_decay,
-                   int ema_enabled, float ema_decay, float ema_min_decay, int ema_update_after_step, int ema_update_every,
-                   int ema_use_warmup, float ema_inv_gamma, float ema_power, cudaStream_t s) {
+int muse_adamw_ema_step(const void* entries_host, int n_entries, float* scal_dev, long long* step_dev,
+                        const float* lr_dev, float lr_host, float beta1, float beta2, float eps, float weight_decay,
+                        int ema_enabled, float ema_decay, float ema_min_decay, int ema_update_after_step, int ema_update_every,
+                        int ema_use_warmup, float ema_inv_gamma, float ema_power, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n_entries <= 0) return MUSE_OK;
   OptHyper h;
   h.beta1 = beta1; h.beta2 = beta2; h.eps = eps; h.weight_decay = weight_decay;
@@ -151,4 +157,4 @@ int adamw_ema_step(const void* entries_host, int n_entries, float* scal_dev, lon
   return MUSE_OK;
 }
 
-}  // namespace muse
+}  // extern "C"

@@ -137,11 +137,17 @@ sample_remask_kernel(const long long* __restrict__ input_ids, const long long* _
 }
 
 }  // namespace
+}  // namespace muse
 
-int sample_step(const void* logits, const void* logits_unc, long long row_stride, long long batch_stride,
-                float guidance, const long long* input_ids, const float* q_exp, const float* u,
-                long long* sampled, long long* next_ids, float* conf_out, int B, int L, int K, long long mask_id,
-                int mask_len, float temperature, cudaStream_t s) {
+using namespace muse;
+
+extern "C" {
+
+int muse_sample_step(const void* logits, const void* logits_unc, long long row_stride, long long batch_stride,
+                     float guidance, const long long* input_ids, const float* q_exp, const float* u,
+                     long long* sampled, long long* next_ids, float* conf_out, int B, int L, int K, long long mask_id,
+                     int mask_len, float temperature, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (B <= 0 || L <= 0) return MUSE_OK;
   if (L > 4096) { set_last_error("sample_step: L=%d too long (max 4096)", L); return MUSE_ERR_UNSUPPORTED; }
   if (conf_out == nullptr) { set_last_error("sample_step: conf_out (B*L floats) is required"); return MUSE_ERR_INVALID; }
@@ -156,4 +162,4 @@ int sample_step(const void* logits, const void* logits_unc, long long row_stride
   return check_launch("sample_remask");
 }
 
-}  // namespace muse
+}  // extern "C"

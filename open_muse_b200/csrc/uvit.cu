@@ -281,10 +281,16 @@ int launch_add_norm(const void* a, const float* r, const float* w, const float* 
 }
 
 }  // namespace
+}  // namespace muse
 
-int add_norm_mod_fwd(const void* a, int a_dt, const float* r, const float* w, const float* ss, long long ss_stride,
-                     int rows_per_sample, float* r_out, void* y, int y_dt, int rows, int H, float eps, int rms,
-                     cudaStream_t s) {
+using namespace muse;
+
+extern "C" {
+
+int muse_add_norm_mod_fwd(const void* a, int a_dt, const float* r, const float* w, const float* ss, long long ss_stride,
+                          int rows_per_sample, float* r_out, void* y, int y_dt, int rows, int H, float eps, int rms,
+                          void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024) { set_last_error("add_norm_mod: H=%d must be a multiple of 8 and <= 1024", H); return MUSE_ERR_UNSUPPORTED; }
   if (ss != nullptr && (rows_per_sample <= 0 || ss_stride % 4 != 0)) { set_last_error("add_norm_mod: bad modulation layout"); return MUSE_ERR_INVALID; }
@@ -297,8 +303,9 @@ int add_norm_mod_fwd(const void* a, int a_dt, const float* r, const float* w, co
   return MUSE_ERR_INVALID;
 }
 
-int dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y, void* conv_out, int B, int hh, int ww,
-                       int C, float eps, int rms, cudaStream_t s) {
+int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y, void* conv_out, int B, int hh, int ww,
+                            int C, float eps, int rms, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const long long pixels = static_cast<long long>(B) * hh * ww;
   if (pixels <= 0) return MUSE_OK;
   if (C % 8 != 0 || C > 1024) { set_last_error("dwconv3x3_norm: C=%d must be a multiple of 8 and <= 1024", C); return MUSE_ERR_UNSUPPORTED; }
@@ -312,11 +319,14 @@ int dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y
   return check_launch("dwconv3x3_norm");
 }
 
-namespace {
-
-template <bool DROP>
-int launch_grn(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws, int B, int HW,
-               int C, const philox::ElemDrop& drop, cudaStream_t s) {
+// x bf16 [B, HW, C] -> out bf16 [B, HW, C]; sumsq_ws / nx_ws fp32 [B, C] (kept by the caller for the backward pass).
+// bits != nullptr: the ResBlock's dropout (:607) fused into the apply pass, out is the dropped output and bits
+// [B * HW, ceil(C / 32)] uint32 words are written (philox.cuh elementwise mapping, seed read from *seed).
+int muse_grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws,
+                 unsigned int* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C,
+                 void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (bits != nullptr && seed == nullptr) { set_last_error("grn_fwd: dropout needs a seed"); return MUSE_ERR_INVALID; }
   if (B <= 0 || HW <= 0) return MUSE_OK;
   if (C % 8 != 0) { set_last_error("grn: C must be a multiple of 8"); return MUSE_ERR_UNSUPPORTED; }
   const bf16* xp = reinterpret_cast<const bf16*>(x);
@@ -327,28 +337,13 @@ int launch_grn(const void* x, const float* gamma, const float* beta, void* out, 
   rc = check_launch("grn_finalize");
   if (rc) return rc;
   const long long total8 = static_cast<long long>(B) * HW * (C / 8);
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(grn_apply_kernel<DROP>, xp, nx_ws, gamma, beta,
-                                                                         reinterpret_cast<bf16*>(out), total8, HW, C, drop);
-  return check_launch(DROP ? "grn_apply_dropout" : "grn_apply");
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(bits ? grn_apply_kernel<true> : grn_apply_kernel<false>,
+      xp, nx_ws, gamma, beta, reinterpret_cast<bf16*>(out), total8, HW, C, philox::elem_drop(bits, seed, site, p, C));
+  return check_launch(bits ? "grn_apply_dropout" : "grn_apply");
 }
 
-}  // namespace
-
-// x bf16 [B, HW, C] -> out bf16 [B, HW, C]; sumsq_ws / nx_ws fp32 [B, C] (kept by the caller for the backward pass)
-int grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws, int B, int HW,
-            int C, cudaStream_t s) {
-  return launch_grn<false>(x, gamma, beta, out, stat_ws, nx_ws, B, HW, C, philox::ElemDrop{}, s);
-}
-
-// grn_fwd followed by the ResBlock's dropout (:607): out is the dropped output, bits [B * HW, ceil(C / 32)] uint32
-// words written (philox.cuh elementwise mapping, seed read from *seed)
-int grn_fwd_dropout(const void* x, const float* gamma, const float* beta, void* out, float* stat_ws, float* nx_ws,
-                    void* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C, cudaStream_t s) {
-  if (bits == nullptr || seed == nullptr) { set_last_error("grn_fwd_dropout: bits and seed are required"); return MUSE_ERR_INVALID; }
-  return launch_grn<true>(x, gamma, beta, out, stat_ws, nx_ws, B, HW, C, philox::elem_drop(bits, seed, site, p, C), s);
-}
-
-int adaln_apply(float* x, const float* ss, long long ss_stride, int B, int rows_per_sample, int C, cudaStream_t s) {
+int muse_adaln_apply(float* x, const float* ss, long long ss_stride, int B, int rows_per_sample, int C, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (C % 4 != 0 || ss_stride % 4 != 0) { set_last_error("adaln_apply: C and the modulation stride must be multiples of 4"); return MUSE_ERR_UNSUPPORTED; }
   const long long total4 = static_cast<long long>(B) * rows_per_sample * (C / 4);
   if (total4 <= 0) return MUSE_OK;
@@ -356,7 +351,8 @@ int adaln_apply(float* x, const float* ss, long long ss_stride, int B, int rows_
   return check_launch("adaln_apply");
 }
 
-int silu_bf16(const void* x, int x_dt, void* y, long long n, cudaStream_t s) {
+int muse_silu_bf16(const void* x, int x_dt, void* y, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
   if (n % 8 != 0) { set_last_error("silu: n must be a multiple of 8"); return MUSE_ERR_INVALID; }
   const long long n8 = n / 8;
@@ -366,4 +362,4 @@ int silu_bf16(const void* x, int x_dt, void* y, long long n, cudaStream_t s) {
   return check_launch("silu");
 }
 
-}  // namespace muse
+}  // extern "C"

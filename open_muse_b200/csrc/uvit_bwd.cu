@@ -457,12 +457,18 @@ int launch_anm_bwd(const void* dy, const float* dr_out, const float* x, const fl
 }
 
 }  // namespace
+}  // namespace muse
+
+using namespace muse;
+
+extern "C" {
 
 // dy: grad wrt y (dtype code), dr_out: grad wrt the prenorm residual output (fp32, nullable), x: saved r_out;
 // outputs da (dtype code) and dr (fp32, nullable) both = g; dw [H] and dss [B, ss_stride] accumulate (+=).
-int add_norm_mod_bwd(const void* dy, int dy_dt, const float* dr_out, const float* x, const float* w, const float* ss,
-                     long long ss_stride, int rows_per_sample, void* da, int da_dt, float* dr, float* dw, float* dss,
-                     int rows, int H, float eps, int rms, cudaStream_t s) {
+int muse_add_norm_mod_bwd(const void* dy, int dy_dt, const float* dr_out, const float* x, const float* w, const float* ss,
+                          long long ss_stride, int rows_per_sample, void* da, int da_dt, float* dr, float* dw, float* dss,
+                          int rows, int H, float eps, int rms, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024) { set_last_error("add_norm_mod_bwd: H=%d must be a multiple of 8 and <= 1024", H); return MUSE_ERR_UNSUPPORTED; }
   if (ss == nullptr) { rows_per_sample = 1; dss = nullptr; }
@@ -476,9 +482,10 @@ int add_norm_mod_bwd(const void* dy, int dy_dt, const float* dr_out, const float
 
 // dy bf16 (grad wrt the normalised output), conv bf16 (saved conv output), x fp32 (block input), wk fp32 [9,C];
 // dc_ws fp32 [pixels, C] scratch; dx fp32 = dres + conv-transpose(d_c); dwk [9,C] and dnw [C] accumulate.
-int dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, const float* wk, const float* nw, const float* dres,
-                       float* dc_ws, float* dx, float* dwk, float* dnw, int B, int hh, int ww, int C, float eps, int rms,
-                       cudaStream_t s) {
+int muse_dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, const float* wk, const float* nw, const float* dres,
+                            float* dc_ws, float* dx, float* dwk, float* dnw, int B, int hh, int ww, int C, float eps, int rms,
+                            void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const long long pixels = static_cast<long long>(B) * hh * ww;
   if (pixels <= 0) return MUSE_OK;
   if (C % 8 != 0 || C > 1024) { set_last_error("dwconv3x3_norm_bwd: C=%d unsupported", C); return MUSE_ERR_UNSUPPORTED; }
@@ -497,52 +504,41 @@ int dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, const f
   return check_launch("dwconv_bwd");
 }
 
-namespace {
-
-template <bool DROP>
-int launch_grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
-                   void* dx, float* dgamma, float* dbeta, int B, int HW, int C, const philox::ElemDrop& drop, cudaStream_t s) {
+// x bf16 (GEMM output before GELU), dout bf16, nx / sumsq fp32 [B,C] saved by the forward; s1_ws fp32 [B,C] scratch;
+// dx bf16; dgamma / dbeta [C] accumulate.  bits != nullptr: those muse_grn_fwd wrote; dout (the gradient of the dropped
+// output) is scaled by them as it is read.
+int muse_grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
+                 void* dx, float* dgamma, float* dbeta, const unsigned int* bits, float p, int B, int HW, int C,
+                 void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (B <= 0 || HW <= 0) return MUSE_OK;
   if (C % 8 != 0) { set_last_error("grn_bwd: C must be a multiple of 8"); return MUSE_ERR_UNSUPPORTED; }
   const bf16* xp = reinterpret_cast<const bf16*>(x);
   const bf16* dp = reinterpret_cast<const bf16*>(dout);
-  pdl_launch(dim3(ceil_div(C, 256), B), 128, 0, s)(grn_bwd_stats_kernel<DROP>, xp, dp, nx, s1_ws, dgamma, dbeta, HW, C, drop);
-  int rc = check_launch(DROP ? "grn_bwd_stats_dropout" : "grn_bwd_stats");
+  const philox::ElemDrop drop = philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, C);
+  pdl_launch(dim3(ceil_div(C, 256), B), 128, 0, s)(bits ? grn_bwd_stats_kernel<true> : grn_bwd_stats_kernel<false>, xp, dp,
+                                                   nx, s1_ws, dgamma, dbeta, HW, C, drop);
+  int rc = check_launch(bits ? "grn_bwd_stats_dropout" : "grn_bwd_stats");
   if (rc) return rc;
   pdl_launch(B, 256, 0, s)(grn_bwd_finalize_kernel, s1_ws, sumsq, gamma, C);
   rc = check_launch("grn_bwd_finalize");
   if (rc) return rc;
   const long long total8 = static_cast<long long>(B) * HW * (C / 8);
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(grn_bwd_apply_kernel<DROP>, xp, dp, nx, s1_ws, gamma,
-                                                                         reinterpret_cast<bf16*>(dx), total8, HW, C, drop);
-  return check_launch(DROP ? "grn_bwd_apply_dropout" : "grn_bwd_apply");
+  pdl_launch(static_cast<unsigned>(ceil_div_ll(total8, 256)), 256, 0, s)(bits ? grn_bwd_apply_kernel<true> : grn_bwd_apply_kernel<false>,
+      xp, dp, nx, s1_ws, gamma, reinterpret_cast<bf16*>(dx), total8, HW, C, drop);
+  return check_launch(bits ? "grn_bwd_apply_dropout" : "grn_bwd_apply");
 }
 
-}  // namespace
-
-// x bf16 (GEMM output before GELU), dout bf16, nx / sumsq fp32 [B,C] saved by the forward; s1_ws fp32 [B,C] scratch;
-// dx bf16; dgamma / dbeta [C] accumulate.
-int grn_bwd(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws, void* dx,
-            float* dgamma, float* dbeta, int B, int HW, int C, cudaStream_t s) {
-  return launch_grn_bwd<false>(x, dout, nx, sumsq, gamma, s1_ws, dx, dgamma, dbeta, B, HW, C, philox::ElemDrop{}, s);
-}
-
-// backward of grn_fwd_dropout: dout (the gradient of the dropped output) is scaled by the bits as it is read
-int grn_bwd_dropout(const void* x, const void* dout, const float* nx, const float* sumsq, const float* gamma, float* s1_ws,
-                    void* dx, float* dgamma, float* dbeta, const void* bits, float p, int B, int HW, int C, cudaStream_t s) {
-  if (bits == nullptr) { set_last_error("grn_bwd_dropout: bits are required"); return MUSE_ERR_INVALID; }
-  return launch_grn_bwd<true>(x, dout, nx, sumsq, gamma, s1_ws, dx, dgamma, dbeta, B, HW, C,
-                              philox::elem_drop(const_cast<void*>(bits), nullptr, 0, p, C), s);
-}
-
-int adaln_bwd(const float* dy, const float* x, const float* ss, long long ss_stride, float* dx, float* dss, int B,
-              int rows_per_sample, int C, cudaStream_t s) {
+int muse_adaln_bwd(const float* dy, const float* x, const float* ss, long long ss_stride, float* dx, float* dss, int B,
+                   int rows_per_sample, int C, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (B <= 0 || rows_per_sample <= 0) return MUSE_OK;
   pdl_launch(dim3(ceil_div(C, 128), B), 128, 0, s)(adaln_bwd_kernel, dy, x, ss, ss_stride, dx, dss, rows_per_sample, C);
   return check_launch("adaln_bwd");
 }
 
-int silu_bwd(const void* dy, const void* x, int x_dt, void* dx, int dx_dt, long long n, int accumulate, cudaStream_t s) {
+int muse_silu_bwd(const void* dy, const void* x, int x_dt, void* dx, int dx_dt, long long n, int accumulate, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
   if (n % 8 != 0) { set_last_error("silu_bwd: n must be a multiple of 8"); return MUSE_ERR_INVALID; }
   const long long n8 = n / 8;
@@ -555,4 +551,4 @@ int silu_bwd(const void* dy, const void* x, int x_dt, void* dx, int dx_dt, long 
   return check_launch("silu_bwd");
 }
 
-}  // namespace muse
+}  // extern "C"

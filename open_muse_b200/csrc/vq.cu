@@ -180,9 +180,15 @@ vq_lookup_nchw_kernel(const long long* __restrict__ ids, const float* __restrict
 }
 
 }  // namespace
+}  // namespace muse
 
-int vq_argmin(const float* z, const float* codebook, float* enorm_ws, long long* ids, float* dmin, int n, int ncodes,
-              int D, cudaStream_t s) {
+using namespace muse;
+
+extern "C" {
+
+int muse_vq_argmin(const float* z, const float* codebook, float* enorm_ws, long long* ids, float* dmin, int n, int ncodes,
+                   int D, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
   if (D % TKK != 0) { set_last_error("vq_argmin: D=%d must be a multiple of %d", D, TKK); return MUSE_ERR_UNSUPPORTED; }
   pdl_launch(ceil_div(ncodes, 256), 256, 0, s)(sqnorm_kernel, codebook, enorm_ws, ncodes, D);
@@ -192,8 +198,9 @@ int vq_argmin(const float* z, const float* codebook, float* enorm_ws, long long*
   return check_launch("vq_argmin");
 }
 
-int vq_soft_code(const float* z, const float* codebook, float* enorm_ws, float* soft, long long* ids, const float* expo,
-                 float temp, int n, int ncodes, int D, cudaStream_t s) {
+int muse_vq_soft_code(const float* z, const float* codebook, float* enorm_ws, float* soft, long long* ids, const float* expo,
+                      float temp, int n, int ncodes, int D, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
   if (D % TKK != 0) { set_last_error("vq_soft_code: D=%d must be a multiple of %d", D, TKK); return MUSE_ERR_UNSUPPORTED; }
   if (!(temp > 0.f)) { set_last_error("vq_soft_code: temp must be > 0"); return MUSE_ERR_INVALID; }
@@ -207,12 +214,13 @@ int vq_soft_code(const float* z, const float* codebook, float* enorm_ws, float* 
   return check_launch("vq_soft");
 }
 
-int vq_lookup_nchw(const long long* ids, const float* codebook, float* out, int B, int P, int D, int ncodes,
-                   cudaStream_t s) {
+int muse_vq_lookup_nchw(const long long* ids, const float* codebook, float* out, int B, int P, int D, int ncodes,
+                        void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const long long total = static_cast<long long>(B) * D * P;
   if (total <= 0) return MUSE_OK;
   pdl_launch(static_cast<unsigned>(ceil_div_ll(total, 256)), 256, 0, s)(vq_lookup_nchw_kernel, ids, codebook, out, B, P, D, ncodes);
   return check_launch("vq_lookup_nchw");
 }
 
-}  // namespace muse
+}  // extern "C"

@@ -63,9 +63,8 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
-_KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_attn_bwd_dropout": 2, "muse_norm_bwd_glu_dropout": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
-                     "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3, "muse_grn_fwd_dropout": 3,
-                     "muse_grn_bwd_dropout": 3,
+_KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
+                     "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3,
                      "muse_dwconv3x3_norm_bwd": 2}
 _prof = {"on": False, "events": []}
 
@@ -236,15 +235,10 @@ def norm_fwd(x, w, eps, out_dtype, res=None, act=0, rms=0, save_stats=True, drop
         stats = mean = rstd = None
     if dropout is not None:
         assert act == 2 and x.dtype == torch.bfloat16 and out_dtype == torch.bfloat16 and res is None
-        p, seed, site = dropout
-        bits = torch.empty(rows, (H + 31) // 32, dtype=torch.int32, device=x.device)
-        _call("muse_norm_fwd_glu_dropout", _p(x), _p(w), _p(y), _p(mean), _p(rstd), _p(bits), _p(seed), int(site), float(p),
-              rows, H, float(eps), rms, st)
-        _drop_record(site, bits)
-        return y, stats, bits
-    _call("muse_norm_fwd", _p(x), _dt(x), _p(w), _p(res), _p(y), _dt(y), _p(mean), _p(rstd), rows, H, float(eps),
-          act, rms, st)
-    return y, stats
+    bits, seed, site, p = _drop_fwd_args(dropout, x.device, rows, cols=H)
+    _call("muse_norm_fwd", _p(x), _dt(x), _p(w), _p(res), _p(y), _dt(y), _p(mean), _p(rstd), _p(bits), _p(seed), site, p,
+          rows, H, float(eps), act, rms, st)
+    return (y, stats) if bits is None else (y, stats, bits)
 
 
 _bf16_copies = {}
@@ -269,18 +263,10 @@ def norm_bwd(dy, x, w, stats, dx_dtype, dw=None, dres=None, act=0, rms=0, y_fwd=
     rows = x.shape[0]
     H = x.shape[1] // 2 if act == 2 else x.shape[1]
     dx = torch.empty(x.shape, dtype=dx_dtype, device=x.device)
+    p, bits = dropout if dropout is not None else (0.0, None)
     if dropout is not None:
         assert act == 2 and dy.dtype == x.dtype == dx_dtype == torch.bfloat16 and dres is None and not bf16_copy
-        p, bits = dropout
-        ws = None
-        if want_dw:
-            dw = torch.empty(H, dtype=torch.float32, device=x.device)
-            ws = torch.empty(max(1, _lib.load().muse_norm_bwd_workspace_floats(rows, H, act)), dtype=torch.float32,
-                             device=x.device)
-            _state["launches"] += 1  # the ordered column sum
-        _call("muse_norm_bwd_glu_dropout", _p(dy), _p(x), _p(w), _p(stats[0]), _p(stats[1]), _p(bits), float(p), _p(dx),
-              _p(dw), _p(ws), rows, H, rms, st)
-        return (dx, dw) if want_dw else dx
+        y_fwd = None
     if y_fwd is not None and not (act == 2 and y_fwd.dtype == torch.bfloat16 and y_fwd.is_contiguous()):
         y_fwd = None
     copy = None
@@ -294,8 +280,8 @@ def norm_bwd(dy, x, w, stats, dx_dtype, dw=None, dres=None, act=0, rms=0, y_fwd=
         dw = torch.empty(H, dtype=torch.float32, device=x.device)
         ws = torch.empty(max(1, _lib.load().muse_norm_bwd_workspace_floats(rows, H, act)), dtype=torch.float32, device=x.device)
         _state["launches"] += 1  # the ordered column sum
-    _call("muse_norm_bwd", _p(dy), _dt(dy), _p(x), _dt(x), _p(w), _p(stats[0]), _p(stats[1]), _p(dres), _p(y_fwd), _p(dx),
-          _dt(dx), _p(copy), _p(dw), _p(ws), rows, H, act, rms, st)
+    _call("muse_norm_bwd", _p(dy), _dt(dy), _p(x), _dt(x), _p(w), _p(stats[0]), _p(stats[1]), _p(dres), _p(y_fwd), _p(bits),
+          float(p), _p(dx), _dt(dx), _p(copy), _p(dw), _p(ws), rows, H, act, rms, st)
     return (dx, dw) if want_dw else dx
 
 
@@ -333,14 +319,9 @@ def glu_fwd(ab, dropout=None):
     st = _prep(ab)
     rows, two_i = ab.shape
     out = torch.empty(rows, two_i // 2, dtype=torch.bfloat16, device=ab.device)
-    if dropout is not None:
-        p, seed, site = dropout
-        bits = torch.empty(rows, (two_i // 2 + 31) // 32, dtype=torch.int32, device=ab.device)
-        _call("muse_glu_fwd_dropout", _p(ab), _p(out), _p(bits), _p(seed), int(site), float(p), rows, two_i // 2, st)
-        _drop_record(site, bits)
-        return out, bits
-    _call("muse_glu_fwd", _p(ab), _p(out), rows, two_i // 2, st)
-    return out
+    bits, seed, site, p = _drop_fwd_args(dropout, ab.device, rows, cols=two_i // 2)
+    _call("muse_glu_fwd", _p(ab), _p(out), _p(bits), _p(seed), site, p, rows, two_i // 2, st)
+    return out if bits is None else (out, bits)
 
 
 def glu_bwd(ab, dout, dropout=None):
@@ -348,11 +329,8 @@ def glu_bwd(ab, dout, dropout=None):
     st = _prep(ab)
     rows, two_i = ab.shape
     dab = torch.empty_like(ab)
-    if dropout is not None:
-        p, bits = dropout
-        _call("muse_glu_bwd_dropout", _p(ab), _p(dout), _p(bits), float(p), _p(dab), rows, two_i // 2, st)
-        return dab
-    _call("muse_glu_bwd", _p(ab), _p(dout), _p(dab), rows, two_i // 2, st)
+    p, bits = dropout if dropout is not None else (0.0, None)
+    _call("muse_glu_bwd", _p(ab), _p(dout), _p(bits), float(p), _p(dab), rows, two_i // 2, st)
     return dab
 
 
@@ -366,30 +344,20 @@ def attn_fwd(q, k, v, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
     hd = int(head_dim)
     o = torch.empty(B * Sq, nh * hd, dtype=torch.bfloat16, device=q.device)
     lse = torch.empty(B, nh, Sq, dtype=torch.float32, device=q.device)
-    if dropout is not None:
-        p, seed, site = dropout
-        bits = torch.empty(B, nh, Sq, (Skv + 31) // 32, dtype=torch.int32, device=q.device)
-        _call("muse_attn_fwd_dropout", _p(q), _p(k), _p(v), _p(o), _p(lse), _p(bits), _p(seed), int(site), float(p), B, nh,
-              Sq, Skv, hd, q.stride(0), k.stride(0), v.stride(0), o.stride(0), float(scale), st)
-        _drop_record(site, bits)
-        return o, lse, bits
-    _call("muse_attn_fwd", _p(q), _p(k), _p(v), _p(o), _p(lse), B, nh, Sq, Skv, hd, q.stride(0), k.stride(0),
-          v.stride(0), o.stride(0), float(scale), st)
-    return o, lse
+    bits, seed, site, p = _drop_fwd_args(dropout, q.device, B, nh, Sq, cols=Skv)
+    _call("muse_attn_fwd", _p(q), _p(k), _p(v), _p(o), _p(lse), _p(bits), _p(seed), site, p, B, nh, Sq, Skv, hd,
+          q.stride(0), k.stride(0), v.stride(0), o.stride(0), float(scale), st)
+    return (o, lse) if bits is None else (o, lse, bits)
 
 
 def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
-    """dropout = (p, bits): the rate and the keep bits attn_fwd(..., dropout=...) returned."""
+    """dropout = (p, bits): the rate and the keep bits attn_fwd(..., dropout=...) returned.  o is not read: the kernels
+    recompute what they need from q, k, v and lse."""
     st = _prep(q)
     dvec = torch.empty(B, nh, Sq, dtype=torch.float32, device=q.device)
-    if dropout is not None:
-        p, bits = dropout
-        _call("muse_attn_bwd_dropout", _p(q), _p(k), _p(v), _p(do), _p(lse), _p(bits), float(p), _p(dvec), _p(dq), _p(dk),
-              _p(dv), B, nh, Sq, Skv, int(head_dim), q.stride(0), k.stride(0), v.stride(0), do.stride(0), dq.stride(0),
-              dk.stride(0), dv.stride(0), float(scale), st)
-        return
-    _call("muse_attn_bwd", _p(q), _p(k), _p(v), _p(o), _p(do), _p(lse), _p(dvec), _p(dq), _p(dk), _p(dv), B, nh, Sq,
-          Skv, int(head_dim), q.stride(0), k.stride(0), v.stride(0), o.stride(0), do.stride(0), dq.stride(0), dk.stride(0),
+    p, bits = dropout if dropout is not None else (0.0, None)
+    _call("muse_attn_bwd", _p(q), _p(k), _p(v), _p(do), _p(lse), _p(bits), float(p), _p(dvec), _p(dq), _p(dk), _p(dv), B,
+          nh, Sq, Skv, int(head_dim), q.stride(0), k.stride(0), v.stride(0), do.stride(0), dq.stride(0), dk.stride(0),
           dv.stride(0), float(scale), st)
 
 
@@ -423,15 +391,25 @@ def _drop_record(site, bits):
         _drop_state["log"].append((int(site), bits))
 
 
+def _drop_fwd_args(dropout, device, *lead, cols):
+    """(bits, seed, site, p) for a forward that takes dropout = (p, seed, site): fresh int32 keep-bit words
+    [*lead, ceil(cols / 32)], recorded for dropout_record.  dropout None: (None, None, 0, 0.0), i.e. no dropout."""
+    if dropout is None:
+        return None, None, 0, 0.0
+    p, seed, site = dropout
+    bits = torch.empty(*lead, (cols + 31) // 32, dtype=torch.int32, device=device)
+    _drop_record(site, bits)
+    return bits, seed, int(site), float(p)
+
+
 def dropout_fwd(x, p, seed, site):
     """x contiguous fp32 / bf16 [rows, cols] (cols % 8 == 0) is dropped IN PLACE: x * keep / (1 - p_eff).  Returns
     (x, bits) with bits int32 [rows, ceil(cols / 32)]."""
     st = _prep(x)
     rows, cols = x.shape
     assert x.is_contiguous()
-    bits = torch.empty(rows, (cols + 31) // 32, dtype=torch.int32, device=x.device)
-    _call("muse_dropout_fwd", _p(x), _p(x), _dt(x), _p(bits), _p(seed), int(site), float(p), rows, cols, st)
-    _drop_record(site, bits)
+    bits, seed, site, p = _drop_fwd_args((p, seed, site), x.device, rows, cols=cols)
+    _call("muse_dropout_fwd", _p(x), _p(x), _dt(x), _p(bits), _p(seed), site, p, rows, cols, st)
     return x, bits
 
 
@@ -497,14 +475,11 @@ def grn(x, gamma, beta, B, HW, save_stats=False, dropout=None):
     C = x.shape[1]
     out = torch.empty_like(x)
     ws = torch.empty(2, B, C, dtype=torch.float32, device=x.device)
-    if dropout is not None:
-        p, seed, site = dropout
-        bits = torch.empty(B * HW, (C + 31) // 32, dtype=torch.int32, device=x.device)
-        _call("muse_grn_fwd_dropout", _p(x), _p(gamma), _p(beta), _p(out), _p(ws[0]), _p(ws[1]), _p(bits), _p(seed),
-              int(site), float(p), B, HW, C, st)
-        _drop_record(site, bits)
+    bits, seed, site, p = _drop_fwd_args(dropout, x.device, B * HW, cols=C)
+    _call("muse_grn_fwd", _p(x), _p(gamma), _p(beta), _p(out), _p(ws[0]), _p(ws[1]), _p(bits), _p(seed), site, p, B, HW, C,
+          st)
+    if bits is not None:
         return out, ws, bits
-    _call("muse_grn_fwd", _p(x), _p(gamma), _p(beta), _p(out), _p(ws[0]), _p(ws[1]), B, HW, C, st)
     return (out, ws) if save_stats else out
 
 
@@ -537,13 +512,9 @@ def grn_bwd(x, dout, stats, gamma, dgamma, dbeta, B, HW, dropout=None):
     C = x.shape[1]
     dx = torch.empty_like(x)
     ws = torch.empty(B, C, dtype=torch.float32, device=x.device)
-    if dropout is not None:
-        p, bits = dropout
-        _call("muse_grn_bwd_dropout", _p(x), _p(dout), _p(stats[1]), _p(stats[0]), _p(gamma), _p(ws), _p(dx), _p(dgamma),
-              _p(dbeta), _p(bits), float(p), B, HW, C, st)
-        return dx
-    _call("muse_grn_bwd", _p(x), _p(dout), _p(stats[1]), _p(stats[0]), _p(gamma), _p(ws), _p(dx), _p(dgamma), _p(dbeta), B, HW,
-          C, st)
+    p, bits = dropout if dropout is not None else (0.0, None)
+    _call("muse_grn_bwd", _p(x), _p(dout), _p(stats[1]), _p(stats[0]), _p(gamma), _p(ws), _p(dx), _p(dgamma), _p(dbeta),
+          _p(bits), float(p), B, HW, C, st)
     return dx
 
 

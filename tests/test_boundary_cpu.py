@@ -10,17 +10,39 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
+def _c_kind(decl):
+    """'pointer', 'int', 'long long' or 'float' for a return type or a named parameter of the header."""
+    if "*" in decl:
+        return "pointer"
+    return " ".join(w for w in decl.split() if w in ("int", "long", "float"))
+
+
+def _ctypes_kind(t):
+    import ctypes
+
+    if t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, ctypes._Pointer):
+        return "pointer"
+    return {ctypes.c_int: "int", ctypes.c_longlong: "long long", ctypes.c_float: "float"}[t]
+
+
 def test_library_exports_every_declared_symbol():
+    """Every declaration of the header has a ctypes entry with the same return type and the same kind of value in each
+    parameter slot (so a long long bound as an int, or a missing argument, is caught without a GPU)."""
     from open_muse_b200 import _lib, build
 
     build.build()
     lib = _lib.load()
-    header = open(os.path.join(ROOT, "include", "muse_b200.h")).read()
-    declared = set(re.findall(r"\b(muse_[a-z0-9_]+)\s*\(", header))
+    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "muse_b200.h")).read(), flags=re.S)
+    declared = {name: (ret, params) for ret, name, params in
+                re.findall(r"^([A-Za-z][\w ]*?\**)\s*\b(muse_\w+)\(([^)]*)\);", header, flags=re.M)}
     assert declared, "no declarations parsed"
-    assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
-    for name in declared:
+    assert set(declared) == set(_lib.SIGNATURES), set(declared) ^ set(_lib.SIGNATURES)
+    for name, (ret, params) in declared.items():
         assert hasattr(lib, name), name
+        params = [p for p in (p.strip() for p in params.split(",")) if p and p != "void"]
+        restype, argtypes = _lib.SIGNATURES[name]
+        assert _c_kind(ret) == _ctypes_kind(restype), name
+        assert [_c_kind(p) for p in params] == [_ctypes_kind(t) for t in argtypes], name
     assert lib.muse_abi_version() == _lib.ABI_VERSION
 
 
