@@ -302,6 +302,13 @@ static int gemm_tc(const void* A, const void* B, void* C, const float* res, int 
     set_last_error("gemm: ldc=%d must be a multiple of %d", ldc, epi == EPI_BF16 ? 8 : 4);
     return MUSE_ERR_INVALID;
   }
+  // The TMA-store epilogues do not clip a partial 16-byte unit at column N: they would overwrite the pad columns of that
+  // unit (N = 2025 into ldc = 2048 zeroes columns 2025..).  Only the atomic epilogue, which stores per element, takes any N.
+  if (epi != EPI_ATOMIC_F32 && N % (epi == EPI_BF16 ? 8 : 4) != 0) {
+    set_last_error("gemm: N=%d must be a multiple of %d for this epilogue (its TMA stores write whole 16-byte units)", N,
+                   epi == EPI_BF16 ? 8 : 4);
+    return MUSE_ERR_INVALID;
+  }
   if ((reinterpret_cast<uintptr_t>(C) & 15) != 0) {
     set_last_error("gemm: C must be 16B aligned");
     return MUSE_ERR_INVALID;

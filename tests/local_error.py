@@ -1,0 +1,153 @@
+"""Local error checks for the bf16 training kernels: the error of every row, tile or head against an fp64 reference.
+
+A whole-tensor ||out - ref|| / ||ref|| divides the error of one wrong row by the square root of the number of rows, so a
+tiled kernel that gets one row, one tile or one head wrong (a ragged tail tile, an off-by-one mask, state carried from
+one tile to the next) can stay under it.  check_local() splits both tensors into groups -- rows of the kernel's output,
+output tiles, (batch, head, row) of attention -- and bounds the error of each group on its own:
+
+    e_g    = ||out_g - ref_g|| / max(||ref_g||, median_g ||ref_g|| / 16)
+    elem_g = max |out_g - ref_g| / (the same denominator / sqrt(n))     (n = elements per group)
+
+The floor keeps near-zero groups (a key nobody attends to, an ignored row) from dividing by nothing.  A failure names
+the worst group in the kernel's own coordinates and gives the next-worst one.
+
+BOUNDS holds one (group bound, elementwise bound) pair per kernel output.  Each group bound is about twice the worst
+per-group error measured on an H100 SXM over all cases of tests/test_kernel_local_gpu.py (value in the comment), rounded
+up; bf16 outputs stay at or below 2e-2, where tests/test_local_error_cpu.py shows that the bounds reject subtly wrong
+kernels."""
+from __future__ import annotations
+
+import math
+from dataclasses import dataclass
+from typing import Callable
+
+import torch
+
+
+@dataclass
+class Groups:
+    """view: tensor -> [G, n] (one group per row); where: group index -> its coordinates in the kernel's terms;
+    sizes: elements per group when the view pads groups with zeros (default: n each)."""
+    view: Callable[[torch.Tensor], torch.Tensor]
+    where: Callable[[int], str]
+    sizes: torch.Tensor | None = None
+
+
+@dataclass
+class Local:
+    worst: float          # largest e_g
+    where: str            # its group
+    second: float         # next-largest e_g
+    second_where: str
+    elem: float           # largest elem_g
+    elem_where: str
+    whole: float          # whole-tensor rel-L2, the old single-number check
+
+
+def rows(n_rows: int, label: str = "row") -> Groups:
+    return Groups(lambda t: t.reshape(n_rows, -1), lambda g: f"{label} {g}")
+
+
+def balanced_rows(S: int) -> int:
+    """Rows per owned tile of the attention kernels: ceil(S / 64) tiles of equal height (attention_tc.cu balanced_tiles)."""
+    return -(-S // -(-S // 64))
+
+
+def attn_rows(B: int, nh: int, S: int, hd: int) -> Groups:
+    """[B * S, nh * hd] token-major attention operand -> one group per (b, h, row); the owned tile is the 64-row-box CTA
+    whose kept rows include `row` (q rows for O / dQ, kv rows for dK / dV)."""
+    R = balanced_rows(S)
+
+    def view(t):
+        return t.reshape(B, S, nh, hd).permute(0, 2, 1, 3).reshape(B * nh * S, hd)
+
+    def where(g):
+        b, h, r = g // (nh * S), (g // S) % nh, g % S
+        return f"(b {b}, h {h}, row {r}, owned tile {r // R} of {R} rows)"
+
+    return Groups(view, where)
+
+
+def gemm_rows(M: int, N: int, BM: int = 128) -> Groups:
+    return Groups(lambda t: t[:, :N].reshape(M, N), lambda g: f"(m tile {g // BM}, all n tiles, row {g})")
+
+
+def gemm_tiles(M: int, N: int, BN: int, BM: int = 128) -> Groups:
+    """One group per BM x BN output tile; the ragged M / N tails are zero-padded in both tensors (adding nothing)."""
+    nm, nn = -(-M // BM), -(-N // BN)
+
+    def view(t):
+        p = t.new_zeros(nm * BM, nn * BN)
+        p[:M, :N] = t[:, :N]
+        return p.reshape(nm, BM, nn, BN).permute(0, 2, 1, 3).reshape(nm * nn, BM * BN)
+
+    sizes = (torch.arange(nm)[:, None] * BM).neg().add(M).clamp(max=BM) * \
+        (torch.arange(nn)[None] * BN).neg().add(N).clamp(max=BN)
+    return Groups(view, lambda g: f"(m tile {g // nn}, n tile {g % nn}, rows {g // nn * BM}..{min(M, g // nn * BM + BM) - 1})",
+                  sizes.reshape(-1).double())
+
+
+def check_local(out, ref, groups: Groups, bound: float, elem_bound: float, what: str) -> Local:
+    d = groups.view(out.detach().double()) - groups.view(ref.detach().double())
+    r = groups.view(ref.detach().double())
+    n = torch.full((r.shape[0],), float(r.shape[1]), dtype=r.dtype) if groups.sizes is None else groups.sizes
+    nrm = r.norm(dim=1)
+    floor = max(float(nrm.median()) / 16, 1e-300)
+    den = nrm.clamp_min(floor)
+    e = torch.nan_to_num(d.norm(dim=1) / den, nan=math.inf)
+    el = torch.nan_to_num(d.abs().amax(dim=1) / (den / n.to(den.device).sqrt()), nan=math.inf)
+    top = torch.topk(e, min(2, e.numel()))
+    gi = [int(i) for i in top.indices]
+    ei = int(el.argmax())
+    whole = float(d.norm() / r.norm().clamp_min(1e-300))
+    res = Local(float(top.values[0]), groups.where(gi[0]), float(top.values[-1]) if len(gi) > 1 else 0.0,
+                groups.where(gi[-1]) if len(gi) > 1 else "-", float(el[ei]), groups.where(ei), whole)
+    msg = (f"{what}: worst group error {res.worst:.3e} at {res.where} (bound {bound:.1e}); next worst {res.second:.3e} "
+           f"at {res.second_where}; worst elementwise {res.elem:.3e} at {res.elem_where} (bound {elem_bound:.1e}); "
+           f"whole-tensor rel-L2 {res.whole:.3e}")
+    assert res.worst <= bound and res.elem <= elem_bound, msg
+    return res
+
+
+# (group bound, elementwise bound) per kernel output; the comment gives the worst group / elementwise error measured on
+# an H100 SXM (700 W) over all cases of tests/test_kernel_local_gpu.py.
+BOUNDS = {
+    # attention (ops.attn_fwd / attn_bwd), bf16 outputs
+    "attn.o": (1e-2, 4e-2),        # 4.87e-3 / 1.84e-2
+    "attn.dq": (1e-2, 4e-2),       # 4.86e-3 / 1.87e-2
+    "attn.dk": (1.4e-2, 5e-2),     # 6.59e-3 / 2.19e-2
+    "attn.dv": (1e-2, 4e-2),       # 4.85e-3 / 1.78e-2
+    # GEMM epilogues
+    "gemm.bf16": (5e-3, 7e-2),     # 2.16e-3 / 3.05e-2 (an element of the 2^3 column tile in a row of 2^-4 .. 2^3 tiles)
+    "gemm.f32": (6e-7, 4e-6),      # 2.68e-7 / 1.89e-6
+    "gemm.resadd": (4e-3, 2e-2),   # 1.69e-3 / 7.89e-3
+    "gemm.splitk": (6e-7, 4e-6),   # 2.68e-7 / 1.89e-6
+    "gemm.atomic": (4e-7, 4e-6),   # 1.90e-7 / 1.62e-6
+    # row norms; a row with one element 1e3 x the others puts that element at 64 x the row's rms
+    "norm.y_bf16": (5e-3, 3e-1),   # 2.27e-3 / 1.45e-1
+    "norm.dx": (3e-5, 4e-5),       # 1.38e-5 / 1.52e-5
+    "norm.dw": (2e-4, 2e-4),       # 8.46e-5 / 8.46e-5
+    "norm2.dx2": (3e-7, 1.5e-6),   # 1.09e-7 / 6.36e-7
+    "norm2.da": (4e-3, 3e-2),      # 1.94e-3 / 1.36e-2
+    "norm2.dw": (1.5e-5, 1.5e-5),  # 7.18e-6 / 7.18e-6
+    "glu_norm.y": (5e-3, 1.5e-1),  # 2.05e-3 / 6.23e-2
+    "glu_norm.dab": (5e-3, 1.5e-1),  # 2.04e-3 / 5.83e-2
+    "glu_norm.dw": (3e-5, 3e-5),   # 1.34e-5 / 1.34e-5
+    # cross-entropy; a row dominated by one +60 logit has its gradient in two elements
+    "ce.dlogits": (8e-3, 4e-1),    # 3.60e-3 / 1.62e-1
+    # U-ViT
+    "anm.y": (5e-3, 3e-2),         # 2.31e-3 / 1.34e-2
+    "anm.da_bf16": (5e-3, 3e-2),   # 2.19e-3 / 1.24e-2
+    "anm.da_f32": (3e-7, 1.5e-6),  # 1.17e-7 / 6.77e-7
+    "anm.dw": (2e-5, 2e-5),        # 8.49e-6 / 8.49e-6
+    "anm.dmod": (4e-7, 1.5e-6),    # 1.54e-7 / 5.65e-7
+    "dwconv.y": (5e-3, 4e-2),      # 2.03e-3 / 1.55e-2
+    "dwconv.dx": (3e-5, 6e-4),     # 1.37e-5 / 2.68e-4
+    "dwconv.dwk": (4e-6, 8e-5),    # 1.89e-6 / 3.39e-5
+    "dwconv.dnw": (6e-3, 6e-3),    # 2.55e-3 / 2.55e-3 (from the bf16 conv output the kernel saves)
+    "grn.out": (6e-3, 4e-2),       # 2.51e-3 / 1.56e-2
+    "grn.dx": (5e-3, 5e-2),        # 2.25e-3 / 2.13e-2
+    "grn.dgamma": (1.2e-4, 1.2e-4),  # 5.20e-5 / 5.20e-5
+    "grn.dbeta": (8e-7, 8e-7),     # 3.18e-7 / 3.18e-7
+}
+ATTN_LSE_ABS = 4e-5  # max |lse - lse_ref| in natural-log units; measured 1.53e-5
