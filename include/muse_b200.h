@@ -27,7 +27,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 6
+#define MUSE_B200_ABI_VERSION 7
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -274,10 +274,14 @@ int muse_sample_step(const void* logits, const void* logits_unc, long long row_s
 int muse_conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H,
                      int W, int Cin, int Cout, int ksize, int upsample2x, void* stream);
 /* nn.GroupNorm(groups, C, eps) + F.silu (:61-79), deterministic (no atomics). Scratch: partials_ws float
- * [muse_groupnorm_workspace_floats(B,HW,C)] (-1 if the shape is unsupported), scale_shift_ws float [B*C*2].
+ * [muse_groupnorm_workspace_floats(B,HW,C)] (-1 if the shape is unsupported), scale_shift_ws float [B*C*3].
  * Output either y (fp32) or the pair y_hi / y_lo (bf16 planes with y = hi + lo, the operand form of
- * muse_conv2d_nhwc_tc); the unused form is NULL.  precomputed_tiles > 0: partials_ws already holds the {sum, sumsq}
- * per [image][tile][C] written by muse_conv2d_nhwc_tc(stats=...) for x and the statistics pass is skipped. */
+ * muse_conv2d_nhwc_tc); the unused form is NULL.  partials_ws holds per [image][pixel block][C] {sum, M2}: the sum of the
+ * block's values less the image's first pixel x[b, 0, c] and the sum of their squared deviations from the block's own
+ * mean; the blocks are merged in fp64.
+ * precomputed_tiles > 0: partials_ws already holds them (sums of the values themselves) per [image][tile][C] (HW / tiles
+ * pixels each), written by
+ * muse_conv2d_nhwc_tc(stats=...) for x, and the statistics pass is skipped. */
 long long muse_groupnorm_workspace_floats(int B, int HW, int C);
 int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* beta, float* y, void* y_hi, void* y_lo,
                              float* partials_ws, float* scale_shift_ws, int B, int HW, int C, int groups, float eps,
@@ -287,8 +291,9 @@ int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* be
  * fp32 accumulation): x_hi/x_lo bf16 [B,H,W,Cin], w_hi/w_lo bf16 [Cout, ksize*ksize*Cin] (tap-major, then input
  * channel), optional bias [Cout] and residual [B,H,W,Cout] -> y fp32 [B,H,W,Cout].
  * muse_conv2d_tc_supported says whether the geometry is handled (Cin % 64 == 0, W a multiple or a divisor of 128 ...);
- * other shapes use muse_conv2d_nhwc.  stats (nullable, Cout > 16): fp32 [B][tiles][Cout][2] receives {sum, sumsq} of y
- * per pixel tile, tiles = muse_conv2d_tc_tiles_per_image(...) -- the GroupNorm statistics of the next layer for free.
+ * other shapes use muse_conv2d_nhwc.  stats (nullable, Cout > 16): fp32 [B][tiles][Cout][2] receives {sum, M2} of y per
+ * pixel tile (M2: sum of squared deviations from the tile's mean), tiles = muse_conv2d_tc_tiles_per_image(...) -- the
+ * GroupNorm statistics of the next layer for free.
  * upsample2x (UpsamplingBlock :141-149, ksize 3): H, W are the output dims, x_hi/x_lo the LOW-resolution input
  * [B,H/2,W/2,Cin] and w_hi/w_lo the four 2x2 parity matrices stacked as [4*Cout, 4*Cin] (row = parity*Cout + co with
  * parity = 2*(y&1) + (x&1); column = (a*2+b)*Cin + ci for window offset (a,b); entries are sums of the 3x3 taps that

@@ -77,7 +77,7 @@ SIGNATURES = {
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 
 class MuseB200Error(RuntimeError):

@@ -137,14 +137,18 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
 }
 
 // ---------------------------------------------------------------- GroupNorm + SiLU (NHWC)
-// pass 1: per-(image, channel) moments {sum, sumsq} in fp64 (atomics across pixel chunks)
-// pass 2: fold channels into groups -> per-(image, channel) scale = rstd*gamma, shift = beta - mean*scale
-// pass 3: y = silu(x * scale + shift)
+// pass 1: per-(image, pixel block, channel) partials {sum, M2}, M2 = sum of squared deviations from the block's own mean
+//         (or the same per pixel tile from the epilogue of the tensor-core convolution that produced x)
+// pass 2: merge the partials of each group in fp64 (Chan et al.) -> per-(image, channel) scale = rstd*gamma,
+//         shift = beta - mean*scale (fp64, kept as two floats hi + lo)
+// pass 3: y = silu(fma(x, scale, shift_hi) + shift_lo)
+// A variance taken as E[x^2] - mean^2 from fp32 sums loses ~2^-24 (mean^2 + var) / var of itself: at |mean| = 100 std the
+// GroupNorm output would be off by ~3e-4.  Deviations from a partial's own mean keep the error independent of the mean.
 __global__ void __launch_bounds__(256)
 gn_stats_kernel(const float* __restrict__ x, float* __restrict__ partials, int HW, int C, int rows_per_block) {
   pdl_enter();
-  // deterministic: fixed thread->data mapping, fixed-order in-block reduction, per-block partials (no atomics)
-  extern __shared__ float s_part[];  // [rstep][C][2]
+  // deterministic: fixed thread->data mapping, fixed-order in-block merge, per-block partials (no atomics)
+  extern __shared__ float s_part[];  // [rstep][C][2]: {mean of v - K, M2} of each row lane's rows
   const int b = blockIdx.y;
   const int c4 = C / 4;
   const int r0 = blockIdx.x * rows_per_block;
@@ -153,31 +157,56 @@ gn_stats_kernel(const float* __restrict__ x, float* __restrict__ partials, int H
   const int q = threadIdx.x % c4;          // fixed channel quad per thread (256 % c4 == 0)
   const int lane_r = threadIdx.x / c4;
   const int rstep = blockDim.x / c4;
-  float s[4] = {0.f, 0.f, 0.f, 0.f}, ss[4] = {0.f, 0.f, 0.f, 0.f};
+  // Welford per thread over its rows r0 + lane_r, r0 + lane_r + rstep, ... of v - K, K = the image's first pixel: the
+  // stored sum is then of values ~ the spread, and its fp32 rounding no longer scales with the mean
+  const float4 k4 = *reinterpret_cast<const float4*>(base + q * 4);
+  const float K[4] = {k4.x, k4.y, k4.z, k4.w};
+  float mu[4] = {0.f, 0.f, 0.f, 0.f}, m2[4] = {0.f, 0.f, 0.f, 0.f};
+  int cnt = 0;
   for (int r = r0 + lane_r; r < r1; r += rstep) {
-    const float4 v = *reinterpret_cast<const float4*>(base + static_cast<long long>(r) * C + q * 4);
-    s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
-    ss[0] += v.x * v.x; ss[1] += v.y * v.y; ss[2] += v.z * v.z; ss[3] += v.w * v.w;
+    const float4 v4 = *reinterpret_cast<const float4*>(base + static_cast<long long>(r) * C + q * 4);
+    const float v[4] = {v4.x, v4.y, v4.z, v4.w};
+    const float inv = __frcp_rn(static_cast<float>(++cnt));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float u = v[j] - K[j];
+      const float d = u - mu[j];
+      mu[j] = fmaf(d, inv, mu[j]);
+      m2[j] = fmaf(d, u - mu[j], m2[j]);
+    }
   }
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    s_part[(lane_r * C + q * 4 + j) * 2] = s[j];
-    s_part[(lane_r * C + q * 4 + j) * 2 + 1] = ss[j];
+    s_part[(lane_r * C + q * 4 + j) * 2] = mu[j];
+    s_part[(lane_r * C + q * 4 + j) * 2 + 1] = m2[j];
   }
   __syncthreads();
   float* out = partials + (static_cast<long long>(b) * gridDim.x + blockIdx.x) * C * 2;  // [image][block][C][2]
-  for (int i = threadIdx.x; i < C * 2; i += blockDim.x) {
-    float acc = 0.f;
-    for (int k = 0; k < rstep; ++k) acc += s_part[k * C * 2 + i];
-    out[i] = acc;
+  const int rows = r1 - r0;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    // merge the row lanes in order; lane k holds rows k, k + rstep, ... of the block
+    float n = 0.f, mean = 0.f, M2 = 0.f;
+    for (int k = 0; k < rstep && k < rows; ++k) {
+      const float nk = static_cast<float>((rows - k + rstep - 1) / rstep);
+      const float mk = s_part[(k * C + c) * 2], m2k = s_part[(k * C + c) * 2 + 1];
+      const float d = mk - mean, nn = n + nk;
+      mean = fmaf(d, nk / nn, mean);
+      M2 += m2k + d * d * (n * nk / nn);
+      n = nn;
+    }
+    out[c * 2] = mean * n;
+    out[c * 2 + 1] = M2;
   }
 }
 
-// one warp per (image, group): fp64 sum of the per-block partials [image][block][C][2] in a fixed order (deterministic)
+// one warp per (image, group): fp64 merge of the per-block partials {sum, M2} [image][block][C][2] in a fixed order
+// (deterministic).  Block blk covers min(rows_per_block, HW - blk * rows_per_block) pixels.  shift_x (nullable): the
+// sums are of x - K with K the image's first pixel x[b, 0, c] (the statistics pass); NULL: of x (conv epilogue tiles).
 __global__ void __launch_bounds__(256)
-gn_finalize_kernel(const float* __restrict__ partials, int nblocks, const float* __restrict__ gamma,
-                   const float* __restrict__ beta, float* __restrict__ scale_shift, int B, int HW, int C, int groups,
-                   float eps) {
+gn_finalize_kernel(const float* __restrict__ partials, int nblocks, int rows_per_block, const float* __restrict__ shift_x,
+                   const float* __restrict__ gamma,
+                   const float* __restrict__ beta, float* __restrict__ scale_shift, float* __restrict__ shift_lo, int B,
+                   int HW, int C, int groups, float eps) {
   pdl_enter();
   const int w = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (w >= B * groups) return;
@@ -185,37 +214,53 @@ gn_finalize_kernel(const float* __restrict__ partials, int nblocks, const float*
   const int b = w / groups, g = w % groups;
   const int cpg = C / groups;
   const float* base = partials + static_cast<long long>(b) * nblocks * C * 2;
-  double sum = 0.0, sq = 0.0;
   const int items = nblocks * cpg;
-  for (int i = lane; i < items; i += 32) {
+  auto partial = [&](int i) {
     const int blk = i / cpg, k = i % cpg;
-    const float2 v = *reinterpret_cast<const float2*>(base + (static_cast<long long>(blk) * C + g * cpg + k) * 2);
-    sum += static_cast<double>(v.x);
-    sq += static_cast<double>(v.y);
-  }
+    return *reinterpret_cast<const float2*>(base + (static_cast<long long>(blk) * C + g * cpg + k) * 2);
+  };
+  auto warp_sum_d = [](double v) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  }
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+  };
+  auto rows_of = [&](int i) { return static_cast<double>(min(rows_per_block, HW - (i / cpg) * rows_per_block)); };
+  auto shift = [&](int i) {
+    return shift_x ? static_cast<double>(shift_x[static_cast<long long>(b) * HW * C + g * cpg + i % cpg]) : 0.0;
+  };
+  double sum = 0.0;
+  for (int i = lane; i < items; i += 32) sum += static_cast<double>(partial(i).x) + rows_of(i) * shift(i);
   const double n = static_cast<double>(HW) * cpg;
-  const double mean = sum / n;
-  double var = sq / n - mean * mean;
-  if (var < 0) var = 0;
+  const double mean = warp_sum_d(sum) / n;
+  // Chan et al.: M2 = sum_i M2_i + n_i (mean_i - mean)^2
+  double m2 = 0.0;
+  for (int i = lane; i < items; i += 32) {
+    const float2 v = partial(i);
+    const double ni = rows_of(i);
+    const double d = static_cast<double>(v.x) / ni + shift(i) - mean;
+    m2 += static_cast<double>(v.y) + ni * d * d;
+  }
+  const double var = warp_sum_d(m2) / n;
   const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  // shift = beta - mean * scale in fp64 with the fp32 scale, carried as hi + lo: y = fma(x, scale, hi) + lo is
+  // (x - mean) * scale + beta to fp32 rounding however large the mean (a one-float shift is off by ~2^-25 |mean| scale).
   for (int k = lane; k < cpg; k += 32) {
     const int c = g * cpg + k;
     const float sc = rstd * gamma[c];
+    const double sh = static_cast<double>(beta[c]) - mean * static_cast<double>(sc);
+    const float sh_hi = static_cast<float>(sh);
     scale_shift[(static_cast<long long>(b) * C + c) * 2] = sc;
-    scale_shift[(static_cast<long long>(b) * C + c) * 2 + 1] = beta[c] - static_cast<float>(mean) * sc;
+    scale_shift[(static_cast<long long>(b) * C + c) * 2 + 1] = sh_hi;
+    shift_lo[static_cast<long long>(b) * C + c] = static_cast<float>(sh - static_cast<double>(sh_hi));
   }
 }
 
 // SPLIT: instead of fp32 y, emit the bf16 hi/lo planes (y = hi + lo) the tensor-core convolution consumes (conv_tc.cu)
 template <bool SPLIT>
 __global__ void __launch_bounds__(256)
-gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scale_shift, float* __restrict__ y,
-                     bf16* __restrict__ y_hi, bf16* __restrict__ y_lo, long long total4, int HW, int C, int silu) {
+gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scale_shift, const float* __restrict__ shift_lo,
+                     float* __restrict__ y, bf16* __restrict__ y_hi, bf16* __restrict__ y_lo, long long total4, int HW, int C,
+                     int silu) {
   pdl_enter();
   const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= total4) return;
@@ -225,7 +270,9 @@ gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scal
   const float4 v = *reinterpret_cast<const float4*>(x + i * 4);
   const float4 s0 = *reinterpret_cast<const float4*>(scale_shift + (static_cast<long long>(b) * C + q * 4) * 2);
   const float4 s1 = *reinterpret_cast<const float4*>(scale_shift + (static_cast<long long>(b) * C + q * 4) * 2 + 4);
-  float o[4] = {fmaf(v.x, s0.x, s0.y), fmaf(v.y, s0.z, s0.w), fmaf(v.z, s1.x, s1.y), fmaf(v.w, s1.z, s1.w)};
+  const float4 l = *reinterpret_cast<const float4*>(shift_lo + static_cast<long long>(b) * C + q * 4);
+  float o[4] = {fmaf(v.x, s0.x, s0.y) + l.x, fmaf(v.y, s0.z, s0.w) + l.y, fmaf(v.z, s1.x, s1.y) + l.z,
+                fmaf(v.w, s1.z, s1.w) + l.w};
 #pragma unroll
   for (int j = 0; j < 4; ++j) o[j] = silu ? o[j] / (1.f + expf(-o[j])) : o[j];
   if (SPLIT) {
@@ -244,22 +291,24 @@ gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scal
 
 // 8 channels per thread variant of the SPLIT apply (two 16-byte loads in flight, 16-byte stores per plane)
 __global__ void __launch_bounds__(256)
-gn_apply_silu_split8_kernel(const float* __restrict__ x, const float* __restrict__ scale_shift, bf16* __restrict__ y_hi,
-                            bf16* __restrict__ y_lo, long long total8, int HW, int C, int silu) {
+gn_apply_silu_split8_kernel(const float* __restrict__ x, const float* __restrict__ scale_shift,
+                            const float* __restrict__ shift_lo, bf16* __restrict__ y_hi, bf16* __restrict__ y_lo,
+                            long long total8, int HW, int C, int silu) {
   pdl_enter();
   const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= total8) return;
   const int c8 = C / 8;
   const int q = static_cast<int>(i % c8);
   const int b = static_cast<int>(i / (static_cast<long long>(c8) * HW));
-  float v[8];
+  float v[8], sl[8];
   load8(x + i * 8, v);
+  load8(shift_lo + static_cast<long long>(b) * C + q * 8, sl);
   const float4* ssp = reinterpret_cast<const float4*>(scale_shift + (static_cast<long long>(b) * C + q * 8) * 2);
   float h[8], l[8];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const float4 s2 = ssp[j];  // {scale, shift} of channels 2j, 2j+1
-    float o0 = fmaf(v[2 * j], s2.x, s2.y), o1 = fmaf(v[2 * j + 1], s2.z, s2.w);
+    float o0 = fmaf(v[2 * j], s2.x, s2.y) + sl[2 * j], o1 = fmaf(v[2 * j + 1], s2.z, s2.w) + sl[2 * j + 1];
     if (silu) {
       o0 = o0 / (1.f + expf(-o0));
       o1 = o1 / (1.f + expf(-o1));
@@ -389,31 +438,37 @@ int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* be
     return MUSE_ERR_UNSUPPORTED;
   }
   if (B <= 0 || HW <= 0) return MUSE_OK;
-  // precomputed_tiles > 0: partials_ws already holds {sum, sumsq} per [image][tile][C], written by the epilogue of the
-  // tensor-core convolution that produced x (conv_tc.cu), and the statistics pass over x is skipped.
+  // precomputed_tiles > 0: partials_ws already holds {sum, M2} per [image][tile][C] (HW / tiles pixels each), written by the
+  // epilogue of the tensor-core convolution that produced x (conv_tc.cu), and the statistics pass over x is skipped.
   int nblocks = precomputed_tiles;
+  int rows_per_block = precomputed_tiles > 0 ? HW / precomputed_tiles : gn_rows_per_block(C);
   int rc;
+  if (precomputed_tiles > 0 && HW % precomputed_tiles != 0) {
+    set_last_error("groupnorm: %d precomputed tiles do not split HW=%d evenly", precomputed_tiles, HW);
+    return MUSE_ERR_INVALID;
+  }
   if (precomputed_tiles <= 0) {
-    const int rows_per_block = gn_rows_per_block(C);
     nblocks = ceil_div(HW, rows_per_block);
     const int rstep = 256 / (C / 4);
     pdl_launch(dim3(nblocks, B), 256, rstep * C * 2 * sizeof(float), s)(gn_stats_kernel, x, partials_ws, HW, C, rows_per_block);
     rc = check_launch("gn_stats");
     if (rc) return rc;
   }
-  pdl_launch(ceil_div(B * groups, 8), 256, 0, s)(gn_finalize_kernel, partials_ws, nblocks, gamma, beta, scale_shift_ws, B, HW, C,
-                                                             groups, eps);
+  float* shift_lo = scale_shift_ws + 2LL * B * C;
+  pdl_launch(ceil_div(B * groups, 8), 256, 0, s)(gn_finalize_kernel, partials_ws, nblocks, rows_per_block,
+                                                             precomputed_tiles > 0 ? nullptr : x, gamma, beta,
+                                                             scale_shift_ws, shift_lo, B, HW, C, groups, eps);
   rc = check_launch("gn_finalize");
   if (rc) return rc;
   const long long total4 = static_cast<long long>(B) * HW * (C / 4);
   const unsigned blocks = static_cast<unsigned>(ceil_div_ll(total4, 256));
   if (y != nullptr)
-    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<false>, x, scale_shift_ws, y, nullptr, nullptr, total4, HW, C, apply_silu);
+    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<false>, x, scale_shift_ws, shift_lo, y, nullptr, nullptr, total4, HW, C, apply_silu);
   else if (C % 8 == 0)
     pdl_launch(static_cast<unsigned>(ceil_div_ll(total4 / 2, 256)), 256, 0, s)(gn_apply_silu_split8_kernel,
-        x, scale_shift_ws, reinterpret_cast<bf16*>(y_hi), reinterpret_cast<bf16*>(y_lo), total4 / 2, HW, C, apply_silu);
+        x, scale_shift_ws, shift_lo, reinterpret_cast<bf16*>(y_hi), reinterpret_cast<bf16*>(y_lo), total4 / 2, HW, C, apply_silu);
   else
-    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<true>, x, scale_shift_ws, nullptr, reinterpret_cast<bf16*>(y_hi),
+    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<true>, x, scale_shift_ws, shift_lo, nullptr, reinterpret_cast<bf16*>(y_hi),
                                                       reinterpret_cast<bf16*>(y_lo), total4, HW, C, apply_silu);
   return check_launch("gn_apply_silu");
 }

@@ -21,7 +21,7 @@
 //   whose tile rows scatter to every other output pixel.
 // * The persistent warp-specialised pipeline of tc_pipeline.cuh (wgmma m64 x BN x k16 on the two 64-pixel halves of the
 //   tile); the epilogue adds bias / residual to the accumulator registers, writes fp32 NHWC rows and folds the
-//   per-channel GroupNorm statistics of the tile.
+//   per-channel GroupNorm statistics of the tile: its sum, then the squared deviations from the tile mean (M2).
 #include "common.cuh"
 #include "tc_host.cuh"
 #include "tc_pipeline.cuh"
@@ -32,8 +32,8 @@ namespace {
 
 using tc::BK;
 
-// Stages of the ring: a multiple of 1024 B for BN in {16, 128, 256}.  Behind them, per consumer warp, {sum, sumsq} of
-// every tile column.
+// Stages of the ring: a multiple of 1024 B for BN in {16, 128, 256}.  Behind them, per consumer warp, {sum, M2} of
+// every tile column over the warp's 16 pixels.
 template <int BN>
 using Ring = tc::Ring<BN, (BN == 256) ? 4 : (BN == 128 ? 6 : 8), 8 * BN * 2 * 4>;
 
@@ -41,7 +41,7 @@ struct ConvParams {
   float* y;
   const float* bias;
   const float* res;
-  float* stats;  // nullable: per [pixel tile][C_out] {sum, sumsq} of y, the GroupNorm statistics of the next layer
+  float* stats;  // nullable: per [pixel tile][C_out] {sum, M2} of y (M2 about the tile mean), the next GroupNorm's statistics
   int N;  // C_out
   int H, W, Cin, ksize;
   int tile_w, tile_h, tiles_x, tiles_per_img;
@@ -137,7 +137,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = n0 + 8 * j + lc;
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
         if (BN == 16) {  // narrow head (C_out <= 16, e.g. the 3-channel pixel output): element-wise, no statistics
 #pragma unroll
           for (int hr = 0; hr < 2; ++hr)
@@ -163,15 +162,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
               o.x += r2.x; o.y += r2.y;
             }
             *reinterpret_cast<float2*>(p.y + off) = o;
-            s0 += o.x; s1 += o.y;
-            q0 = fmaf(o.x, o.x, q0); q1 = fmaf(o.y, o.y, q1);
+            acc[4 * j + 2 * hr] = o.x; acc[4 * j + 2 * hr + 1] = o.y;  // y, for the statistics (the next tile overwrites acc)
           }
         }
-        if (BN != 16 && p.stats != nullptr) {  // fold the 8 row groups of the warp (lane >> 2); lanes 0-3 publish
+        if (BN != 16 && p.stats != nullptr) {
+          // the warp's 16 pixels of columns col, col + 1: sum over the 8 row groups (lane >> 2; the xor tree leaves it in
+          // every lane), then M2 about the warp's own mean.  Lanes 0-3 publish {sum, M2}.
+          float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
 #pragma unroll
           for (int o = 4; o < 32; o <<= 1) {
             s0 += __shfl_xor_sync(0xffffffffu, s0, o);
             s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+          }
+          const float m0 = s0 * (1.f / 16), m1 = s1 * (1.f / 16);
+          const float d00 = acc[4 * j] - m0, d01 = acc[4 * j + 2] - m0;
+          const float d10 = acc[4 * j + 1] - m1, d11 = acc[4 * j + 3] - m1;
+          float q0 = fmaf(d01, d01, d00 * d00), q1 = fmaf(d11, d11, d10 * d10);
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
             q0 += __shfl_xor_sync(0xffffffffu, q0, o);
             q1 += __shfl_xor_sync(0xffffffffu, q1, o);
           }
@@ -183,13 +191,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
         asm volatile("bar.sync 1, 256;" ::: "memory");  // the eight consumer warps
         for (int col = threadIdx.x - 128; col < BN; col += 256) {
           if (n0 + col < p.N) {
-            float2 a = make_float2(0.f, 0.f);
+            // the tile's {sum, M2} from the eight warps' {sum, M2} of 16 pixels each (Chan et al.), in warp order
+            float sw[8], s = 0.f, m2 = 0.f;
 #pragma unroll
             for (int wq = 0; wq < 8; ++wq) {
               const float2 v = *reinterpret_cast<const float2*>(stat_smem + ((wq * BN) + col) * 2);
-              a.x += v.x; a.y += v.y;
+              sw[wq] = v.x;
+              s += v.x; m2 += v.y;
             }
-            *reinterpret_cast<float2*>(p.stats + (stat_row * p.N + n0 + col) * 2) = a;
+            const float mean = s * (1.f / 128);
+#pragma unroll
+            for (int wq = 0; wq < 8; ++wq) {
+              const float d = fmaf(sw[wq], 1.f / 16, -mean);
+              m2 = fmaf(16.f * d, d, m2);
+            }
+            *reinterpret_cast<float2*>(p.stats + (stat_row * p.N + n0 + col) * 2) = make_float2(s, m2);
           }
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");

@@ -724,7 +724,7 @@ def _gn_scratch(x):
     if n_ws < 0:
         raise _lib.MuseB200Error(f"groupnorm: unsupported channel count {C}")
     return (torch.empty(n_ws, dtype=torch.float32, device=x.device),
-            torch.empty(B * C * 2, dtype=torch.float32, device=x.device))
+            torch.empty(B * C * 3, dtype=torch.float32, device=x.device))
 
 
 def _packed_conv_weight_upsample(w):
@@ -761,13 +761,14 @@ def _packed_conv_weight_upsample(w):
 
 
 def _conv_stats_buffer(y, H, W, Cin, Cout, k, up=0):
-    """The tensor-core convolution's epilogue leaves per-tile {sum, sumsq} of its output: they ride along on the output
-    tensor (``y._gn_stats``) so that a following conv2d(gn=...) skips the GroupNorm statistics pass over y."""
+    """The tensor-core convolution's epilogue leaves per-tile {sum, M2} of its output (M2: squared deviations from the tile
+    mean): they ride along on the output tensor (``y._gn_stats``, with y's version counter) so that a following
+    conv2d(gn=...) skips the GroupNorm statistics pass over y -- unless y was modified in place since."""
     if Cout <= 16 or Cout % 32 != 0:
         return None, 0
     tiles = _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, k, up)
     stats = torch.empty(y.shape[0], tiles, Cout, 2, dtype=torch.float32, device=y.device)
-    y._gn_stats = (stats, tiles)
+    y._gn_stats = (stats, tiles, y._version)
     return stats, tiles
 
 
@@ -809,10 +810,10 @@ def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None):
         lo = _lo_like(hi)
         if gn is not None:
             assert not upsample2x
-            pre = getattr(x, "_gn_stats", None)  # {sum, sumsq} tiles left by the convolution that produced x
-            if pre is not None:
-                ws, tiles = pre
-                ss = torch.empty(B * Cin * 2, dtype=torch.float32, device=x.device)
+            pre = getattr(x, "_gn_stats", None)  # {sum, M2} tiles left by the convolution that produced x
+            if pre is not None and pre[2] == x._version:
+                ws, tiles, _ = pre
+                ss = torch.empty(B * Cin * 3, dtype=torch.float32, device=x.device)
             else:
                 (ws, ss), tiles = _gn_scratch(x), 0
             _call("muse_groupnorm_silu_nhwc", _p(x), _p(gn[0].detach().float()), _p(gn[1].detach().float()), None, _p(hi),

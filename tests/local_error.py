@@ -87,6 +87,61 @@ def gemm_tiles(M: int, N: int, BN: int, BM: int = 128) -> Groups:
                   sizes.reshape(-1).double())
 
 
+def conv_bn(Cout: int) -> int:
+    """N tile of the tensor-core convolution (conv_tc.cu): 256, 128 or 16 output channels."""
+    return 256 if Cout >= 256 else (128 if Cout > 16 else 16)
+
+
+def conv_tile_pixels(t: torch.Tensor, up: bool = False) -> torch.Tensor:
+    """NHWC [B, H, W, C] -> [B, parities, tiles, 128, C]: the pixels of each 128-pixel tile of the tensor-core convolution,
+    tile_w = min(W, 128) wide and 128 / tile_w high, in the kernel's tile order.  up: the tiles are taken per parity
+    (py, px) on the H/2 x W/2 grid, parity = 2 py + px (the layout of the upsample statistics)."""
+    B, H, W, C = t.shape
+    if up:
+        H, W = H // 2, W // 2
+        t = t.reshape(B, H, 2, W, 2, C).permute(0, 2, 4, 1, 3, 5).reshape(B * 4, H, W, C)
+    tw = min(W, 128)
+    th = 128 // tw
+    t = t.reshape(-1, H // th, th, W // tw, tw, C).permute(0, 1, 3, 2, 4, 5)
+    return t.reshape(B, 4 if up else 1, (H // th) * (W // tw), 128, C)
+
+
+def conv_tiles(B: int, H: int, W: int, Cout: int, up: bool = False) -> Groups:
+    """NHWC output [B, H, W, Cout] of the tensor-core convolution -> one group per (image, parity, pixel tile, n tile).
+    The ragged last n tile is zero-padded in both tensors."""
+    BN = conv_bn(Cout)
+    nn = -(-Cout // BN)
+    h, w = (H // 2, W // 2) if up else (H, W)
+    tw = min(w, 128)
+    th = 128 // tw
+    tiles = (h // th) * (w // tw)
+    P = 4 if up else 1
+
+    def view(t):
+        p = conv_tile_pixels(t, up)
+        if nn * BN != Cout:
+            p = torch.cat([p, p.new_zeros(*p.shape[:-1], nn * BN - Cout)], -1)
+        return p.reshape(B, P, tiles, 128, nn, BN).permute(0, 1, 2, 4, 3, 5).reshape(-1, 128 * BN)
+
+    def where(g):
+        n, rest = g % nn, g // nn
+        tt, rest = rest % tiles, rest // tiles
+        par, img = rest % P, rest // P
+        y0, x0 = (tt // (w // tw)) * th, (tt % (w // tw)) * tw
+        return f"(image {img}, parity {par}, tile y0 {y0} x0 {x0}, n tile {n})" if up else \
+            f"(image {img}, tile y0 {y0} x0 {x0}, n tile {n})"
+
+    sizes = torch.tensor([128.0 * min(BN, Cout - n * BN) for n in range(nn)], dtype=torch.float64).repeat(B * P * tiles)
+    return Groups(view, where, sizes)
+
+
+def gn_groups(B: int, HW: int, C: int, G: int) -> Groups:
+    """NHWC [B, HW, C] -> one group per (image, GroupNorm group)."""
+    cpg = C // G
+    return Groups(lambda t: t.reshape(B, HW, G, cpg).permute(0, 2, 1, 3).reshape(B * G, HW * cpg),
+                  lambda g: f"(image {g // G}, group {g % G})")
+
+
 def check_local(out, ref, groups: Groups, bound: float, elem_bound: float, what: str) -> Local:
     d = groups.view(out.detach().double()) - groups.view(ref.detach().double())
     r = groups.view(ref.detach().double())
@@ -149,5 +204,15 @@ BOUNDS = {
     "grn.dx": (5e-3, 5e-2),        # 2.25e-3 / 2.13e-2
     "grn.dgamma": (1.2e-4, 1.2e-4),  # 5.20e-5 / 5.20e-5
     "grn.dbeta": (8e-7, 8e-7),     # 3.18e-7 / 3.18e-7
+    # tokenizer kernels (tests/test_tokenizer_local_gpu.py, same H100 SXM at 700 W), fp32 outputs against fp64 of the
+    # exact fp32 operands
+    "conv.bf16x3": (3.2e-5, 8e-4),   # 1.55e-5 / 3.98e-4
+    "conv.bf16": (5e-3, 7e-2),       # 2.38e-3 / 3.44e-2 (single-pass bf16 mode)
+    "conv.stats_sum": (2e-7, 1e-6),  # 9.12e-8 / 4.83e-7 (epilogue statistics against fp64 sums of the y written)
+    "conv.stats_m2": (3e-7, 2.5e-6),  # 1.51e-7 / 1.20e-6
+    "conv.simt": (6e-7, 1.2e-5),     # 2.61e-7 / 5.91e-6
+    "attn1.out": (3e-5, 3e-4),       # 1.50e-5 / 1.39e-4
+    "softmax.split": (1e-5, 3e-4),   # 4.97e-6 / 1.48e-4 (hi + lo: representation error 2^-18)
+    "softmax.f32": (3e-7, 4e-6),     # 1.46e-7 / 2.03e-6
 }
 ATTN_LSE_ABS = 4e-5  # max |lse - lse_ref| in natural-log units; measured 1.53e-5
