@@ -16,11 +16,29 @@ import torch
 from . import _lib, ops
 
 
+def _check_lr(lr, device=None):
+    """the kernel reads a tensor learning rate as ONE fp32 value at a device address: a host tensor would hand it a host
+    address, another dtype the wrong bits"""
+    if torch.is_tensor(lr) and (lr.numel() != 1 or lr.dtype != torch.float32 or (device is not None and lr.device != device)):
+        raise ValueError(f"FusedAdamW: a tensor lr must be a one-element float32 tensor on the parameters' device"
+                         f"{'' if device is None else ' ' + str(device)}; got {lr.numel()} element(s) of {lr.dtype} "
+                         f"on {lr.device}")
+
+
 class FusedAdamW(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, ema=None, model=None):
         """ema: an ``open_muse_b200.EMAModel`` built over the SAME parameter list (its shadow params are updated in the fused
         pass; do not also call ``ema.step``).  model: a ``MaskGitTransformer`` whose packed bf16 operand cache receives
-        the updated weights directly (saves the re-pack launch of the next forward)."""
+        the updated weights directly (saves the re-pack launch of the next forward).
+
+        lr: a Python number, or (for a CUDA-graph-capturable schedule) a one-element float32 tensor on the parameters'
+        device, read by the kernel at every step; ``step`` raises ValueError for any other tensor.
+
+        Every parameter of the groups is expected to have a gradient at every step, as in the training scripts.  A parameter
+        without one is left out of that step's pass: its EMA shadow does not move (``EMAModel.step`` would move it toward
+        the parameter), and its bias correction follows its group's step counter, which a group without any gradient does
+        not advance."""
+        _check_lr(lr)
         if lr < 0 or eps < 0 or not 0 <= betas[0] < 1 or not 0 <= betas[1] < 1 or weight_decay < 0:
             raise ValueError("invalid AdamW hyper-parameters")
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
@@ -43,23 +61,29 @@ class FusedAdamW(torch.optim.Optimizer):
 
     def _plan(self, gi, group, shadow_of, packed_dst):
         params = [p for p in group["params"] if p.grad is not None]
-        key = tuple((p.data_ptr(), p.grad.data_ptr()) for p in params)
+        # every address the kernel writes through is part of the key: EMAModel.load_state_dict / .to replace the shadow
+        # tensors while parameters and gradients stay where they are
+        key = tuple((p.data_ptr(), p.grad.data_ptr(), 0 if shadow_of.get(id(p)) is None else shadow_of[id(p)].data_ptr(),
+                     packed_dst.get(p.data_ptr(), 0)) for p in params)
         plan = self._plans.get(gi)
         if plan is not None and plan["key"] == key:
             return plan
         entries = []
         dev = params[0].device
-        for p in params:
+        for p, (_, _, sh_ptr, packed_ptr) in zip(params, key):
             if p.dtype != torch.float32 or p.grad.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous() \
                     or p.numel() % 4 != 0 or p.grad.is_sparse:
                 raise RuntimeError("FusedAdamW needs contiguous fp32 parameters / gradients with numel % 4 == 0")
+            sh = shadow_of.get(id(p))
+            if sh is not None and (sh.dtype != torch.float32 or sh.device != p.device or sh.shape != p.shape
+                                   or not sh.is_contiguous()):
+                raise RuntimeError("FusedAdamW(ema=...) needs contiguous fp32 EMA shadows shaped and placed like the parameters")
             st = self.state[p]
             if not st:
                 st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                 st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-            sh = shadow_of.get(id(p))
             entries.append((p.data_ptr(), p.grad.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(),
-                            0 if sh is None else sh.data_ptr(), packed_dst.get(p.data_ptr(), 0), p.numel(), 0))
+                            sh_ptr, packed_ptr, p.numel(), 0))
         plan = self._plans.get(gi) or {}
         if "step" not in plan:
             # one device-resident step counter per group, shared by the group's parameters' state entries so that
@@ -90,9 +114,10 @@ class FusedAdamW(torch.optim.Optimizer):
             flat = [p for g in self.param_groups for p in g["params"]]
             shadow_of = {id(p): s for p, s in zip(flat, ema.shadow_params)}
         packed_dst = self._packed_dst()
-        for gi, group in enumerate(self.param_groups):
-            if not any(p.grad is not None for p in group["params"]):
-                continue
+        live = [(gi, group) for gi, group in enumerate(self.param_groups) if any(p.grad is not None for p in group["params"])]
+        for _, group in live:  # every group before the first launch (a scheduler may have assigned any tensor)
+            _check_lr(group["lr"], next(p.device for p in group["params"] if p.grad is not None))
+        for gi, group in live:
             plan = self._plan(gi, group, shadow_of, packed_dst)
             lr = group["lr"]
             lr_dev = lr if torch.is_tensor(lr) else None

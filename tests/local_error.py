@@ -164,6 +164,119 @@ def check_local(out, ref, groups: Groups, bound: float, elem_bound: float, what:
     return res
 
 
+def check_abs(out, ref, where: Callable[[int], str], bound: float, what: str) -> Local:
+    """one value per row (a log-sum-exp, a row's loss): the largest absolute error and its row"""
+    d = torch.nan_to_num((out.detach().double() - ref.detach().double()).abs().reshape(-1), nan=math.inf)
+    top = torch.topk(d, min(2, d.numel()))
+    gi = [int(i) for i in top.indices]
+    whole = float(d.norm() / ref.detach().double().norm().clamp_min(1e-300))
+    res = Local(float(top.values[0]), where(gi[0]), float(top.values[-1]), where(gi[-1]), float(top.values[0]),
+                where(gi[0]), whole)
+    assert res.worst <= bound, (f"{what}: worst absolute error {res.worst:.3e} at {res.where} (bound {bound:.1e}); "
+                                f"next worst {res.second:.3e} at {res.second_where}; whole-tensor rel-L2 {whole:.3e}")
+    return res
+
+
+# ------------------------------------------------------------------------------------------------ element-wise fp32 kernels
+ULP32 = 2.0 ** -24  # unit roundoff of fp32
+
+
+def check_ulps(out, ref, terms, group, where: Callable[[int], str], bound: float, what: str) -> Local:
+    """Element-wise kernels (no reduction): the error of each element in fp32 units of its own terms,
+    |out - ref| / (2^-24 * terms), where `terms` is the sum of the magnitudes of what the kernel adds up for that element.
+    A whole-tensor rel-L2 of an updated parameter is dominated by the unchanged part and hides a wrong update; this does
+    not.  An element whose terms are all zero must be exact.  group: int64 id per element (a kernel block); the failure
+    names the group with the largest error."""
+    d = (out.detach().double() - ref.detach().double()).abs()
+    den = terms.detach().double() * ULP32
+    e = torch.where(d == 0, torch.zeros_like(d), d / den)  # d != 0 over zero terms: inf
+    e = torch.nan_to_num(e, nan=math.inf)
+    n = int(group.max()) + 1
+    per = torch.zeros(n, dtype=e.dtype, device=e.device).scatter_reduce_(0, group, e, "amax", include_self=True)
+    top = torch.topk(per, min(2, n))
+    gi = [int(i) for i in top.indices]
+    whole = float(d.norm() / ref.detach().double().norm().clamp_min(1e-300))
+    res = Local(float(top.values[0]), where(gi[0]), float(top.values[-1]) if n > 1 else 0.0,
+                where(gi[-1]) if n > 1 else "-", float(top.values[0]), where(gi[0]), whole)
+    assert res.worst <= bound, (f"{what}: worst element {res.worst:.2f} ulps of its terms at {res.where} (bound {bound}); "
+                                f"next worst group {res.second:.2f} at {res.second_where}; whole-tensor rel-L2 {whole:.3e}")
+    return res
+
+
+@dataclass
+class AdamHyper:
+    """what the kernel receives, as fp64 values of its fp32 arguments; inv_bc1 / inv_sqrt_bc2 / omd in fp64 from the
+    formulas (omd = 1 - EMA decay, None: no EMA update this step)"""
+    lr: float
+    beta1: float
+    beta2: float
+    eps: float
+    weight_decay: float
+    step: int
+    omd: float | None
+
+    @property
+    def inv_bc1(self):
+        return 1.0 / (1.0 - self.beta1 ** self.step)
+
+    @property
+    def inv_sqrt_bc2(self):
+        return 1.0 / math.sqrt(1.0 - self.beta2 ** self.step)
+
+
+def f32(x: float) -> float:
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def adamw_ref(p, g, m, v, h: AdamHyper):
+    """fp64 AdamW of csrc/optim.cu from fp32 operands: {name: (reference, terms)} for p, m, v (terms for check_ulps)"""
+    p, g, m, v = (t.double() for t in (p, g, m, v))
+    c1, c2 = 1.0 - h.beta1, 1.0 - h.beta2
+    wd = h.lr * h.weight_decay * p
+    m1 = m + c1 * (g - m)
+    m1_terms = m.abs() + c1 * (g - m).abs()
+    v1 = h.beta2 * v + c2 * g * g
+    den = v1.sqrt() * h.inv_sqrt_bc2 + h.eps
+    step = h.lr * h.inv_bc1
+    p1 = p - wd - step * m1 / den
+    return {"p": (p1, p.abs() + wd.abs() + step * m1_terms / den), "m": (m1, m1_terms), "v": (v1, v1)}
+
+
+def ema_ref(s, p_new, omd: float):
+    """fp64 EMA step s - (1 - decay) (s - p') from the kernel's own updated p' (its error is measured on its own)"""
+    s, p_new = s.double(), p_new.double()
+    return s - omd * (s - p_new), s.abs() + omd * (s - p_new).abs()
+
+
+# ------------------------------------------------------------------------------------------------ cross-entropy forward
+def ce_inputs(rows: int, V: int, ld: int, seed: int):
+    """fp32 logits [rows, ld] (bf16-exact, zero pad columns) and int64 labels: random rows plus the special ones -- a
+    dominant +60 logit (labelled elsewhere / on the label), an all-equal row, labels at columns 0 and V - 1, a dominant
+    logit in the scalar-tail column V - 1, ignored rows"""
+    g = torch.Generator().manual_seed(seed)
+    logits = torch.zeros(rows, ld)
+    logits[:, :V] = torch.randn(rows, V, generator=g) * 2
+    labels = torch.randint(0, V, (rows,), generator=g)
+    labels[torch.rand(rows, generator=g) < 0.3] = -100
+    labels[0], labels[1], labels[rows - 1] = 0, V - 1, V - 1
+    logits[2, 5], labels[2] = 60.0, 7          # one +60 logit, labelled elsewhere
+    logits[3, 9], labels[3] = 60.0, 9          # one +60 logit on the label
+    logits[4, :V], labels[4] = 1.5, 11         # all-equal row
+    logits[5, V - 1], labels[5] = 12.0, 3      # dominant logit in the last column
+    labels[6] = labels[rows - 2] = -100
+    return logits.to(torch.bfloat16).float(), labels
+
+
+def ce_fwd_ref(logits, labels, V: int, ls: float):
+    """fp64 (lse, row loss) of the label-smoothed cross-entropy per row; ignored rows have loss 0"""
+    x = logits[:, :V].double()
+    lse = torch.logsumexp(x, -1)
+    valid = labels != -100
+    zy = x.gather(1, labels.clamp_min(0)[:, None])[:, 0]
+    loss = (1 - ls) * (lse - zy) + ls * (lse - x.mean(-1))
+    return lse, torch.where(valid, loss, torch.zeros_like(loss))
+
+
 # (group bound, elementwise bound) per kernel output; the comment gives the worst group / elementwise error measured on
 # an H100 SXM (700 W) over all cases of tests/test_kernel_local_gpu.py.
 BOUNDS = {
@@ -214,5 +327,16 @@ BOUNDS = {
     "attn1.out": (3e-5, 3e-4),       # 1.50e-5 / 1.39e-4
     "softmax.split": (1e-5, 3e-4),   # 4.97e-6 / 1.48e-4 (hi + lo: representation error 2^-18)
     "softmax.f32": (3e-7, 4e-6),     # 1.46e-7 / 2.03e-6
+    # fused AdamW + EMA step (tests/test_optim_local_gpu.py, same H100 SXM at 700 W): worst element error in fp32 ulps
+    # of its own terms (check_ulps), the same number for the group and the element
+    "adamw.p": (10.0, 10.0),       # 4.91
+    "adamw.m": (4.0, 4.0),         # 1.80
+    "adamw.v": (6.0, 6.0),         # 2.82
+    "adamw.ema": (5.0, 5.0),       # 2.48
+    # cross-entropy forward per row (tests/test_kernel_local_gpu.py): absolute error of the row's log-sum-exp and loss
+    # (natural-log units); relative error of the mean and of the row_scale-weighted sum
+    "ce.lse": (1.5e-6, 1.5e-6),    # 7.47e-7
+    "ce.loss": (4e-6, 4e-6),       # 2.01e-6 (the +60 logit row)
+    "ce.mean": (2.5e-7, 2.5e-7),   # 1.03e-7
 }
 ATTN_LSE_ABS = 4e-5  # max |lse - lse_ref| in natural-log units; measured 1.53e-5

@@ -14,8 +14,8 @@ import pytest
 import torch
 
 from open_muse_b200 import ops
-from tests.local_error import (ATTN_LSE_ABS, BOUNDS, Groups, attn_rows, balanced_rows, check_local, gemm_rows,
-                               gemm_tiles)
+from tests.local_error import (ATTN_LSE_ABS, BOUNDS, Groups, Local, attn_rows, balanced_rows, ce_fwd_ref, ce_inputs,
+                               check_abs, check_local, gemm_rows, gemm_tiles)
 from tests.local_error import rows as by_row
 from tests.test_dropout_cpu import keep_scale, unpack_bits
 from tests.test_gemm_epilogue_gpu import EPI_SPLITK_F32, _gemm
@@ -338,6 +338,57 @@ def test_ce_bwd_local(ls, weighted):
     ref[~valid] = 0
     _check("ce.dlogits", dl[:, :V], ref, by_row(rows), case)
     assert bool((dl[:, V:] == 0).all()) and bool((dl[~valid] == 0).all()), case  # exact zeros
+
+
+def _check_abs(key, out, ref, case):
+    res = check_abs(out, ref, lambda r: f"row {r}", BOUNDS[key][0], f"{key} {case}")
+    if key not in _worst or res.worst > _worst[key][0].worst:
+        _worst[key] = (res, case)
+
+
+def _check_rel(key, out, ref, case):
+    err = abs(float(out) - float(ref)) / abs(float(ref))
+    assert err <= BOUNDS[key][0], f"{key} {case}: relative error {err:.3e} (bound {BOUNDS[key][0]:.1e})"
+    if key not in _worst or err > _worst[key][0].worst:
+        _worst[key] = (Local(err, "-", 0.0, "-", err, "-", err), case)
+
+
+@pytest.mark.parametrize("ls", [0.0, 0.1])
+@pytest.mark.parametrize("V,ld", [(2025, 2048), (1024, 1024), (8192, 8192)])
+def test_ce_fwd_local(V, ld, ls):
+    """every row's log-sum-exp and loss (U-ViT v2 weights the row losses directly), the mean, the valid count and the
+    row_scale-weighted loss as uvit_v2_train.TailFn forms it; V = 2025 sends column 2024 through the scalar tail loop"""
+    rows = 389
+    case = f"(rows {rows}, V {V}, ld {ld}, label smoothing {ls})"
+    logits, labels = ce_inputs(rows, V, ld, 15)
+    logits, labels = logits.to(BF).to(DEV), labels.to(DEV)
+    out, ws = ops.ce_fwd(logits, labels, V, ls)
+    lw = (torch.rand(rows, generator=torch.Generator().manual_seed(16)) + 0.1).to(DEV)
+    row_scale = lw / lw.sum()
+    weighted = (ws[1] * row_scale).sum()
+    torch.cuda.synchronize()
+    lse_ref, loss_ref = ce_fwd_ref(logits, labels, V, ls)
+    valid = labels != -100
+    _check_abs("ce.lse", ws[0], lse_ref, case)
+    _check_abs("ce.loss", ws[1], loss_ref, case)
+    assert bool((ws[1][~valid] == 0).all()), f"{case}: an ignored row has a non-zero loss"
+    assert float(out[1]) == float(valid.sum()), case
+    _check_rel("ce.mean", out[0], loss_ref[valid].mean(), case + " mean")
+    _check_rel("ce.mean", weighted, (loss_ref * row_scale.double()).sum(), case + " row_scale-weighted")
+
+
+def test_ce_fwd_all_rows_ignored():
+    """no valid row: the mean is NaN and the count 0, as torch's mean cross-entropy gives"""
+    rows, V, ld = 37, 2025, 2048
+    logits, _ = ce_inputs(rows, V, ld, 17)
+    labels = torch.full((rows,), -100, dtype=torch.int64)
+    out, ws = ops.ce_fwd(logits.to(BF).to(DEV), labels.to(DEV), V, 0.1)
+    torch.cuda.synchronize()
+    want = torch.nn.functional.cross_entropy(logits[:, :V].to(BF).double(), labels, ignore_index=-100, label_smoothing=0.1)
+    assert math.isnan(float(want)) and math.isnan(float(out[0])) and float(out[1]) == 0.0
+    assert bool((ws[1] == 0).all())
+    lse_ref = ce_fwd_ref(logits.to(BF).to(DEV), labels.to(DEV), V, 0.1)[0]
+    check_abs(ws[0], lse_ref, lambda r: f"row {r}", BOUNDS["ce.lse"][0], "ce.lse (all rows ignored)")
 
 
 # ------------------------------------------------------------------------------------------------------------ U-ViT

@@ -9,7 +9,8 @@ import math
 import pytest
 import torch
 
-from tests.local_error import BOUNDS, attn_rows, balanced_rows, check_local, gemm_rows, gemm_tiles, rows
+from tests.local_error import (BOUNDS, attn_rows, balanced_rows, ce_fwd_ref, ce_inputs, check_abs, check_local, gemm_rows,
+                               gemm_tiles, rows)
 
 F64 = torch.float64
 
@@ -191,6 +192,43 @@ def test_add_norm_mod_bwd_mutant_is_rejected():
     print(f"\ndmod of one sample missing its last row: whole-tensor rel-L2 {_whole(out, ref):.2e} (old tolerance 1.0e-04)")
     with pytest.raises(AssertionError, match="worst group error"):
         check_local(out.view(2 * NB, NH), ref.view(2 * NB, NH), _dmod_groups(), *BOUNDS["anm.dmod"], "anm.dmod")
+
+
+# ------------------------------------------------------------------------------------------------------------ CE forward
+CR, CV, CLD = 389, 2025, 2048  # the real vocabulary: column 2024 is the scalar tail of the kernel's 8-wide loop
+
+
+def _ce_fwd(ls, mutant=None):
+    """(lse, row loss) of an fp32 emulation of ce_fwd (max, sum of exp, log and the logit sum in fp32) and the fp64
+    reference"""
+    logits, labels = ce_inputs(CR, CV, CLD, 15)
+    x = logits[:, :CV - 1] if mutant == "tail column V - 1 dropped from the LSE" else logits[:, :CV]
+    m = x.amax(-1)
+    lse = m + torch.exp(x - m[:, None]).sum(-1).log()
+    z = logits[:, :CV]
+    div = CV - 1 if mutant == "smoothing term divides by V - 1" else CV
+    zy = z.gather(1, labels.clamp_min(0)[:, None])[:, 0]
+    loss = (1 - ls) * (lse - zy) + ls * (lse - z.sum(-1) / div)
+    loss = torch.where(labels != -100, loss, torch.zeros_like(loss))
+    return (lse, loss), ce_fwd_ref(logits, labels, CV, ls)
+
+
+@pytest.mark.parametrize("ls", [0.0, 0.1])
+def test_ce_fwd_emulation_is_accepted(ls):
+    (lse, loss), (lse_ref, loss_ref) = _ce_fwd(ls)
+    check_abs(lse, lse_ref, lambda r: f"row {r}", BOUNDS["ce.lse"][0], "ce.lse")
+    check_abs(loss, loss_ref, lambda r: f"row {r}", BOUNDS["ce.loss"][0], "ce.loss")
+
+
+@pytest.mark.parametrize("mutant,output", [("tail column V - 1 dropped from the LSE", 0),
+                                           ("smoothing term divides by V - 1", 1)])
+def test_ce_fwd_mutant_is_rejected(mutant, output):
+    out, ref = _ce_fwd(0.1, mutant)
+    key = ("ce.lse", "ce.loss")[output]
+    print(f"\n{mutant}: {key} whole-tensor rel-L2 {_whole(out[output].double(), ref[output]):.2e}, mean loss error "
+          f"{abs(float(out[1][ref[1] != 0].double().mean() - ref[1][ref[1] != 0].mean())):.2e}")
+    with pytest.raises(AssertionError, match="worst absolute error"):
+        check_abs(out[output], ref[output], lambda r: f"row {r}", BOUNDS[key][0], key)
 
 
 def test_bf16_bounds_stay_below_the_mutation_floor():
