@@ -114,7 +114,8 @@ int muse_embed_bwd_sorted(const long long* order, const long long* bounds, const
 /* LayerNorm (weight only, :124-137) / RMSNorm (:79-100) over the last dim of [rows,H].
  *   y = (res ? res : 0) + norm(v) * w ; mean/rstd [rows] are saved for backward.  v = x (act 0), gelu(x) (act 1: the
  *   exact-erf GELU of MlmLayer :980-983) or, with act 2, x is [rows, 2H] = [a | b] and v = bf16(gelu(a)) * b: the
- *   FeedForward GLU product (:789-792) feeding mid_mlp_layer_norm (:795-796) without materialising it.
+ *   FeedForward GLU product (:789-792) feeding mid_mlp_layer_norm (:795-796) without materialising it; act 2 takes
+ *   bf16 x and y only (an fp32 one returns MUSE_ERR_UNSUPPORTED).
  *   rms = 1 selects RMSNorm.
  * bits (nullable; act 2, bf16 x / y, no res): FeedForward.dropout (:797) fused into the pass that produces the wo
  * operand: y is the dropped output, bits [rows, ceil(H / 32)] written. */
@@ -127,6 +128,7 @@ int muse_norm_fwd(const void* x, int x_dtype, const float* w, const float* res, 
  *   dw_ws given (muse_norm_bwd_workspace_floats(rows, H, act) floats): dw is STORED, reduced in a fixed order -> run-to-run
  *   bit-identical, no zero fill needed; dw_ws null: dw += ... with atomics (caller zero-fills; order-dependent).
  * act 2: dx is [rows, 2H] = d[a | b] (LayerNorm backward and GLU backward in one pass; v is recomputed from x).
+ *   act 2 takes bf16 dy, x and dx only: an fp32 one returns MUSE_ERR_UNSUPPORTED.
  * y_fwd (nullable, act 2 with bf16 tensors only): the forward output bf16 [rows, H]; when given, the row reductions of
  * the first pass come from (dy, y_fwd) alone instead of re-evaluating the GELU over [a | b].
  * bits (nullable; act 2, bf16 dy / x / dx, no dres, no dx_bf16_copy, no y_fwd): the bits muse_norm_fwd wrote; dy (the

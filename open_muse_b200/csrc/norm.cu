@@ -11,15 +11,15 @@
 //   * backward: dx = norm_bwd(dy) (+ dres), so the residual-stream gradient add is free.
 //   * act=2 with dropout: FeedForward.dropout (:797) on the normalised output -- the forward draws the keep bits
 //              (philox.cuh) and writes the dropped bf16 output and the bits, the backward scales dy by them as it reads it
-#include "common.cuh"
 #include "philox.cuh"
+#include "row_norm.cuh"
 
 namespace muse {
 namespace {
 
 constexpr int ACT_NONE = 0, ACT_GELU = 1, ACT_GLU = 2;
 
-// ---- warp-per-row kernels (H <= 1024, no GLU): the whole row lives in registers, no block barriers
+// ---- warp-per-row kernels (H <= 1024, no GLU): the whole row lives in registers (row_norm.cuh), no block barriers
 constexpr int kWarpsPerBlock = 4;
 
 template <typename TX, typename TY, int CH>
@@ -33,39 +33,16 @@ norm_fwd_warp_kernel(const TX* __restrict__ x, const float* __restrict__ w, cons
   if (row >= rows) return;
   const TX* xr = x + static_cast<size_t>(row) * H;
   float v[CH][8];
-  float sum = 0.f;
-#pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < H) {
-      load8(xr + col, v[c]);
-      if (act) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[c][j] = gelu_f(v[c][j]);
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += v[c][j];
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[c][j] = 0.f;
-    }
-  }
   const float inv_h = 1.0f / static_cast<float>(H);
-  float mean = rms ? 0.f : warp_sum(sum) * inv_h;
-  float sq = 0.f;
+  const float sum = row_load(v, H, lane, [&](int col, float (&vc)[8]) {
+    load8(xr + col, vc);
+    if (act) {
 #pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < H) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = v[c][j] - mean;
-        sq += d * d;
-      }
+      for (int j = 0; j < 8; ++j) vc[j] = gelu_f(vc[j]);
     }
-  }
-  const float var = warp_sum(sq) * inv_h;
-  const float rstd = rsqrtf(var + eps);
+  });
+  float mean, rstd;
+  row_stats(v, sum, H, inv_h, lane, eps, rms, mean, rstd);
   if (lane == 0) {
     if (mean_out) mean_out[row] = mean;
     if (rstd_out) rstd_out[row] = rstd;
@@ -74,7 +51,7 @@ norm_fwd_warp_kernel(const TX* __restrict__ x, const float* __restrict__ w, cons
   const float* rr = res ? res + static_cast<size_t>(row) * H : nullptr;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    const int col = row_col(c, lane);
     if (col < H) {
       float o[8], wv[8];
       if (w) load8(w + col, wv);
@@ -134,22 +111,20 @@ __global__ void __launch_bounds__(1024) colsum_ordered_kernel(const float* __res
 // exposed load latency rather than by issue slots or DRAM bandwidth.  A warp walks its rows strictly one after the
 // other, so the lines of the row it will touch NEXT are requested from HBM while the current row is processed and the demand
 // loads become L2 hits.  prefetch_row: the lanes of a warp cover the 128-byte lines of one row of H elements.
+// The GLU + LayerNorm backward prefetches two loop iterations ahead instead (see glu_norm_bwd_kernel).
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 template <typename T>
 __device__ __forceinline__ void prefetch_row(const T* row, int H, int lane) {
   const int bytes = H * static_cast<int>(sizeof(T));
   for (int off = lane * 128; off < bytes; off += 32 * 128) prefetch_l2(reinterpret_cast<const char*>(row) + off);
 }
-// Next-row prefetch for the LayerNorm backward, two iterations ahead for GLU + LayerNorm backward.  The kernels take the
-// switch as an argument so that an A/B comparison needs one binary.
-constexpr int kRowPrefetch = 1;
 
 template <typename TDY, typename TX, typename TDX, int CH>
 __global__ void __launch_bounds__(kBwdWarps * 32)
 norm_bwd_warp_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const float* __restrict__ w,
                 const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                 const float* __restrict__ dres, TDX* __restrict__ dx, bf16* __restrict__ dx_copy, float* __restrict__ dw,
-                float* __restrict__ dw_ws, int rows, int H, int act, int rms, int pf) {
+                float* __restrict__ dw_ws, int rows, int H, int act, int rms) {
   pdl_enter();
   extern __shared__ float s_dw[];  // [kBwdWarps][H] private rows
   const int lane = threadIdx.x & 31;
@@ -170,14 +145,14 @@ norm_bwd_warp_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
     float s1 = 0.f, s2 = 0.f;
     const float* drr = dres ? dres + static_cast<size_t>(row) * H : nullptr;
     const int next = row + gridDim.x * kBwdWarps;
-    if (pf && next < rows) {  // this warp's next row (see prefetch_row)
+    if (next < rows) {  // this warp's next row (see prefetch_row)
       prefetch_row(x + static_cast<size_t>(next) * H, H, lane);
       prefetch_row(dy + static_cast<size_t>(next) * H, H, lane);
       if (dres) prefetch_row(dres + static_cast<size_t>(next) * H, H, lane);
     }
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float xv[8], dv[8], wv[8];
         load8(xr + col, xv);
@@ -190,21 +165,19 @@ norm_bwd_warp_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
           xh[c][j] = (a - mean) * rstd;
           dw_acc[c][j] += dv[j] * xh[c][j];
           g[c][j] = dv[j] * (w ? wv[j] : 1.f);
-          s1 += g[c][j];
-          s2 += g[c][j] * xh[c][j];
+          row_bwd_acc(g[c][j], xh[c][j], s1, s2);
         }
       }
     }
-    s1 = rms ? 0.f : warp_sum(s1) * inv_h;
-    s2 = warp_sum(s2) * inv_h;
+    row_bwd_sums(inv_h, rms, s1, s2);
     TDX* dxr = dx + static_cast<size_t>(row) * H;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float o[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = rstd * (g[c][j] - s1 - xh[c][j] * s2);
+        for (int j = 0; j < 8; ++j) o[j] = row_dx(g[c][j], xh[c][j], s1, s2, rstd);
         if (act) {
           float xv[8];
           load8(xr + col, xv);
@@ -226,7 +199,7 @@ norm_bwd_warp_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
     float* my_dw = s_dw + static_cast<size_t>(warp) * H;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) store8(my_dw + col, dw_acc[c]);
     }
     flush_cta_dw(s_dw, kBwdWarps, H, dw, dw_ws);
@@ -251,33 +224,14 @@ norm2_fwd_warp_kernel(const bf16* __restrict__ a, const float* __restrict__ res,
   if (row >= rows) return;
   const float inv_h = 1.0f / static_cast<float>(H);
   float v[CH][8];
-  float sum = 0.f;
-#pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < H) {
-      load8(a + static_cast<size_t>(row) * H + col, v[c]);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += v[c][j];
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[c][j] = 0.f;
-    }
-  }
-  const float mean1 = rms1 ? 0.f : warp_sum(sum) * inv_h;
-  float sq = 0.f;
-#pragma unroll
-  for (int c = 0; c < CH; ++c)
-    if ((c * 32 + lane) * 8 < H) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { const float d = v[c][j] - mean1; sq += d * d; }
-    }
-  const float rstd1 = rsqrtf(warp_sum(sq) * inv_h + eps);
+  const float sum1 = row_load(v, H, lane, [&](int col, float (&vc)[8]) { load8(a + static_cast<size_t>(row) * H + col, vc); });
+  float mean1, rstd1;
+  row_stats(v, sum1, H, inv_h, lane, eps, rms1, mean1, rstd1);
   // x2 = res + norm1(a) * w1  (kept in v), second statistics over x2
   float sum2 = 0.f;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    const int col = row_col(c, lane);
     if (col < H) {
       float wv[8], r8[8];
       load8(w1 + col, wv);
@@ -290,21 +244,14 @@ norm2_fwd_warp_kernel(const bf16* __restrict__ a, const float* __restrict__ res,
       store8(x2 + static_cast<size_t>(row) * H + col, v[c]);
     }
   }
-  const float mean2 = rms2 ? 0.f : warp_sum(sum2) * inv_h;
-  float sq2 = 0.f;
-#pragma unroll
-  for (int c = 0; c < CH; ++c)
-    if ((c * 32 + lane) * 8 < H) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { const float d = v[c][j] - mean2; sq2 += d * d; }
-    }
-  const float rstd2 = rsqrtf(warp_sum(sq2) * inv_h + eps);
+  float mean2, rstd2;
+  row_stats(v, sum2, H, inv_h, lane, eps, rms2, mean2, rstd2);
   if (lane == 0) {
     if (mean1_out) { mean1_out[row] = mean1; rstd1_out[row] = rstd1; mean2_out[row] = mean2; rstd2_out[row] = rstd2; }
   }
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    const int col = row_col(c, lane);
     if (col < H) {
       float wv[8], o[8];
       load8(w2 + col, wv);
@@ -322,7 +269,7 @@ norm2_bwd_warp_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x
                       const float* __restrict__ mean2_in, const float* __restrict__ rstd2_in, const float* __restrict__ dres,
                       const bf16* __restrict__ a, const float* __restrict__ w1, const float* __restrict__ mean1_in,
                       const float* __restrict__ rstd1_in, float* __restrict__ dx2, bf16* __restrict__ d_a,
-                      float* __restrict__ dw2_ws, float* __restrict__ dw1_ws, int rows, int H, int rms1, int rms2, int pf) {
+                      float* __restrict__ dw2_ws, float* __restrict__ dw1_ws, int rows, int H, int rms1, int rms2) {
   pdl_enter();
   extern __shared__ float s_dw[];  // [2][kBwdWarps][H] private rows (dw2 then dw1)
   const int lane = threadIdx.x & 31;
@@ -340,7 +287,7 @@ norm2_bwd_warp_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x
     float xh[CH][8], g[CH][8], rs[CH][8], av[CH][8];
     float s1 = 0.f, s2 = 0.f;
     const int next = row + gridDim.x * kBwdWarps;
-    if (pf && next < rows) {  // this warp's next row (see prefetch_row)
+    if (next < rows) {  // this warp's next row (see prefetch_row)
       const size_t noff = static_cast<size_t>(next) * H;
       prefetch_row(x2 + noff, H, lane);
       prefetch_row(d_h2 + noff, H, lane);
@@ -349,7 +296,7 @@ norm2_bwd_warp_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x
     }
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float xv[8], dv[8], wv[8];
         load8(x2 + off + col, xv);
@@ -362,43 +309,39 @@ norm2_bwd_warp_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x
           xh[c][j] = (xv[j] - mean2) * rstd2;
           acc2[c][j] += dv[j] * xh[c][j];
           g[c][j] = dv[j] * wv[j];
-          s1 += g[c][j];
-          s2 += g[c][j] * xh[c][j];
+          row_bwd_acc(g[c][j], xh[c][j], s1, s2);
         }
       }
     }
-    s1 = rms2 ? 0.f : warp_sum(s1) * inv_h;
-    s2 = warp_sum(s2) * inv_h;
+    row_bwd_sums(inv_h, rms2, s1, s2);
     float t1 = 0.f, t2 = 0.f;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float wv[8];
         load8(w1 + col, wv);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const float d2 = rstd2 * (g[c][j] - s1 - xh[c][j] * s2) + rs[c][j];  // dx2
+          const float d2 = row_dx(g[c][j], xh[c][j], s1, s2, rstd2) + rs[c][j];  // dx2
           rs[c][j] = d2;
           const float ah = (av[c][j] - mean1) * rstd1;
           av[c][j] = ah;
           acc1[c][j] += d2 * ah;
           g[c][j] = d2 * wv[j];
-          t1 += g[c][j];
-          t2 += g[c][j] * ah;
+          row_bwd_acc(g[c][j], ah, t1, t2);
         }
         store8(dx2 + off + col, rs[c]);
       }
     }
-    t1 = rms1 ? 0.f : warp_sum(t1) * inv_h;
-    t2 = warp_sum(t2) * inv_h;
+    row_bwd_sums(inv_h, rms1, t1, t2);
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float o[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = rstd1 * (g[c][j] - t1 - av[c][j] * t2);
+        for (int j = 0; j < 8; ++j) o[j] = row_dx(g[c][j], av[c][j], t1, t2, rstd1);
         store8(d_a + off + col, o);
       }
     }
@@ -407,7 +350,7 @@ norm2_bwd_warp_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x
   float* my1 = s_dw + static_cast<size_t>(kBwdWarps + warp) * H;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    const int col = row_col(c, lane);
     if (col < H) { store8(my2 + col, acc2[c]); store8(my1 + col, acc1[c]); }
   }
   __syncthreads();
@@ -422,35 +365,21 @@ norm2_bwd_warp_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x
   }
 }
 
-// ---- wide rows (H > 1024) and GLU mode: warp-per-row STREAMING kernels.  Nothing row-sized lives in registers:
+// ---- wide rows (H > 1024): warp-per-row STREAMING kernels.  Nothing row-sized lives in registers:
 // pass 1 streams the row for the statistics, pass 2 streams it again (L1/L2 hits) to produce the output.  Few
 // registers -> many resident warps -> enough bytes in flight to approach HBM bandwidth without any block barrier.
 // (A CTA-per-row variant with barriers measured 2-3x below the HBM roofline: two resident rows per SM.)
 
-// v = value to normalise; gv8 = bf16(gelu(a)) and ga8 = gelu'(a) (GLU / GELU modes), b8 = the linear GLU half
+// v = value to normalise; ga8 = gelu'(x) (GELU mode)
 template <typename TX>
-__device__ __forceinline__ void load_value(const TX* xr, int col, int H, int act, float (&v)[8], float (&gv8)[8],
-                                           float (&ga8)[8], float (&b8)[8]) {
-  if (act == ACT_GLU) {
-    float a8[8];
-    load8(xr + col, a8);
-    load8(xr + H + col, b8);
+__device__ __forceinline__ void load_value(const TX* xr, int col, int act, float (&v)[8], float (&ga8)[8]) {
+  load8(xr + col, v);
+  if (act == ACT_GELU) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       float gv;
-      gelu_eval(a8[j], gv, ga8[j]);
-      gv8[j] = bf16_round(gv);
-      v[j] = bf16_round(gv8[j] * b8[j]);
-    }
-  } else {
-    load8(xr + col, v);
-    if (act == ACT_GELU) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float gv;
-        gelu_eval(v[j], gv, ga8[j]);
-        v[j] = gv;
-      }
+      gelu_eval(v[j], gv, ga8[j]);
+      v[j] = gv;
     }
   }
 }
@@ -466,20 +395,19 @@ norm_fwd_wide_kernel(const TX* __restrict__ x, const float* __restrict__ w, cons
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kWideWarps + (threadIdx.x >> 5);
   if (row >= rows) return;
-  const int xs = (act == ACT_GLU) ? 2 * H : H;
-  const TX* xr = x + static_cast<size_t>(row) * xs;
-  float gv8[8], ga8[8], b8[8];
+  const TX* xr = x + static_cast<size_t>(row) * H;
+  float ga8[8];
   // pass 1: shifted single-pass moments (shift = first element of the row kills the cancellation in E[v^2]-E[v]^2)
   float shift;
   {
     float v0[8];
-    if (lane == 0) load_value(xr, 0, H, act, v0, gv8, ga8, b8);
+    if (lane == 0) load_value(xr, 0, act, v0, ga8);
     shift = rms ? 0.f : __shfl_sync(0xffffffffu, v0[0], 0);
   }
   float s = 0.f, ss = 0.f;
   for (int col = lane * 8; col < H; col += 256) {
     float v[8];
-    load_value(xr, col, H, act, v, gv8, ga8, b8);
+    load_value(xr, col, act, v, ga8);
 #pragma unroll
     for (int j = 0; j < 8; ++j) { const float d = v[j] - shift; s += d; ss += d * d; }
   }
@@ -498,7 +426,7 @@ norm_fwd_wide_kernel(const TX* __restrict__ x, const float* __restrict__ w, cons
   const float* rr = res ? res + static_cast<size_t>(row) * H : nullptr;
   for (int col = lane * 8; col < H; col += 256) {
     float v[8], o[8], wv[8];
-    load_value(xr, col, H, act, v, gv8, ga8, b8);
+    load_value(xr, col, act, v, ga8);
     if (w) load8(w + col, wv);
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = (v[j] - mean) * rstd * (w ? wv[j] : 1.f);
@@ -512,8 +440,9 @@ norm_fwd_wide_kernel(const TX* __restrict__ x, const float* __restrict__ w, cons
   }
 }
 
+// Four CTAs per SM, the residency bwd_grid sizes the grid for (and 64 registers, so no spill).
 template <typename TDY, typename TX, typename TDX>
-__global__ void __launch_bounds__(kWideWarps * 32)
+__global__ void __launch_bounds__(kWideWarps * 32, 4)
 norm_bwd_wide_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const float* __restrict__ w,
                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                      const float* __restrict__ dres, TDX* __restrict__ dx, float* __restrict__ dw,
@@ -527,17 +456,16 @@ norm_bwd_wide_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
     for (int i = lane * 4; i < H; i += 128) *reinterpret_cast<float4*>(my_dw + i) = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncwarp();
   }
-  const int xs = (act == ACT_GLU) ? 2 * H : H;
   const float inv_h = 1.0f / static_cast<float>(H);
   for (int row = blockIdx.x * kWideWarps + warp; row < rows; row += gridDim.x * kWideWarps) {
-    const TX* xr = x + static_cast<size_t>(row) * xs;
+    const TX* xr = x + static_cast<size_t>(row) * H;
     const TDY* dyr = dy + static_cast<size_t>(row) * H;
     const float mean = rms ? 0.f : mean_in[row];
     const float rstd = rstd_in[row];
     float s1 = 0.f, s2 = 0.f;
     for (int col = lane * 8; col < H; col += 256) {
-      float v[8], gv8[8], ga8[8], b8[8], dv[8], wv[8], pr[8];
-      load_value(xr, col, H, act, v, gv8, ga8, b8);
+      float v[8], ga8[8], dv[8], wv[8], pr[8];
+      load_value(xr, col, act, v, ga8);
       load8(dyr + col, dv);
       if (w) load8(w + col, wv);
 #pragma unroll
@@ -558,11 +486,11 @@ norm_bwd_wide_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
     }
     s1 = rms ? 0.f : warp_sum(s1) * inv_h;
     s2 = warp_sum(s2) * inv_h;
-    TDX* dxr = dx + static_cast<size_t>(row) * xs;
+    TDX* dxr = dx + static_cast<size_t>(row) * H;
     const float* drr = dres ? dres + static_cast<size_t>(row) * H : nullptr;
     for (int col = lane * 8; col < H; col += 256) {
-      float v[8], gv8[8], ga8[8], b8[8], dv[8], wv[8], o[8];
-      load_value(xr, col, H, act, v, gv8, ga8, b8);
+      float v[8], ga8[8], dv[8], wv[8], o[8];
+      load_value(xr, col, act, v, ga8);
       load8(dyr + col, dv);
       if (w) load8(w + col, wv);
 #pragma unroll
@@ -571,25 +499,17 @@ norm_bwd_wide_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
         const float g = dv[j] * (w ? wv[j] : 1.f);
         o[j] = rstd * (g - s1 - xh * s2);
       }
-      if (act == ACT_GLU) {
-        float da[8], db[8];
+      if (act == ACT_GELU) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { da[j] = o[j] * b8[j] * ga8[j]; db[j] = o[j] * gv8[j]; }
-        store8(dxr + col, da);
-        store8(dxr + H + col, db);
-      } else {
-        if (act == ACT_GELU) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] *= ga8[j];
-        }
-        if (drr) {
-          float r8[8];
-          load8(drr + col, r8);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] += r8[j];
-        }
-        store8(dxr + col, o);
+        for (int j = 0; j < 8; ++j) o[j] *= ga8[j];
       }
+      if (drr) {
+        float r8[8];
+        load8(drr + col, r8);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] += r8[j];
+      }
+      store8(dxr + col, o);
     }
   }
   if (dw) flush_cta_dw(s_dw, kWideWarps, H, dw, dw_ws);
@@ -734,7 +654,7 @@ __global__ void __launch_bounds__(kGluWarps * 32, 3)
 glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, const float* __restrict__ w,
                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in, bf16* __restrict__ dab,
                     float* __restrict__ dw, float* __restrict__ dw_ws, const bf16* __restrict__ yf, int rows, int H,
-                    int rms, int pf, const philox::ElemDrop drop) {
+                    int rms, const philox::ElemDrop drop) {
   static_assert(!(HAVE_Y && DROP), "the dropout backward recomputes the GLU product");
   pdl_enter();
   extern __shared__ __align__(16) float s_dw[];  // [kGluWarps][H] private rows
@@ -760,7 +680,7 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
     if (HAVE_Y) {
       const bf16* yr = yf + static_cast<size_t>(row) * H;
       for (int col = lane * 8; col < H; col += 256) {
-        if (pf && lane < 4) {
+        if (lane < 4) {
           const int nb = col - lane * 8 + 512 + lane * 64;
           if (nb < H) { prefetch_l2(dyr + nb); prefetch_l2(yr + nb); }
           else if (nb - H < H) { prefetch_l2(xr + (nb - H)); prefetch_l2(xr + H + (nb - H)); }
@@ -818,7 +738,7 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
     s2 = warp_sum(s2) * inv_h;
     bf16* dr = dab + static_cast<size_t>(row) * 2 * H;
     for (int col = lane * 8; col < H; col += 256) {
-      if (pf && HAVE_Y && lane < 4) {
+      if (HAVE_Y && lane < 4) {
         const int nb = col - lane * 8 + 512 + lane * 64;
         if (nb < H) { prefetch_l2(xr + nb); prefetch_l2(xr + H + nb); }
         else if (next < rows && nb - H < H) {
@@ -879,21 +799,17 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
 template <typename TX, typename TY>
 int fwd_dispatch(const void* x, const float* w, const float* res, void* y, float* mean, float* rstd, int rows, int H,
                  float eps, int act, int rms, cudaStream_t s) {
-  if (H <= 1024 && act != ACT_GLU) {
-    const int grid = ceil_div(rows, kWarpsPerBlock);
-    const int ch = ceil_div(H, 256);
-#define MUSE_NF(CH)                                                                                                \
-  pdl_launch(grid, kWarpsPerBlock * 32, 0, s)(norm_fwd_warp_kernel<TX, TY, CH>, reinterpret_cast<const TX*>(x), w, res,    \
-                                                                         reinterpret_cast<TY*>(y), mean, rstd, rows, \
-                                                                         H, eps, act, rms)
-    if (ch <= 1) MUSE_NF(1);
-    else if (ch <= 2) MUSE_NF(2);
-    else MUSE_NF(4);
-#undef MUSE_NF
-    return check_launch("norm_fwd");
+  const TX* xp = reinterpret_cast<const TX*>(x);
+  TY* yp = reinterpret_cast<TY*>(y);
+  if (H <= 1024) {
+    with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+      pdl_launch(ceil_div(rows, kWarpsPerBlock), kWarpsPerBlock * 32, 0, s)(
+          norm_fwd_warp_kernel<TX, TY, decltype(ch)::value>, xp, w, res, yp, mean, rstd, rows, H, eps, act, rms);
+    });
+  } else {
+    pdl_launch(ceil_div(rows, kWideWarps), kWideWarps * 32, 0, s)(norm_fwd_wide_kernel<TX, TY>, xp, w, res, yp, mean, rstd,
+                                                                  rows, H, eps, act, rms);
   }
-  pdl_launch(ceil_div(rows, kWideWarps), kWideWarps * 32, 0, s)(norm_fwd_wide_kernel<TX, TY>,
-      reinterpret_cast<const TX*>(x), w, res, reinterpret_cast<TY*>(y), mean, rstd, rows, H, eps, act, rms);
   return check_launch("norm_fwd");
 }
 
@@ -914,42 +830,26 @@ int bwd_dispatch(const void* dy, const void* x, const float* w, const float* mea
                  const float* dres, void* dx, void* dx_copy, float* dw, float* dw_ws, int rows, int H, int act, int rms,
                  cudaStream_t s) {
   const int grid = bwd_grid(rows, H, act);
-  if (H <= 1024 && act != ACT_GLU) {
-    const int ch = ceil_div(H, 256);
+  const TDY* dyp = reinterpret_cast<const TDY*>(dy);
+  const TX* xp = reinterpret_cast<const TX*>(x);
+  TDX* dxp = reinterpret_cast<TDX*>(dx);
+  if (H <= 1024) {
     const size_t smem = dw ? static_cast<size_t>(kBwdWarps) * H * sizeof(float) : 0;
-#define MUSE_NB(CH)                                                                                          \
-  pdl_launch(grid, kBwdWarps * 32, smem, s)(norm_bwd_warp_kernel<TDY, TX, TDX, CH>,                                  \
-      reinterpret_cast<const TDY*>(dy), reinterpret_cast<const TX*>(x), w, mean, rstd, dres,                 \
-      reinterpret_cast<TDX*>(dx), reinterpret_cast<bf16*>(dx_copy), dw, dw_ws, rows, H, act, rms, kRowPrefetch)
-    if (ch <= 1) MUSE_NB(1);
-    else if (ch <= 2) MUSE_NB(2);
-    else MUSE_NB(4);
-#undef MUSE_NB
+    with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+      pdl_launch(grid, kBwdWarps * 32, smem, s)(norm_bwd_warp_kernel<TDY, TX, TDX, decltype(ch)::value>, dyp, xp, w, mean,
+                                                rstd, dres, dxp, reinterpret_cast<bf16*>(dx_copy), dw, dw_ws, rows, H, act,
+                                                rms);
+    });
   } else {
-    if (dx_copy) { set_last_error("norm_bwd: the bf16 copy of dx is only produced for H <= 1024 without GLU"); return MUSE_ERR_UNSUPPORTED; }
+    if (dx_copy) { set_last_error("norm_bwd: the bf16 copy of dx is only produced for H <= 1024"); return MUSE_ERR_UNSUPPORTED; }
     const size_t smem = dw ? static_cast<size_t>(kWideWarps) * H * sizeof(float) : 0;
-    auto kern = norm_bwd_wide_kernel<TDY, TX, TDX>;
-    static bool attr = false;
-    if (!attr) {
-      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideWarps * 4096 * 4);
-      attr = true;
-    }
-    pdl_launch(grid, kWideWarps * 32, smem, s)(kern, reinterpret_cast<const TDY*>(dy), reinterpret_cast<const TX*>(x), w, mean, rstd,
-                                             dres, reinterpret_cast<TDX*>(dx), dw, dw_ws, rows, H, act, rms);
+    allow_dynamic_smem_once<norm_bwd_wide_kernel<TDY, TX, TDX>>(kWideWarps * 4096 * 4);
+    pdl_launch(grid, kWideWarps * 32, smem, s)(norm_bwd_wide_kernel<TDY, TX, TDX>, dyp, xp, w, mean, rstd, dres, dxp, dw,
+                                               dw_ws, rows, H, act, rms);
   }
   int rc = check_launch("norm_bwd");
   if (rc || !dw || !dw_ws) return rc;
   return reduce_dw(dw_ws, dw, grid, H, s);
-}
-
-void glu_bwd_smem_attr() {
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(glu_norm_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
-    cudaFuncSetAttribute(glu_norm_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
-    cudaFuncSetAttribute(glu_norm_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGluWarps * 4096 * 4);
-    attr = true;
-  }
 }
 
 int check_args(const char* who, int H, int act, const void* res_or_dres) {
@@ -983,21 +883,23 @@ int muse_norm_fwd(const void* x, int x_dt, const float* w, const float* res, voi
     set_last_error("norm_fwd: dropout needs act 2, bf16 x and y, and a seed");
     return MUSE_ERR_INVALID;
   }
-  if (act == ACT_GLU && x_dt == 1 && y_dt == 1 && H <= 4096) {
+  if (act == ACT_GLU && (x_dt == 0 || y_dt == 0)) {
+    set_last_error("norm_fwd: GLU mode (act 2) takes bf16 x and y only");
+    return MUSE_ERR_UNSUPPORTED;
+  }
+  if (act == ACT_GLU && x_dt == 1 && y_dt == 1) {
     const philox::ElemDrop drop = philox::elem_drop(bits, seed, site, p, H);
-    const int grid = ceil_div(rows, kGluWarps);
-    const int ch = ceil_div(H, 256);
-#define MUSE_GF(CH) pdl_launch(grid, kGluWarps * 32, 0, s)(bits ? glu_norm_fwd_kernel<CH, true> : glu_norm_fwd_kernel<CH, false>, reinterpret_cast<const bf16*>(x), w, reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop)
-    if (ch <= 1) MUSE_GF(1); else if (ch <= 2) MUSE_GF(2); else if (ch <= 4) MUSE_GF(4); else if (ch <= 8) MUSE_GF(8); else MUSE_GF(16);
-#undef MUSE_GF
+    with_row_chunks<1, 2, 4, 8, 16>(H, [&](auto ch) {
+      constexpr int CH = decltype(ch)::value;
+      pdl_launch(ceil_div(rows, kGluWarps), kGluWarps * 32, 0, s)(
+          bits ? glu_norm_fwd_kernel<CH, true> : glu_norm_fwd_kernel<CH, false>, reinterpret_cast<const bf16*>(x), w,
+          reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop);
+    });
     return check_launch("glu_norm_fwd");
   }
-  if (x_dt == 0 && y_dt == 1) return fwd_dispatch<float, bf16>(x, w, res, y, mean, rstd, rows, H, eps, act, rms, s);
-  if (x_dt == 1 && y_dt == 1) return fwd_dispatch<bf16, bf16>(x, w, res, y, mean, rstd, rows, H, eps, act, rms, s);
-  if (x_dt == 1 && y_dt == 0) return fwd_dispatch<bf16, float>(x, w, res, y, mean, rstd, rows, H, eps, act, rms, s);
-  if (x_dt == 0 && y_dt == 0) return fwd_dispatch<float, float>(x, w, res, y, mean, rstd, rows, H, eps, act, rms, s);
-  set_last_error("norm_fwd: bad dtype codes %d %d", x_dt, y_dt);
-  return MUSE_ERR_INVALID;
+  return dtype_dispatch("norm_fwd", [&](auto x_t, auto y_t) {
+    return fwd_dispatch<decltype(x_t), decltype(y_t)>(x, w, res, y, mean, rstd, rows, H, eps, act, rms, s);
+  }, x_dt, y_dt);
 }
 
 // x2 = res + norm1(a) * w1 ; h2 = norm2(x2) * w2  (a bf16 [rows,H], res / x2 fp32, h2 bf16; H % 8 == 0, H <= 1024)
@@ -1006,11 +908,11 @@ int muse_norm2_fwd(const void* a, const float* res, const float* w1, const float
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024 || H < 8) { set_last_error("norm2_fwd: H=%d must be a multiple of 8 in [8, 1024]", H); return MUSE_ERR_UNSUPPORTED; }
-  const int grid = ceil_div(rows, kWarpsPerBlock);
-  const int ch = ceil_div(H, 256);
-#define MUSE_N2F(CH) pdl_launch(grid, kWarpsPerBlock * 32, 0, s)(norm2_fwd_warp_kernel<CH>, reinterpret_cast<const bf16*>(a), res, w1, w2, x2, reinterpret_cast<bf16*>(h2), mean1, rstd1, mean2, rstd2, rows, H, eps, rms1, rms2)
-  if (ch <= 1) MUSE_N2F(1); else if (ch <= 2) MUSE_N2F(2); else MUSE_N2F(4);
-#undef MUSE_N2F
+  with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+    pdl_launch(ceil_div(rows, kWarpsPerBlock), kWarpsPerBlock * 32, 0, s)(
+        norm2_fwd_warp_kernel<decltype(ch)::value>, reinterpret_cast<const bf16*>(a), res, w1, w2, x2,
+        reinterpret_cast<bf16*>(h2), mean1, rstd1, mean2, rstd2, rows, H, eps, rms1, rms2);
+  });
   return check_launch("norm2_fwd");
 }
 
@@ -1022,20 +924,16 @@ int muse_norm2_bwd(const void* d_h2, const float* x2, const float* w2, const flo
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024 || H < 8) { set_last_error("norm2_bwd: H=%d must be a multiple of 8 in [8, 1024]", H); return MUSE_ERR_UNSUPPORTED; }
   const int grid = bwd_grid(rows, H, 0);
-  const int ch = ceil_div(H, 256);
   float* ws2 = ws;
   float* ws1 = ws + static_cast<size_t>(grid) * H;
   const size_t smem = static_cast<size_t>(2) * kBwdWarps * H * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(norm2_bwd_warp_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kBwdWarps * 1024 * 4);
-    cudaFuncSetAttribute(norm2_bwd_warp_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kBwdWarps * 1024 * 4);
-    cudaFuncSetAttribute(norm2_bwd_warp_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kBwdWarps * 1024 * 4);
-    attr = true;
-  }
-#define MUSE_N2B(CH) pdl_launch(grid, kBwdWarps * 32, smem, s)(norm2_bwd_warp_kernel<CH>, reinterpret_cast<const bf16*>(d_h2), x2, w2, mean2, rstd2, dres, reinterpret_cast<const bf16*>(a), w1, mean1, rstd1, dx2, reinterpret_cast<bf16*>(d_a), ws2, ws1, rows, H, rms1, rms2, kRowPrefetch)
-  if (ch <= 1) MUSE_N2B(1); else if (ch <= 2) MUSE_N2B(2); else MUSE_N2B(4);
-#undef MUSE_N2B
+  with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+    constexpr int CH = decltype(ch)::value;
+    allow_dynamic_smem_once<norm2_bwd_warp_kernel<CH>>(2 * kBwdWarps * 1024 * 4);
+    pdl_launch(grid, kBwdWarps * 32, smem, s)(norm2_bwd_warp_kernel<CH>, reinterpret_cast<const bf16*>(d_h2), x2, w2, mean2,
+                                              rstd2, dres, reinterpret_cast<const bf16*>(a), w1, mean1, rstd1, dx2,
+                                              reinterpret_cast<bf16*>(d_a), ws2, ws1, rows, H, rms1, rms2);
+  });
   int rc = check_launch("norm2_bwd");
   if (rc) return rc;
   if ((rc = reduce_dw(ws2, dw2, grid, H, s))) return rc;
@@ -1061,36 +959,32 @@ int muse_norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const floa
     set_last_error("norm_bwd: dropout needs act 2, bf16 dy, x and dx, and no y_fwd");
     return MUSE_ERR_INVALID;
   }
-  if (act == ACT_GLU && dy_dt == 1 && x_dt == 1 && dx_dt == 1 && H <= 4096) {
+  if (act == ACT_GLU && (dy_dt == 0 || x_dt == 0 || dx_dt == 0)) {
+    set_last_error("norm_bwd: GLU mode (act 2) takes bf16 dy, x and dx only");
+    return MUSE_ERR_UNSUPPORTED;
+  }
+  if (act == ACT_GLU && dy_dt == 1 && x_dt == 1 && dx_dt == 1) {
     const int grid = bwd_grid(rows, H, act);
     const size_t smem = dw ? static_cast<size_t>(kGluWarps) * H * sizeof(float) : 0;
     const philox::ElemDrop drop = philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, H);
-    glu_bwd_smem_attr();
+    allow_dynamic_smem_once<glu_norm_bwd_kernel<false, false>, glu_norm_bwd_kernel<true, false>,
+                            glu_norm_bwd_kernel<false, true>>(kGluWarps * 4096 * 4);
     if (y_fwd != nullptr)
       pdl_launch(grid, kGluWarps * 32, smem, s)(glu_norm_bwd_kernel<true, false>,
           reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-          dw_ws, reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, kRowPrefetch, drop);
+          dw_ws, reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, drop);
     else
       pdl_launch(grid, kGluWarps * 32, smem, s)(bits ? glu_norm_bwd_kernel<false, true> : glu_norm_bwd_kernel<false, false>,
           reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw,
-          dw_ws, nullptr, rows, H, rms, 0, drop);
+          dw_ws, nullptr, rows, H, rms, drop);
     rc = check_launch("glu_norm_bwd");
     if (rc || !dw || !dw_ws) return rc;
     return reduce_dw(dw_ws, dw, grid, H, s);
   }
-  const int key = dy_dt * 4 + x_dt * 2 + dx_dt;
-  switch (key) {
-    case 0: return bwd_dispatch<float, float, float>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 1: return bwd_dispatch<float, float, bf16>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 2: return bwd_dispatch<float, bf16, float>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 3: return bwd_dispatch<float, bf16, bf16>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 4: return bwd_dispatch<bf16, float, float>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 5: return bwd_dispatch<bf16, float, bf16>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 6: return bwd_dispatch<bf16, bf16, float>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-    case 7: return bwd_dispatch<bf16, bf16, bf16>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws, rows, H, act, rms, s);
-  }
-  set_last_error("norm_bwd: bad dtype codes");
-  return MUSE_ERR_INVALID;
+  return dtype_dispatch("norm_bwd", [&](auto dy_t, auto x_t, auto dx_t) {
+    return bwd_dispatch<decltype(dy_t), decltype(x_t), decltype(dx_t)>(dy, x, w, mean, rstd, dres, dx, dx_copy, dw, dw_ws,
+                                                                       rows, H, act, rms, s);
+  }, dy_dt, x_dt, dx_dt);
 }
 
 }  // extern "C"

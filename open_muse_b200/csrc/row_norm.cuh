@@ -1,0 +1,105 @@
+// Warp-per-row LayerNorm / RMSNorm core of the H <= 1024 norm kernels (norm.cu, uvit.cu, uvit_bwd.cu).
+// One warp owns one row and holds it in registers as float v[CH][8]: chunk c of lane `lane` is the 8 columns starting at
+// row_col(c, lane), and chunks at or past H are zero.  Each helper fixes the order of its floating-point operations, so
+// every kernel built on them produces the same bits for the same row.  The GLU and wide streaming kernels of norm.cu
+// keep their own loops: they do not hold the row as floats (packed bf16 pairs, or no row at all).
+#pragma once
+#include <type_traits>
+
+#include "common.cuh"
+
+namespace muse {
+
+__device__ __forceinline__ int row_col(int c, int lane) { return (c * 32 + lane) * 8; }
+
+// Fills the register row: load(col, v[c]) for every chunk inside the row, zeros past H.  Returns the lane's sum of
+// the loaded values, accumulated chunk by chunk as they arrive.
+template <int CH, typename Load>
+__device__ __forceinline__ float row_load(float (&v)[CH][8], int H, int lane, Load&& load) {
+  float sum = 0.f;
+#pragma unroll
+  for (int c = 0; c < CH; ++c) {
+    const int col = row_col(c, lane);
+    if (col < H) {
+      load(col, v[c]);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sum += v[c][j];
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[c][j] = 0.f;
+    }
+  }
+  return sum;
+}
+
+// Two-pass forward statistics of the register row from the lane sums `sum` of its values (row_load): mean (0 for
+// RMSNorm), then rstd = 1 / sqrt(mean((v - mean)^2) + eps).  inv_h = 1 / H is computed once by the caller, outside any
+// row loop.
+template <int CH>
+__device__ __forceinline__ void row_stats(const float (&v)[CH][8], float sum, int H, float inv_h, int lane, float eps,
+                                          int rms, float& mean, float& rstd) {
+  mean = rms ? 0.f : warp_sum(sum) * inv_h;
+  float sq = 0.f;
+#pragma unroll
+  for (int c = 0; c < CH; ++c)
+    if (row_col(c, lane) < H) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float d = v[c][j] - mean;
+        sq = fmaf(d, d, sq);
+      }
+    }
+  rstd = rsqrtf(warp_sum(sq) * inv_h + eps);
+}
+
+// Backward, with g = dL/dxhat: each lane accumulates s1 += g and s2 += g * xhat over its elements (element by element,
+// inside the kernel's own loop), row_bwd_sums turns the lane sums into s1 = mean(g) (0 for RMSNorm) and
+// s2 = mean(g * xhat), and row_dx gives dL/dv = rstd * (g - s1 - xhat * s2).
+__device__ __forceinline__ void row_bwd_acc(float g, float xh, float& s1, float& s2) {
+  s1 += g;
+  s2 = fmaf(g, xh, s2);
+}
+__device__ __forceinline__ void row_bwd_sums(float inv_h, int rms, float& s1, float& s2) {
+  s1 = rms ? 0.f : warp_sum(s1) * inv_h;
+  s2 = warp_sum(s2) * inv_h;
+}
+__device__ __forceinline__ float row_dx(float g, float xh, float s1, float s2, float rstd) {
+  return rstd * (g - s1 - xh * s2);
+}
+
+// ---- host side
+
+// Calls f(std::integral_constant<int, CH>()) with the first CH of the list whose CH * 256 columns cover H, or the last one.
+// Each call site lists the chunk counts its kernel is instantiated for.
+template <int CH, int... More, typename F>
+void with_row_chunks(int H, F&& f) {
+  if constexpr (sizeof...(More) == 0) {
+    f(std::integral_constant<int, CH>());
+  } else {
+    if (H <= CH * 256) f(std::integral_constant<int, CH>());
+    else with_row_chunks<More...>(H, f);
+  }
+}
+
+// Calls f(T0(), T1(), ...) with Ti = float for dtype code 0 and bf16 for code 1, one type per code, and returns its status.
+template <typename... Ts, typename F>
+int dtype_dispatch(const char* who, F&& f) {
+  return f(Ts()...);
+}
+template <typename... Ts, typename F, typename... Codes>
+int dtype_dispatch(const char* who, F&& f, int code, Codes... more) {
+  if (code == 0) return dtype_dispatch<Ts..., float>(who, f, more...);
+  if (code == 1) return dtype_dispatch<Ts..., bf16>(who, f, more...);
+  set_last_error("%s: bad dtype code %d", who, code);
+  return MUSE_ERR_INVALID;
+}
+
+// Raises the dynamic shared-memory limit of each listed kernel to `bytes`, the first time it is called for that list.
+template <auto... Kernels>
+void allow_dynamic_smem_once(int bytes) {
+  static const bool done =
+      ((cudaFuncSetAttribute(Kernels, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes), ...), true);
+  (void)done;
+}
+
+}  // namespace muse

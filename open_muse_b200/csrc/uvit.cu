@@ -10,8 +10,8 @@
 //                     apply pass, which draws the keep bits (philox.cuh) and writes the dropped output and the bits.
 //   * adaln_apply   : in-place fp32 x * (1 + scale_b) + shift_b at the end of a ResBlock.
 //   * silu          : SiLU of the conditioning vectors / text states feeding the adaLN and kv mappers.
-#include "common.cuh"
 #include "philox.cuh"
+#include "row_norm.cuh"
 
 namespace muse {
 namespace {
@@ -32,45 +32,22 @@ add_norm_mod_kernel(const TA* __restrict__ a, const float* __restrict__ r, const
   if (row >= rows) return;
   const size_t base = static_cast<size_t>(row) * H;
   float v[CH][8];
-  float sum = 0.f;
+  const float sum = row_load(v, H, lane, [&](int col, float (&vc)[8]) {
+    load8(a + base + col, vc);
+    if (r != nullptr) {
+      float rv[8];
+      load8(r + base + col, rv);
 #pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < H) {
-      load8(a + base + col, v[c]);
-      if (r != nullptr) {
-        float rv[8];
-        load8(r + base + col, rv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[c][j] += rv[j];
-      }
-      if (r_out != nullptr) store8(r_out + base + col, v[c]);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += v[c][j];
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[c][j] = 0.f;
+      for (int j = 0; j < 8; ++j) vc[j] += rv[j];
     }
-  }
-  const float inv_h = 1.0f / static_cast<float>(H);
-  const float mean = rms ? 0.f : warp_sum(sum) * inv_h;
-  float sq = 0.f;
-#pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < H) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = v[c][j] - mean;
-        sq += d * d;
-      }
-    }
-  }
-  const float rstd = rsqrtf(warp_sum(sq) * inv_h + eps);
+    if (r_out != nullptr) store8(r_out + base + col, vc);
+  });
+  float mean, rstd;
+  row_stats(v, sum, H, 1.0f / static_cast<float>(H), lane, eps, rms, mean, rstd);
   const float* sc = ss ? ss + static_cast<size_t>(row / rows_per_sample) * ss_stride : nullptr;
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    const int col = row_col(c, lane);
     if (col < H) {
       float o[8], wv[8];
       if (w) load8(w + col, wv);
@@ -104,50 +81,29 @@ dwconv3x3_norm_kernel(const float* __restrict__ x, const float* __restrict__ wk,
   const int py = static_cast<int>((pix / ww) % hh);
   const long long b = pix / (static_cast<long long>(ww) * hh);
   float v[CH][8];
-  float sum = 0.f;
+  const float sum = row_load(v, C, lane, [&](int col, float (&vc)[8]) {
 #pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    for (int j = 0; j < 8; ++j) vc[j] = 0.f;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[c][j] = 0.f;
-    if (col < C) {
+    for (int t = 0; t < 9; ++t) {
+      const int iy = py + t / 3 - 1, ix = px + t % 3 - 1;
+      if (iy >= 0 && iy < hh && ix >= 0 && ix < ww) {
+        float xv[8], kv[8];
+        load8(x + ((b * hh + iy) * ww + ix) * C + col, xv);
+        load8(wk + t * C + col, kv);
 #pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const int iy = py + t / 3 - 1, ix = px + t % 3 - 1;
-        if (iy >= 0 && iy < hh && ix >= 0 && ix < ww) {
-          float xv[8], kv[8];
-          load8(x + ((b * hh + iy) * ww + ix) * C + col, xv);
-          load8(wk + t * C + col, kv);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[c][j] = fmaf(xv[j], kv[j], v[c][j]);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        v[c][j] = bf16_round(v[c][j]);  // the conv output is a bf16 tensor under autocast
-        sum += v[c][j];
-      }
-      if (conv_out != nullptr) store8(conv_out + pix * C + col, v[c]);  // saved for the backward pass
-    }
-  }
-  const float inv_c = 1.0f / static_cast<float>(C);
-  const float mean = rms ? 0.f : warp_sum(sum) * inv_c;
-  float sq = 0.f;
-#pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
-    if (col < C) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = v[c][j] - mean;
-        sq += d * d;
+        for (int j = 0; j < 8; ++j) vc[j] = fmaf(xv[j], kv[j], vc[j]);
       }
     }
-  }
-  const float rstd = rsqrtf(warp_sum(sq) * inv_c + eps);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) vc[j] = bf16_round(vc[j]);  // the conv output is a bf16 tensor under autocast
+    if (conv_out != nullptr) store8(conv_out + pix * C + col, vc);  // saved for the backward pass
+  });
+  float mean, rstd;
+  row_stats(v, sum, C, 1.0f / static_cast<float>(C), lane, eps, rms, mean, rstd);
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
-    const int col = (c * 32 + lane) * 8;
+    const int col = row_col(c, lane);
     if (col < C) {
       float o[8], wv[8];
       if (nw) load8(nw + col, wv);
@@ -265,21 +221,6 @@ __global__ void __launch_bounds__(256) silu_kernel(const TX* __restrict__ x, bf1
   store8(y + i * 8, v);
 }
 
-template <typename TA, typename TY>
-int launch_add_norm(const void* a, const float* r, const float* w, const float* ss, long long ss_stride,
-                    int rows_per_sample, float* r_out, void* y, int rows, int H, float eps, int rms, cudaStream_t s) {
-  const int grid = ceil_div(rows, kWarps);
-  const TA* ap = reinterpret_cast<const TA*>(a);
-  TY* yp = reinterpret_cast<TY*>(y);
-#define MUSE_AN(CH) pdl_launch(grid, kWarps * 32, 0, s)(add_norm_mod_kernel<TA, TY, CH>, ap, r, w, ss, ss_stride, rows_per_sample, r_out, yp, rows, H, eps, rms)
-  if (H <= 256) MUSE_AN(1);
-  else if (H <= 512) MUSE_AN(2);
-  else if (H <= 768) MUSE_AN(3);
-  else MUSE_AN(4);
-#undef MUSE_AN
-  return check_launch("add_norm_mod");
-}
-
 }  // namespace
 }  // namespace muse
 
@@ -295,12 +236,16 @@ int muse_add_norm_mod_fwd(const void* a, int a_dt, const float* r, const float* 
   if (H % 8 != 0 || H > 1024) { set_last_error("add_norm_mod: H=%d must be a multiple of 8 and <= 1024", H); return MUSE_ERR_UNSUPPORTED; }
   if (ss != nullptr && (rows_per_sample <= 0 || ss_stride % 4 != 0)) { set_last_error("add_norm_mod: bad modulation layout"); return MUSE_ERR_INVALID; }
   if (ss == nullptr) rows_per_sample = 1;
-  if (a_dt == 1 && y_dt == 1) return launch_add_norm<bf16, bf16>(a, r, w, ss, ss_stride, rows_per_sample, r_out, y, rows, H, eps, rms, s);
-  if (a_dt == 0 && y_dt == 1) return launch_add_norm<float, bf16>(a, r, w, ss, ss_stride, rows_per_sample, r_out, y, rows, H, eps, rms, s);
-  if (a_dt == 1 && y_dt == 0) return launch_add_norm<bf16, float>(a, r, w, ss, ss_stride, rows_per_sample, r_out, y, rows, H, eps, rms, s);
-  if (a_dt == 0 && y_dt == 0) return launch_add_norm<float, float>(a, r, w, ss, ss_stride, rows_per_sample, r_out, y, rows, H, eps, rms, s);
-  set_last_error("add_norm_mod: bad dtype codes %d %d", a_dt, y_dt);
-  return MUSE_ERR_INVALID;
+  return dtype_dispatch("add_norm_mod", [&](auto a_t, auto y_t) {
+    using TA = decltype(a_t);
+    using TY = decltype(y_t);
+    with_row_chunks<1, 2, 3, 4>(H, [&](auto ch) {
+      pdl_launch(ceil_div(rows, kWarps), kWarps * 32, 0, s)(
+          add_norm_mod_kernel<TA, TY, decltype(ch)::value>, reinterpret_cast<const TA*>(a), r, w, ss, ss_stride,
+          rows_per_sample, r_out, reinterpret_cast<TY*>(y), rows, H, eps, rms);
+    });
+    return check_launch("add_norm_mod");
+  }, a_dt, y_dt);
 }
 
 int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y, void* conv_out, int B, int hh, int ww,
@@ -310,12 +255,10 @@ int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, vo
   if (pixels <= 0) return MUSE_OK;
   if (C % 8 != 0 || C > 1024) { set_last_error("dwconv3x3_norm: C=%d must be a multiple of 8 and <= 1024", C); return MUSE_ERR_UNSUPPORTED; }
   const unsigned grid = static_cast<unsigned>(ceil_div_ll(pixels, kWarps));
-  bf16* yp = reinterpret_cast<bf16*>(y);
-  bf16* cp = reinterpret_cast<bf16*>(conv_out);
-  if (C <= 256) pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<1>, x, wk, nw, yp, cp, B, hh, ww, C, eps, rms);
-  else if (C <= 512) pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<2>, x, wk, nw, yp, cp, B, hh, ww, C, eps, rms);
-  else if (C <= 768) pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<3>, x, wk, nw, yp, cp, B, hh, ww, C, eps, rms);
-  else pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<4>, x, wk, nw, yp, cp, B, hh, ww, C, eps, rms);
+  with_row_chunks<1, 2, 3, 4>(C, [&](auto ch) {
+    pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<decltype(ch)::value>, x, wk, nw, reinterpret_cast<bf16*>(y),
+                                        reinterpret_cast<bf16*>(conv_out), B, hh, ww, C, eps, rms);
+  });
   return check_launch("dwconv3x3_norm");
 }
 

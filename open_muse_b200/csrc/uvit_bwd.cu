@@ -1,8 +1,10 @@
 // Backward kernels of the MaskGiTUViT_v2-specific ops of uvit.cu (the GEMM dgrad/wgrad, attention, GLU, cross-entropy and
 // embedding backward are shared with the v1 path).  All HBM-bound; parameter / per-sample reductions are folded in
 // registers and shared memory before touching global atomics.
-#include "common.cuh"
+#include <limits.h>
+
 #include "philox.cuh"
+#include "row_norm.cuh"
 
 namespace muse {
 namespace {
@@ -14,10 +16,11 @@ constexpr int kRowsPerWarp = 8;
 //   g  = norm_bwd(dy * (1 + s_b)) + dr_out         -> da (TA) and dr (fp32, optional): both equal g
 //   dw += sum_rows dy (1 + s) xhat ;  ds_b += sum_{rows of b} dy * n ;  dt_b += sum_{rows of b} dy
 // One warp walks kRowsPerWarp consecutive rows, keeps the three reductions in registers and flushes the per-sample ones
-// whenever the sample index changes (rows of one sample are contiguous).
-template <typename TDY, typename TA, int CH>
+// whenever the sample index changes (rows of one sample are contiguous).  MOD = false: no modulation (ss, dss unused),
+// no per-sample reductions.  Also step 1 of the depthwise conv + Norm2D backward (x = the saved bf16 conv output).
+template <typename TDY, typename TX, typename TA, bool MOD, int CH>
 __global__ void __launch_bounds__(kWarps * 32)
-add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr_out, const float* __restrict__ x,
+add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr_out, const TX* __restrict__ x,
                         const float* __restrict__ w, const float* __restrict__ ss, long long ss_stride, int rows_per_sample,
                         TA* __restrict__ da, float* __restrict__ dr, float* __restrict__ dw, float* __restrict__ dss,
                         int rows, int H, float eps, int rms) {
@@ -37,11 +40,11 @@ add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr
   const int row0 = (blockIdx.x * kWarps + warp) * kRowsPerWarp;
   int cur_b = -1;
   auto flush = [&](int b) {
-    if (dss == nullptr || b < 0) return;
+    if (!MOD || dss == nullptr || b < 0) return;
     float* d = dss + static_cast<size_t>(b) * ss_stride;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -55,42 +58,18 @@ add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr
   for (int k = 0; k < kRowsPerWarp; ++k) {
     const int row = row0 + k;
     if (row >= rows) break;
-    const int b = ss ? row / rows_per_sample : 0;
+    const int b = (MOD && ss) ? row / rows_per_sample : 0;
     if (b != cur_b) { flush(cur_b); cur_b = b; }
+    const float* sc = (MOD && ss) ? ss + static_cast<size_t>(b) * ss_stride : nullptr;
     const size_t base = static_cast<size_t>(row) * H;
-    const float* sc = ss ? ss + static_cast<size_t>(b) * ss_stride : nullptr;
     float xv[CH][8], gv[CH][8];
-    float sum = 0.f;
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < H) {
-        load8(x + base + col, xv[c]);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sum += xv[c][j];
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) xv[c][j] = 0.f;
-      }
-    }
-    const float mean = rms ? 0.f : warp_sum(sum) * inv_h;
-    float sq = 0.f;
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < H) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float d = xv[c][j] - mean;
-          sq += d * d;
-        }
-      }
-    }
-    const float rstd = rsqrtf(warp_sum(sq) * inv_h + eps);
+    const float sum = row_load(xv, H, lane, [&](int col, float (&vc)[8]) { load8(x + base + col, vc); });
+    float mean, rstd;
+    row_stats(xv, sum, H, inv_h, lane, eps, rms, mean, rstd);
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float dv[8], wv[8], s8[8];
         load8(dy + base + col, dv);
@@ -101,25 +80,25 @@ add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr
           const float xh = (xv[c][j] - mean) * rstd;
           const float wj = w ? wv[j] : 1.f;
           const float dn = sc ? dv[j] * (1.f + s8[j]) : dv[j];  // grad wrt n = xhat * w
-          ds_acc[c][j] = fmaf(dv[j], xh * wj, ds_acc[c][j]);
-          dt_acc[c][j] += dv[j];
+          if (MOD) {
+            ds_acc[c][j] = fmaf(dv[j], xh * wj, ds_acc[c][j]);
+            dt_acc[c][j] += dv[j];
+          }
           dw_acc[c][j] = fmaf(dn, xh, dw_acc[c][j]);
           gv[c][j] = dn * wj;  // grad wrt xhat
           xv[c][j] = xh;
-          s1 += gv[c][j];
-          s2 = fmaf(gv[c][j], xh, s2);
+          row_bwd_acc(gv[c][j], xh, s1, s2);
         }
       }
     }
-    s1 = rms ? 0.f : warp_sum(s1) * inv_h;
-    s2 = warp_sum(s2) * inv_h;
+    row_bwd_sums(inv_h, rms, s1, s2);
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
         float o[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = rstd * (gv[c][j] - s1 - xv[c][j] * s2);
+        for (int j = 0; j < 8; ++j) o[j] = row_dx(gv[c][j], xv[c][j], s1, s2, rstd);
         if (dr_out) {
           float r8[8];
           load8(dr_out + base + col, r8);
@@ -135,7 +114,7 @@ add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr
   if (dw) {
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
+      const int col = row_col(c, lane);
       if (col < H) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) atomicAdd(&s_dw[col + j], dw_acc[c][j]);
@@ -147,103 +126,8 @@ add_norm_mod_bwd_kernel(const TDY* __restrict__ dy, const float* __restrict__ dr
 }
 
 // ---- depthwise conv + Norm2D backward -----------------------------------------------------------------------------
-// step 1 (warp per pixel): norm backward on the saved conv output c (bf16): d_c fp32, dnw += sum dy * xhat
-template <int CH>
-__global__ void __launch_bounds__(kWarps * 32)
-dwnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ cv, const float* __restrict__ nw,
-                  float* __restrict__ dc, float* __restrict__ dnw, long long pixels, int C, float eps, int rms) {
-  pdl_enter();
-  extern __shared__ float s_dw[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (dnw) {
-    for (int i = threadIdx.x; i < C; i += blockDim.x) s_dw[i] = 0.f;
-    __syncthreads();
-  }
-  float dw_acc[CH][8];
-#pragma unroll
-  for (int c = 0; c < CH; ++c)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dw_acc[c][j] = 0.f;
-  const float inv_c = 1.0f / static_cast<float>(C);
-  const long long p0 = (static_cast<long long>(blockIdx.x) * kWarps + warp) * kRowsPerWarp;
-  for (int k = 0; k < kRowsPerWarp; ++k) {
-    const long long pix = p0 + k;
-    if (pix >= pixels) break;
-    const size_t base = static_cast<size_t>(pix) * C;
-    float xv[CH][8], gv[CH][8];
-    float sum = 0.f;
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < C) {
-        load8(cv + base + col, xv[c]);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sum += xv[c][j];
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) xv[c][j] = 0.f;
-      }
-    }
-    const float mean = rms ? 0.f : warp_sum(sum) * inv_c;
-    float sq = 0.f;
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < C) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float d = xv[c][j] - mean;
-          sq += d * d;
-        }
-      }
-    }
-    const float rstd = rsqrtf(warp_sum(sq) * inv_c + eps);
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < C) {
-        float dv[8], wv[8];
-        load8(dy + base + col, dv);
-        if (nw) load8(nw + col, wv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float xh = (xv[c][j] - mean) * rstd;
-          dw_acc[c][j] = fmaf(dv[j], xh, dw_acc[c][j]);
-          gv[c][j] = dv[j] * (nw ? wv[j] : 1.f);
-          xv[c][j] = xh;
-          s1 += gv[c][j];
-          s2 = fmaf(gv[c][j], xh, s2);
-        }
-      }
-    }
-    s1 = rms ? 0.f : warp_sum(s1) * inv_c;
-    s2 = warp_sum(s2) * inv_c;
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < C) {
-        float o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = rstd * (gv[c][j] - s1 - xv[c][j] * s2);
-        store8(dc + base + col, o);
-      }
-    }
-  }
-  if (dnw) {
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int col = (c * 32 + lane) * 8;
-      if (col < C) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) atomicAdd(&s_dw[col + j], dw_acc[c][j]);
-      }
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(&dnw[i], s_dw[i]);
-  }
-}
-
+// step 1 (add_norm_mod_bwd_kernel, warp per pixel): norm backward on the saved conv output c (bf16): d_c fp32,
+// dnw += sum dy * xhat
 // step 2: dx[p] = dres[p] + sum_t wk[t] * d_c[p - off(t)]   and   dwk[t] += sum_p d_c[p] * x[p + off(t)]
 // thread = (pixel strip, 4 channels); each thread walks kStrip pixels of one image row keeping dwk[9][4] in registers.
 constexpr int kStrip = 16;
@@ -439,20 +323,19 @@ silu_bwd_kernel(const bf16* __restrict__ dy, const TX* __restrict__ x, TDX* __re
   store8(dx + i * 8, o);
 }
 
-template <typename TDY, typename TA>
-int launch_anm_bwd(const void* dy, const float* dr_out, const float* x, const float* w, const float* ss, long long ss_stride,
+// ss == nullptr selects the kernel without modulation
+template <typename TDY, typename TX, typename TA>
+int launch_anm_bwd(const void* dy, const float* dr_out, const void* x, const float* w, const float* ss, long long ss_stride,
                    int rows_per_sample, void* da, float* dr, float* dw, float* dss, int rows, int H, float eps, int rms,
                    cudaStream_t s) {
-  const int grid = ceil_div(rows, kWarps * kRowsPerWarp);
   const size_t smem = dw ? static_cast<size_t>(H) * sizeof(float) : 0;
-  const TDY* dyp = reinterpret_cast<const TDY*>(dy);
-  TA* dap = reinterpret_cast<TA*>(da);
-#define MUSE_ANB(CH) pdl_launch(grid, kWarps * 32, smem, s)(add_norm_mod_bwd_kernel<TDY, TA, CH>, dyp, dr_out, x, w, ss, ss_stride, rows_per_sample, dap, dr, dw, dss, rows, H, eps, rms)
-  if (H <= 256) MUSE_ANB(1);
-  else if (H <= 512) MUSE_ANB(2);
-  else if (H <= 768) MUSE_ANB(3);
-  else MUSE_ANB(4);
-#undef MUSE_ANB
+  with_row_chunks<1, 2, 3, 4>(H, [&](auto ch) {
+    constexpr int CH = decltype(ch)::value;
+    pdl_launch(ceil_div(rows, kWarps * kRowsPerWarp), kWarps * 32, smem, s)(
+        ss ? add_norm_mod_bwd_kernel<TDY, TX, TA, true, CH> : add_norm_mod_bwd_kernel<TDY, TX, TA, false, CH>,
+        reinterpret_cast<const TDY*>(dy), dr_out, reinterpret_cast<const TX*>(x), w, ss, ss_stride, rows_per_sample,
+        reinterpret_cast<TA*>(da), dr, dw, dss, rows, H, eps, rms);
+  });
   return check_launch("add_norm_mod_bwd");
 }
 
@@ -471,13 +354,10 @@ int muse_add_norm_mod_bwd(const void* dy, int dy_dt, const float* dr_out, const 
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024) { set_last_error("add_norm_mod_bwd: H=%d must be a multiple of 8 and <= 1024", H); return MUSE_ERR_UNSUPPORTED; }
-  if (ss == nullptr) { rows_per_sample = 1; dss = nullptr; }
-  if (dy_dt == 1 && da_dt == 1) return launch_anm_bwd<bf16, bf16>(dy, dr_out, x, w, ss, ss_stride, rows_per_sample, da, dr, dw, dss, rows, H, eps, rms, s);
-  if (dy_dt == 1 && da_dt == 0) return launch_anm_bwd<bf16, float>(dy, dr_out, x, w, ss, ss_stride, rows_per_sample, da, dr, dw, dss, rows, H, eps, rms, s);
-  if (dy_dt == 0 && da_dt == 1) return launch_anm_bwd<float, bf16>(dy, dr_out, x, w, ss, ss_stride, rows_per_sample, da, dr, dw, dss, rows, H, eps, rms, s);
-  if (dy_dt == 0 && da_dt == 0) return launch_anm_bwd<float, float>(dy, dr_out, x, w, ss, ss_stride, rows_per_sample, da, dr, dw, dss, rows, H, eps, rms, s);
-  set_last_error("add_norm_mod_bwd: bad dtype codes");
-  return MUSE_ERR_INVALID;
+  return dtype_dispatch("add_norm_mod_bwd", [&](auto dy_t, auto da_t) {
+    return launch_anm_bwd<decltype(dy_t), float, decltype(da_t)>(dy, dr_out, x, w, ss, ss_stride, rows_per_sample, da, dr,
+                                                                  dw, dss, rows, H, eps, rms, s);
+  }, dy_dt, da_dt);
 }
 
 // dy bf16 (grad wrt the normalised output), conv bf16 (saved conv output), x fp32 (block input), wk fp32 [9,C];
@@ -489,15 +369,9 @@ int muse_dwconv3x3_norm_bwd(const void* dy, const void* conv, const float* x, co
   const long long pixels = static_cast<long long>(B) * hh * ww;
   if (pixels <= 0) return MUSE_OK;
   if (C % 8 != 0 || C > 1024) { set_last_error("dwconv3x3_norm_bwd: C=%d unsupported", C); return MUSE_ERR_UNSUPPORTED; }
-  const unsigned grid = static_cast<unsigned>(ceil_div_ll(pixels, kWarps * kRowsPerWarp));
-  const size_t smem = dnw ? static_cast<size_t>(C) * sizeof(float) : 0;
-  const bf16* dyp = reinterpret_cast<const bf16*>(dy);
-  const bf16* cp = reinterpret_cast<const bf16*>(conv);
-  if (C <= 256) pdl_launch(grid, kWarps * 32, smem, s)(dwnorm_bwd_kernel<1>, dyp, cp, nw, dc_ws, dnw, pixels, C, eps, rms);
-  else if (C <= 512) pdl_launch(grid, kWarps * 32, smem, s)(dwnorm_bwd_kernel<2>, dyp, cp, nw, dc_ws, dnw, pixels, C, eps, rms);
-  else if (C <= 768) pdl_launch(grid, kWarps * 32, smem, s)(dwnorm_bwd_kernel<3>, dyp, cp, nw, dc_ws, dnw, pixels, C, eps, rms);
-  else pdl_launch(grid, kWarps * 32, smem, s)(dwnorm_bwd_kernel<4>, dyp, cp, nw, dc_ws, dnw, pixels, C, eps, rms);
-  int rc = check_launch("dwnorm_bwd");
+  if (pixels > INT_MAX) { set_last_error("dwconv3x3_norm_bwd: %lld pixels, at most INT_MAX supported", pixels); return MUSE_ERR_UNSUPPORTED; }
+  int rc = launch_anm_bwd<bf16, bf16, float>(dy, nullptr, conv, nw, nullptr, 0, 1, dc_ws, nullptr, dnw, nullptr,
+                                             static_cast<int>(pixels), C, eps, rms, s);
   if (rc) return rc;
   const long long strips = static_cast<long long>(B) * hh * ((ww + kStrip - 1) / kStrip) * (C / 4);
   pdl_launch(static_cast<unsigned>(ceil_div_ll(strips, 256)), 256, 0, s)(dwconv_bwd_kernel, dc_ws, x, wk, dres, dx, dwk, B, hh, ww, C);

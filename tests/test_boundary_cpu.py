@@ -46,6 +46,20 @@ def test_library_exports_every_declared_symbol():
     assert lib.muse_abi_version() == _lib.ABI_VERSION
 
 
+def test_norm_glu_mode_refuses_fp32_operands():
+    """act 2 (GLU) runs on bf16 tensors only: an fp32 operand is refused before anything is launched."""
+    from open_muse_b200 import _lib
+
+    lib = _lib.load()
+    MUSE_ERR_UNSUPPORTED = 3
+    for x_dt, y_dt in ((0, 1), (1, 0), (0, 0)):
+        assert lib.muse_norm_fwd(None, x_dt, None, None, None, y_dt, None, None, None, None, 0, 0.0, 4, 64, 1e-6, 2, 0,
+                                 None) == MUSE_ERR_UNSUPPORTED
+    for dy_dt, x_dt, dx_dt in ((0, 1, 1), (1, 0, 1), (1, 1, 0), (0, 0, 0)):
+        assert lib.muse_norm_bwd(None, dy_dt, None, x_dt, None, None, None, None, None, None, 0.0, None, dx_dt, None, None,
+                                 None, 4, 64, 2, 0, None) == MUSE_ERR_UNSUPPORTED
+
+
 def test_ops_refuse_cpu_tensors():
     from open_muse_b200 import _lib, ops
 

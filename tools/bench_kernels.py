@@ -1,6 +1,16 @@
 #!/usr/bin/env python
 """Per-kernel timings at the base-256 shapes (B=256, T=65792, H=512, I=2048) with CUDA events.
-Prints achieved GB/s (algorithmic bytes) or TFLOP/s per op -- the inner optimisation loop of the round."""
+Prints achieved GB/s (algorithmic bytes) or TFLOP/s per op -- the inner optimisation loop of the round.
+
+    python tools/bench_kernels.py [GROUP ...] [--dump DIR]
+
+GROUP selects the groups whose name contains it (glu, rownorm, norm, attn, gemm, resgemm; default all).  rownorm times every entry
+point of the warp-per-row LayerNorm / RMSNorm kernels at the shapes training runs, on seeded inputs; with --dump DIR it
+also writes DIR/rownorm_outputs.json, the SHA-256 of every run-to-run deterministic output, and DIR/rownorm_atomic.pt,
+the weight gradients accumulated with atomics (order-dependent, so two builds are compared with a tolerance)."""
+import argparse
+import hashlib
+import json
 import os
 import sys
 
@@ -41,11 +51,101 @@ def bf(*shape):
     return torch.randn(*shape, device=dev).to(torch.bfloat16)
 
 
-only = sys.argv[1:] or None
+ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+ap.add_argument("groups", nargs="*")
+ap.add_argument("--dump", help="directory for the digests / tensors of the rownorm outputs")
+args = ap.parse_args()
+only = args.groups or None
 
 
 def want(tag):
     return only is None or any(o in tag for o in only)
+
+
+def rownorm(dump):
+    """(name, call, atomic) for each entry point of the warp-per-row norm kernels: call() returns the outputs as a dict,
+    atomic names the outputs that accumulate with atomics (zeroed before the dumped call)."""
+    gen = torch.Generator(device=dev)
+
+    def rnd(seed, *shape, dtype=torch.float32):
+        gen.manual_seed(seed)
+        return torch.randn(*shape, device=dev, generator=gen).to(dtype)
+
+    cases = []
+    for Hn in (512, 1024):  # base-256 width; cc12m width (4 chunks of 256 columns per lane)
+        x, xb, res, dres = rnd(1, T, Hn), rnd(2, T, Hn, dtype=torch.bfloat16), rnd(3, T, Hn), rnd(4, T, Hn)
+        dyb, w, w2 = rnd(5, T, Hn, dtype=torch.bfloat16), 1 + 0.1 * rnd(6, Hn), 1 + 0.1 * rnd(7, Hn)
+        st = ops.norm_fwd(x, w, 1e-6, torch.bfloat16)[1]
+        dw = torch.zeros(Hn, device=dev)
+        x2, _, st2 = ops.norm2_fwd(xb, res, w, w2, 1e-6)
+
+        def bwd_copy(x=x, w=w, st=st, dyb=dyb, dres=dres):
+            dx, dwo = ops.norm_bwd(dyb, x, w, st, torch.float32, dres=dres, want_dw=True, bf16_copy=True)
+            return {"dx": dx, "dx_copy": ops.take_bf16_copy(dx), "dw": dwo}
+
+        def bwd_atomic(x=x, w=w, st=st, dyb=dyb, dres=dres, dw=dw):
+            return {"dx": ops.norm_bwd(dyb, x, w, st, torch.float32, dw=dw, dres=dres), "dw": dw}
+
+        cases += [
+            (f"norm_fwd fp32->bf16 H={Hn}", lambda x=x, w=w: dict(zip(("y", "stats"), ops.norm_fwd(x, w, 1e-6, torch.bfloat16))), ()),
+            (f"norm_fwd bf16->fp32 +res H={Hn}",
+             lambda xb=xb, w=w, res=res: dict(zip(("y", "stats"), ops.norm_fwd(xb, w, 1e-6, torch.float32, res=res))), ()),
+            (f"norm_bwd +dres, bf16 copy, ordered dw H={Hn}", bwd_copy, ()),
+            (f"norm_bwd +dres, atomic dw H={Hn}", bwd_atomic, ("dw",)),
+            (f"norm2_fwd H={Hn}", lambda xb=xb, res=res, w=w, w2=w2: dict(zip(("x2", "h2", "stats"), ops.norm2_fwd(xb, res, w, w2, 1e-6))), ()),
+            (f"norm2_bwd H={Hn}", lambda dyb=dyb, x2=x2, w2=w2, dres=dres, xb=xb, w=w, st2=st2: dict(zip(
+                ("dx2", "d_a", "dw1", "dw2"), ops.norm2_bwd(dyb, x2, w2, dres, xb, w, st2))), ()),
+        ]
+    Bu, S = 32, 256  # MaskGiTUViT_v2 defaults: batch 32, 16 x 16 = 256 tokens
+    for Hn, with_mod, rms in ((1024, True, 1), (768, False, 0)):
+        a, r, w = rnd(11, Bu * S, Hn, dtype=torch.bfloat16), rnd(12, Bu * S, Hn), 1 + 0.1 * rnd(13, Hn)
+        mod = 0.1 * rnd(14, Bu, 2 * Hn) if with_mod else None
+        dy, dr_out = rnd(15, Bu * S, Hn, dtype=torch.bfloat16), rnd(16, Bu * S, Hn)
+        r_out = ops.add_norm_mod(a, w, 1e-6, rms, residual=r, mod=mod, rows_per_sample=S)[0]
+        dw = torch.zeros(Hn, device=dev)
+        dmod = torch.zeros(Bu, 2 * Hn, device=dev) if with_mod else None
+        tag = f"H={Hn}" + (" +mod" if with_mod else "")
+
+        def anm_bwd(dy=dy, dr_out=dr_out, r_out=r_out, w=w, rms=rms, mod=mod, dw=dw, dmod=dmod):
+            da, dr = ops.add_norm_mod_bwd(dy, dr_out, r_out, w, 1e-6, rms, torch.bfloat16, mod=mod, rows_per_sample=S, dw=dw,
+                                          dmod=dmod)
+            return {"da": da, "dr": dr, "dw": dw, **({"dmod": dmod} if dmod is not None else {})}
+
+        cases += [
+            (f"add_norm_mod {tag}", lambda a=a, w=w, rms=rms, r=r, mod=mod: dict(zip(("r_out", "y"), ops.add_norm_mod(
+                a, w, 1e-6, rms, residual=r, mod=mod, rows_per_sample=S))), ()),
+            (f"add_norm_mod_bwd {tag}", anm_bwd, ("dw", "dmod")),
+        ]
+    C, hw = 768, 16
+    xd, wk, nw = rnd(21, Bu * hw * hw, C), 0.3 * rnd(22, 9, C), 1 + 0.1 * rnd(23, C)
+    dyd, dresd = rnd(24, Bu * hw * hw, C, dtype=torch.bfloat16), rnd(25, Bu * hw * hw, C)
+    conv = ops.dwconv3x3_norm(xd, wk, nw, Bu, hw, hw, 1e-6, 0, save_conv=True)[1]
+    dwk, dnw = torch.zeros(9, C, device=dev), torch.zeros(C, device=dev)
+    cases += [
+        (f"dwconv3x3_norm C={C}", lambda: dict(zip(("y", "conv"), ops.dwconv3x3_norm(xd, wk, nw, Bu, hw, hw, 1e-6, 0, save_conv=True))), ()),
+        (f"dwconv3x3_norm_bwd C={C}", lambda: {"dx": ops.dwconv3x3_norm_bwd(dyd, conv, xd, wk, nw, dresd, dwk, dnw, Bu, hw, hw, 1e-6, 0),
+                                               "dwk": dwk, "dnw": dnw}, ("dwk", "dnw")),
+    ]
+    digests, atomic = {}, {}
+    for name, call, acc in cases:
+        report(name, timeit(call, n=20, warm=5))
+        if dump:
+            outs = call()  # the buffers to zero are the ones this call returns
+            for k in acc:
+                if k in outs:
+                    outs[k].zero_()
+            outs = call()
+            torch.cuda.synchronize()
+            for k, t in outs.items():
+                if k in acc:
+                    atomic[f"{name}/{k}"] = t.cpu()
+                else:
+                    digests[f"{name}/{k}"] = hashlib.sha256(t.contiguous().view(torch.uint8).cpu().numpy().tobytes()).hexdigest()
+    if dump:
+        os.makedirs(dump, exist_ok=True)
+        with open(os.path.join(dump, "rownorm_outputs.json"), "w") as f:
+            json.dump(digests, f, indent=1, sort_keys=True)
+        torch.save(atomic, os.path.join(dump, "rownorm_atomic.pt"))
 
 
 u = T * H * 2 / 1e6  # MB of one bf16 [T,H]
@@ -65,6 +165,8 @@ if want("glu"):
     report("LN fwd [T,2048] bf16->bf16", timeit(lambda: ops.norm_fwd(gl, w, 1e-6, torch.bfloat16)), 8 * u)
     report("LN bwd [T,2048] bf16", timeit(lambda: ops.norm_bwd(dy, gl, w, st2, torch.bfloat16, dw=dw)), 12 * u)
     del ab, dy, gl, y, y2
+if want("rownorm"):
+    rownorm(args.dump)
 if want("norm"):
     x = torch.randn(T, H, device=dev)
     w = torch.ones(H, device=dev)
