@@ -27,7 +27,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 7
+#define MUSE_B200_ABI_VERSION 8
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -95,6 +95,17 @@ int muse_adamw_ema_step(const void* entries_host, int n_entries, float* scal_dev
                         const float* lr_dev, float lr_host, float beta1, float beta2, float eps, float weight_decay,
                         int ema_enabled, float ema_decay, float ema_min_decay, int ema_update_after_step,
                         int ema_update_every, int ema_use_warmup, float ema_inv_gamma, float ema_power, void* stream);
+
+/* One pass over all parameters: Lion (training/optimizer.py::Lion, the scripts' optimizer.name: lion) + the same EMA and
+ * bf16 copy as muse_adamw_ema_step, through the same table (the v slot is unused), step counter and scalar array.
+ * Per element, in the reference's operation order: p *= wd_scale; u = m * beta1 + g * one_minus_beta1; p -= lr * sign(u);
+ * m = m * beta2 + one_minus_beta2 * g.  wd_scale (1 - lr * weight_decay), one_minus_beta1 and one_minus_beta2 are formed
+ * in double by the caller and rounded once; with lr_dev the kernel forms 1 - lr * weight_decay in fp32 instead. */
+int muse_lion_ema_step(const void* entries_host, int n_entries, float* scal_dev, long long* step_dev,
+                       const float* lr_dev, float lr_host, float wd_scale, float beta1, float beta2, float one_minus_beta1,
+                       float one_minus_beta2, float weight_decay, int ema_enabled, float ema_decay, float ema_min_decay,
+                       int ema_update_after_step, int ema_update_every, int ema_use_warmup, float ema_inv_gamma,
+                       float ema_power, void* stream);
 
 /* Embed.forward (muse/modeling_transformer.py:942-957): out[b,s,:] = word[ids[b,s],:] + pos[s,:] (fp32). */
 int muse_embed_fwd(const long long* ids, const float* word, const float* pos, float* out, int B, int S, int H,

@@ -30,6 +30,7 @@ SIGNATURES = {
     "muse_gemm_bf16_splitk": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
     "muse_pack_bf16": (c_int, [_P, _I, _L, _P]),
     "muse_adamw_ema_step": (c_int, [_P, _I, _P, _P, _P, _F, _F, _F, _F, _F, _I, _F, _F, _I, _I, _I, _F, _F, _P]),
+    "muse_lion_ema_step": (c_int, [_P, _I, _P, _P, _P, _F, _F, _F, _F, _F, _F, _F, _I, _F, _F, _I, _I, _I, _F, _F, _P]),
     "muse_cast_bf16": (c_int, [_P, _P, _L, _P]),
     "muse_embed_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "muse_embed_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
@@ -77,7 +78,7 @@ SIGNATURES = {
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class MuseB200Error(RuntimeError):

@@ -200,14 +200,23 @@ class _PackedWeights:
             groups.append((-1, "logits", [m.to_logits.weight], m.padded_output_size))
         return groups
 
+    def _key(self, groups):
+        return tuple((p.data_ptr(), p._version, p.dtype) for _, _, ps, _ in groups for p in ps)
+
+    def sync(self):
+        """after a fused optimizer step that wrote every packed copy through ``dst_of``: the cache is current, so its key
+        follows the parameters' new version counters (no re-pack on the next forward)"""
+        if self.key is not None:
+            self.key = self._key(self._plan())
+
     def refresh(self):
         m = self.model
-        params = [p for _, _, ps, _ in self._plan() for p in ps]
-        key = tuple((p.data_ptr(), p._version, p.dtype) for p in params)
+        groups = self._plan()
+        params = [p for _, _, ps, _ in groups for p in ps]
+        key = self._key(groups)
         if key == self.key:
             return self
         dev = params[0].device
-        groups = self._plan()
         layout_key = tuple(p.data_ptr() for p in params)
         if getattr(self, "layout_key", None) != layout_key:
             total = 0
@@ -237,7 +246,7 @@ class _PackedWeights:
                         self.slow.append((p, dst))
                     r += p.shape[0]
             self.n_entries, self.n_blocks = len(entries), block
-            self.dst_of = {e[0]: e[1] for e in entries}  # parameter pointer -> bf16 copy (used by FusedAdamW)
+            self.dst_of = {e[0]: e[1] for e in entries}  # parameter pointer -> bf16 copy (used by the fused optimizers)
             self.table = torch.tensor(entries, dtype=torch.int64).to(dev) if entries else None
             self.layout_key = layout_key
         if self.table is not None:

@@ -192,6 +192,30 @@ class ConvMlmLayer(nn.Module):
 
 
 # ---------------------------------------------------------------------------------------------------------- the model
+class _OperandCache:
+    """The fused optimizers' view of ``MaskGiTUViT_v2._weights()``, the same protocol as ``MaskGitTransformer._packed``:
+    ``refresh()`` brings the cache up to date and returns an object whose ``dst_of`` maps a parameter's data_ptr to its bf16
+    copy, which the optimizer's pass writes; after the step ``sync()`` recomputes the few operands that are not such a copy
+    (``derived``: the transposed depthwise weights, the permuted down / up-sample weights) in place -- graph-capturable
+    copies -- and moves the cache's key to the parameters' new version counters, so the next forward rebuilds nothing."""
+
+    def __init__(self, model):
+        self.model = model
+        self.dst_of, self.derived = {}, []
+
+    def refresh(self):
+        self.model._weights()
+        return self
+
+    def sync(self):
+        m = self.model
+        if m._cache_key is None:
+            return
+        for dst, src in self.derived:
+            dst.copy_(src())
+        m._cache_key = m._weights_key()
+
+
 class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
     _supports_gradient_checkpointing = True
 
@@ -241,6 +265,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
             if isinstance(m, AdaLNModulation):
                 nn.init.constant_(m.mapper.weight, 0)
         self._cache_key, self._cache = None, None
+        self._packed = _OperandCache(self)  # the fused optimizers' handle on the cache (model=)
         self._debug_stages = None  # tests set this to a dict to receive the block-boundary activations
         self._graph = None         # CUDA graph of one decode-step forward (generate2), keyed by shapes and weight versions
 
@@ -260,14 +285,43 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         assert False  # (reference :326-328)
 
     # ------------------------------------------------------------------------------------ bf16 operand cache
+    def _weights_key(self):
+        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+
     def _weights(self):
         """bf16 GEMM operands (fused [k;v], [q;k;v], [wi_0;wi_1], all adaLN mappers stacked into one matrix, logits rows
-        padded to 64), rebuilt only when a parameter changes -- never inside generate2."""
-        params = list(self.parameters())
-        key = tuple((p.data_ptr(), p._version) for p in params)
+        padded to 64), rebuilt only when a parameter changes -- never inside generate2, and not after a fused optimizer
+        step with ``model=``, which writes them itself (``_packed``)."""
+        key = self._weights_key()
         if key == self._cache_key:
             return self._cache
-        bf = lambda *ws: torch.cat([w.detach().reshape(w.shape[0], -1) for w in ws], dim=0).to(torch.bfloat16).contiguous()
+        W, self._packed.dst_of, self._packed.derived = self._build_weights()
+        self._cache_key, self._cache = key, W
+        return W
+
+    def _build_weights(self):
+        """(W, dst_of, derived): the operand dict; parameter data_ptr -> address of its bf16 copy, for every parameter whose
+        operand is a plain row block of one bf16 matrix; and (destination, source view) of the operands that are not: the
+        transposed fp32 depthwise weights and the permuted down / up-sample weights."""
+        dev = next(self.parameters()).device
+        dst_of, derived = {}, []
+
+        def bf(*ws):
+            out = torch.cat([w.detach().reshape(w.shape[0], -1) for w in ws], dim=0).to(torch.bfloat16).contiguous()
+            r = 0
+            for w in ws:
+                dst_of[w.data_ptr()] = out[r: r + w.shape[0]].data_ptr()
+                r += w.shape[0]
+            return out
+
+        def derive(dtype, shape, src):  # src() is a view of the parameter laid out as the operand viewed as `shape`
+            out = torch.empty(shape, dtype=dtype, device=dev)
+            view = out.view(src().shape)
+            view.copy_(src())
+            derived.append((view, src))
+            return out
+
+        # fp32 operands of contiguous fp32 parameters are the parameters themselves (no copy to keep current)
         f32 = lambda w: None if w is None else w.detach().float().contiguous()
         W = {"encoder_proj": bf(self.encoder_proj.weight), "enc_norm": f32(self.encoder_proj_layer_norm.weight),
              "cond0": bf(self.cond_embed[0].weight), "cond2": bf(self.cond_embed[2].weight),
@@ -278,8 +332,9 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
              "mlm_norm": f32(self.mlm_layer.layer_norm.norm.weight)}
         V = self.config.codebook_size
         vpad = ((V + 63) // 64) * 64
-        w2 = torch.zeros(vpad, self.config.in_channels, dtype=torch.bfloat16, device=params[0].device)
+        w2 = torch.zeros(vpad, self.config.in_channels, dtype=torch.bfloat16, device=dev)
         w2[:V] = self.mlm_layer.conv2.weight.detach().reshape(V, -1).to(torch.bfloat16)
+        dst_of[self.mlm_layer.conv2.weight.data_ptr()] = w2[:V].data_ptr()  # the padding rows stay zero
         W["mlm2"], W["vpad"] = w2, vpad
         mappers, off = [], 0
 
@@ -292,19 +347,19 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
 
         def attn(a, fuse_q):
             hd = a.out.weight.shape[0] // a.num_heads  # 64: scale 0.125 exactly; 48 for 768-wide / 16-head layers
-            d = {"kv": bf(a.key.weight, a.value.weight), "o": bf(a.out.weight), "nh": a.num_heads, "hd": hd,
-                 "sc": 1.0 / math.sqrt(hd)}
-            if fuse_q:
+            d = {"o": bf(a.out.weight), "nh": a.num_heads, "hd": hd, "sc": 1.0 / math.sqrt(hd)}
+            if fuse_q:  # self-attention reads k and v from [q;k;v] only: no separate [k;v] copy of the same weights
                 d["qkv"] = bf(a.query.weight, a.key.weight, a.value.weight)
             else:
-                d["q"] = bf(a.query.weight)
+                d["q"], d["kv"] = bf(a.query.weight), bf(a.key.weight, a.value.weight)
             return d
 
         def block(blk):
             out = []
             for rb, ab in zip(blk.res_blocks, blk.attention_blocks):
+                dw = rb.depthwise.weight
                 out.append({
-                    "dw": f32(rb.depthwise.weight.detach().reshape(rb.depthwise.weight.shape[0], 9).t()),
+                    "dw": derive(torch.float32, (9, dw.shape[0]), lambda dw=dw: dw.detach().reshape(dw.shape[0], 9).t()),
                     "dw_norm": f32(rb.norm.norm.weight), "cw0": bf(rb.channelwise[0].weight),
                     "gamma": f32(rb.channelwise[2].gamma.reshape(-1)), "beta": f32(rb.channelwise[2].beta.reshape(-1)),
                     "cw4": bf(rb.channelwise[4].weight), "mod": mapper(rb.adaLN_modulation),
@@ -315,10 +370,12 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
 
         if c_down := self.down_blocks[0].downsample:  # [co, ci, dy, dx] -> [co, (dy, dx, ci)]: a GEMM over 2x2 patches
             W["ds_norm"] = f32(c_down[0].norm.weight)
-            W["ds"] = bf(c_down[1].weight.detach().permute(0, 2, 3, 1))
+            wd = c_down[1].weight
+            W["ds"] = derive(torch.bfloat16, (wd.shape[0], wd[0].numel()), lambda: wd.detach().permute(0, 2, 3, 1))
             c_up = self.up_blocks[0].upsample  # ConvTranspose2d weight [ci, co, dy, dx] -> [(dy, dx, co), ci]
             W["us_norm"] = f32(c_up[0].norm.weight)
-            W["us"] = bf(c_up[1].weight.detach().permute(2, 3, 1, 0).reshape(-1, c_up[1].weight.shape[0]))
+            wu = c_up[1].weight
+            W["us"] = derive(torch.bfloat16, (wu[0].numel(), wu.shape[0]), lambda: wu.detach().permute(2, 3, 1, 0))
         W["down"] = block(self.down_blocks[0])
         W["layers"] = []
         for l in self.transformer_layers:
@@ -330,8 +387,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
                 "wo": bf(l.ffn.wo.weight)})
         W["up"] = block(self.up_blocks[0])
         W["mappers"] = bf(*mappers)
-        self._cache_key, self._cache = key, W
-        return W
+        return W, dst_of, derived
 
     # ------------------------------------------------------------------------------------------- forward
     def _forward_tokens(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, drop=None):

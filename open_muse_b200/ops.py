@@ -63,7 +63,7 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
-_KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
+_KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_lion_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
                      "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3,
                      "muse_dwconv3x3_norm_bwd": 2}
 _prof = {"on": False, "events": []}

@@ -6,7 +6,10 @@ Reference: the training scripts step ``torch.optim.AdamW`` / apex ``FusedAdam`` 
 forward.  Here one kernel reads p, g, m, v (and the EMA shadow) once and writes p, m, v, the shadow and the packed bf16
 GEMM operand.  A ``torch.optim.Optimizer`` subclass, so LR schedulers, ``state_dict`` / ``load_state_dict``,
 ``zero_grad`` and ``accelerate`` treat it like AdamW.  CUDA-graph capturable (step counter and per-step scalars live on
-the device)."""
+the device).
+
+``FusedLion`` is the reference's ``training/optimizer.py::Lion`` (the scripts' ``optimizer.name: lion``; one moment instead
+of two) on the same machinery.  Both optimizers keep a model's bf16 operand cache current (see ``_FusedOptimizer``)."""
 from __future__ import annotations
 
 from typing import Optional
@@ -16,50 +19,52 @@ import torch
 from . import _lib, ops
 
 
-def _check_lr(lr, device=None):
+def _check_lr(lr, device=None, who="FusedAdamW"):
     """the kernel reads a tensor learning rate as ONE fp32 value at a device address: a host tensor would hand it a host
     address, another dtype the wrong bits"""
     if torch.is_tensor(lr) and (lr.numel() != 1 or lr.dtype != torch.float32 or (device is not None and lr.device != device)):
-        raise ValueError(f"FusedAdamW: a tensor lr must be a one-element float32 tensor on the parameters' device"
+        raise ValueError(f"{who}: a tensor lr must be a one-element float32 tensor on the parameters' device"
                          f"{'' if device is None else ' ' + str(device)}; got {lr.numel()} element(s) of {lr.dtype} "
                          f"on {lr.device}")
 
 
-class FusedAdamW(torch.optim.Optimizer):
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, ema=None, model=None):
-        """ema: an ``open_muse_b200.EMAModel`` built over the SAME parameter list (its shadow params are updated in the fused
-        pass; do not also call ``ema.step``).  model: a ``MaskGitTransformer`` whose packed bf16 operand cache receives
-        the updated weights directly (saves the re-pack launch of the next forward).
+class _FusedOptimizer(torch.optim.Optimizer):
+    """The launch plan, EMA wiring and operand-cache protocol shared by ``FusedAdamW`` and ``FusedLion``.
 
-        lr: a Python number, or (for a CUDA-graph-capturable schedule) a one-element float32 tensor on the parameters'
-        device, read by the kernel at every step; ``step`` raises ValueError for any other tensor.
+    A subclass names its per-parameter moment buffers (``_moments``: the table's m and v slots) and launches its kernel in
+    ``_launch``.  The kernels write parameters through raw pointers, which autograd does not see, so after every step the
+    written parameters' version counters are bumped: a model's operand cache keyed on ``(data_ptr, _version)`` then
+    rebuilds on its next forward.  With ``model=`` the step also writes the bf16 operands itself: ``model._packed``
+    provides ``refresh()`` (bring the cache up to date; returns an object whose ``dst_of`` maps a parameter's data_ptr to
+    its bf16 copy) and ``sync()`` (after the step: refresh the few operands that are not a plain copy of one parameter and
+    move the cache's key to the new versions), so no re-pack follows the step."""
 
-        Every parameter of the groups is expected to have a gradient at every step, as in the training scripts.  A parameter
-        without one is left out of that step's pass: its EMA shadow does not move (``EMAModel.step`` would move it toward
-        the parameter), and its bias correction follows its group's step counter, which a group without any gradient does
-        not advance."""
-        _check_lr(lr)
-        if lr < 0 or eps < 0 or not 0 <= betas[0] < 1 or not 0 <= betas[1] < 1 or weight_decay < 0:
-            raise ValueError("invalid AdamW hyper-parameters")
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+    _moments = ()
+
+    def __init__(self, params, defaults, ema, model):
+        super().__init__(params, defaults)
         self.ema, self.model = ema, model
         self._plans = {}
         if ema is not None:
             flat = [p for g in self.param_groups for p in g["params"]]
             if len(flat) != len(ema.shadow_params) or any(p.shape != s.shape for p, s in zip(flat, ema.shadow_params)):
-                raise ValueError("FusedAdamW(ema=...): the EMAModel must be built over the same parameter list")
+                raise ValueError(f"{type(self).__name__}(ema=...): the EMAModel must be built over the same parameter list")
 
     # ---- per-group launch plan (device table), rebuilt when pointers change (new grads storage, .to(device), ...)
-    def _packed_dst(self):
+    def _packed_cache(self):
+        m = self.model
+        return None if m is None or not hasattr(m, "_packed") else m._packed
+
+    def _packed_dst(self, cache):
         """parameter data_ptr -> address of its bf16 copy in the model's packed operand cache (host-side bookkeeping kept
         by the cache itself: no device read, so this is legal during graph capture)."""
-        m = self.model
-        if m is None or not hasattr(m, "_packed"):
+        if cache is None:
             return {}
-        pk = m._packed.refresh()
+        pk = cache.refresh()
         return dict(getattr(pk, "dst_of", {}) or {})
 
     def _plan(self, gi, group, shadow_of, packed_dst):
+        name = type(self).__name__
         params = [p for p in group["params"] if p.grad is not None]
         # every address the kernel writes through is part of the key: EMAModel.load_state_dict / .to replace the shadow
         # tensors while parameters and gradients stay where they are
@@ -73,21 +78,22 @@ class FusedAdamW(torch.optim.Optimizer):
         for p, (_, _, sh_ptr, packed_ptr) in zip(params, key):
             if p.dtype != torch.float32 or p.grad.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous() \
                     or p.numel() % 4 != 0 or p.grad.is_sparse:
-                raise RuntimeError("FusedAdamW needs contiguous fp32 parameters / gradients with numel % 4 == 0")
+                raise RuntimeError(f"{name} needs contiguous fp32 parameters / gradients with numel % 4 == 0")
             sh = shadow_of.get(id(p))
             if sh is not None and (sh.dtype != torch.float32 or sh.device != p.device or sh.shape != p.shape
                                    or not sh.is_contiguous()):
-                raise RuntimeError("FusedAdamW(ema=...) needs contiguous fp32 EMA shadows shaped and placed like the parameters")
+                raise RuntimeError(f"{name}(ema=...) needs contiguous fp32 EMA shadows shaped and placed like the parameters")
             st = self.state[p]
-            if not st:
-                st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-            entries.append((p.data_ptr(), p.grad.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(),
-                            sh_ptr, packed_ptr, p.numel(), 0))
+            for k in self._moments:
+                if k not in st:
+                    st[k] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            m, v = (st[k].data_ptr() for k in self._moments) if len(self._moments) == 2 else (st[self._moments[0]].data_ptr(), 0)
+            entries.append((p.data_ptr(), p.grad.data_ptr(), m, v, sh_ptr, packed_ptr, p.numel(), 0))
         plan = self._plans.get(gi) or {}
         if "step" not in plan:
             # one device-resident step counter per group, shared by the group's parameters' state entries so that
-            # state_dict() / load_state_dict() carry it (a freshly loaded state brings its own copy per parameter)
+            # state_dict() / load_state_dict() carry it (a freshly loaded state brings its own copy per parameter; a
+            # state without one -- e.g. the reference Lion's -- starts at 0)
             loaded = self.state[params[0]].get("step")
             step = loaded.to(device=dev, dtype=torch.int64).reshape(1).clone() if torch.is_tensor(loaded) else \
                 torch.zeros(1, dtype=torch.int64, device=dev)
@@ -102,6 +108,17 @@ class FusedAdamW(torch.optim.Optimizer):
         self._plans[gi] = plan
         return plan
 
+    @staticmethod
+    def _ema_args(ema):
+        """(enabled, decay, min_decay, update_after_step, update_every, use_warmup, inv_gamma, power) of the kernels"""
+        if ema is None:
+            return 0, 0.0, 0.0, 0, 1, 0, 1.0, 1.0
+        return (1, float(ema.decay), float(ema.min_decay), int(ema.update_after_step), int(ema.update_every),
+                1 if ema.use_ema_warmup else 0, float(ema.inv_gamma), float(ema.power))
+
+    def _launch(self, plan, group, lr_dev, ema_args, stream):
+        raise NotImplementedError
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = None
@@ -113,26 +130,82 @@ class FusedAdamW(torch.optim.Optimizer):
         if ema is not None:
             flat = [p for g in self.param_groups for p in g["params"]]
             shadow_of = {id(p): s for p, s in zip(flat, ema.shadow_params)}
-        packed_dst = self._packed_dst()
+        cache = self._packed_cache()
+        packed_dst = self._packed_dst(cache)
         live = [(gi, group) for gi, group in enumerate(self.param_groups) if any(p.grad is not None for p in group["params"])]
         for _, group in live:  # every group before the first launch (a scheduler may have assigned any tensor)
-            _check_lr(group["lr"], next(p.device for p in group["params"] if p.grad is not None))
+            _check_lr(group["lr"], next(p.device for p in group["params"] if p.grad is not None), type(self).__name__)
+        ema_args = self._ema_args(ema)
+        written = []
         for gi, group in live:
             plan = self._plan(gi, group, shadow_of, packed_dst)
             lr = group["lr"]
-            lr_dev = lr if torch.is_tensor(lr) else None
-            st = ops._prep(plan["scal"])
-            b1, b2 = group["betas"]
-            ops._call("muse_adamw_ema_step", plan["table"].ctypes.data, plan["n"], plan["scal"].data_ptr(),
-                      plan["step"].data_ptr(), None if lr_dev is None else lr_dev.data_ptr(),
-                      0.0 if lr_dev is not None else float(lr), float(b1), float(b2), float(group["eps"]),
-                      float(group["weight_decay"]), 1 if ema is not None else 0,
-                      float(ema.decay) if ema is not None else 0.0, float(ema.min_decay) if ema is not None else 0.0,
-                      int(ema.update_after_step) if ema is not None else 0, int(ema.update_every) if ema is not None else 1,
-                      1 if (ema is not None and ema.use_ema_warmup) else 0, float(ema.inv_gamma) if ema is not None else 1.0,
-                      float(ema.power) if ema is not None else 1.0, st)
+            self._launch(plan, group, lr if torch.is_tensor(lr) else None, ema_args, ops._prep(plan["scal"]))
+            written += plan["params"]
+        if written:
+            torch.autograd.graph.increment_version(written)
+            if cache is not None:
+                cache.sync()
         if ema is not None:  # host mirror of the device-side schedule (state_dict / logging), same rule as EMAModel.step
             ema.optimization_step += 1
             if (ema.optimization_step - 1) % ema.update_every == 0:
                 ema.cur_decay_value = ema.get_decay(ema.optimization_step)
         return loss
+
+
+class FusedAdamW(_FusedOptimizer):
+    _moments = ("exp_avg", "exp_avg_sq")
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, ema=None, model=None):
+        """ema: an ``open_muse_b200.EMAModel`` built over the SAME parameter list (its shadow params are updated in the fused
+        pass; do not also call ``ema.step``).  model: a ``MaskGitTransformer`` or ``MaskGiTUViT_v2`` whose bf16 operand
+        cache receives the updated weights directly (saves the re-pack of the next forward).
+
+        lr: a Python number, or (for a CUDA-graph-capturable schedule) a one-element float32 tensor on the parameters'
+        device, read by the kernel at every step; ``step`` raises ValueError for any other tensor.
+
+        Every parameter of the groups is expected to have a gradient at every step, as in the training scripts.  A parameter
+        without one is left out of that step's pass: its EMA shadow does not move (``EMAModel.step`` would move it toward
+        the parameter), and its bias correction follows its group's step counter, which a group without any gradient does
+        not advance."""
+        _check_lr(lr)
+        if lr < 0 or eps < 0 or not 0 <= betas[0] < 1 or not 0 <= betas[1] < 1 or weight_decay < 0:
+            raise ValueError("invalid AdamW hyper-parameters")
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), ema, model)
+
+    def _launch(self, plan, group, lr_dev, ema_args, stream):
+        b1, b2 = group["betas"]
+        ops._call("muse_adamw_ema_step", plan["table"].ctypes.data, plan["n"], plan["scal"].data_ptr(),
+                  plan["step"].data_ptr(), None if lr_dev is None else lr_dev.data_ptr(),
+                  0.0 if lr_dev is not None else float(group["lr"]), float(b1), float(b2), float(group["eps"]),
+                  float(group["weight_decay"]), *ema_args, stream)
+
+
+class FusedLion(_FusedOptimizer):
+    _moments = ("exp_avg",)
+
+    def __init__(self, params, lr=1e-4, betas=(0.9, 0.99), weight_decay=0.0, ema=None, model=None, **kwargs):
+        """Lion (training/optimizer.py::Lion) + EMA + bf16 operand copy in one pass; ``ema`` / ``model`` / a tensor ``lr``
+        as in ``FusedAdamW``.  Other keywords (the training script passes ``eps`` to every optimizer class) are accepted
+        and ignored, as the reference does.
+
+        With a Python-number lr, parameters and ``exp_avg`` equal the reference's on the same GPU bit for bit
+        (``1 - lr * weight_decay``, ``1 - beta1`` and ``1 - beta2`` are formed in double as the reference's Python
+        scalars are).  With a tensor lr, ``1 - lr * weight_decay`` is formed in fp32 on the device.  The state of each
+        parameter is ``exp_avg`` (loads into the reference ``Lion`` and back) plus the group's device-resident ``step``
+        (the EMA schedule's counter; 0 when a reference state without one is loaded)."""
+        _check_lr(lr, who="FusedLion")
+        if not 0.0 <= lr:
+            raise ValueError(f"FusedLion: invalid learning rate {lr}")
+        for i in (0, 1):
+            if not 0.0 <= betas[i] < 1.0:
+                raise ValueError(f"FusedLion: invalid beta parameter at index {i}: {betas[i]}")
+        super().__init__(params, dict(lr=lr, betas=betas, weight_decay=weight_decay), ema, model)
+
+    def _launch(self, plan, group, lr_dev, ema_args, stream):
+        b1, b2 = group["betas"]
+        lr, wd = group["lr"], float(group["weight_decay"])
+        ops._call("muse_lion_ema_step", plan["table"].ctypes.data, plan["n"], plan["scal"].data_ptr(),
+                  plan["step"].data_ptr(), None if lr_dev is None else lr_dev.data_ptr(),
+                  0.0 if lr_dev is not None else float(lr), 1.0 if lr_dev is not None else 1.0 - float(lr) * wd,
+                  float(b1), float(b2), 1.0 - float(b1), 1.0 - float(b2), wd, *ema_args, stream)
