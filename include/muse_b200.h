@@ -27,7 +27,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 8
+#define MUSE_B200_ABI_VERSION 9
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -286,6 +286,15 @@ int muse_sample_step(const void* logits, const void* logits_unc, long long row_s
  * residual [B,H,W,Cout] (ResnetBlock :82-85) -> y [B,H,W,Cout]. */
 int muse_conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H,
                      int W, int Cin, int Cout, int ksize, int upsample2x, void* stream);
+/* Further values of upsample2x (the mode) for the Paella tokenizer (muse/modeling_paella_vq.py):
+ *   2 with ksize 2: stride 2, pad 0, 2x2 taps -- PixelUnshuffle(2) + 1x1 conv (in_block), wk from the 1x1 weight viewed
+ *     as [Cout, Cin, 2, 2];
+ *   3: Conv2d(k=4, s=2, p=1), x [B,2H,2W,Cin], ksize 4;
+ *   4: ConvTranspose2d(k=4, s=2, p=1), x [B,H/2,W/2,Cin], ksize 4, wk the four parity matrices [4][4*Cin][Cout] (parity
+ *     2*(y&1) + (x&1); row (a*2+b)*Cin + ci for window offset (a,b) at input pixel (y>>1) + a + (y&1) - 1; kernel tap
+ *     3 - 2a - (y&1), likewise for columns);
+ *   | 8: y = GELU(conv + bias) (exact erf form, no residual);
+ *   | 16: PixelShuffle(2) folded into the store (mode 0, Cout % 4 == 0): y [B,2H,2W,Cout/4]. */
 /* nn.GroupNorm(groups, C, eps) + F.silu (:61-79), deterministic (no atomics). Scratch: partials_ws float
  * [muse_groupnorm_workspace_floats(B,HW,C)] (-1 if the shape is unsupported), scale_shift_ws float [B*C*3].
  * Output either y (fp32) or the pair y_hi / y_lo (bf16 planes with y = hi + lo, the operand form of
@@ -316,6 +325,14 @@ int muse_conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, i
 int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias,
                         const float* res, float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize,
                         int mode, void* stream);
+/* mode & 16 (Cout <= 16, Cout % 4 == 0, stride 1, no residual): PixelShuffle(2) folded into the store, y [B,2H,2W,Cout/4]
+ * (the Paella out_block).
+ * muse_conv2d_nhwc_tc_gelu_split: y = GELU(conv + bias) (exact erf form) stored as the bf16 planes y_hi / y_lo
+ * [B,H,W,Cout] (y_lo unused with mode & 8) that the next muse_conv2d_nhwc_tc consumes: the c -> 4c Linear + GELU of the
+ * Paella ResBlock.  Cout > 16, stride-1 modes (mode & 7 == 0), no residual, no statistics. */
+int muse_conv2d_nhwc_tc_gelu_split(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo,
+                                   const float* bias, void* y_hi, void* y_lo, int B, int H, int W, int Cin, int Cout,
+                                   int ksize, int mode, void* stream);
 /* mode & 3: 0 plain, 1 upsample2x (above), 2 = ksize 2 with taps at offsets (0,0),(0,1),(1,0),(1,1) and zeros beyond the
  * right / bottom edge: the stride-2 3x3 convolution with pad (0,1,0,1) of the taming Downsample
  * (modeling_taming_vqgan.py:47-62) after muse_split_s2d_bf16_nhwc, weights [Cout, 4 taps * 4 Cin].  mode & 4: per-image
@@ -332,7 +349,15 @@ int muse_softmax_split_rows(const float* x, void* hi, void* lo, float* out_f32, 
 int muse_split_bf16_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int C, int upsample2x, void* stream);
 /* Stem convolutions with ksize*ksize*Cin <= 64 (3 -> 128 conv_in): im2col of the taps into 64-wide bf16 hi/lo rows
  * [B,H,W,64] (tap-major, zero padded), consumed by muse_conv2d_nhwc_tc as a 1x1 convolution with Cin = 64. */
+/* ksize 2: x is [B,2H,2W,Cin] and each row is the pixel's PixelUnshuffle(2) block, column c*4 + dy*2 + dx (Paella in_block). */
 int muse_im2col_split_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int Cin, int ksize, void* stream);
+/* Spatial half of the Paella ResBlock (muse/modeling_paella_vq.py:136-139), fp32 NHWC x [B,H,W,C], C % 8 == 0, C <= 1024:
+ * x1 = x + bias + depthwise3x3(ReplicationPad2d(1)(LN1(x))) with wk [9][C] (tap-major), then n2 = LN2(x1); both LayerNorms
+ * without affine, eps given (the ResBlock's gammas are folded into wk / bias and the Linears by the caller).
+ * stats_ws: float [2*B*H*W] (per-pixel LN1 mean, rstd).  n2 goes to fp32 n2 or to the bf16 planes n2_hi (+ n2_lo, NULL in
+ * single-pass mode) -- exactly one of the two forms. */
+int muse_paella_resblock_spatial(const float* x, const float* wk, const float* bias, float* stats_ws, float* x1, float* n2,
+                                 void* n2_hi, void* n2_lo, int B, int H, int W, int C, float eps, void* stream);
 /* F.avg_pool2d(2,2) (:112): x [B,2Ho,2Wo,C] -> y [B,Ho,Wo,C]. */
 int muse_avgpool2_nhwc(const float* x, float* y, int B, int Ho, int Wo, int C, void* stream);
 /* Decoder output (fp32, any layout; the caller passes the NHWC tensor) -> display bytes with the reference's recipe

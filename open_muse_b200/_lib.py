@@ -71,14 +71,16 @@ SIGNATURES = {
     "muse_conv2d_tc_tiles_per_image": (c_int, [_I, _I, _I, _I, _I, _I]),
     "muse_conv2d_tc_supported": (c_int, [_I, _I, _I, _I, _I]),
     "muse_conv2d_nhwc_tc": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "muse_conv2d_nhwc_tc_gelu_split": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "muse_im2col_split_nhwc": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "muse_paella_resblock_spatial": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "muse_split_bf16_nhwc": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "muse_avgpool2_nhwc": (c_int, [_P, _P, _I, _I, _I, _I, _P]),
     "muse_image_to_uint8": (c_int, [_P, _P, _L, _P]),
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 
 class MuseB200Error(RuntimeError):

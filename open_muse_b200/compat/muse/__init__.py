@@ -19,13 +19,14 @@ from . import logging, lr_schedulers  # noqa: F401,E402
 
 
 class _OutOfScopeTokenizer:
-    """MOVQ / PaellaVQModel are other tokenizers the training scripts import by name (training/train_muse.py:49-58,
-    train_maskgit_imagenet.py:38); they are outside this package's hot path (DESIGN.md section 7) and fail loudly if a
-    config actually selects them."""
+    """MOVQ is another tokenizer the training scripts import by name (training/train_muse.py:49-58,
+    train_maskgit_imagenet.py:38); it is outside this package's hot path (DESIGN.md section 7) and fails loudly if a
+    config actually selects it."""
 
     def __init__(self, *a, **k):
         raise NotImplementedError(f"open_muse_b200: {type(self).__name__} is not part of the H100 hot path; use "
-                                  "MaskGitVQGAN (model.vq_model.type: maskgit_vqgan) or VQGANModel (taming)")
+                                  "MaskGitVQGAN (model.vq_model.type: maskgit_vqgan), VQGANModel (taming) or PaellaVQModel "
+                                  "(paella_vq)")
 
     @classmethod
     def from_pretrained(cls, *a, **k):
@@ -36,5 +37,4 @@ class MOVQ(_OutOfScopeTokenizer):
     pass
 
 
-class PaellaVQModel(_OutOfScopeTokenizer):
-    pass
+from open_muse_b200.modeling_paella_vq import PaellaVQModel  # noqa: F401,E402

@@ -26,15 +26,25 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
   constexpr int BM = 16 * TM, BN = 16 * TN;
   __shared__ __align__(16) float sA[KT][BM];
   __shared__ __align__(16) float sB[KT][BN];
-  const long long M = static_cast<long long>(B) * H * W;
-  const int K = ksize * ksize * Cin;
+  // up & 7 (geometry): 0 plain 'same'; 1 nearest x2 upsample folded into the gather; 2 stride 2, pad 0 (ksize 3: the taming
+  // Downsample with pad (0,1,0,1); ksize 2: PixelUnshuffle(2) + 1x1 of the Paella in_block); 3 stride 2, pad 1, ksize 4
+  // (Paella Conv2d(4, 2, 1)); 4 ConvTranspose2d(4, 2, 1) as four 2x2 parity convolutions on the H/2 x W/2 input, parity
+  // blockIdx.z, weights [4][4*Cin][Cout].  up & 8: GELU epilogue; up & 16: PixelShuffle(2) folded into the store.
+  const int md = up & 7, gelu = up & 8, shuf = up & 16;
+  const int s2 = (md == 2 || md == 3), tr = (md == 4);
+  const int par = tr ? static_cast<int>(blockIdx.z) : 0;
+  const int Hg = tr ? H / 2 : H, Wg = tr ? W / 2 : W;  // the grid the output rows m run over
+  const long long M = static_cast<long long>(B) * Hg * Wg;
+  const int kk_size = tr ? 2 : ksize;
+  const int K = kk_size * kk_size * Cin;
+  wk += static_cast<long long>(par) * K * Cout;
   const long long m0 = static_cast<long long>(blockIdx.x) * BM;
   const int n0 = blockIdx.y * BN;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  // up: 0 plain 'same'; 1 nearest x2 upsample folded into the gather; 2 stride 2 with pad (0,1,0,1) (taming Downsample)
-  const int s2 = (up == 2);
-  const int Hi = up == 1 ? H / 2 : (s2 ? 2 * H : H), Wi = up == 1 ? W / 2 : (s2 ? 2 * W : W);
-  const int pad = s2 ? 0 : ksize / 2;
+  const int Hi = md == 1 ? H / 2 : (s2 ? 2 * H : Hg), Wi = md == 1 ? W / 2 : (s2 ? 2 * W : Wg);
+  const int Hb = md == 1 ? H : Hi, Wb = md == 1 ? W : Wi;  // bounds of the (virtual) input grid the taps index
+  const int offy = tr ? (par >> 1) - 1 : (md == 3 ? -1 : (s2 ? 0 : -(ksize / 2)));
+  const int offx = tr ? (par & 1) - 1 : offy;
   const int st = s2 ? 2 : 1;
 
   // A-loader role: BM rows x 8 k per stage. VEC: one float4 per (row, half); scalar: BM*8/256 elements.
@@ -57,9 +67,9 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
     const long long m = m0 + a_row[i];
     a_ok[i] = m < M;
     const long long mm = a_ok[i] ? m : 0;
-    ax[i] = static_cast<int>(mm % W);
-    ay[i] = static_cast<int>((mm / W) % H);
-    ab[i] = static_cast<int>(mm / (static_cast<long long>(W) * H));
+    ax[i] = static_cast<int>(mm % Wg);
+    ay[i] = static_cast<int>((mm / Wg) % Hg);
+    ab[i] = static_cast<int>(mm / (static_cast<long long>(Wg) * Hg));
   }
 
   float acc[TM][TN];
@@ -73,11 +83,10 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
     if (VEC) {
       const int k = k0 + a_k[0];
       const int tap = k / Cin, ci = k % Cin;
-      const int iy = ay[0] * st + tap / ksize - pad, ix = ax[0] * st + tap % ksize - pad;
+      const int iy = ay[0] * st + tap / kk_size + offy, ix = ax[0] * st + tap % kk_size + offx;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      const int Hb = s2 ? Hi : H, Wb = s2 ? Wi : W;  // bounds of the (virtual) input grid the taps index
       if (a_ok[0] && iy >= 0 && iy < Hb && ix >= 0 && ix < Wb) {
-        const int sy = up == 1 ? (iy >> 1) : iy, sx = up == 1 ? (ix >> 1) : ix;
+        const int sy = md == 1 ? (iy >> 1) : iy, sx = md == 1 ? (ix >> 1) : ix;
         v = *reinterpret_cast<const float4*>(x + ((static_cast<long long>(ab[0]) * Hi + sy) * Wi + sx) * Cin + ci);
       }
       sA[a_k[0] + 0][a_row[0]] = v.x; sA[a_k[0] + 1][a_row[0]] = v.y;
@@ -89,10 +98,9 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
         float v = 0.f;
         if (k < K && a_ok[i]) {
           const int tap = k / Cin, ci = k % Cin;
-          const int iy = ay[i] * st + tap / ksize - pad, ix = ax[i] * st + tap % ksize - pad;
-          const int Hb = s2 ? Hi : H, Wb = s2 ? Wi : W;
+          const int iy = ay[i] * st + tap / kk_size + offy, ix = ax[i] * st + tap % kk_size + offx;
           if (iy >= 0 && iy < Hb && ix >= 0 && ix < Wb) {
-            const int sy = up == 1 ? (iy >> 1) : iy, sx = up == 1 ? (ix >> 1) : ix;
+            const int sy = md == 1 ? (iy >> 1) : iy, sx = md == 1 ? (ix >> 1) : ix;
             v = x[((static_cast<long long>(ab[i]) * Hi + sy) * Wi + sx) * Cin + ci];
           }
         }
@@ -123,14 +131,19 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
   for (int i = 0; i < TM; ++i) {
     const long long m = m0 + ty * TM + i;
     if (m >= M) continue;
+    const long long gx = m % Wg, gy = (m / Wg) % Hg, gb = m / (static_cast<long long>(Wg) * Hg);
+    const long long orow = tr ? (gb * H + 2 * gy + (par >> 1)) * W + 2 * gx + (par & 1) : m;
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
       const int n = n0 + tx * TN + j;
       if (n < Cout) {
         float v = acc[i][j];
         if (bias) v += bias[n];
-        if (res) v += res[m * Cout + n];
-        y[m * Cout + n] = v;
+        if (res) v += res[orow * Cout + n];
+        if (gelu) v = 0.5f * v * (1.f + erff(v * 0.70710678118654752440f));
+        long long off = orow * Cout + n;
+        if (shuf) off = ((gb * 2 * H + 2 * gy + ((n >> 1) & 1)) * 2 * W + 2 * gx + (n & 1)) * (Cout / 4) + (n >> 2);
+        y[off] = v;
       }
     }
   }
@@ -399,22 +412,30 @@ using namespace muse;
 extern "C" {
 
 int muse_conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H, int W,
-                     int Cin, int Cout, int ksize, int upsample2x, void* stream) {
+                     int Cin, int Cout, int ksize, int mode, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (ksize != 1 && ksize != 3) { set_last_error("conv2d: kernel size %d unsupported (1 or 3)", ksize); return MUSE_ERR_UNSUPPORTED; }
-  if (upsample2x == 1 && ((H | W) & 1)) { set_last_error("conv2d: upsample2x needs even output dims"); return MUSE_ERR_INVALID; }
-  if (upsample2x == 2 && ksize != 3) { set_last_error("conv2d: the stride-2 mode is the 3x3 taming Downsample"); return MUSE_ERR_INVALID; }
-  const long long M = static_cast<long long>(B) * H * W;
+  const int md = mode & 7;
+  if (md > 4 || (mode & ~31) != 0) { set_last_error("conv2d: bad mode %d", mode); return MUSE_ERR_INVALID; }
+  const bool k_ok = md == 2 ? (ksize == 2 || ksize == 3) : (md >= 3 ? ksize == 4 : (ksize == 1 || ksize == 3));
+  if (!k_ok) { set_last_error("conv2d: kernel size %d unsupported in mode %d", ksize, md); return MUSE_ERR_UNSUPPORTED; }
+  if ((md == 1 || md == 4) && ((H | W) & 1)) { set_last_error("conv2d: upsampling modes need even output dims"); return MUSE_ERR_INVALID; }
+  if ((mode & 8) && res) { set_last_error("conv2d: the GELU epilogue takes no residual"); return MUSE_ERR_INVALID; }
+  if ((mode & 16) && (res || md != 0 || Cout % 4 != 0)) {
+    set_last_error("conv2d: the PixelShuffle store needs Cout %% 4 == 0, stride 1, no residual");
+    return MUSE_ERR_INVALID;
+  }
+  const long long M = static_cast<long long>(B) * H * W / (md == 4 ? 4 : 1);
   if (M <= 0) return MUSE_OK;
   const bool vec = (Cin % 8 == 0);
+  const unsigned gz = md == 4 ? 4 : 1;
   if (Cout > 16) {
-    dim3 grid(static_cast<unsigned>(ceil_div_ll(M, 128)), ceil_div(Cout, 128));
-    if (vec) pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 8, true>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, upsample2x);
-    else pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 8, false>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, upsample2x);
+    dim3 grid(static_cast<unsigned>(ceil_div_ll(M, 128)), ceil_div(Cout, 128), gz);
+    if (vec) pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 8, true>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, mode);
+    else pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 8, false>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, mode);
   } else {
-    dim3 grid(static_cast<unsigned>(ceil_div_ll(M, 128)), 1);
-    if (vec) pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 1, true>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, upsample2x);
-    else pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 1, false>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, upsample2x);
+    dim3 grid(static_cast<unsigned>(ceil_div_ll(M, 128)), 1, gz);
+    if (vec) pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 1, true>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, mode);
+    else pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 1, false>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, mode);
   }
   return check_launch("conv2d_nhwc");
 }

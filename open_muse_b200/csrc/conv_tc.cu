@@ -50,7 +50,13 @@ struct ConvParams {
   int wbatch;           // weights are per image: [B][C_out][K] (attention scores / values as 1x1 convolutions)
   int num_m, num_n, cchunks, num_kb;
   int passes;           // 3: bf16x3 (hi*hi + lo*hi + hi*lo, fp32-faithful); 1: hi*hi only (plain bf16 operands, fast mode)
+  bf16* yh;             // non-null: y = GELU(acc + bias) is stored as these bf16 planes (yl: lo, nullable) instead of fp32 y
+  bf16* yl;
+  int shuffle;          // C_out <= 16: PixelShuffle(2) folded into the store, y is [B, 2H, 2W, C_out / 4]
 };
+
+// nn.GELU() (exact erf form) of the Paella ResBlock's channelwise MLP
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
 
 template <int BN>
 __global__ void __launch_bounds__(tc::kThreads, 1)
@@ -143,10 +149,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               if (col + e < p.N) {
-                const size_t off = static_cast<size_t>(orow[hr]) * p.N + col + e;
+                size_t off = static_cast<size_t>(orow[hr]) * p.N + col + e;
                 float v = acc[4 * j + 2 * hr + e];
                 if (p.bias != nullptr) v += p.bias[col + e];
                 if (p.res != nullptr) v += p.res[off];
+                if (p.shuffle) {  // channel c*4 + dy*2 + dx of pixel (y, x) -> channel c of pixel (2y + dy, 2x + dx)
+                  const long long px = orow[hr], xx = px % p.W, yy = (px / p.W) % p.H, b = px / (static_cast<long long>(p.W) * p.H);
+                  const int ch = col + e;
+                  off = static_cast<size_t>(((b * 2 * p.H + 2 * yy + ((ch >> 1) & 1)) * 2 * p.W + 2 * xx + (ch & 1)) * (p.N / 4) + (ch >> 2));
+                }
                 p.y[off] = v;
               }
             }
@@ -157,6 +168,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
           for (int hr = 0; hr < 2; ++hr) {
             const size_t off = static_cast<size_t>(orow[hr]) * p.N + col;
             float2 o = make_float2(acc[4 * j + 2 * hr] + b2.x, acc[4 * j + 2 * hr + 1] + b2.y);
+            if (p.yh != nullptr) {  // GELU, stored as the operand planes of the next 1x1 convolution
+              const float g0 = gelu_erf(o.x), g1 = gelu_erf(o.y);
+              const float h0 = bf16_round(g0), h1 = bf16_round(g1);
+              *reinterpret_cast<uint32_t*>(p.yh + off) = pack_bf16(h0, h1);
+              if (p.yl != nullptr) *reinterpret_cast<uint32_t*>(p.yl + off) = pack_bf16(g0 - h0, g1 - h1);
+              continue;
+            }
             if (p.res != nullptr) {
               const float2 r2 = *reinterpret_cast<const float2*>(p.res + off);
               o.x += r2.x; o.y += r2.y;
@@ -244,6 +262,8 @@ split_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ hi, bf16* __re
 
 // Small-C_in stem (3 -> 128 at full resolution): im2col of the k*k*C_in <= 64 taps into 64-wide bf16 hi/lo rows, so the
 // stem runs as a 1x1 tensor-core convolution with C_in = 64 (zero columns past k*k*C_in).  8 threads per pixel.
+// ksize 2: nn.PixelUnshuffle(2) of the [B, 2H, 2W, C_in] input (Paella in_block), column c*4 + dy*2 + dx of output pixel
+// (y, x) = x[2y + dy, 2x + dx, c].
 __global__ void __launch_bounds__(256)
 im2col_split_kernel(const float* __restrict__ x, bf16* __restrict__ hi, bf16* __restrict__ lo, long long pixels, int H, int W,
                     int Cin, int ksize) {
@@ -261,7 +281,9 @@ im2col_split_kernel(const float* __restrict__ x, bf16* __restrict__ hi, bf16* __
   for (int j = 0; j < 8; ++j) {
     const int k = chunk * 8 + j;
     float v = 0.f;
-    if (k < K) {
+    if (k < K && ksize == 2) {
+      v = x[((b * 2 * H + 2 * oy + ((k >> 1) & 1)) * 2 * W + 2 * ox + (k & 1)) * Cin + (k >> 2)];
+    } else if (k < K) {
       const int tap = k / Cin, ci = k % Cin;
       const int iy = oy + tap / ksize - pad, ix = ox + tap % ksize - pad;
       if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = x[((b * H + iy) * W + ix) * Cin + ci];
@@ -369,10 +391,23 @@ int muse_conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, i
 // mode & 8: single-pass bf16 (fast tokenizer mode): only the hi planes are multiplied (x_lo / w_lo may be null): one tensor-core
 //   product per fp32 product instead of three, bf16-operand accuracy (~4e-3 per layer instead of ~2e-5).
 // x_hi/x_lo: bf16 [B,H,W,Cin]; w_hi/w_lo: bf16 [Cout, k*k*Cin] (tap-major, then input channel); y fp32 [B,H,W,Cout].
-int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias, const float* res,
-                        float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode, void* stream) {
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+}  // extern "C"
+
+namespace {
+// muse_conv2d_nhwc_tc, and with yh != nullptr muse_conv2d_nhwc_tc_gelu_split
+int conv_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias, const float* res,
+            float* y, bf16* yh, bf16* yl, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode,
+            cudaStream_t s) {
   if (B <= 0) return MUSE_OK;
+  const int shuffle = (mode & 16) ? 1 : 0;
+  if (shuffle && (Cout > 16 || Cout % 4 != 0 || res != nullptr || (mode & 3) != 0)) {
+    set_last_error("conv2d_tc: the PixelShuffle store needs C_out <= 16, C_out %% 4 == 0, no residual, stride 1");
+    return MUSE_ERR_UNSUPPORTED;
+  }
+  if (yh != nullptr && (Cout <= 16 || res != nullptr || (mode & 7) != 0)) {
+    set_last_error("conv2d_tc: the GELU split epilogue needs C_out > 16, no residual, a plain stride-1 convolution");
+    return MUSE_ERR_UNSUPPORTED;
+  }
   const int upsample2x = (mode & 3) == 1;
   const int fwd2x2 = (mode & 3) == 2;
   if (fwd2x2 != (ksize == 2)) { set_last_error("conv2d_tc: ksize 2 and mode 2 go together"); return MUSE_ERR_INVALID; }
@@ -387,13 +422,15 @@ int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, co
     set_last_error("conv2d_tc: unsupported shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W, Cin, Cout, ksize);
     return MUSE_ERR_UNSUPPORTED;
   }
-  if ((reinterpret_cast<uintptr_t>(y) & 15) || (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) ||
+  if ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(yh) & 15) || (reinterpret_cast<uintptr_t>(yl) & 15) ||
+      (bias && (reinterpret_cast<uintptr_t>(bias) & 15)) ||
       (res && (reinterpret_cast<uintptr_t>(res) & 15))) {
     set_last_error("conv2d_tc: y / bias / res must be 16B aligned");
     return MUSE_ERR_INVALID;
   }
   ConvParams p;
-  p.y = y; p.bias = bias; p.res = res; p.stats = (Cout > 16) ? stats : nullptr;
+  p.y = y; p.bias = bias; p.res = res; p.stats = (Cout > 16 && yh == nullptr) ? stats : nullptr;
+  p.yh = yh; p.yl = (mode & 8) ? nullptr : yl; p.shuffle = shuffle;
   p.N = Cout; p.H = H; p.W = W; p.Cin = Cin; p.ksize = ksize;
   const int tile_px = 128;
   p.tile_w = W >= tile_px ? tile_px : W;
@@ -434,11 +471,34 @@ int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, co
   if (BN == 128) return launch_conv<128>(ah, al, bh, bl, p, s);
   return launch_conv<16>(ah, al, bh, bl, p, s);
 }
+}  // namespace
 
-// x fp32 [B,H,W,Cin] with k*k*Cin <= 64 -> hi, lo bf16 [B,H,W,64]: row = the k*k*Cin taps of the pixel (tap-major), zero padded
+extern "C" {
+
+int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias, const float* res,
+                        float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode, void* stream) {
+  return conv_tc(x_hi, x_lo, w_hi, w_lo, bias, res, y, nullptr, nullptr, stats, B, H, W, Cin, Cout, ksize, mode,
+                 static_cast<cudaStream_t>(stream));
+}
+
+// y = GELU(conv(x) + bias) written as bf16 planes y_hi [B,H,W,Cout] (+ y_lo unless mode & 8), the operands of the next
+// tensor-core convolution: the c -> 4c Linear + GELU of the Paella ResBlock.  Stride-1 modes only (mode & 7 == 0).
+int muse_conv2d_nhwc_tc_gelu_split(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias,
+                                   void* y_hi, void* y_lo, int B, int H, int W, int Cin, int Cout, int ksize, int mode,
+                                   void* stream) {
+  if (y_hi == nullptr || ((mode & 8) == 0 && y_lo == nullptr)) {
+    set_last_error("conv2d_tc_gelu_split: y_hi (and y_lo unless single-pass) are required");
+    return MUSE_ERR_INVALID;
+  }
+  return conv_tc(x_hi, x_lo, w_hi, w_lo, bias, nullptr, nullptr, reinterpret_cast<bf16*>(y_hi), reinterpret_cast<bf16*>(y_lo),
+                 nullptr, B, H, W, Cin, Cout, ksize, mode, static_cast<cudaStream_t>(stream));
+}
+
+// x fp32 [B,H,W,Cin] with k*k*Cin <= 64 -> hi, lo bf16 [B,H,W,64]: row = the k*k*Cin taps of the pixel (tap-major), zero padded;
+// ksize 2: x is [B,2H,2W,Cin] and the row is its PixelUnshuffle(2) (column c*4 + dy*2 + dx)
 int muse_im2col_split_nhwc(const float* x, void* hi, void* lo, int B, int H, int W, int Cin, int ksize, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (ksize * ksize * Cin > 64 || (ksize != 1 && ksize != 3)) {
+  if (ksize * ksize * Cin > 64 || (ksize != 1 && ksize != 2 && ksize != 3)) {
     set_last_error("im2col_split: k*k*Cin = %d must be <= 64", ksize * ksize * Cin);
     return MUSE_ERR_UNSUPPORTED;
   }

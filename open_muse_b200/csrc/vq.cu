@@ -68,10 +68,13 @@ vq_argmin_kernel(const float* __restrict__ z, const float* __restrict__ cb, cons
         const int idx = threadIdx.x + it * 256;  // 128 rows x 4 float4
         const int r = idx >> 2, kq = (idx & 3) * 4;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row0 + r < n) v = *reinterpret_cast<const float4*>(z + static_cast<size_t>(row0 + r) * D + k0 + kq);
+        // k past D (D % 16 != 0, e.g. the Paella latent D = 4) loads zeros: fmaf(0, 0, acc) == acc, so every chain is
+        // the same as if it stopped at D
+        const bool kin = k0 + kq < D;
+        if (row0 + r < n && kin) v = *reinterpret_cast<const float4*>(z + static_cast<size_t>(row0 + r) * D + k0 + kq);
         sZ[kq + 0][r] = v.x; sZ[kq + 1][r] = v.y; sZ[kq + 2][r] = v.z; sZ[kq + 3][r] = v.w;
         float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c0 + r < ncodes) e = *reinterpret_cast<const float4*>(cb + static_cast<size_t>(c0 + r) * D + k0 + kq);
+        if (c0 + r < ncodes && kin) e = *reinterpret_cast<const float4*>(cb + static_cast<size_t>(c0 + r) * D + k0 + kq);
         sE[kq + 0][r] = e.x; sE[kq + 1][r] = e.y; sE[kq + 2][r] = e.z; sE[kq + 3][r] = e.w;
       }
       __syncthreads();
@@ -190,7 +193,7 @@ int muse_vq_argmin(const float* z, const float* codebook, float* enorm_ws, long 
                    int D, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
-  if (D % TKK != 0) { set_last_error("vq_argmin: D=%d must be a multiple of %d", D, TKK); return MUSE_ERR_UNSUPPORTED; }
+  if (D % 4 != 0 || D <= 0) { set_last_error("vq_argmin: D=%d must be a positive multiple of 4", D); return MUSE_ERR_UNSUPPORTED; }
   pdl_launch(ceil_div(ncodes, 256), 256, 0, s)(sqnorm_kernel, codebook, enorm_ws, ncodes, D);
   int rc = check_launch("vq_sqnorm");
   if (rc) return rc;
@@ -202,7 +205,7 @@ int muse_vq_soft_code(const float* z, const float* codebook, float* enorm_ws, fl
                       float temp, int n, int ncodes, int D, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return MUSE_OK;
-  if (D % TKK != 0) { set_last_error("vq_soft_code: D=%d must be a multiple of %d", D, TKK); return MUSE_ERR_UNSUPPORTED; }
+  if (D % 4 != 0 || D <= 0) { set_last_error("vq_soft_code: D=%d must be a positive multiple of 4", D); return MUSE_ERR_UNSUPPORTED; }
   if (!(temp > 0.f)) { set_last_error("vq_soft_code: temp must be > 0"); return MUSE_ERR_INVALID; }
   pdl_launch(ceil_div(ncodes, 256), 256, 0, s)(sqnorm_kernel, codebook, enorm_ws, ncodes, D);
   int rc = check_launch("vq_sqnorm");

@@ -971,3 +971,180 @@ def image_to_uint8(x):
     y = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
     _call("muse_image_to_uint8", _p(x), _p(y), x.numel(), st)
     return y
+
+
+# ------------------------------------------------------------------------------------------ Paella tokenizer (fp32 NHWC)
+# muse/modeling_paella_vq.py.  Each op takes the nn weights (already gamma / BatchNorm-folded where the model folds them)
+# and picks the tensor-core route when the geometry has a TMA tiling, else the fp32 SIMT kernels of conv.cu.
+_KERNELS_PER_CALL["muse_paella_resblock_spatial"] = 2
+
+
+def _cached_pack(tag, w, pack):
+    """pack(w) cached per live tensor w under `tag` (same keying as _packed_conv_weight)."""
+    import weakref
+
+    key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
+    hit = _wk_cache.get((tag, id(w)))
+    if hit is not None and hit[0]() is w and hit[1] == key:
+        return hit[2]
+    out = pack(w.detach().float())
+    if len(_wk_cache) > 4096:
+        _wk_cache.clear()
+    _wk_cache[(tag, id(w))] = (weakref.ref(w), key, out)
+    return out
+
+
+def _planes(wk):
+    hi = wk.to(torch.bfloat16)
+    return hi, (wk - hi.float()).to(torch.bfloat16)
+
+
+def _tc_route(H, W, Cin, Cout, k):
+    return _conv_state["route"] != "simt" and bool(_lib.load().muse_conv2d_tc_supported(H, W, Cin, Cout, k))
+
+
+def _split(x, st):
+    hi = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    lo = _lo_like(hi)
+    B, H, W, C = x.shape
+    _call("muse_split_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, C, 0, st)
+    return hi, lo
+
+
+def paella_resblock(x, wk, bias, w1, b1, w2, b2, eps=1e-6):
+    """Paella ResBlock (modeling_paella_vq.py:112-145) on fp32 NHWC x [B,H,W,C] with its gammas folded into the weights:
+    wk fp32 [9, C] and bias [C] of the depthwise 3x3 (tap-major), w1 [4C, C, 1, 1] / b1 and w2 [C, 4C, 1, 1] / b2 of the
+    two Linears.  Four launches: LN1 statistics, the spatial pass (x1 = x + dw(LN1 x), LN2(x1)), Linear + GELU, Linear
+    + residual x1."""
+    st = _prep(x)
+    B, H, W, C = x.shape
+    Ch = w1.shape[0]
+    x1 = torch.empty_like(x)
+    stats = torch.empty(2 * B * H * W, dtype=torch.float32, device=x.device)
+    y = torch.empty_like(x)
+    if _tc_route(H, W, C, Ch, 1) and _tc_route(H, W, Ch, C, 1):
+        n_hi = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+        n_lo = _lo_like(n_hi)
+        _call("muse_paella_resblock_spatial", _p(x), _p(wk), _p(bias), _p(stats), _p(x1), None, _p(n_hi), _p(n_lo), B, H, W,
+              C, float(eps), st)
+        g_hi = torch.empty(B, H, W, Ch, dtype=torch.bfloat16, device=x.device)
+        g_lo = _lo_like(g_hi)
+        w1h, w1l = _packed_conv_weight_split(w1)
+        _call("muse_conv2d_nhwc_tc_gelu_split", _p(n_hi), _p(n_lo), _p(w1h), _p(w1l), _p(b1), _p(g_hi), _p(g_lo), B, H, W, C,
+              Ch, 1, _tc_mode(0), st)
+        w2h, w2l = _packed_conv_weight_split(w2)
+        _call("muse_conv2d_nhwc_tc", _p(g_hi), _p(g_lo), _p(w2h), _p(w2l), _p(b2), _p(x1), _p(y), None, B, H, W, Ch, C, 1,
+              _tc_mode(0), st)
+        return y
+    n2 = torch.empty_like(x)
+    _call("muse_paella_resblock_spatial", _p(x), _p(wk), _p(bias), _p(stats), _p(x1), _p(n2), None, None, B, H, W, C,
+          float(eps), st)
+    g = torch.empty(B, H, W, Ch, dtype=torch.float32, device=x.device)
+    _call("muse_conv2d_nhwc", _p(n2), _p(_packed_conv_weight(w1)), _p(b1), None, _p(g), B, H, W, C, Ch, 1, 8, st)
+    _call("muse_conv2d_nhwc", _p(g), _p(_packed_conv_weight(w2)), _p(b2), _p(x1), _p(y), B, H, W, Ch, C, 1, 0, st)
+    return y
+
+
+def conv2d_unshuffle(x, w, bias=None):
+    """nn.PixelUnshuffle(2) then the 1x1 conv w [Cout, 4*Cin, 1, 1] (Paella in_block): fp32 NHWC [B,2H,2W,Cin] ->
+    [B,H,W,Cout].  Tensor cores: an im2col of the 2x2 blocks into 64 columns, then one 1x1 convolution; SIMT: the same
+    weights as a 2x2 stride-2 convolution."""
+    st = _prep(x)
+    B, Hi, Wi, Cin = x.shape
+    H, W, Cout = Hi // 2, Wi // 2, w.shape[0]
+    y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
+    b = None if bias is None else bias.detach().float()
+    if 4 * Cin <= 64 and _tc_route(H, W, 64, Cout, 1):
+        hi = torch.empty(B, H, W, 64, dtype=torch.bfloat16, device=x.device)
+        lo = _lo_like(hi)
+        _call("muse_im2col_split_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, 2, st)
+        w_hi, w_lo = _packed_conv_weight_split_stem(w)
+        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, 64, Cout, 1,
+              _tc_mode(0), st)
+        return y
+    wk = _cached_pack("unshuffle", w, lambda wf: wf.view(Cout, Cin, 2, 2).permute(2, 3, 1, 0).reshape(-1, Cout).contiguous())
+    _call("muse_conv2d_nhwc", _p(x), _p(wk), _p(b), None, _p(y), B, H, W, Cin, Cout, 2, 2, st)
+    return y
+
+
+def _pack_s2p1(wf):
+    """Conv2d(4, 2, 1) weight [Cout, Cin, 4, 4] -> [Cout, 9 taps * 4 * Cin] for a 3x3 pad-1 convolution over the
+    space-to-depth grid: tap (a, b) and plane (p, q) hold w[:, :, 2a + p - 1, 2b + q - 1] (zero outside 0..3)."""
+    Cout, Cin = wf.shape[0], wf.shape[1]
+    wk = torch.zeros(Cout, 3, 3, 2, 2, Cin, dtype=torch.float32, device=wf.device)  # [co, a, b, p, q, ci]
+    for a in range(3):
+        for b in range(3):
+            for p_ in (0, 1):
+                for q in (0, 1):
+                    kh, kw = 2 * a + p_ - 1, 2 * b + q - 1
+                    if 0 <= kh <= 3 and 0 <= kw <= 3:
+                        wk[:, a, b, p_, q] = wf[:, :, kh, kw]
+    return _planes(wk.reshape(Cout, -1).contiguous())
+
+
+def conv2d_s2p1(x, w, bias=None):
+    """nn.Conv2d(k=4, s=2, p=1) on fp32 NHWC [B,2H,2W,Cin] -> [B,H,W,Cout].  Tensor cores: space-to-depth + hi/lo split,
+    then a stride-1 3x3 convolution over the 4*Cin planes (16 of the 36 weight taps are non-zero); SIMT: stride-2 mode."""
+    st = _prep(x)
+    B, Hi, Wi, Cin = x.shape
+    H, W, Cout = Hi // 2, Wi // 2, w.shape[0]
+    y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
+    b = None if bias is None else bias.detach().float()
+    if (4 * Cin) % 64 == 0 and _tc_route(H, W, 4 * Cin, Cout, 3):
+        hi = torch.empty(B, H, W, 4 * Cin, dtype=torch.bfloat16, device=x.device)
+        lo = _lo_like(hi)
+        _call("muse_split_s2d_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, st)
+        w_hi, w_lo = _cached_pack("s2p1", w, _pack_s2p1)
+        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, 4 * Cin, Cout, 3,
+              _tc_mode(0), st)
+        return y
+    _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), None, _p(y), B, H, W, Cin, Cout, 4, 3, st)
+    return y
+
+
+def _pack_transpose_parities(wf):
+    """ConvTranspose2d(4, 2, 1) weight [Cin, Cout, 4, 4] -> [4 parities][Cout][4 taps * Cin]: output pixel (2i + py, 2j + px)
+    reads input (i + a + py - 1, j + b + px - 1) with kernel tap (3 - 2a - py, 3 - 2b - px), a, b in {0, 1}."""
+    mats = []
+    for py in (0, 1):
+        for px in (0, 1):
+            taps = [wf[:, :, 3 - 2 * a - py, 3 - 2 * b - px].t() for a in (0, 1) for b in (0, 1)]  # [Cout, Cin] each
+            mats.append(torch.stack(taps, dim=1).reshape(wf.shape[1], -1))  # [Cout, 4*Cin], column (a*2+b)*Cin + ci
+    return torch.stack(mats)
+
+
+def conv_transpose2d_s2(x, w, bias=None):
+    """nn.ConvTranspose2d(k=4, s=2, p=1) on fp32 NHWC [B,H,W,Cin] with w [Cin, Cout, 4, 4] -> [B,2H,2W,Cout]: four 2x2
+    parity convolutions of the input (the upsample mode of muse_conv2d_nhwc_tc, or mode 4 of the SIMT kernel)."""
+    st = _prep(x)
+    B, Hi, Wi, Cin = x.shape
+    H, W, Cout = 2 * Hi, 2 * Wi, w.shape[1]
+    y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
+    b = None if bias is None else bias.detach().float()
+    if _conv_state["route"] != "simt" and _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, 3, 1) > 0:
+        hi, lo = _split(x, st)
+        w_hi, w_lo = _cached_pack("convT", w, lambda wf: _planes(_pack_transpose_parities(wf).reshape(4 * Cout, -1).contiguous()))
+        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, Cin, Cout, 3,
+              _tc_mode(1), st)
+        return y
+    wk = _cached_pack("convT_simt", w, lambda wf: _pack_transpose_parities(wf).transpose(1, 2).contiguous())
+    _call("muse_conv2d_nhwc", _p(x), _p(wk), _p(b), None, _p(y), B, H, W, Cin, Cout, 4, 4, st)
+    return y
+
+
+def conv1x1_pixel_shuffle(x, w, bias=None):
+    """1x1 conv w [Cout, Cin, 1, 1] then nn.PixelShuffle(2) (Paella out_block), folded into the convolution's store:
+    fp32 NHWC [B,H,W,Cin] -> [B,2H,2W,Cout/4]."""
+    st = _prep(x)
+    B, H, W, Cin = x.shape
+    Cout = w.shape[0]
+    y = torch.empty(B, 2 * H, 2 * W, Cout // 4, dtype=torch.float32, device=x.device)
+    b = None if bias is None else bias.detach().float()
+    if _tc_route(H, W, Cin, Cout, 1):
+        hi, lo = _split(x, st)
+        w_hi, w_lo = _packed_conv_weight_split(w)
+        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, Cin, Cout, 1,
+              _tc_mode(16), st)
+        return y
+    _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), None, _p(y), B, H, W, Cin, Cout, 1, 16, st)
+    return y
