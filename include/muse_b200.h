@@ -27,7 +27,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 9
+#define MUSE_B200_ABI_VERSION 10
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -309,6 +309,16 @@ int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* be
                              float* partials_ws, float* scale_shift_ws, int B, int HW, int C, int groups, float eps,
                              int precomputed_tiles, int apply_silu, void* stream);  /* apply_silu 0: plain GroupNorm
                              (AttnBlock.norm of the taming VQGAN, modeling_taming_vqgan.py:137-150) */
+/* MoVQ SpatialNorm (muse/modeling_movq.py:21-49) + optional F.silu: the GroupNorm above (same statistics, workspaces,
+ * precomputed_tiles and output forms) with its output modulated per pixel by the quantised latent zq before the SiLU:
+ *   out[b,y,x,c] = GN(x)[b,y,x,c] * Ym + Bm,  Ym = by[c] + sum_d wy[c][d] zq[b, y / ry, x / rx, d]  (Bm from wb / bb),
+ * i.e. GN(f) * conv_y(up(zq)) + conv_b(up(zq)) with `up` the nearest resize to H x W.  x [B,H,W,C], zq [B,hz,wz,dq] fp32
+ * NHWC; wy / wb the 1x1 conv weights [C][dq], by / bb [C].  ry = H / hz and rx = W / wz must be integers and dq a
+ * multiple of 4 up to 16 (else MUSE_ERR_UNSUPPORTED); zq, wy, wb 16-byte aligned.  Checked before any launch. */
+int muse_spatial_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* beta, const float* zq, const float* wy,
+                                     const float* by, const float* wb, const float* bb, float* y, void* y_hi, void* y_lo,
+                                     float* partials_ws, float* scale_shift_ws, int B, int H, int W, int C, int groups,
+                                     float eps, int hz, int wz, int dq, int precomputed_tiles, int apply_silu, void* stream);
 /* Conv2dSame (:33-45) on the Hopper (wgmma) tensor cores with fp32-level accuracy (3 bf16 products hi*hi + lo*hi + hi*lo,
  * fp32 accumulation): x_hi/x_lo bf16 [B,H,W,Cin], w_hi/w_lo bf16 [Cout, ksize*ksize*Cin] (tap-major, then input
  * channel), optional bias [Cout] and residual [B,H,W,Cout] -> y fp32 [B,H,W,Cout].

@@ -8,6 +8,7 @@ __version__ = "0.1.0"
 
 from .modeling_ema import EMAModel  # noqa: F401
 from .modeling_maskgit_vqgan import MaskGitVQGAN  # noqa: F401
+from .modeling_movq import MOVQ  # noqa: F401
 from .modeling_paella_vq import PaellaVQModel  # noqa: F401
 from .modeling_taming_vqgan import VQGANModel  # noqa: F401
 from .modeling_transformer import MaskGitTransformer  # noqa: F401

@@ -66,6 +66,7 @@ SIGNATURES = {
     "muse_conv2d_nhwc": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "muse_groupnorm_workspace_floats": (c_longlong, [_I, _I, _I]),
     "muse_groupnorm_silu_nhwc": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _I, _P]),
+    "muse_spatial_groupnorm_silu_nhwc": (c_int, [_P] * 13 + [_I, _I, _I, _I, _I, _F, _I, _I, _I, _I, _I, _P]),
     "muse_split_s2d_bf16_nhwc": (c_int, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "muse_softmax_split_rows": (c_int, [_P, _P, _P, _P, _L, _I, _F, _P]),
     "muse_conv2d_tc_tiles_per_image": (c_int, [_I, _I, _I, _I, _I, _I]),
@@ -80,7 +81,7 @@ SIGNATURES = {
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 
 class MuseB200Error(RuntimeError):

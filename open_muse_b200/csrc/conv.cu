@@ -268,12 +268,47 @@ gn_finalize_kernel(const float* __restrict__ partials, int nblocks, int rows_per
   }
 }
 
+// Spatial modulation of the apply pass (MoVQ SpatialNorm, muse/modeling_movq.py:21-49): out = GN(x) * Ym + Bm with
+// Ym[c] = by[c] + sum_d wy[c][d] zq[b, y / ry, x / rx, d] and Bm likewise from wb / bb, the 1x1 conv_y / conv_b of the
+// nearest-upsampled latent computed per pixel from its latent pixel (never written out: at C = 512 Ym and Bm would be
+// twice the bytes of x).  Integer ratios ry = H / Hz, rx = W / Wz; dq % 4 == 0, dq <= 16.
+struct GnMod {
+  const float* zq;                  // [B, Hz, Wz, dq] NHWC latent
+  const float* wy; const float* wb;  // [C][dq]
+  const float* by; const float* bb;  // [C]
+  int W, Hz, Wz, ry, rx, dq;
+};
+
+// o[j] = fma(o[j], Ym[c0 + j], Bm[c0 + j]) for pixel p (flat over the batch), channels c0 .. c0 + N - 1
+template <int N>
+__device__ __forceinline__ void gn_modulate(const GnMod& m, long long p, int HW, int c0, float (&o)[N]) {
+  const int b = static_cast<int>(p / HW), r = static_cast<int>(p - static_cast<long long>(b) * HW);
+  const int zy = (r / m.W) / m.ry, zx = (r % m.W) / m.rx;
+  const float* z = m.zq + ((static_cast<long long>(b) * m.Hz + zy) * m.Wz + zx) * m.dq;
+  float ym[N], bm[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) { ym[j] = m.by[c0 + j]; bm[j] = m.bb[c0 + j]; }
+  for (int k = 0; k < m.dq; k += 4) {
+    const float4 z4 = *reinterpret_cast<const float4*>(z + k);
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+      const float4 a = *reinterpret_cast<const float4*>(m.wy + (c0 + j) * m.dq + k);
+      const float4 e = *reinterpret_cast<const float4*>(m.wb + (c0 + j) * m.dq + k);
+      ym[j] = fmaf(a.w, z4.w, fmaf(a.z, z4.z, fmaf(a.y, z4.y, fmaf(a.x, z4.x, ym[j]))));
+      bm[j] = fmaf(e.w, z4.w, fmaf(e.z, z4.z, fmaf(e.y, z4.y, fmaf(e.x, z4.x, bm[j]))));
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) o[j] = fmaf(o[j], ym[j], bm[j]);
+}
+
 // SPLIT: instead of fp32 y, emit the bf16 hi/lo planes (y = hi + lo) the tensor-core convolution consumes (conv_tc.cu)
-template <bool SPLIT>
+// MOD: the SpatialNorm modulation above, before the SiLU
+template <bool SPLIT, bool MOD>
 __global__ void __launch_bounds__(256)
 gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scale_shift, const float* __restrict__ shift_lo,
                      float* __restrict__ y, bf16* __restrict__ y_hi, bf16* __restrict__ y_lo, long long total4, int HW, int C,
-                     int silu) {
+                     int silu, GnMod mod) {
   pdl_enter();
   const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= total4) return;
@@ -286,6 +321,7 @@ gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scal
   const float4 l = *reinterpret_cast<const float4*>(shift_lo + static_cast<long long>(b) * C + q * 4);
   float o[4] = {fmaf(v.x, s0.x, s0.y) + l.x, fmaf(v.y, s0.z, s0.w) + l.y, fmaf(v.z, s1.x, s1.y) + l.z,
                 fmaf(v.w, s1.z, s1.w) + l.w};
+  if (MOD) gn_modulate<4>(mod, i / c4, HW, q * 4, o);
 #pragma unroll
   for (int j = 0; j < 4; ++j) o[j] = silu ? o[j] / (1.f + expf(-o[j])) : o[j];
   if (SPLIT) {
@@ -303,10 +339,11 @@ gn_apply_silu_kernel(const float* __restrict__ x, const float* __restrict__ scal
 }
 
 // 8 channels per thread variant of the SPLIT apply (two 16-byte loads in flight, 16-byte stores per plane)
+template <bool MOD>
 __global__ void __launch_bounds__(256)
 gn_apply_silu_split8_kernel(const float* __restrict__ x, const float* __restrict__ scale_shift,
                             const float* __restrict__ shift_lo, bf16* __restrict__ y_hi, bf16* __restrict__ y_lo,
-                            long long total8, int HW, int C, int silu) {
+                            long long total8, int HW, int C, int silu, GnMod mod) {
   pdl_enter();
   const long long i = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= total8) return;
@@ -318,16 +355,33 @@ gn_apply_silu_split8_kernel(const float* __restrict__ x, const float* __restrict
   load8(shift_lo + static_cast<long long>(b) * C + q * 8, sl);
   const float4* ssp = reinterpret_cast<const float4*>(scale_shift + (static_cast<long long>(b) * C + q * 8) * 2);
   float h[8], l[8];
+  if (MOD) {
+    float o[8];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float4 s2 = ssp[j];  // {scale, shift} of channels 2j, 2j+1
-    float o0 = fmaf(v[2 * j], s2.x, s2.y) + sl[2 * j], o1 = fmaf(v[2 * j + 1], s2.z, s2.w) + sl[2 * j + 1];
-    if (silu) {
-      o0 = o0 / (1.f + expf(-o0));
-      o1 = o1 / (1.f + expf(-o1));
+    for (int j = 0; j < 4; ++j) {
+      const float4 s2 = ssp[j];
+      o[2 * j] = fmaf(v[2 * j], s2.x, s2.y) + sl[2 * j];
+      o[2 * j + 1] = fmaf(v[2 * j + 1], s2.z, s2.w) + sl[2 * j + 1];
     }
-    h[2 * j] = bf16_round(o0); h[2 * j + 1] = bf16_round(o1);
-    l[2 * j] = o0 - h[2 * j]; l[2 * j + 1] = o1 - h[2 * j + 1];
+    gn_modulate<8>(mod, i / c8, HW, q * 8, o);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float t = silu ? o[j] / (1.f + expf(-o[j])) : o[j];
+      h[j] = bf16_round(t);
+      l[j] = t - h[j];
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float4 s2 = ssp[j];  // {scale, shift} of channels 2j, 2j+1
+      float o0 = fmaf(v[2 * j], s2.x, s2.y) + sl[2 * j], o1 = fmaf(v[2 * j + 1], s2.z, s2.w) + sl[2 * j + 1];
+      if (silu) {
+        o0 = o0 / (1.f + expf(-o0));
+        o1 = o1 / (1.f + expf(-o1));
+      }
+      h[2 * j] = bf16_round(o0); h[2 * j + 1] = bf16_round(o1);
+      l[2 * j] = o0 - h[2 * j]; l[2 * j + 1] = o1 - h[2 * j + 1];
+    }
   }
   store8(y_hi + i * 8, h);
   if (y_lo) store8(y_lo + i * 8, l);  // single-pass bf16 tokenizer mode needs the hi plane only
@@ -405,6 +459,65 @@ image_to_uint8_kernel(const float* __restrict__ x, unsigned char* __restrict__ y
 // workspace: partials float [nblocks*B*C*2] with nblocks = ceil(HW / rows_per_block) (see muse_groupnorm_workspace_floats)
 static int gn_rows_per_block(int C) { return (256 / (C / 4)) * 64; }
 
+// argument checks shared by both GroupNorm entry points; run before any launch
+static int gn_check(const char* what, const float* y, const void* y_hi, const void* y_lo, int C, int groups) {
+  if ((y != nullptr) == (y_hi != nullptr) || (y_hi == nullptr && y_lo != nullptr)) {
+    set_last_error("%s: give either y (fp32) or y_hi (+ y_lo unless the single-pass bf16 mode is used)", what);
+    return MUSE_ERR_INVALID;
+  }
+  if (C % groups != 0 || C % 4 != 0 || C > 1024 || 256 % (C / 4) != 0) {
+    set_last_error("%s: C=%d groups=%d unsupported (C must divide into groups, C/4 must divide 256)", what, C, groups);
+    return MUSE_ERR_UNSUPPORTED;
+  }
+  return MUSE_OK;
+}
+
+// statistics pass (or the conv epilogue's tiles) + fp64 finalize: per-(image, channel) {scale, shift_hi} in
+// scale_shift_ws, shift_lo after them
+static int gn_scale_shift(const float* x, const float* gamma, const float* beta, float* partials_ws, float* scale_shift_ws, int B,
+                   int HW, int C, int groups, float eps, int precomputed_tiles, cudaStream_t s) {
+  // precomputed_tiles > 0: partials_ws already holds {sum, M2} per [image][tile][C] (HW / tiles pixels each), written by the
+  // epilogue of the tensor-core convolution that produced x (conv_tc.cu), and the statistics pass over x is skipped.
+  int nblocks = precomputed_tiles;
+  int rows_per_block = precomputed_tiles > 0 ? HW / precomputed_tiles : gn_rows_per_block(C);
+  int rc;
+  if (precomputed_tiles > 0 && HW % precomputed_tiles != 0) {
+    set_last_error("groupnorm: %d precomputed tiles do not split HW=%d evenly", precomputed_tiles, HW);
+    return MUSE_ERR_INVALID;
+  }
+  if (precomputed_tiles <= 0) {
+    nblocks = ceil_div(HW, rows_per_block);
+    const int rstep = 256 / (C / 4);
+    pdl_launch(dim3(nblocks, B), 256, rstep * C * 2 * sizeof(float), s)(gn_stats_kernel, x, partials_ws, HW, C, rows_per_block);
+    rc = check_launch("gn_stats");
+    if (rc) return rc;
+  }
+  float* shift_lo = scale_shift_ws + 2LL * B * C;
+  pdl_launch(ceil_div(B * groups, 8), 256, 0, s)(gn_finalize_kernel, partials_ws, nblocks, rows_per_block,
+                                                             precomputed_tiles > 0 ? nullptr : x, gamma, beta,
+                                                             scale_shift_ws, shift_lo, B, HW, C, groups, eps);
+  return check_launch("gn_finalize");
+}
+
+template <bool MOD>
+static int gn_apply(const float* x, const float* scale_shift_ws, float* y, void* y_hi, void* y_lo, int B, int HW, int C,
+             int apply_silu, const GnMod& mod, cudaStream_t s) {
+  const float* shift_lo = scale_shift_ws + 2LL * B * C;
+  const long long total4 = static_cast<long long>(B) * HW * (C / 4);
+  const unsigned blocks = static_cast<unsigned>(ceil_div_ll(total4, 256));
+  if (y != nullptr)
+    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<false, MOD>, x, scale_shift_ws, shift_lo, y, nullptr, nullptr, total4, HW,
+                                  C, apply_silu, mod);
+  else if (C % 8 == 0)
+    pdl_launch(static_cast<unsigned>(ceil_div_ll(total4 / 2, 256)), 256, 0, s)(gn_apply_silu_split8_kernel<MOD>,
+        x, scale_shift_ws, shift_lo, reinterpret_cast<bf16*>(y_hi), reinterpret_cast<bf16*>(y_lo), total4 / 2, HW, C, apply_silu,
+        mod);
+  else
+    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<true, MOD>, x, scale_shift_ws, shift_lo, nullptr, reinterpret_cast<bf16*>(y_hi),
+                                  reinterpret_cast<bf16*>(y_lo), total4, HW, C, apply_silu, mod);
+  return check_launch(MOD ? "spatial_gn_apply_silu" : "gn_apply_silu");
+}
+
 }  // namespace muse
 
 using namespace muse;
@@ -450,48 +563,40 @@ int muse_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* be
                              float* partials_ws, float* scale_shift_ws, int B, int HW, int C, int groups, float eps,
                              int precomputed_tiles, int apply_silu, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if ((y != nullptr) == (y_hi != nullptr) || (y_hi == nullptr && y_lo != nullptr)) {
-    set_last_error("groupnorm: give either y (fp32) or y_hi (+ y_lo unless the single-pass bf16 mode is used)");
-    return MUSE_ERR_INVALID;
-  }
-  if (C % groups != 0 || C % 4 != 0 || C > 1024 || 256 % (C / 4) != 0) {
-    set_last_error("groupnorm: C=%d groups=%d unsupported (C must divide into groups, C/4 must divide 256)", C, groups);
+  int rc = gn_check("groupnorm", y, y_hi, y_lo, C, groups);
+  if (rc) return rc;
+  if (B <= 0 || HW <= 0) return MUSE_OK;
+  rc = gn_scale_shift(x, gamma, beta, partials_ws, scale_shift_ws, B, HW, C, groups, eps, precomputed_tiles, s);
+  if (rc) return rc;
+  return gn_apply<false>(x, scale_shift_ws, y, y_hi, y_lo, B, HW, C, apply_silu, GnMod{}, s);
+}
+
+int muse_spatial_groupnorm_silu_nhwc(const float* x, const float* gamma, const float* beta, const float* zq, const float* wy,
+                                     const float* by, const float* wb, const float* bb, float* y, void* y_hi, void* y_lo,
+                                     float* partials_ws, float* scale_shift_ws, int B, int H, int W, int C, int groups,
+                                     float eps, int hz, int wz, int dq, int precomputed_tiles, int apply_silu, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc = gn_check("spatial groupnorm", y, y_hi, y_lo, C, groups);
+  if (rc) return rc;
+  if (dq <= 0 || dq % 4 != 0 || dq > 16) {
+    set_last_error("spatial groupnorm: latent channels %d unsupported (a multiple of 4, at most 16)", dq);
     return MUSE_ERR_UNSUPPORTED;
   }
-  if (B <= 0 || HW <= 0) return MUSE_OK;
-  // precomputed_tiles > 0: partials_ws already holds {sum, M2} per [image][tile][C] (HW / tiles pixels each), written by the
-  // epilogue of the tensor-core convolution that produced x (conv_tc.cu), and the statistics pass over x is skipped.
-  int nblocks = precomputed_tiles;
-  int rows_per_block = precomputed_tiles > 0 ? HW / precomputed_tiles : gn_rows_per_block(C);
-  int rc;
-  if (precomputed_tiles > 0 && HW % precomputed_tiles != 0) {
-    set_last_error("groupnorm: %d precomputed tiles do not split HW=%d evenly", precomputed_tiles, HW);
+  if (hz <= 0 || wz <= 0 || H <= 0 || W <= 0 || H % hz != 0 || W % wz != 0) {
+    set_last_error("spatial groupnorm: %dx%d is not an integer multiple of the %dx%d latent grid", H, W, hz, wz);
+    return MUSE_ERR_UNSUPPORTED;
+  }
+  if (!zq || !wy || !by || !wb || !bb ||
+      ((reinterpret_cast<uintptr_t>(zq) | reinterpret_cast<uintptr_t>(wy) | reinterpret_cast<uintptr_t>(wb)) & 15)) {
+    set_last_error("spatial groupnorm: zq, wy, wb, by, bb are required; zq, wy and wb 16-byte aligned");
     return MUSE_ERR_INVALID;
   }
-  if (precomputed_tiles <= 0) {
-    nblocks = ceil_div(HW, rows_per_block);
-    const int rstep = 256 / (C / 4);
-    pdl_launch(dim3(nblocks, B), 256, rstep * C * 2 * sizeof(float), s)(gn_stats_kernel, x, partials_ws, HW, C, rows_per_block);
-    rc = check_launch("gn_stats");
-    if (rc) return rc;
-  }
-  float* shift_lo = scale_shift_ws + 2LL * B * C;
-  pdl_launch(ceil_div(B * groups, 8), 256, 0, s)(gn_finalize_kernel, partials_ws, nblocks, rows_per_block,
-                                                             precomputed_tiles > 0 ? nullptr : x, gamma, beta,
-                                                             scale_shift_ws, shift_lo, B, HW, C, groups, eps);
-  rc = check_launch("gn_finalize");
+  if (B <= 0) return MUSE_OK;
+  const int HW = H * W;
+  rc = gn_scale_shift(x, gamma, beta, partials_ws, scale_shift_ws, B, HW, C, groups, eps, precomputed_tiles, s);
   if (rc) return rc;
-  const long long total4 = static_cast<long long>(B) * HW * (C / 4);
-  const unsigned blocks = static_cast<unsigned>(ceil_div_ll(total4, 256));
-  if (y != nullptr)
-    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<false>, x, scale_shift_ws, shift_lo, y, nullptr, nullptr, total4, HW, C, apply_silu);
-  else if (C % 8 == 0)
-    pdl_launch(static_cast<unsigned>(ceil_div_ll(total4 / 2, 256)), 256, 0, s)(gn_apply_silu_split8_kernel,
-        x, scale_shift_ws, shift_lo, reinterpret_cast<bf16*>(y_hi), reinterpret_cast<bf16*>(y_lo), total4 / 2, HW, C, apply_silu);
-  else
-    pdl_launch(blocks, 256, 0, s)(gn_apply_silu_kernel<true>, x, scale_shift_ws, shift_lo, nullptr, reinterpret_cast<bf16*>(y_hi),
-                                                      reinterpret_cast<bf16*>(y_lo), total4, HW, C, apply_silu);
-  return check_launch("gn_apply_silu");
+  const GnMod mod{zq, wy, wb, by, bb, W, hz, wz, H / hz, W / wz, dq};
+  return gn_apply<true>(x, scale_shift_ws, y, y_hi, y_lo, B, HW, C, apply_silu, mod, s);
 }
 
 int muse_image_to_uint8(const float* x, unsigned char* y, long long n, void* stream) {

@@ -13,6 +13,9 @@ layers with fp32-faithful tensor-core convolutions (csrc/conv_tc.cu):
   * AttnBlock (:137-174): GroupNorm -> q, k, v 1x1 convs -> one 512-wide head over the 16x16 tokens; both attention
     products are 1x1 convolutions with per-image weights (keys / values), softmax in fp32 -> proj_out (+ residual).
   * quantiser: the bit-exact arg-min / lookup kernels of MaskGitVQGAN.
+
+The blocks also build the MoVQ tokenizer (modeling_movq.py): ``norm`` makes its decoder norms SpatialNorms, modulated by
+the latent ``zq`` that ``run`` then passes down, and ``linear`` gives the AttnBlocks nn.Linear projections.
 """
 from __future__ import annotations
 
@@ -31,6 +34,30 @@ _GN = dict(num_groups=32, eps=1e-6, affine=True)
 
 def _gn(norm, silu=1):
     return (norm.weight, norm.bias, 32, 1e-6, silu)
+
+
+def _group_norm(channels):
+    return nn.GroupNorm(num_channels=channels, **_GN)
+
+
+def _norm(norm, zq, silu=1):
+    """ops.conv2d / ops.groupnorm_silu arguments of a block norm: an nn.GroupNorm, or with the latent zq (fp32 NHWC) a MoVQ
+    SpatialNorm, whose GroupNorm output is modulated by its 1x1 conv_y / conv_b of zq."""
+    if zq is None:
+        return dict(gn=_gn(norm, silu))
+    return dict(gn=_gn(norm.norm_layer, silu), spatial=(zq, norm.conv_y, norm.conv_b))
+
+
+def _conv1x1(w):
+    """the [C, C, 1, 1] weight ops.conv2d takes, for an nn.Conv2d or an nn.Linear [C, C] weight; the Linear's view is kept on
+    the parameter so that the packed-weight caches, keyed per tensor, keep hitting"""
+    if w.dim() == 4:
+        return w
+    v = getattr(w, "_conv_view", None)
+    if v is None or v.data_ptr() != w.data_ptr() or v.device != w.device:
+        v = w.detach().view(*w.shape, 1, 1)
+        w._conv_view = v
+    return v
 
 
 class Upsample(nn.Module):
@@ -60,14 +87,14 @@ class Downsample(nn.Module):
 
 
 class ResnetBlock(nn.Module):
-    def __init__(self, in_channels, out_channels=None, use_conv_shortcut=False, dropout_prob=0.0):
+    def __init__(self, in_channels, out_channels=None, use_conv_shortcut=False, dropout_prob=0.0, norm=_group_norm):
         super().__init__()
         self.in_channels = in_channels
         self.out_channels_ = in_channels if out_channels is None else out_channels
         self.use_conv_shortcut = use_conv_shortcut
-        self.norm1 = nn.GroupNorm(num_channels=in_channels, **_GN)
+        self.norm1 = norm(in_channels)
         self.conv1 = nn.Conv2d(in_channels, self.out_channels_, kernel_size=3, stride=1, padding=1)
-        self.norm2 = nn.GroupNorm(num_channels=self.out_channels_, **_GN)
+        self.norm2 = norm(self.out_channels_)
         self.dropout = nn.Dropout(dropout_prob)
         self.conv2 = nn.Conv2d(self.out_channels_, self.out_channels_, kernel_size=3, stride=(1, 1), padding=1)
         if self.in_channels != self.out_channels_:
@@ -76,36 +103,40 @@ class ResnetBlock(nn.Module):
             else:
                 self.nin_shortcut = nn.Conv2d(in_channels, self.out_channels_, kernel_size=1, stride=1, padding=0)
 
-    def run(self, x):
-        h = ops.conv2d(x, self.conv1.weight, bias=self.conv1.bias, gn=_gn(self.norm1))
+    def run(self, x, zq=None):
+        h = ops.conv2d(x, self.conv1.weight, bias=self.conv1.bias, **_norm(self.norm1, zq))
         res = x
         if self.in_channels != self.out_channels_:
             sc = self.conv_shortcut if self.use_conv_shortcut else self.nin_shortcut
             res = ops.conv2d(x, sc.weight, bias=sc.bias)
-        return ops.conv2d(h, self.conv2.weight, bias=self.conv2.bias, residual=res, gn=_gn(self.norm2))
+        return ops.conv2d(h, self.conv2.weight, bias=self.conv2.bias, residual=res, **_norm(self.norm2, zq))
 
 
 class AttnBlock(nn.Module):
-    def __init__(self, in_channels):
+    def __init__(self, in_channels, norm=_group_norm, linear=False):
         super().__init__()
         self.in_channels = in_channels
-        conv = partial(nn.Conv2d, in_channels, in_channels, kernel_size=1, stride=1, padding=0)
-        self.norm = nn.GroupNorm(num_channels=in_channels, **_GN)
+        if linear:  # MoVQ: nn.Linear(C, C) projections over the tokens, the same products as 1x1 convolutions
+            conv = partial(nn.Linear, in_channels, in_channels)
+        else:
+            conv = partial(nn.Conv2d, in_channels, in_channels, kernel_size=1, stride=1, padding=0)
+        self.norm = norm(in_channels)
         self.q, self.k, self.v = conv(), conv(), conv()
         self.proj_out = conv()
 
-    def run(self, x):
+    def run(self, x, zq=None):
         B, hh, ww, C = x.shape
-        n = ops.groupnorm_silu(x, self.norm.weight, self.norm.bias, 32, 1e-6, silu=0)
-        q = ops.conv2d(n, self.q.weight, bias=self.q.bias)
-        k = ops.conv2d(n, self.k.weight, bias=self.k.bias)
-        v = ops.conv2d(n, self.v.weight, bias=self.v.bias)
+        a = _norm(self.norm, zq, silu=0)
+        n = ops.groupnorm_silu(x, *a.pop("gn"), **a)
+        q = ops.conv2d(n, _conv1x1(self.q.weight), bias=self.q.bias)
+        k = ops.conv2d(n, _conv1x1(self.k.weight), bias=self.k.bias)
+        v = ops.conv2d(n, _conv1x1(self.v.weight), bias=self.v.bias)
         a = ops.attention_single_head(q.view(-1, C), k.view(-1, C), v.view(-1, C), B, hh, ww).view(B, hh, ww, C)
-        return ops.conv2d(a, self.proj_out.weight, bias=self.proj_out.bias, residual=x)
+        return ops.conv2d(a, _conv1x1(self.proj_out.weight), bias=self.proj_out.bias, residual=x)
 
 
 class UpsamplingBlock(nn.Module):
-    def __init__(self, config, curr_res, block_idx):
+    def __init__(self, config, curr_res, block_idx, norm=_group_norm, linear=False):
         super().__init__()
         self.block_idx = block_idx
         if block_idx == config.num_resolutions - 1:
@@ -115,24 +146,24 @@ class UpsamplingBlock(nn.Module):
         block_out = config.hidden_channels * config.channel_mult[block_idx]
         res_blocks, attn_blocks = [], []
         for _ in range(config.num_res_blocks + 1):  # creation order interleaved like the reference (seeded init)
-            res_blocks.append(ResnetBlock(block_in, block_out, dropout_prob=config.dropout))
+            res_blocks.append(ResnetBlock(block_in, block_out, dropout_prob=config.dropout, norm=norm))
             block_in = block_out
             if curr_res in config.attn_resolutions:
-                attn_blocks.append(AttnBlock(block_in))
+                attn_blocks.append(AttnBlock(block_in, norm=norm, linear=linear))
         self.block = nn.ModuleList(res_blocks)
         self.attn = nn.ModuleList(attn_blocks)
         self.upsample = Upsample(block_in, config.resample_with_conv) if block_idx != 0 else None
 
-    def run(self, x):
+    def run(self, x, zq=None):
         for i, blk in enumerate(self.block):
-            x = blk.run(x)
+            x = blk.run(x, zq)
             if len(self.attn) > 1:  # (sic, :211)
-                x = self.attn[i].run(x)
+                x = self.attn[i].run(x, zq)
         return self.upsample.run(x) if self.upsample is not None else x
 
 
 class DownsamplingBlock(nn.Module):
-    def __init__(self, config, curr_res, block_idx):
+    def __init__(self, config, curr_res, block_idx, linear=False):
         super().__init__()
         in_mult = (1,) + tuple(config.channel_mult)
         block_in = config.hidden_channels * in_mult[block_idx]
@@ -142,7 +173,7 @@ class DownsamplingBlock(nn.Module):
             res_blocks.append(ResnetBlock(block_in, block_out, dropout_prob=config.dropout))
             block_in = block_out
             if curr_res in config.attn_resolutions:
-                attn_blocks.append(AttnBlock(block_in))
+                attn_blocks.append(AttnBlock(block_in, linear=linear))
         self.block = res_blocks
         self.attn = attn_blocks
         self.downsample = Downsample(block_in, config.resample_with_conv) if block_idx != config.num_resolutions - 1 else None
@@ -156,33 +187,36 @@ class DownsamplingBlock(nn.Module):
 
 
 class MidBlock(nn.Module):
-    def __init__(self, config, in_channels, no_attn, dropout):
+    def __init__(self, config, in_channels, no_attn, dropout, norm=_group_norm, linear=False):
         super().__init__()
         self.no_attn = no_attn
-        self.block_1 = ResnetBlock(in_channels, in_channels, dropout_prob=dropout)
+        self.block_1 = ResnetBlock(in_channels, in_channels, dropout_prob=dropout, norm=norm)
         if not no_attn:
-            self.attn_1 = AttnBlock(in_channels)
-        self.block_2 = ResnetBlock(in_channels, in_channels, dropout_prob=dropout)
+            self.attn_1 = AttnBlock(in_channels, norm=norm, linear=linear)
+        self.block_2 = ResnetBlock(in_channels, in_channels, dropout_prob=dropout, norm=norm)
 
-    def run(self, x):
-        x = self.block_1.run(x)
+    def run(self, x, zq=None):
+        x = self.block_1.run(x, zq)
         if not self.no_attn:
-            x = self.attn_1.run(x)
-        return self.block_2.run(x)
+            x = self.attn_1.run(x, zq)
+        return self.block_2.run(x, zq)
 
 
 class Encoder(nn.Module):
-    def __init__(self, config):
+    """linear: nn.Linear attention projections (MoVQ, whose configs have no no_attn_mid_block: the mid attention is always
+    built)"""
+
+    def __init__(self, config, linear=False):
         super().__init__()
         self.conv_in = nn.Conv2d(config.num_channels, config.hidden_channels, kernel_size=3, stride=1, padding=1)
         curr_res, blocks = config.resolution, []
         for i in range(config.num_resolutions):
-            blocks.append(DownsamplingBlock(config, curr_res, block_idx=i))
+            blocks.append(DownsamplingBlock(config, curr_res, block_idx=i, linear=linear))
             if i != config.num_resolutions - 1:
                 curr_res //= 2
         self.down = nn.ModuleList(blocks)
         mid = config.hidden_channels * config.channel_mult[-1]
-        self.mid = MidBlock(config, mid, config.no_attn_mid_block, config.dropout)
+        self.mid = MidBlock(config, mid, getattr(config, "no_attn_mid_block", False), config.dropout, linear=linear)
         self.norm_out = nn.GroupNorm(num_channels=mid, **_GN)
         self.conv_out = nn.Conv2d(mid, config.z_channels, kernel_size=3, stride=1, padding=1)
 
@@ -195,29 +229,33 @@ class Encoder(nn.Module):
 
 
 class Decoder(nn.Module):
-    def __init__(self, config):
+    """norm / linear: the MoVQ decoder (SpatialNorm norms, nn.Linear attention projections, mid attention always built),
+    whose run() takes the latent zq every norm is modulated by"""
+
+    def __init__(self, config, norm=_group_norm, linear=False):
         super().__init__()
         block_in = config.hidden_channels * config.channel_mult[config.num_resolutions - 1]
         curr_res = config.resolution // 2 ** (config.num_resolutions - 1)
         self.z_shape = (1, config.z_channels, curr_res, curr_res)
         self.conv_in = nn.Conv2d(config.z_channels, block_in, kernel_size=3, stride=1, padding=1)
-        self.mid = MidBlock(config, block_in, config.no_attn_mid_block, config.dropout)
+        self.mid = MidBlock(config, block_in, getattr(config, "no_attn_mid_block", False), config.dropout, norm=norm,
+                            linear=linear)
         ups = []
         for i in reversed(range(config.num_resolutions)):
-            ups.append(UpsamplingBlock(config, curr_res, block_idx=i))
+            ups.append(UpsamplingBlock(config, curr_res, block_idx=i, norm=norm, linear=linear))
             if i != 0:
                 curr_res *= 2
         self.up = nn.ModuleList(list(reversed(ups)))
         block_out = config.hidden_channels * config.channel_mult[0]
-        self.norm_out = nn.GroupNorm(num_channels=block_out, **_GN)
+        self.norm_out = norm(block_out)
         self.conv_out = nn.Conv2d(block_out, config.num_channels, kernel_size=3, stride=1, padding=1)
 
-    def run(self, z):
+    def run(self, z, zq=None):
         h = ops.conv2d(z, self.conv_in.weight, bias=self.conv_in.bias)
-        h = self.mid.run(h)
+        h = self.mid.run(h, zq)
         for blk in reversed(self.up):
-            h = blk.run(h)
-        return ops.conv2d(h, self.conv_out.weight, bias=self.conv_out.bias, gn=_gn(self.norm_out))
+            h = blk.run(h, zq)
+        return ops.conv2d(h, self.conv_out.weight, bias=self.conv_out.bias, **_norm(self.norm_out, zq))
 
 
 class VectorQuantizer(nn.Module):

@@ -64,7 +64,7 @@ def _p(t):
 
 
 _KERNELS_PER_CALL = {"muse_norm2_bwd": 3, "muse_sample_step": 2, "muse_gemm_bf16_splitk": 2, "muse_adamw_ema_step": 4, "muse_lion_ema_step": 4, "muse_ce_fwd": 2, "muse_attn_bwd": 2, "muse_embed_bwd": 2, "muse_embed_bwd_sorted": 4, "muse_vq_argmin": 2, "muse_vq_soft_code": 3,
-                     "muse_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3,
+                     "muse_groupnorm_silu_nhwc": 3, "muse_spatial_groupnorm_silu_nhwc": 3, "muse_grn_fwd": 3, "muse_grn_bwd": 3,
                      "muse_dwconv3x3_norm_bwd": 2}
 _prof = {"on": False, "events": []}
 
@@ -772,12 +772,13 @@ def _conv_stats_buffer(y, H, W, Cin, Cout, k, up=0):
     return stats, tiles
 
 
-def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None):
+def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None, spatial=None):
     """Conv2dSame on fp32 NHWC x [B,Hi,Wi,Cin] with the nn.Conv2d weight w [Cout,Cin,k,k] -> fp32 NHWC [B,H,W,Cout].
 
     gn = (gamma, beta, groups, eps) applies GroupNorm+SiLU to x first (the ResnetBlock pattern); upsample2x applies the
     nearest x2 upsample first.  Heavy layers run on the tensor cores (csrc/conv_tc.cu) with operands carried as bf16
-    hi/lo planes; the GroupNorm kernel emits the planes directly."""
+    hi/lo planes; the GroupNorm kernel emits the planes directly.  spatial = (zq, conv_y, conv_b) turns the GroupNorm
+    into the MoVQ SpatialNorm (see groupnorm_silu)."""
     st = _prep(x)
     B, Hi, Wi, Cin = x.shape
     H, W = (Hi * 2, Wi * 2) if upsample2x else (Hi, Wi)
@@ -816,8 +817,15 @@ def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None):
                 ss = torch.empty(B * Cin * 3, dtype=torch.float32, device=x.device)
             else:
                 (ws, ss), tiles = _gn_scratch(x), 0
-            _call("muse_groupnorm_silu_nhwc", _p(x), _p(gn[0].detach().float()), _p(gn[1].detach().float()), None, _p(hi),
-                  _p(lo), _p(ws), _p(ss), B, H * W, Cin, int(gn[2]), float(gn[3]), tiles, int(gn[4]) if len(gn) > 4 else 1, st)
+            if spatial is None:
+                _call("muse_groupnorm_silu_nhwc", _p(x), _p(gn[0].detach().float()), _p(gn[1].detach().float()), None,
+                      _p(hi), _p(lo), _p(ws), _p(ss), B, H * W, Cin, int(gn[2]), float(gn[3]), tiles,
+                      int(gn[4]) if len(gn) > 4 else 1, st)
+            else:
+                zq, mod, hz, wz, dq = _spatial_args(spatial)
+                _call("muse_spatial_groupnorm_silu_nhwc", _p(x), _p(gn[0].detach().float()), _p(gn[1].detach().float()),
+                      _p(zq), *mod, None, _p(hi), _p(lo), _p(ws), _p(ss), B, H, W, Cin, int(gn[2]), float(gn[3]), hz, wz,
+                      dq, tiles, int(gn[4]) if len(gn) > 4 else 1, st)
         else:
             _call("muse_split_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, 1 if upsample2x else 0, st)
         w_hi, w_lo = _packed_conv_weight_split(w)
@@ -826,21 +834,41 @@ def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None):
               Cout, k, _tc_mode(0), st)
         return y
     if gn is not None:
-        x = groupnorm_silu(x, *gn)
+        x = groupnorm_silu(x, *gn) if spatial is None else groupnorm_silu(x, *gn, spatial=spatial)
     _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), _p(residual), _p(y), B, H, W, Cin, Cout, k,
           1 if upsample2x else 0, st)
     return y
 
 
-def groupnorm_silu(x, gamma, beta, groups, eps, silu=1):
-    """GroupNorm (+ SiLU unless silu=0), fp32 NHWC in and out."""
+def groupnorm_silu(x, gamma, beta, groups, eps, silu=1, spatial=None):
+    """GroupNorm (+ SiLU unless silu=0), fp32 NHWC in and out.
+
+    spatial = (zq, conv_y, conv_b): the MoVQ SpatialNorm (muse/modeling_movq.py:21-49) before the SiLU,
+    GN(x) * conv_y(up(zq)) + conv_b(up(zq)), with zq the fp32 NHWC latent [B, hz, wz, dq] (H / hz and W / wz integers),
+    conv_y / conv_b its 1x1 nn.Conv2d(dq, C) modules and `up` the nearest resize; computed per pixel inside the apply pass."""
     st = _prep(x)
     B, H, W, C = x.shape
     y = torch.empty_like(x)
     ws, ss = _gn_scratch(x)
-    _call("muse_groupnorm_silu_nhwc", _p(x), _p(gamma.detach().float()), _p(beta.detach().float()), _p(y), None, None,
-          _p(ws), _p(ss), B, H * W, C, groups, float(eps), 0, int(silu), st)
+    if spatial is None:
+        _call("muse_groupnorm_silu_nhwc", _p(x), _p(gamma.detach().float()), _p(beta.detach().float()), _p(y), None, None,
+              _p(ws), _p(ss), B, H * W, C, groups, float(eps), 0, int(silu), st)
+        return y
+    zq, mod, hz, wz, dq = _spatial_args(spatial)
+    _call("muse_spatial_groupnorm_silu_nhwc", _p(x), _p(gamma.detach().float()), _p(beta.detach().float()), _p(zq), *mod,
+          _p(y), None, None, _p(ws), _p(ss), B, H, W, C, groups, float(eps), hz, wz, dq, 0, int(silu), st)
     return y
+
+
+def _spatial_args(spatial):
+    """(zq, conv_y, conv_b) -> zq, the (wy, by, wb, bb) pointers, hz, wz, dq of muse_spatial_groupnorm_silu_nhwc; the 1x1
+    weights are packed to [C, dq] once per parameter version"""
+    zq, cy, cb = spatial
+    zq = zq.float().contiguous()
+    pack = lambda w: w.reshape(w.shape[0], -1).clone()  # noqa: E731  (a fresh, 16-byte aligned [C, dq] copy)
+    wy, wb = _cached_pack("spatial_w", cy.weight, pack), _cached_pack("spatial_w", cb.weight, pack)
+    by, bb = _cached_pack("spatial_b", cy.bias, torch.clone), _cached_pack("spatial_b", cb.bias, torch.clone)
+    return zq, (_p(wy), _p(by), _p(wb), _p(bb)), zq.shape[1], zq.shape[2], zq.shape[3]
 
 
 def _packed_conv_weight_down(w):

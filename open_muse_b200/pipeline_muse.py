@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 from .modeling_maskgit_vqgan import MaskGitVQGAN
+from .modeling_movq import MOVQ
 from .modeling_paella_vq import PaellaVQModel
 from .modeling_taming_vqgan import VQGANModel
 from .modeling_transformer import MaskGitTransformer
@@ -238,12 +239,14 @@ class PipelineMuse:
             name = class_name(path, folder)
             if name == "VQGANModel":  # (reference :327-328)
                 vae = VQGANModel.from_pretrained(path, subfolder=folder)
+            elif name == "MOVQ":  # (reference :334-335)
+                vae = MOVQ.from_pretrained(path, subfolder=folder)
             elif name == "PaellaVQModel":  # (reference :336-337)
                 vae = PaellaVQModel.from_pretrained(path, subfolder=folder)
             elif name in (None, "MaskGitVQGAN"):
                 vae = MaskGitVQGAN.from_pretrained(path, subfolder=folder)
             else:
-                raise NotImplementedError(f"tokenizer class {name} is out of scope (MaskGitVQGAN, VQGANModel and PaellaVQModel "
+                raise NotImplementedError(f"unknown tokenizer class {name} (MaskGitVQGAN, VQGANModel, MOVQ and PaellaVQModel "
                                           "are built)")
         if transformer is None:
             path, folder = sub(transformer_path, "transformer")
