@@ -280,21 +280,25 @@ int muse_sample_step(const void* logits, const void* logits_unc, long long row_s
                      long long mask_id, int mask_len, float temperature, void* stream);
 
 /* MaskGitVQGAN encoder/decoder blocks, fp32 NHWC (muse/modeling_maskgit_vqgan.py).
- * conv2d: Conv2dSame (:33-45) stride 1, ksize 1|3, x [B,Hi,Wi,Cin] (upsample2x = 2: stride 2, pad (0,1,0,1), Hi = 2H;
- * Hi=H/2 if upsample2x == 1: nearest x2 of :146 folded
- * into the gather), wk [ksize*ksize*Cin, Cout] packed (tap-major, then input channel), optional bias [Cout] and
- * residual [B,H,W,Cout] (ResnetBlock :82-85) -> y [B,H,W,Cout]. */
+ * conv2d: x [B,Hi,Wi,Cin], wk [ksize*ksize*Cin, Cout] packed (tap-major, then input channel), optional bias [Cout] and
+ * residual [B,H,W,Cout] (ResnetBlock :82-85) -> y [B,H,W,Cout].  mode: one geometry (mode & MUSE_CONV_GEOMETRY) plus
+ * flags. */
+enum muse_conv_mode {
+  MUSE_CONV_SAME = 0,          /* Conv2dSame (:33-45): stride 1, ksize 1|3, Hi = H */
+  MUSE_CONV_UPSAMPLE2X = 1,    /* nearest x2 of :146 folded into the gather, Hi = H/2 */
+  MUSE_CONV_STRIDE2 = 2,       /* stride 2, pad 0, Hi = 2H.  ksize 3: the taming Downsample (pad (0,1,0,1));
+                                  ksize 2: PixelUnshuffle(2) + 1x1 conv of the Paella in_block (muse/modeling_paella_vq.py),
+                                  wk from the 1x1 weight viewed as [Cout, Cin, 2, 2] */
+  MUSE_CONV_S2P1 = 3,          /* Conv2d(k=4, s=2, p=1), x [B,2H,2W,Cin], ksize 4 */
+  MUSE_CONV_TRANSPOSE_S2 = 4,  /* ConvTranspose2d(k=4, s=2, p=1), x [B,H/2,W/2,Cin], ksize 4, wk the four parity matrices
+                                  [4][4*Cin][Cout] (parity 2*(y&1) + (x&1); row (a*2+b)*Cin + ci for window offset (a,b) at
+                                  input pixel (y>>1) + a + (y&1) - 1; kernel tap 3 - 2a - (y&1), likewise for columns) */
+  MUSE_CONV_GEOMETRY = 7,      /* mask of the geometry values above */
+  MUSE_CONV_GELU = 8,          /* y = GELU(conv + bias) (exact erf form, no residual) */
+  MUSE_CONV_PIXEL_SHUFFLE = 16 /* PixelShuffle(2) folded into the store (MUSE_CONV_SAME, Cout % 4 == 0): y [B,2H,2W,Cout/4] */
+};
 int muse_conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H,
-                     int W, int Cin, int Cout, int ksize, int upsample2x, void* stream);
-/* Further values of upsample2x (the mode) for the Paella tokenizer (muse/modeling_paella_vq.py):
- *   2 with ksize 2: stride 2, pad 0, 2x2 taps -- PixelUnshuffle(2) + 1x1 conv (in_block), wk from the 1x1 weight viewed
- *     as [Cout, Cin, 2, 2];
- *   3: Conv2d(k=4, s=2, p=1), x [B,2H,2W,Cin], ksize 4;
- *   4: ConvTranspose2d(k=4, s=2, p=1), x [B,H/2,W/2,Cin], ksize 4, wk the four parity matrices [4][4*Cin][Cout] (parity
- *     2*(y&1) + (x&1); row (a*2+b)*Cin + ci for window offset (a,b) at input pixel (y>>1) + a + (y&1) - 1; kernel tap
- *     3 - 2a - (y&1), likewise for columns);
- *   | 8: y = GELU(conv + bias) (exact erf form, no residual);
- *   | 16: PixelShuffle(2) folded into the store (mode 0, Cout % 4 == 0): y [B,2H,2W,Cout/4]. */
+                     int W, int Cin, int Cout, int ksize, int mode, void* stream);
 /* nn.GroupNorm(groups, C, eps) + F.silu (:61-79), deterministic (no atomics). Scratch: partials_ws float
  * [muse_groupnorm_workspace_floats(B,HW,C)] (-1 if the shape is unsupported), scale_shift_ws float [B*C*3].
  * Output either y (fp32) or the pair y_hi / y_lo (bf16 planes with y = hi + lo, the operand form of
@@ -325,29 +329,40 @@ int muse_spatial_groupnorm_silu_nhwc(const float* x, const float* gamma, const f
  * muse_conv2d_tc_supported says whether the geometry is handled (Cin % 64 == 0, W a multiple or a divisor of 128 ...);
  * other shapes use muse_conv2d_nhwc.  stats (nullable, Cout > 16): fp32 [B][tiles][Cout][2] receives {sum, M2} of y per
  * pixel tile (M2: sum of squared deviations from the tile's mean), tiles = muse_conv2d_tc_tiles_per_image(...) -- the
- * GroupNorm statistics of the next layer for free.
- * upsample2x (UpsamplingBlock :141-149, ksize 3): H, W are the output dims, x_hi/x_lo the LOW-resolution input
- * [B,H/2,W/2,Cin] and w_hi/w_lo the four 2x2 parity matrices stacked as [4*Cout, 4*Cin] (row = parity*Cout + co with
- * parity = 2*(y&1) + (x&1); column = (a*2+b)*Cin + ci for window offset (a,b); entries are sums of the 3x3 taps that
- * land on the same low-resolution pixel); tiles_per_image returns 0 when the upsample form is unsupported. */
+ * GroupNorm statistics of the next layer for free.  mode: one geometry (mode & MUSE_CONV_TC_GEOMETRY) plus flags. */
+enum muse_conv_tc_mode {
+  MUSE_CONV_TC_SAME = 0,
+  /* UpsamplingBlock (:141-149, ksize 3): H, W are the output dims, x_hi/x_lo the LOW-resolution input [B,H/2,W/2,Cin] and
+   * w_hi/w_lo the four 2x2 parity matrices stacked as [4*Cout, 4*Cin] (row = parity*Cout + co with parity = 2*(y&1) +
+   * (x&1); column = (a*2+b)*Cin + ci for window offset (a,b); entries are sums of the 3x3 taps that land on the same
+   * low-resolution pixel); tiles_per_image(upsample2x = 1) returns 0 when this form is unsupported. */
+  MUSE_CONV_TC_UPSAMPLE2X = 1,
+  /* ksize 2 with taps at offsets (0,0),(0,1),(1,0),(1,1) and zeros beyond the right / bottom edge: the stride-2 3x3
+   * convolution with pad (0,1,0,1) of the taming Downsample (modeling_taming_vqgan.py:47-62) after
+   * muse_split_s2d_bf16_nhwc, weights [Cout, 4 taps * 4 Cin]. */
+  MUSE_CONV_TC_FWD2X2 = 2,
+  MUSE_CONV_TC_GEOMETRY = 3,
+  /* per-image weights [B][Cout][K]: the attention products of AttnBlock (:160-170) run as 1x1 convolutions whose weights
+   * are the image's own keys / values. */
+  MUSE_CONV_TC_PER_IMAGE_WEIGHTS = 4,
+  /* single-pass bf16 (the fast tokenizer precision): only the hi planes are multiplied (x_lo / w_lo may be NULL), one
+   * tensor-core product per fp32 product instead of three. */
+  MUSE_CONV_TC_SINGLE_PASS = 8,
+  /* Cout <= 16, Cout % 4 == 0, MUSE_CONV_TC_SAME, no residual: PixelShuffle(2) folded into the store, y [B,2H,2W,Cout/4]
+   * (the Paella out_block). */
+  MUSE_CONV_TC_PIXEL_SHUFFLE = 16
+};
 int muse_conv2d_tc_supported(int H, int W, int Cin, int Cout, int ksize);
 int muse_conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, int upsample2x);
 int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias,
                         const float* res, float* y, float* stats, int B, int H, int W, int Cin, int Cout, int ksize,
                         int mode, void* stream);
-/* mode & 16 (Cout <= 16, Cout % 4 == 0, stride 1, no residual): PixelShuffle(2) folded into the store, y [B,2H,2W,Cout/4]
- * (the Paella out_block).
- * muse_conv2d_nhwc_tc_gelu_split: y = GELU(conv + bias) (exact erf form) stored as the bf16 planes y_hi / y_lo
- * [B,H,W,Cout] (y_lo unused with mode & 8) that the next muse_conv2d_nhwc_tc consumes: the c -> 4c Linear + GELU of the
- * Paella ResBlock.  Cout > 16, stride-1 modes (mode & 7 == 0), no residual, no statistics. */
+/* y = GELU(conv + bias) (exact erf form) stored as the bf16 planes y_hi / y_lo [B,H,W,Cout] (y_lo unused with
+ * MUSE_CONV_TC_SINGLE_PASS) that the next muse_conv2d_nhwc_tc consumes: the c -> 4c Linear + GELU of the Paella
+ * ResBlock.  Cout > 16, MUSE_CONV_TC_SAME (plus MUSE_CONV_TC_SINGLE_PASS), no residual, no statistics. */
 int muse_conv2d_nhwc_tc_gelu_split(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo,
                                    const float* bias, void* y_hi, void* y_lo, int B, int H, int W, int Cin, int Cout,
                                    int ksize, int mode, void* stream);
-/* mode & 3: 0 plain, 1 upsample2x (above), 2 = ksize 2 with taps at offsets (0,0),(0,1),(1,0),(1,1) and zeros beyond the
- * right / bottom edge: the stride-2 3x3 convolution with pad (0,1,0,1) of the taming Downsample
- * (modeling_taming_vqgan.py:47-62) after muse_split_s2d_bf16_nhwc, weights [Cout, 4 taps * 4 Cin].  mode & 4: per-image
- * weights [B][Cout][K] -- the attention products of AttnBlock (:160-170) run as 1x1 convolutions whose weights are the
- * image's own keys / values.  */
 /* space-to-depth + split: x fp32 [B,2Ho,2Wo,C] -> bf16 planes [B,Ho,Wo,4C], channel = (row parity*2 + col parity)*C + c. */
 int muse_split_s2d_bf16_nhwc(const float* x, void* hi, void* lo, int B, int Ho, int Wo, int C, void* stream);
 /* softmax(scale * x) over rows of n fp32 values (AttnBlock attention weights :162-163), written as bf16 hi/lo planes, or

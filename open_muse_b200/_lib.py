@@ -83,6 +83,13 @@ SIGNATURES = {
 
 ABI_VERSION = 10
 
+# the mode argument of muse_conv2d_nhwc (enum muse_conv_mode): one geometry plus flags
+CONV_SAME, CONV_UPSAMPLE2X, CONV_STRIDE2, CONV_S2P1, CONV_TRANSPOSE_S2 = 0, 1, 2, 3, 4
+CONV_GEOMETRY, CONV_GELU, CONV_PIXEL_SHUFFLE = 7, 8, 16
+# the mode argument of muse_conv2d_nhwc_tc / muse_conv2d_nhwc_tc_gelu_split (enum muse_conv_tc_mode)
+CONV_TC_SAME, CONV_TC_UPSAMPLE2X, CONV_TC_FWD2X2, CONV_TC_GEOMETRY = 0, 1, 2, 3
+CONV_TC_PER_IMAGE_WEIGHTS, CONV_TC_SINGLE_PASS, CONV_TC_PIXEL_SHUFFLE = 4, 8, 16
+
 
 class MuseB200Error(RuntimeError):
     pass

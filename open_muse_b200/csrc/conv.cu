@@ -21,17 +21,15 @@ template <int TM, int TN, bool VEC>
 __global__ void __launch_bounds__(256)
 conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, const float* __restrict__ bias,
                    const float* __restrict__ res, float* __restrict__ y, int B, int H, int W, int Cin, int Cout,
-                   int ksize, int up) {
+                   int ksize, int mode) {
   pdl_enter();
   constexpr int BM = 16 * TM, BN = 16 * TN;
   __shared__ __align__(16) float sA[KT][BM];
   __shared__ __align__(16) float sB[KT][BN];
-  // up & 7 (geometry): 0 plain 'same'; 1 nearest x2 upsample folded into the gather; 2 stride 2, pad 0 (ksize 3: the taming
-  // Downsample with pad (0,1,0,1); ksize 2: PixelUnshuffle(2) + 1x1 of the Paella in_block); 3 stride 2, pad 1, ksize 4
-  // (Paella Conv2d(4, 2, 1)); 4 ConvTranspose2d(4, 2, 1) as four 2x2 parity convolutions on the H/2 x W/2 input, parity
-  // blockIdx.z, weights [4][4*Cin][Cout].  up & 8: GELU epilogue; up & 16: PixelShuffle(2) folded into the store.
-  const int md = up & 7, gelu = up & 8, shuf = up & 16;
-  const int s2 = (md == 2 || md == 3), tr = (md == 4);
+  // mode: enum muse_conv_mode of include/muse_b200.h.  MUSE_CONV_TRANSPOSE_S2 runs as four 2x2 parity convolutions on the
+  // H/2 x W/2 input, parity blockIdx.z.
+  const int md = mode & MUSE_CONV_GEOMETRY, gelu = mode & MUSE_CONV_GELU, shuf = mode & MUSE_CONV_PIXEL_SHUFFLE;
+  const int s2 = (md == MUSE_CONV_STRIDE2 || md == MUSE_CONV_S2P1), tr = (md == MUSE_CONV_TRANSPOSE_S2);
   const int par = tr ? static_cast<int>(blockIdx.z) : 0;
   const int Hg = tr ? H / 2 : H, Wg = tr ? W / 2 : W;  // the grid the output rows m run over
   const long long M = static_cast<long long>(B) * Hg * Wg;
@@ -41,9 +39,10 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
   const long long m0 = static_cast<long long>(blockIdx.x) * BM;
   const int n0 = blockIdx.y * BN;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int Hi = md == 1 ? H / 2 : (s2 ? 2 * H : Hg), Wi = md == 1 ? W / 2 : (s2 ? 2 * W : Wg);
-  const int Hb = md == 1 ? H : Hi, Wb = md == 1 ? W : Wi;  // bounds of the (virtual) input grid the taps index
-  const int offy = tr ? (par >> 1) - 1 : (md == 3 ? -1 : (s2 ? 0 : -(ksize / 2)));
+  const int up = md == MUSE_CONV_UPSAMPLE2X;
+  const int Hi = up ? H / 2 : (s2 ? 2 * H : Hg), Wi = up ? W / 2 : (s2 ? 2 * W : Wg);
+  const int Hb = up ? H : Hi, Wb = up ? W : Wi;  // bounds of the (virtual) input grid the taps index
+  const int offy = tr ? (par >> 1) - 1 : (md == MUSE_CONV_S2P1 ? -1 : (s2 ? 0 : -(ksize / 2)));
   const int offx = tr ? (par & 1) - 1 : offy;
   const int st = s2 ? 2 : 1;
 
@@ -86,7 +85,7 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
       const int iy = ay[0] * st + tap / kk_size + offy, ix = ax[0] * st + tap % kk_size + offx;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (a_ok[0] && iy >= 0 && iy < Hb && ix >= 0 && ix < Wb) {
-        const int sy = md == 1 ? (iy >> 1) : iy, sx = md == 1 ? (ix >> 1) : ix;
+        const int sy = up ? (iy >> 1) : iy, sx = up ? (ix >> 1) : ix;
         v = *reinterpret_cast<const float4*>(x + ((static_cast<long long>(ab[0]) * Hi + sy) * Wi + sx) * Cin + ci);
       }
       sA[a_k[0] + 0][a_row[0]] = v.x; sA[a_k[0] + 1][a_row[0]] = v.y;
@@ -100,7 +99,7 @@ conv2d_nhwc_kernel(const float* __restrict__ x, const float* __restrict__ wk, co
           const int tap = k / Cin, ci = k % Cin;
           const int iy = ay[i] * st + tap / kk_size + offy, ix = ax[i] * st + tap % kk_size + offx;
           if (iy >= 0 && iy < Hb && ix >= 0 && ix < Wb) {
-            const int sy = md == 1 ? (iy >> 1) : iy, sx = md == 1 ? (ix >> 1) : ix;
+            const int sy = up ? (iy >> 1) : iy, sx = up ? (ix >> 1) : ix;
             v = x[((static_cast<long long>(ab[i]) * Hi + sy) * Wi + sx) * Cin + ci];
           }
         }
@@ -527,20 +526,25 @@ extern "C" {
 int muse_conv2d_nhwc(const float* x, const float* wk, const float* bias, const float* res, float* y, int B, int H, int W,
                      int Cin, int Cout, int ksize, int mode, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int md = mode & 7;
-  if (md > 4 || (mode & ~31) != 0) { set_last_error("conv2d: bad mode %d", mode); return MUSE_ERR_INVALID; }
-  const bool k_ok = md == 2 ? (ksize == 2 || ksize == 3) : (md >= 3 ? ksize == 4 : (ksize == 1 || ksize == 3));
+  const int md = mode & MUSE_CONV_GEOMETRY;
+  if (md > MUSE_CONV_TRANSPOSE_S2 || (mode & ~(MUSE_CONV_GEOMETRY | MUSE_CONV_GELU | MUSE_CONV_PIXEL_SHUFFLE)) != 0) {
+    set_last_error("conv2d: bad mode %d", mode);
+    return MUSE_ERR_INVALID;
+  }
+  const bool k_ok = md == MUSE_CONV_STRIDE2 ? (ksize == 2 || ksize == 3)
+                                            : (md >= MUSE_CONV_S2P1 ? ksize == 4 : (ksize == 1 || ksize == 3));
   if (!k_ok) { set_last_error("conv2d: kernel size %d unsupported in mode %d", ksize, md); return MUSE_ERR_UNSUPPORTED; }
-  if ((md == 1 || md == 4) && ((H | W) & 1)) { set_last_error("conv2d: upsampling modes need even output dims"); return MUSE_ERR_INVALID; }
-  if ((mode & 8) && res) { set_last_error("conv2d: the GELU epilogue takes no residual"); return MUSE_ERR_INVALID; }
-  if ((mode & 16) && (res || md != 0 || Cout % 4 != 0)) {
+  const bool upsampling = md == MUSE_CONV_UPSAMPLE2X || md == MUSE_CONV_TRANSPOSE_S2;
+  if (upsampling && ((H | W) & 1)) { set_last_error("conv2d: upsampling modes need even output dims"); return MUSE_ERR_INVALID; }
+  if ((mode & MUSE_CONV_GELU) && res) { set_last_error("conv2d: the GELU epilogue takes no residual"); return MUSE_ERR_INVALID; }
+  if ((mode & MUSE_CONV_PIXEL_SHUFFLE) && (res || md != MUSE_CONV_SAME || Cout % 4 != 0)) {
     set_last_error("conv2d: the PixelShuffle store needs Cout %% 4 == 0, stride 1, no residual");
     return MUSE_ERR_INVALID;
   }
-  const long long M = static_cast<long long>(B) * H * W / (md == 4 ? 4 : 1);
+  const long long M = static_cast<long long>(B) * H * W / (md == MUSE_CONV_TRANSPOSE_S2 ? 4 : 1);
   if (M <= 0) return MUSE_OK;
   const bool vec = (Cin % 8 == 0);
-  const unsigned gz = md == 4 ? 4 : 1;
+  const unsigned gz = md == MUSE_CONV_TRANSPOSE_S2 ? 4 : 1;
   if (Cout > 16) {
     dim3 grid(static_cast<unsigned>(ceil_div_ll(M, 128)), ceil_div(Cout, 128), gz);
     if (vec) pdl_launch(grid, 256, 0, s)(conv2d_nhwc_kernel<8, 8, true>, x, wk, bias, res, y, B, H, W, Cin, Cout, ksize, mode);

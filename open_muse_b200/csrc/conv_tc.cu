@@ -365,7 +365,7 @@ extern "C" {
 
 // 1 if muse_conv2d_nhwc_tc handles the shape (otherwise the caller uses the fp32 SIMT kernel of conv.cu).
 int muse_conv2d_tc_supported(int H, int W, int Cin, int Cout, int ksize) {
-  if (ksize != 1 && ksize != 3 && ksize != 2) return 0;  // 2: the 2x2 forward-offset window (mode 2 of muse_conv2d_nhwc_tc)
+  if (ksize != 1 && ksize != 3 && ksize != 2) return 0;  // 2: the 2x2 forward-offset window of MUSE_CONV_TC_FWD2X2
   if (Cin % 64 != 0 || Cout < 1 || (Cout > 16 && Cout % 4 != 0)) return 0;
   if (W >= 128) return W % 128 == 0;
   if (W < 8 || 128 % W != 0) return 0;
@@ -383,13 +383,9 @@ int muse_conv2d_tc_tiles_per_image(int H, int W, int Cin, int Cout, int ksize, i
   return (upsample2x ? 4 : 1) * (H * W / 128);
 }
 
-// mode & 3 == 1 (upsample2x): x planes are the LOW-resolution input [B,H/2,W/2,Cin] and w planes the four stacked parity
-//   matrices [4*Cout, 4*Cin] (ops.py packs them); y / res / stats are at the output resolution [B,H,W,Cout].
-// mode & 3 == 2: ksize 2, taps at offsets (0,0),(0,1),(1,0),(1,1), zero beyond the right / bottom edge -- a stride-2 3x3
-//   convolution with pad (0,1,0,1) (taming Downsample) after a space-to-depth of its input (w: [Cout, 4 * Cin]).
-// mode & 4: per-image weights, w planes are [B][Cout][K].
-// mode & 8: single-pass bf16 (fast tokenizer mode): only the hi planes are multiplied (x_lo / w_lo may be null): one tensor-core
-//   product per fp32 product instead of three, bf16-operand accuracy (~4e-3 per layer instead of ~2e-5).
+// mode: enum muse_conv_tc_mode of include/muse_b200.h.  MUSE_CONV_TC_UPSAMPLE2X: y / res / stats are at the output
+// resolution [B,H,W,Cout], the x planes at the input resolution.  MUSE_CONV_TC_SINGLE_PASS: bf16-operand accuracy (~4e-3
+// per layer instead of ~2e-5).
 // x_hi/x_lo: bf16 [B,H,W,Cin]; w_hi/w_lo: bf16 [Cout, k*k*Cin] (tap-major, then input channel); y fp32 [B,H,W,Cout].
 }  // extern "C"
 
@@ -399,18 +395,19 @@ int conv_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_
             float* y, bf16* yh, bf16* yl, float* stats, int B, int H, int W, int Cin, int Cout, int ksize, int mode,
             cudaStream_t s) {
   if (B <= 0) return MUSE_OK;
-  const int shuffle = (mode & 16) ? 1 : 0;
-  if (shuffle && (Cout > 16 || Cout % 4 != 0 || res != nullptr || (mode & 3) != 0)) {
+  const int geometry = mode & MUSE_CONV_TC_GEOMETRY;
+  const int shuffle = (mode & MUSE_CONV_TC_PIXEL_SHUFFLE) ? 1 : 0;
+  if (shuffle && (Cout > 16 || Cout % 4 != 0 || res != nullptr || geometry != MUSE_CONV_TC_SAME)) {
     set_last_error("conv2d_tc: the PixelShuffle store needs C_out <= 16, C_out %% 4 == 0, no residual, stride 1");
     return MUSE_ERR_UNSUPPORTED;
   }
-  if (yh != nullptr && (Cout <= 16 || res != nullptr || (mode & 7) != 0)) {
+  if (yh != nullptr && (Cout <= 16 || res != nullptr || geometry != MUSE_CONV_TC_SAME || (mode & MUSE_CONV_TC_PER_IMAGE_WEIGHTS))) {
     set_last_error("conv2d_tc: the GELU split epilogue needs C_out > 16, no residual, a plain stride-1 convolution");
     return MUSE_ERR_UNSUPPORTED;
   }
-  const int upsample2x = (mode & 3) == 1;
-  const int fwd2x2 = (mode & 3) == 2;
-  if (fwd2x2 != (ksize == 2)) { set_last_error("conv2d_tc: ksize 2 and mode 2 go together"); return MUSE_ERR_INVALID; }
+  const int upsample2x = geometry == MUSE_CONV_TC_UPSAMPLE2X;
+  const int fwd2x2 = geometry == MUSE_CONV_TC_FWD2X2;
+  if (fwd2x2 != (ksize == 2)) { set_last_error("conv2d_tc: ksize 2 and MUSE_CONV_TC_FWD2X2 go together"); return MUSE_ERR_INVALID; }
   if (upsample2x) {
     if (muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, ksize, 1) == 0) {
       set_last_error("conv2d_tc: unsupported upsample shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W, Cin, Cout, ksize);
@@ -430,7 +427,8 @@ int conv_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_
   }
   ConvParams p;
   p.y = y; p.bias = bias; p.res = res; p.stats = (Cout > 16 && yh == nullptr) ? stats : nullptr;
-  p.yh = yh; p.yl = (mode & 8) ? nullptr : yl; p.shuffle = shuffle;
+  const bool single_pass = (mode & MUSE_CONV_TC_SINGLE_PASS) != 0;
+  p.yh = yh; p.yl = single_pass ? nullptr : yl; p.shuffle = shuffle;
   p.N = Cout; p.H = H; p.W = W; p.Cin = Cin; p.ksize = ksize;
   const int tile_px = 128;
   p.tile_w = W >= tile_px ? tile_px : W;
@@ -440,7 +438,7 @@ int conv_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_
   p.num_m = B * p.tiles_per_img;
   p.up = upsample2x ? 1 : 0;
   p.fwd2x2 = fwd2x2;
-  p.wbatch = (mode & 4) ? 1 : 0;
+  p.wbatch = (mode & MUSE_CONV_TC_PER_IMAGE_WEIGHTS) ? 1 : 0;
   p.tile_w_log2 = 0;
   while ((1 << p.tile_w_log2) < p.tile_w) ++p.tile_w_log2;
   if (p.up && (1 << p.tile_w_log2) != p.tile_w) { set_last_error("conv2d_tc: upsample needs a power-of-two tile width"); return MUSE_ERR_UNSUPPORTED; }
@@ -448,7 +446,7 @@ int conv_tc(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_
   p.num_n = ceil_div(Cout, BN);
   p.cchunks = Cin / BK;
   const int taps = (p.up || p.fwd2x2) ? 4 : ksize * ksize;
-  p.passes = (mode & 8) ? 1 : 3;
+  p.passes = single_pass ? 1 : 3;
   p.num_kb = taps * p.cchunks * p.passes;
   if (p.passes == 1) { x_lo = x_hi; w_lo = w_hi; }  // the lo maps are never dereferenced; keep the encodes valid
 
@@ -481,12 +479,12 @@ int muse_conv2d_nhwc_tc(const void* x_hi, const void* x_lo, const void* w_hi, co
                  static_cast<cudaStream_t>(stream));
 }
 
-// y = GELU(conv(x) + bias) written as bf16 planes y_hi [B,H,W,Cout] (+ y_lo unless mode & 8), the operands of the next
-// tensor-core convolution: the c -> 4c Linear + GELU of the Paella ResBlock.  Stride-1 modes only (mode & 7 == 0).
+// y = GELU(conv(x) + bias) written as bf16 planes y_hi [B,H,W,Cout] (+ y_lo unless MUSE_CONV_TC_SINGLE_PASS), the operands
+// of the next tensor-core convolution: the c -> 4c Linear + GELU of the Paella ResBlock.  MUSE_CONV_TC_SAME only.
 int muse_conv2d_nhwc_tc_gelu_split(const void* x_hi, const void* x_lo, const void* w_hi, const void* w_lo, const float* bias,
                                    void* y_hi, void* y_lo, int B, int H, int W, int Cin, int Cout, int ksize, int mode,
                                    void* stream) {
-  if (y_hi == nullptr || ((mode & 8) == 0 && y_lo == nullptr)) {
+  if (y_hi == nullptr || ((mode & MUSE_CONV_TC_SINGLE_PASS) == 0 && y_lo == nullptr)) {
     set_last_error("conv2d_tc_gelu_split: y_hi (and y_lo unless single-pass) are required");
     return MUSE_ERR_INVALID;
   }

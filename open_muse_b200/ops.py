@@ -7,10 +7,14 @@ library is missing or the tensors are not CUDA tensors -- there is no fallback p
 from __future__ import annotations
 
 import os
+import weakref
 
 import torch
 
 from . import _lib
+from ._lib import (CONV_GELU, CONV_PIXEL_SHUFFLE, CONV_S2P1, CONV_SAME, CONV_STRIDE2, CONV_TC_FWD2X2,
+                   CONV_TC_PER_IMAGE_WEIGHTS, CONV_TC_PIXEL_SHUFFLE, CONV_TC_SAME, CONV_TC_SINGLE_PASS, CONV_TC_UPSAMPLE2X,
+                   CONV_TRANSPOSE_S2, CONV_UPSAMPLE2X)
 
 F32, BF16 = 0, 1
 EPI_BF16, EPI_F32, EPI_ATOMIC_F32, EPI_RESADD_F32 = 0, 1, 2, 3
@@ -605,8 +609,6 @@ def sample_step(logits, input_ids, q_exp, u, K, mask_id, mask_len, temperature, 
 
 
 # ------------------------------------------------------------------------------------------ VQGAN blocks (fp32 NHWC)
-_wk_cache = {}
-
 # Tensor-core convolution precision: "bf16x3" (default) carries every fp32 operand as bf16 hi + lo planes and accumulates
 # hi*hi + lo*hi + hi*lo in fp32 -- fp32-faithful, what the bit-exact token-id contract needs.  "bf16" multiplies the hi
 # planes only: one product instead of three and no lo planes written, at bf16-operand accuracy (the reference itself runs
@@ -650,72 +652,116 @@ class conv_route:
         return False
 
 
-def _lo_like(hi):
-    return None if _conv_state["single"] else torch.empty_like(hi)
+_wk_cache = {}
+_WK_CACHE_ENTRIES = 4096
 
 
-def _tc_mode(mode):
-    return mode | 8 if _conv_state["single"] else mode
-
-
-def _packed_conv_weight(w):
-    """[Cout, Cin, kh, kw] -> [kh*kw*Cin, Cout] (tap-major, then input channel); cached per live weight tensor
-    (weakref identity + storage pointer + version counter, so a recycled id() or an in-place update never hits)."""
-    import weakref
-
+def _cached_pack(tag, w, pack):
+    """pack(w as fp32), cached per live weight tensor w under `tag`.  The key holds w's weakref identity, storage pointer,
+    version counter, shape and device, so a recycled id() or an in-place update never hits; the cache is emptied when it
+    outgrows _WK_CACHE_ENTRIES."""
     key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
-    hit = _wk_cache.get(id(w))
+    hit = _wk_cache.get((tag, id(w)))
     if hit is not None and hit[0]() is w and hit[1] == key:
         return hit[2]
-    wk = w.detach().float().permute(2, 3, 1, 0).reshape(-1, w.shape[0]).contiguous()
-    if len(_wk_cache) > 4096:
+    out = pack(w.detach().float())
+    if len(_wk_cache) > _WK_CACHE_ENTRIES:
         _wk_cache.clear()
-    _wk_cache[id(w)] = (weakref.ref(w), key, wk)
-    return wk
+    _wk_cache[(tag, id(w))] = (weakref.ref(w), key, out)
+    return out
 
 
-def _packed_conv_weight_split(w):
-    """[Cout, Cin, kh, kw] -> bf16 planes (hi, lo) of [Cout, kh*kw*Cin] (tap-major, then input channel), w = hi + lo."""
-    import weakref
-
-    key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
-    hit = _wk_cache.get(("split", id(w)))
-    if hit is not None and hit[0]() is w and hit[1] == key:
-        return hit[2]
-    wk = w.detach().float().permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous()
+def _planes(wk):
+    """fp32 -> bf16 planes (hi, lo) with wk = hi + lo: hi = bf16(wk), lo = bf16(wk - hi)."""
     hi = wk.to(torch.bfloat16)
-    lo = (wk - hi.float()).to(torch.bfloat16)
-    if len(_wk_cache) > 4096:
-        _wk_cache.clear()
-    _wk_cache[("split", id(w))] = (weakref.ref(w), key, (hi, lo))
-    return hi, lo
+    return hi, (wk - hi.float()).to(torch.bfloat16)
 
 
-def conv_uses_tensor_cores(H, W, Cin, Cout, k):
-    """Route of conv2d(): wgmma bf16x3 implicit GEMM unless the geometry is unsupported or MUSE_B200_CONV=simt.
-    Stems with k*k*Cin <= 64 go through an im2col to 64 columns and run as a 1x1 convolution."""
-    if _conv_state["route"] == "simt":  # private test hook (ops.conv_route): cross-check against the fp32 FMA kernels
+def _pack_simt(wf):
+    """[Cout, Cin, kh, kw] -> [kh*kw*Cin, Cout] (tap-major, then input channel), the weights of muse_conv2d_nhwc."""
+    return wf.permute(2, 3, 1, 0).reshape(-1, wf.shape[0]).contiguous()
+
+
+def _pack_tc(wf):
+    """[Cout, Cin, kh, kw] -> bf16 planes of [Cout, kh*kw*Cin] (tap-major, then input channel)."""
+    return _planes(wf.permute(0, 2, 3, 1).reshape(wf.shape[0], -1).contiguous())
+
+
+def _pack_stem(wf):
+    """Stem weight [Cout, Cin, k, k] with k*k*Cin <= 64 -> bf16 planes of [Cout, 64], columns tap-major, zero padded: the
+    1x1 convolution over the rows of muse_im2col_split_nhwc."""
+    wk = torch.zeros(wf.shape[0], 64, dtype=torch.float32, device=wf.device)
+    flat = wf.permute(0, 2, 3, 1).reshape(wf.shape[0], -1)
+    wk[:, : flat.shape[1]] = flat
+    return _planes(wk)
+
+
+def _tc_route(H, W, Cin, Cout, k, upsample2x=False):
+    """Whether muse_conv2d_nhwc_tc runs this convolution, H, W the output dims; upsample2x: in the four-parity form of
+    MUSE_CONV_TC_UPSAMPLE2X.  Never under the test hook ops.conv_route("simt")."""
+    if _conv_state["route"] == "simt":
         return False
-    if Cin % 64 != 0 and k * k * Cin <= 64:
-        return bool(_lib.load().muse_conv2d_tc_supported(H, W, 64, Cout, 1))
+    if upsample2x:
+        return _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, k, 1) > 0
     return bool(_lib.load().muse_conv2d_tc_supported(H, W, Cin, Cout, k))
 
 
-def _packed_conv_weight_split_stem(w):
-    """Stem weight [Cout, Cin, k, k] with k*k*Cin <= 64 -> bf16 (hi, lo) of [Cout, 64], columns tap-major, zero padded."""
-    import weakref
+def conv_uses_tensor_cores(H, W, Cin, Cout, k):
+    """Whether conv2d() at output size H x W runs on the tensor cores (the wgmma implicit GEMM of csrc/conv_tc.cu) rather
+    than the fp32 SIMT kernel: unless the geometry is unsupported or ops.conv_route("simt") is active.  Stems with
+    k*k*Cin <= 64 go through an im2col to 64 columns and run as a 1x1 convolution."""
+    if Cin % 64 != 0 and k * k * Cin <= 64:
+        return _tc_route(H, W, 64, Cout, 1)
+    return _tc_route(H, W, Cin, Cout, k)
 
-    key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
-    hit = _wk_cache.get(("stem", id(w)))
-    if hit is not None and hit[0]() is w and hit[1] == key:
-        return hit[2]
-    wk = torch.zeros(w.shape[0], 64, dtype=torch.float32, device=w.device)
-    flat = w.detach().float().permute(0, 2, 3, 1).reshape(w.shape[0], -1)
-    wk[:, : flat.shape[1]] = flat
-    hi = wk.to(torch.bfloat16)
-    lo = (wk - hi.float()).to(torch.bfloat16)
-    _wk_cache[("stem", id(w))] = (weakref.ref(w), key, (hi, lo))
+
+def _new_planes(shape, device, exact=False):
+    """Uninitialised bf16 operand planes (hi, lo); no lo plane in the single-pass precision unless exact."""
+    hi = torch.empty(shape, dtype=torch.bfloat16, device=device)
+    return hi, (torch.empty_like(hi) if exact or not _conv_state["single"] else None)
+
+
+def _split(x, st, upsample2x=False, exact=False):
+    """fp32 NHWC x -> its bf16 planes (hi, lo), those of its nearest x2 upsample with upsample2x.  An x of another rank is
+    split as rows of its last dimension."""
+    *lead, C = x.shape
+    B, H, W = lead if len(lead) == 3 else (1, 1, x.numel() // C)
+    if upsample2x:
+        H, W = 2 * H, 2 * W
+    hi, lo = _new_planes((B, H, W, C) if x.dim() == 4 else x.shape, x.device, exact)
+    _call("muse_split_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, C, int(upsample2x), st)
     return hi, lo
+
+
+def _split_s2d(x, st):
+    """fp32 NHWC x [B, 2H, 2W, C] -> the bf16 planes of its space-to-depth [B, H, W, 4C]."""
+    B, Hi, Wi, C = x.shape
+    hi, lo = _new_planes((B, Hi // 2, Wi // 2, 4 * C), x.device)
+    _call("muse_split_s2d_bf16_nhwc", _p(x), _p(hi), _p(lo), B, Hi // 2, Wi // 2, C, st)
+    return hi, lo
+
+
+def _im2col(x, H, W, k, st):
+    """fp32 NHWC x -> bf16 planes [B, H, W, 64] of the k*k*Cin <= 64 taps per output pixel (k = 2: the PixelUnshuffle(2)
+    block of x [B, 2H, 2W, Cin])."""
+    B, Cin = x.shape[0], x.shape[3]
+    hi, lo = _new_planes((B, H, W, 64), x.device)
+    _call("muse_im2col_split_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, k, st)
+    return hi, lo
+
+
+def _conv_tc(x, w, bias, y, B, H, W, Cin, Cout, k, mode, st, res=None, stats=None, exact=False):
+    """One tensor-core convolution of the activation planes x by the weight planes w, both (hi, lo) pairs.  y is the fp32
+    output, or the (hi, lo) planes that receive GELU(conv + bias) (muse_conv2d_nhwc_tc_gelu_split).  The single-pass
+    precision adds MUSE_CONV_TC_SINGLE_PASS to the mode unless exact."""
+    if _conv_state["single"] and not exact:
+        mode |= CONV_TC_SINGLE_PASS
+    if isinstance(y, tuple):
+        _call("muse_conv2d_nhwc_tc_gelu_split", _p(x[0]), _p(x[1]), _p(w[0]), _p(w[1]), _p(bias), _p(y[0]), _p(y[1]), B, H,
+              W, Cin, Cout, k, mode, st)
+    else:
+        _call("muse_conv2d_nhwc_tc", _p(x[0]), _p(x[1]), _p(w[0]), _p(w[1]), _p(bias), _p(res), _p(y), _p(stats), B, H, W,
+              Cin, Cout, k, mode, st)
 
 
 def _gn_scratch(x):
@@ -727,19 +773,62 @@ def _gn_scratch(x):
             torch.empty(B * C * 3, dtype=torch.float32, device=x.device))
 
 
-def _packed_conv_weight_upsample(w):
-    """3x3 weight of an UpsamplingBlock conv -> bf16 (hi, lo) of the four stacked 2x2 parity matrices [4*Cout, 4*Cin].
+def _groupnorm(x, gn, spatial, st, planes=False):
+    """GroupNorm (+ SiLU) of fp32 NHWC x, gn = (gamma, beta, groups, eps[, silu = 1]); MoVQ SpatialNorm with spatial (see
+    groupnorm_silu).  Returns fp32 y, or with planes the bf16 operand planes of the next tensor-core convolution, which
+    reuse the {sum, M2} tiles the convolution that produced x left on it."""
+    B, H, W, C = x.shape
+    gamma, beta = gn[0].detach().float(), gn[1].detach().float()
+    groups, eps, silu = int(gn[2]), float(gn[3]), int(gn[4]) if len(gn) > 4 else 1
+    pre = getattr(x, "_gn_stats", None) if planes else None
+    if pre is not None and pre[2] == x._version:
+        ws, tiles, _ = pre
+        ss = torch.empty(B * C * 3, dtype=torch.float32, device=x.device)
+    else:
+        (ws, ss), tiles = _gn_scratch(x), 0
+    if planes:
+        y, (hi, lo) = None, _new_planes(x.shape, x.device)
+    else:
+        y, hi, lo = torch.empty_like(x), None, None
+    if spatial is None:
+        _call("muse_groupnorm_silu_nhwc", _p(x), _p(gamma), _p(beta), _p(y), _p(hi), _p(lo), _p(ws), _p(ss), B, H * W, C,
+              groups, eps, tiles, silu, st)
+    else:
+        zq, mod, hz, wz, dq = _spatial_args(spatial)
+        _call("muse_spatial_groupnorm_silu_nhwc", _p(x), _p(gamma), _p(beta), _p(zq), *mod, _p(y), _p(hi), _p(lo), _p(ws),
+              _p(ss), B, H, W, C, groups, eps, hz, wz, dq, tiles, silu, st)
+    return (hi, lo) if planes else y
+
+
+def _spatial_args(spatial):
+    """(zq, conv_y, conv_b) -> zq, the (wy, by, wb, bb) pointers, hz, wz, dq of muse_spatial_groupnorm_silu_nhwc; the 1x1
+    weights are packed to [C, dq] once per parameter version"""
+    zq, cy, cb = spatial
+    zq = zq.float().contiguous()
+    pack = lambda w: w.reshape(w.shape[0], -1).clone()  # noqa: E731  (a fresh, 16-byte aligned [C, dq] copy)
+    wy, wb = _cached_pack("spatial_w", cy.weight, pack), _cached_pack("spatial_w", cb.weight, pack)
+    by, bb = _cached_pack("spatial_b", cy.bias, torch.clone), _cached_pack("spatial_b", cb.bias, torch.clone)
+    return zq, (_p(wy), _p(by), _p(wb), _p(bb)), zq.shape[1], zq.shape[2], zq.shape[3]
+
+
+def _conv_stats_buffer(y, H, W, Cin, Cout, k, up=0):
+    """The tensor-core convolution's epilogue leaves per-tile {sum, M2} of its output (M2: squared deviations from the tile
+    mean): they ride along on the output tensor (``y._gn_stats``, with y's version counter) so that a following
+    conv2d(gn=...) skips the GroupNorm statistics pass over y -- unless y was modified in place since."""
+    if Cout <= 16 or Cout % 32 != 0:
+        return None
+    tiles = _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, k, up)
+    stats = torch.empty(y.shape[0], tiles, Cout, 2, dtype=torch.float32, device=y.device)
+    y._gn_stats = (stats, tiles, y._version)
+    return stats
+
+
+def _pack_upsample(wf):
+    """3x3 weight of an UpsamplingBlock conv -> bf16 planes of the four stacked 2x2 parity matrices [4*Cout, 4*Cin].
 
     Output pixel (2y+py, 2x+px) of conv3x3(nearest_x2(v)) reads only v[y+a+py-1, x+b+px-1] for a, b in {0, 1}; the 3x3
     taps that land on the same low-resolution pixel are summed (fp32): rows R(0,0)={0}, R(0,1)={1,2}, R(1,0)={0,1},
     R(1,1)={2} (same for columns)."""
-    import weakref
-
-    key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
-    hit = _wk_cache.get(("up", id(w)))
-    if hit is not None and hit[0]() is w and hit[1] == key:
-        return hit[2]
-    wf = w.detach().float()  # [Cout, Cin, 3, 3]
     sets = {(0, 0): [0], (0, 1): [1, 2], (1, 0): [0, 1], (1, 1): [2]}
     mats = []
     for py in (0, 1):
@@ -753,23 +842,7 @@ def _packed_conv_weight_upsample(w):
                             acc = acc + wf[:, :, kh, kw]
                     taps.append(acc)  # [Cout, Cin]
             mats.append(torch.stack(taps, dim=1).reshape(wf.shape[0], -1))  # [Cout, 4*Cin], column = (a*2+b)*Cin + ci
-    wk = torch.cat(mats, dim=0).contiguous()  # [4*Cout, 4*Cin], row = parity*Cout + co
-    hi = wk.to(torch.bfloat16)
-    lo = (wk - hi.float()).to(torch.bfloat16)
-    _wk_cache[("up", id(w))] = (weakref.ref(w), key, (hi, lo))
-    return hi, lo
-
-
-def _conv_stats_buffer(y, H, W, Cin, Cout, k, up=0):
-    """The tensor-core convolution's epilogue leaves per-tile {sum, M2} of its output (M2: squared deviations from the tile
-    mean): they ride along on the output tensor (``y._gn_stats``, with y's version counter) so that a following
-    conv2d(gn=...) skips the GroupNorm statistics pass over y -- unless y was modified in place since."""
-    if Cout <= 16 or Cout % 32 != 0:
-        return None, 0
-    tiles = _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, k, up)
-    stats = torch.empty(y.shape[0], tiles, Cout, 2, dtype=torch.float32, device=y.device)
-    y._gn_stats = (stats, tiles, y._version)
-    return stats, tiles
+    return _planes(torch.cat(mats, dim=0).contiguous())  # [4*Cout, 4*Cin], row = parity*Cout + co
 
 
 def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None, spatial=None):
@@ -785,58 +858,29 @@ def conv2d(x, w, bias=None, residual=None, upsample2x=False, gn=None, spatial=No
     Cout, k = w.shape[0], w.shape[2]
     y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
     b = None if bias is None else bias.detach().float()
-    if conv_uses_tensor_cores(H, W, Cin, Cout, k) and Cin % 64 != 0:
-        assert gn is None and not upsample2x
-        hi = torch.empty(B, H, W, 64, dtype=torch.bfloat16, device=x.device)
-        lo = _lo_like(hi)
-        _call("muse_im2col_split_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, k, st)
-        w_hi, w_lo = _packed_conv_weight_split_stem(w)
-        stats, tiles = _conv_stats_buffer(y, H, W, 64, Cout, 1)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), _p(residual), _p(y), _p(stats), B, H, W, 64,
-              Cout, 1, _tc_mode(0), st)
-        return y
-    if upsample2x and gn is None and conv_uses_tensor_cores(H, W, Cin, Cout, k) and \
-            _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, k, 1) > 0:
+    if upsample2x and gn is None and _tc_route(H, W, Cin, Cout, k, upsample2x=True):
         # nearest x2 + 3x3 conv as four 2x2 parity convolutions on the low-resolution planes (2.25x fewer FLOPs)
-        hi = torch.empty(B, Hi, Wi, Cin, dtype=torch.bfloat16, device=x.device)
-        lo = _lo_like(hi)
-        _call("muse_split_bf16_nhwc", _p(x), _p(hi), _p(lo), B, Hi, Wi, Cin, 0, st)
-        w_hi, w_lo = _packed_conv_weight_upsample(w)
-        stats, tiles = _conv_stats_buffer(y, H, W, Cin, Cout, k, 1)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), _p(residual), _p(y), _p(stats), B, H, W, Cin,
-              Cout, k, _tc_mode(1), st)
+        _conv_tc(_split(x, st), _cached_pack("upsample", w, _pack_upsample), b, y, B, H, W, Cin, Cout, k,
+                 CONV_TC_UPSAMPLE2X, st, res=residual, stats=_conv_stats_buffer(y, H, W, Cin, Cout, k, 1))
         return y
-    if conv_uses_tensor_cores(H, W, Cin, Cout, k):
-        hi = torch.empty(B, H, W, Cin, dtype=torch.bfloat16, device=x.device)
-        lo = _lo_like(hi)
+    if not conv_uses_tensor_cores(H, W, Cin, Cout, k):
         if gn is not None:
-            assert not upsample2x
-            pre = getattr(x, "_gn_stats", None)  # {sum, M2} tiles left by the convolution that produced x
-            if pre is not None and pre[2] == x._version:
-                ws, tiles, _ = pre
-                ss = torch.empty(B * Cin * 3, dtype=torch.float32, device=x.device)
-            else:
-                (ws, ss), tiles = _gn_scratch(x), 0
-            if spatial is None:
-                _call("muse_groupnorm_silu_nhwc", _p(x), _p(gn[0].detach().float()), _p(gn[1].detach().float()), None,
-                      _p(hi), _p(lo), _p(ws), _p(ss), B, H * W, Cin, int(gn[2]), float(gn[3]), tiles,
-                      int(gn[4]) if len(gn) > 4 else 1, st)
-            else:
-                zq, mod, hz, wz, dq = _spatial_args(spatial)
-                _call("muse_spatial_groupnorm_silu_nhwc", _p(x), _p(gn[0].detach().float()), _p(gn[1].detach().float()),
-                      _p(zq), *mod, None, _p(hi), _p(lo), _p(ws), _p(ss), B, H, W, Cin, int(gn[2]), float(gn[3]), hz, wz,
-                      dq, tiles, int(gn[4]) if len(gn) > 4 else 1, st)
-        else:
-            _call("muse_split_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, 1 if upsample2x else 0, st)
-        w_hi, w_lo = _packed_conv_weight_split(w)
-        stats, tiles = _conv_stats_buffer(y, H, W, Cin, Cout, k)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), _p(residual), _p(y), _p(stats), B, H, W, Cin,
-              Cout, k, _tc_mode(0), st)
+            x = _groupnorm(x, gn, spatial, st)
+        _call("muse_conv2d_nhwc", _p(x), _p(_cached_pack("simt", w, _pack_simt)), _p(b), _p(residual), _p(y), B, H, W, Cin,
+              Cout, k, CONV_UPSAMPLE2X if upsample2x else CONV_SAME, st)
         return y
-    if gn is not None:
-        x = groupnorm_silu(x, *gn) if spatial is None else groupnorm_silu(x, *gn, spatial=spatial)
-    _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), _p(residual), _p(y), B, H, W, Cin, Cout, k,
-          1 if upsample2x else 0, st)
+    if Cin % 64 != 0:  # stem with k*k*Cin <= 64
+        assert gn is None and not upsample2x
+        _conv_tc(_im2col(x, H, W, k, st), _cached_pack("stem", w, _pack_stem), b, y, B, H, W, 64, Cout, 1, CONV_TC_SAME, st,
+                 res=residual, stats=_conv_stats_buffer(y, H, W, 64, Cout, 1))
+        return y
+    if gn is None:
+        planes = _split(x, st, upsample2x)
+    else:
+        assert not upsample2x
+        planes = _groupnorm(x, gn, spatial, st, planes=True)
+    _conv_tc(planes, _cached_pack("tc", w, _pack_tc), b, y, B, H, W, Cin, Cout, k, CONV_TC_SAME, st, res=residual,
+             stats=_conv_stats_buffer(y, H, W, Cin, Cout, k))
     return y
 
 
@@ -846,43 +890,14 @@ def groupnorm_silu(x, gamma, beta, groups, eps, silu=1, spatial=None):
     spatial = (zq, conv_y, conv_b): the MoVQ SpatialNorm (muse/modeling_movq.py:21-49) before the SiLU,
     GN(x) * conv_y(up(zq)) + conv_b(up(zq)), with zq the fp32 NHWC latent [B, hz, wz, dq] (H / hz and W / wz integers),
     conv_y / conv_b its 1x1 nn.Conv2d(dq, C) modules and `up` the nearest resize; computed per pixel inside the apply pass."""
-    st = _prep(x)
-    B, H, W, C = x.shape
-    y = torch.empty_like(x)
-    ws, ss = _gn_scratch(x)
-    if spatial is None:
-        _call("muse_groupnorm_silu_nhwc", _p(x), _p(gamma.detach().float()), _p(beta.detach().float()), _p(y), None, None,
-              _p(ws), _p(ss), B, H * W, C, groups, float(eps), 0, int(silu), st)
-        return y
-    zq, mod, hz, wz, dq = _spatial_args(spatial)
-    _call("muse_spatial_groupnorm_silu_nhwc", _p(x), _p(gamma.detach().float()), _p(beta.detach().float()), _p(zq), *mod,
-          _p(y), None, None, _p(ws), _p(ss), B, H, W, C, groups, float(eps), hz, wz, dq, 0, int(silu), st)
-    return y
+    return _groupnorm(x, (gamma, beta, groups, eps, silu), spatial, _prep(x))
 
 
-def _spatial_args(spatial):
-    """(zq, conv_y, conv_b) -> zq, the (wy, by, wb, bb) pointers, hz, wz, dq of muse_spatial_groupnorm_silu_nhwc; the 1x1
-    weights are packed to [C, dq] once per parameter version"""
-    zq, cy, cb = spatial
-    zq = zq.float().contiguous()
-    pack = lambda w: w.reshape(w.shape[0], -1).clone()  # noqa: E731  (a fresh, 16-byte aligned [C, dq] copy)
-    wy, wb = _cached_pack("spatial_w", cy.weight, pack), _cached_pack("spatial_w", cb.weight, pack)
-    by, bb = _cached_pack("spatial_b", cy.bias, torch.clone), _cached_pack("spatial_b", cb.bias, torch.clone)
-    return zq, (_p(wy), _p(by), _p(wb), _p(bb)), zq.shape[1], zq.shape[2], zq.shape[3]
-
-
-def _packed_conv_weight_down(w):
-    """3x3 stride-2 weight (pad (0,1,0,1)) -> bf16 (hi, lo) [Cout, 4 taps * 4 * Cin] for the space-to-depth form:
+def _pack_s2d(wf):
+    """3x3 stride-2 weight (pad (0,1,0,1)) -> bf16 planes [Cout, 4 taps * 4 * Cin] for the space-to-depth form:
     tap (a, b) in {0,1}^2 and plane (p, q) hold w[:, :, 2a + p, 2b + q] (zero where 2a + p or 2b + q exceeds 2)."""
-    import weakref
-
-    key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
-    hit = _wk_cache.get(("down", id(w)))
-    if hit is not None and hit[0]() is w and hit[1] == key:
-        return hit[2]
-    wf = w.detach().float()
     Cout, Cin = wf.shape[0], wf.shape[1]
-    wk = torch.zeros(Cout, 2, 2, 2, 2, Cin, dtype=torch.float32, device=w.device)  # [co, a, b, p, q, ci]
+    wk = torch.zeros(Cout, 2, 2, 2, 2, Cin, dtype=torch.float32, device=wf.device)  # [co, a, b, p, q, ci]
     for a in (0, 1):
         for b in (0, 1):
             for p_ in (0, 1):
@@ -890,11 +905,7 @@ def _packed_conv_weight_down(w):
                     kh, kw = 2 * a + p_, 2 * b + q
                     if kh <= 2 and kw <= 2:
                         wk[:, a, b, p_, q] = wf[:, :, kh, kw]
-    wk = wk.reshape(Cout, -1).contiguous()
-    hi = wk.to(torch.bfloat16)
-    lo = (wk - hi.float()).to(torch.bfloat16)
-    _wk_cache[("down", id(w))] = (weakref.ref(w), key, (hi, lo))
-    return hi, lo
+    return _planes(wk.reshape(Cout, -1).contiguous())
 
 
 def conv2d_down(x, w, bias=None):
@@ -907,17 +918,12 @@ def conv2d_down(x, w, bias=None):
     Cout = w.shape[0]
     y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
     b = None if bias is None else bias.detach().float()
-    if _conv_state["route"] != "simt" and (4 * Cin) % 64 == 0 and \
-            _lib.load().muse_conv2d_tc_supported(H, W, 4 * Cin, Cout, 2):
-        hi = torch.empty(B, H, W, 4 * Cin, dtype=torch.bfloat16, device=x.device)
-        lo = _lo_like(hi)
-        _call("muse_split_s2d_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, st)
-        w_hi, w_lo = _packed_conv_weight_down(w)
-        stats, tiles = _conv_stats_buffer(y, H, W, 4 * Cin, Cout, 2)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), _p(stats), B, H, W, 4 * Cin, Cout,
-              2, _tc_mode(2), st)
+    if _tc_route(H, W, 4 * Cin, Cout, 2):
+        _conv_tc(_split_s2d(x, st), _cached_pack("s2d", w, _pack_s2d), b, y, B, H, W, 4 * Cin, Cout, 2, CONV_TC_FWD2X2, st,
+                 stats=_conv_stats_buffer(y, H, W, 4 * Cin, Cout, 2))
         return y
-    _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), None, _p(y), B, H, W, Cin, Cout, 3, 2, st)
+    _call("muse_conv2d_nhwc", _p(x), _p(_cached_pack("simt", w, _pack_simt)), _p(b), None, _p(y), B, H, W, Cin, Cout, 3,
+          CONV_STRIDE2, st)
     return y
 
 
@@ -926,45 +932,32 @@ def attention_single_head(q, k, v, B, hh, ww):
     q, k, v fp32 [B*hh*ww, C] -> fp32 [B*hh*ww, C].  Both products run as 1x1 tensor-core convolutions whose weights are
     the image's own keys / values (per-image weight mode of muse_conv2d_nhwc_tc); small geometries loop over the images
     with the SIMT kernel."""
-    import os
-
     st = _prep(q)
     HW, C = hh * ww, q.shape[1]
-    lib = _lib.load()
     scale = float(C) ** -0.5
     out = torch.empty(B * HW, C, dtype=torch.float32, device=q.device)
     scores = torch.empty(B * HW, HW, dtype=torch.float32, device=q.device)
     vt = torch.empty(B, C, HW, dtype=torch.float32, device=q.device)
     _call("muse_transpose_batched", _p(v), _p(vt), B, HW, C, st)
-    tc = _conv_state["route"] != "simt" and lib.muse_conv2d_tc_supported(hh, ww, C, HW, 1) and \
-        lib.muse_conv2d_tc_supported(hh, ww, HW, C, 1) and HW % 64 == 0 and C % 64 == 0
-
-    def planes(t):
-        hi = torch.empty(t.shape, dtype=torch.bfloat16, device=t.device)
-        lo = torch.empty_like(hi)
-        _call("muse_split_bf16_nhwc", _p(t), _p(hi), _p(lo), 1, 1, t.numel() // t.shape[-1], t.shape[-1], 0, st)
-        return hi, lo
-
-    if tc:
-        qh, ql = planes(q)
-        kh, kl = planes(k)        # per-image weights [B][HW keys][C]
-        _call("muse_conv2d_nhwc_tc", _p(qh), _p(ql), _p(kh), _p(kl), None, None, _p(scores), None, B, hh, ww, C, HW, 1, 4, st)
-        ph = torch.empty(B * HW, HW, dtype=torch.bfloat16, device=q.device)
-        pl = torch.empty_like(ph)
-        _call("muse_softmax_split_rows", _p(scores), _p(ph), _p(pl), None, B * HW, HW, scale, st)
-        vh, vl = planes(vt)       # per-image weights [B][C][HW keys]
-        _call("muse_conv2d_nhwc_tc", _p(ph), _p(pl), _p(vh), _p(vl), None, None, _p(out), None, B, hh, ww, HW, C, 1, 4, st)
+    if _tc_route(hh, ww, C, HW, 1) and _tc_route(hh, ww, HW, C, 1):
+        # exact: both products stay three-pass in the bf16 precision too, as the models' set_conv_precision promises
+        queries, keys = _split(q, st, exact=True), _split(k, st, exact=True)  # keys: per-image weights [B][HW keys][C]
+        _conv_tc(queries, keys, None, scores, B, hh, ww, C, HW, 1, CONV_TC_PER_IMAGE_WEIGHTS, st, exact=True)
+        probs = _new_planes(scores.shape, q.device, exact=True)
+        _call("muse_softmax_split_rows", _p(scores), _p(probs[0]), _p(probs[1]), None, B * HW, HW, scale, st)
+        values = _split(vt, st, exact=True)  # per-image weights [B][C][HW keys]
+        _conv_tc(probs, values, None, out, B, hh, ww, HW, C, 1, CONV_TC_PER_IMAGE_WEIGHTS, st, exact=True)
         return out
     kt = torch.empty(B, C, HW, dtype=torch.float32, device=q.device)
     _call("muse_transpose_batched", _p(k), _p(kt), B, HW, C, st)
     probs = torch.empty_like(scores)
     for b in range(B):  # SIMT weights are [K, Cout]: k_b^T for the scores, v_b for the output
         qb, sb = q[b * HW:(b + 1) * HW], scores[b * HW:(b + 1) * HW]
-        _call("muse_conv2d_nhwc", _p(qb), _p(kt[b]), None, None, _p(sb), 1, hh, ww, C, HW, 1, 0, st)
+        _call("muse_conv2d_nhwc", _p(qb), _p(kt[b]), None, None, _p(sb), 1, hh, ww, C, HW, 1, CONV_SAME, st)
     _call("muse_softmax_split_rows", _p(scores), None, None, _p(probs), B * HW, HW, scale, st)
     for b in range(B):
         pb, ob = probs[b * HW:(b + 1) * HW], out[b * HW:(b + 1) * HW]
-        _call("muse_conv2d_nhwc", _p(pb), _p(v[b * HW:(b + 1) * HW]), None, None, _p(ob), 1, hh, ww, HW, C, 1, 0, st)
+        _call("muse_conv2d_nhwc", _p(pb), _p(v[b * HW:(b + 1) * HW]), None, None, _p(ob), 1, hh, ww, HW, C, 1, CONV_SAME, st)
     return out
 
 
@@ -1007,38 +1000,6 @@ def image_to_uint8(x):
 _KERNELS_PER_CALL["muse_paella_resblock_spatial"] = 2
 
 
-def _cached_pack(tag, w, pack):
-    """pack(w) cached per live tensor w under `tag` (same keying as _packed_conv_weight)."""
-    import weakref
-
-    key = (w.data_ptr(), w._version, tuple(w.shape), w.device)
-    hit = _wk_cache.get((tag, id(w)))
-    if hit is not None and hit[0]() is w and hit[1] == key:
-        return hit[2]
-    out = pack(w.detach().float())
-    if len(_wk_cache) > 4096:
-        _wk_cache.clear()
-    _wk_cache[(tag, id(w))] = (weakref.ref(w), key, out)
-    return out
-
-
-def _planes(wk):
-    hi = wk.to(torch.bfloat16)
-    return hi, (wk - hi.float()).to(torch.bfloat16)
-
-
-def _tc_route(H, W, Cin, Cout, k):
-    return _conv_state["route"] != "simt" and bool(_lib.load().muse_conv2d_tc_supported(H, W, Cin, Cout, k))
-
-
-def _split(x, st):
-    hi = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    lo = _lo_like(hi)
-    B, H, W, C = x.shape
-    _call("muse_split_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, C, 0, st)
-    return hi, lo
-
-
 def paella_resblock(x, wk, bias, w1, b1, w2, b2, eps=1e-6):
     """Paella ResBlock (modeling_paella_vq.py:112-145) on fp32 NHWC x [B,H,W,C] with its gammas folded into the weights:
     wk fp32 [9, C] and bias [C] of the depthwise 3x3 (tap-major), w1 [4C, C, 1, 1] / b1 and w2 [C, 4C, 1, 1] / b2 of the
@@ -1051,25 +1012,21 @@ def paella_resblock(x, wk, bias, w1, b1, w2, b2, eps=1e-6):
     stats = torch.empty(2 * B * H * W, dtype=torch.float32, device=x.device)
     y = torch.empty_like(x)
     if _tc_route(H, W, C, Ch, 1) and _tc_route(H, W, Ch, C, 1):
-        n_hi = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-        n_lo = _lo_like(n_hi)
-        _call("muse_paella_resblock_spatial", _p(x), _p(wk), _p(bias), _p(stats), _p(x1), None, _p(n_hi), _p(n_lo), B, H, W,
+        n = _new_planes(x.shape, x.device)
+        _call("muse_paella_resblock_spatial", _p(x), _p(wk), _p(bias), _p(stats), _p(x1), None, _p(n[0]), _p(n[1]), B, H, W,
               C, float(eps), st)
-        g_hi = torch.empty(B, H, W, Ch, dtype=torch.bfloat16, device=x.device)
-        g_lo = _lo_like(g_hi)
-        w1h, w1l = _packed_conv_weight_split(w1)
-        _call("muse_conv2d_nhwc_tc_gelu_split", _p(n_hi), _p(n_lo), _p(w1h), _p(w1l), _p(b1), _p(g_hi), _p(g_lo), B, H, W, C,
-              Ch, 1, _tc_mode(0), st)
-        w2h, w2l = _packed_conv_weight_split(w2)
-        _call("muse_conv2d_nhwc_tc", _p(g_hi), _p(g_lo), _p(w2h), _p(w2l), _p(b2), _p(x1), _p(y), None, B, H, W, Ch, C, 1,
-              _tc_mode(0), st)
+        g = _new_planes((B, H, W, Ch), x.device)
+        _conv_tc(n, _cached_pack("tc", w1, _pack_tc), b1, g, B, H, W, C, Ch, 1, CONV_TC_SAME, st)
+        _conv_tc(g, _cached_pack("tc", w2, _pack_tc), b2, y, B, H, W, Ch, C, 1, CONV_TC_SAME, st, res=x1)
         return y
     n2 = torch.empty_like(x)
     _call("muse_paella_resblock_spatial", _p(x), _p(wk), _p(bias), _p(stats), _p(x1), _p(n2), None, None, B, H, W, C,
           float(eps), st)
     g = torch.empty(B, H, W, Ch, dtype=torch.float32, device=x.device)
-    _call("muse_conv2d_nhwc", _p(n2), _p(_packed_conv_weight(w1)), _p(b1), None, _p(g), B, H, W, C, Ch, 1, 8, st)
-    _call("muse_conv2d_nhwc", _p(g), _p(_packed_conv_weight(w2)), _p(b2), _p(x1), _p(y), B, H, W, Ch, C, 1, 0, st)
+    _call("muse_conv2d_nhwc", _p(n2), _p(_cached_pack("simt", w1, _pack_simt)), _p(b1), None, _p(g), B, H, W, C, Ch, 1,
+          CONV_GELU, st)
+    _call("muse_conv2d_nhwc", _p(g), _p(_cached_pack("simt", w2, _pack_simt)), _p(b2), _p(x1), _p(y), B, H, W, Ch, C, 1,
+          CONV_SAME, st)
     return y
 
 
@@ -1083,20 +1040,15 @@ def conv2d_unshuffle(x, w, bias=None):
     y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
     b = None if bias is None else bias.detach().float()
     if 4 * Cin <= 64 and _tc_route(H, W, 64, Cout, 1):
-        hi = torch.empty(B, H, W, 64, dtype=torch.bfloat16, device=x.device)
-        lo = _lo_like(hi)
-        _call("muse_im2col_split_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, 2, st)
-        w_hi, w_lo = _packed_conv_weight_split_stem(w)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, 64, Cout, 1,
-              _tc_mode(0), st)
+        _conv_tc(_im2col(x, H, W, 2, st), _cached_pack("stem", w, _pack_stem), b, y, B, H, W, 64, Cout, 1, CONV_TC_SAME, st)
         return y
-    wk = _cached_pack("unshuffle", w, lambda wf: wf.view(Cout, Cin, 2, 2).permute(2, 3, 1, 0).reshape(-1, Cout).contiguous())
-    _call("muse_conv2d_nhwc", _p(x), _p(wk), _p(b), None, _p(y), B, H, W, Cin, Cout, 2, 2, st)
+    wk = _cached_pack("unshuffle", w, lambda wf: _pack_simt(wf.view(Cout, Cin, 2, 2)))
+    _call("muse_conv2d_nhwc", _p(x), _p(wk), _p(b), None, _p(y), B, H, W, Cin, Cout, 2, CONV_STRIDE2, st)
     return y
 
 
 def _pack_s2p1(wf):
-    """Conv2d(4, 2, 1) weight [Cout, Cin, 4, 4] -> [Cout, 9 taps * 4 * Cin] for a 3x3 pad-1 convolution over the
+    """Conv2d(4, 2, 1) weight [Cout, Cin, 4, 4] -> bf16 planes [Cout, 9 taps * 4 * Cin] for a 3x3 pad-1 convolution over the
     space-to-depth grid: tap (a, b) and plane (p, q) hold w[:, :, 2a + p - 1, 2b + q - 1] (zero outside 0..3)."""
     Cout, Cin = wf.shape[0], wf.shape[1]
     wk = torch.zeros(Cout, 3, 3, 2, 2, Cin, dtype=torch.float32, device=wf.device)  # [co, a, b, p, q, ci]
@@ -1118,15 +1070,11 @@ def conv2d_s2p1(x, w, bias=None):
     H, W, Cout = Hi // 2, Wi // 2, w.shape[0]
     y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
     b = None if bias is None else bias.detach().float()
-    if (4 * Cin) % 64 == 0 and _tc_route(H, W, 4 * Cin, Cout, 3):
-        hi = torch.empty(B, H, W, 4 * Cin, dtype=torch.bfloat16, device=x.device)
-        lo = _lo_like(hi)
-        _call("muse_split_s2d_bf16_nhwc", _p(x), _p(hi), _p(lo), B, H, W, Cin, st)
-        w_hi, w_lo = _cached_pack("s2p1", w, _pack_s2p1)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, 4 * Cin, Cout, 3,
-              _tc_mode(0), st)
+    if _tc_route(H, W, 4 * Cin, Cout, 3):
+        _conv_tc(_split_s2d(x, st), _cached_pack("s2p1", w, _pack_s2p1), b, y, B, H, W, 4 * Cin, Cout, 3, CONV_TC_SAME, st)
         return y
-    _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), None, _p(y), B, H, W, Cin, Cout, 4, 3, st)
+    _call("muse_conv2d_nhwc", _p(x), _p(_cached_pack("simt", w, _pack_simt)), _p(b), None, _p(y), B, H, W, Cin, Cout, 4,
+          CONV_S2P1, st)
     return y
 
 
@@ -1143,20 +1091,18 @@ def _pack_transpose_parities(wf):
 
 def conv_transpose2d_s2(x, w, bias=None):
     """nn.ConvTranspose2d(k=4, s=2, p=1) on fp32 NHWC [B,H,W,Cin] with w [Cin, Cout, 4, 4] -> [B,2H,2W,Cout]: four 2x2
-    parity convolutions of the input (the upsample mode of muse_conv2d_nhwc_tc, or mode 4 of the SIMT kernel)."""
+    parity convolutions of the input (MUSE_CONV_TC_UPSAMPLE2X, or MUSE_CONV_TRANSPOSE_S2 of the SIMT kernel)."""
     st = _prep(x)
     B, Hi, Wi, Cin = x.shape
     H, W, Cout = 2 * Hi, 2 * Wi, w.shape[1]
     y = torch.empty(B, H, W, Cout, dtype=torch.float32, device=x.device)
     b = None if bias is None else bias.detach().float()
-    if _conv_state["route"] != "simt" and _lib.load().muse_conv2d_tc_tiles_per_image(H, W, Cin, Cout, 3, 1) > 0:
-        hi, lo = _split(x, st)
-        w_hi, w_lo = _cached_pack("convT", w, lambda wf: _planes(_pack_transpose_parities(wf).reshape(4 * Cout, -1).contiguous()))
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, Cin, Cout, 3,
-              _tc_mode(1), st)
+    if _tc_route(H, W, Cin, Cout, 3, upsample2x=True):
+        wk = _cached_pack("convT", w, lambda wf: _planes(_pack_transpose_parities(wf).reshape(4 * Cout, -1).contiguous()))
+        _conv_tc(_split(x, st), wk, b, y, B, H, W, Cin, Cout, 3, CONV_TC_UPSAMPLE2X, st)
         return y
     wk = _cached_pack("convT_simt", w, lambda wf: _pack_transpose_parities(wf).transpose(1, 2).contiguous())
-    _call("muse_conv2d_nhwc", _p(x), _p(wk), _p(b), None, _p(y), B, H, W, Cin, Cout, 4, 4, st)
+    _call("muse_conv2d_nhwc", _p(x), _p(wk), _p(b), None, _p(y), B, H, W, Cin, Cout, 4, CONV_TRANSPOSE_S2, st)
     return y
 
 
@@ -1169,10 +1115,8 @@ def conv1x1_pixel_shuffle(x, w, bias=None):
     y = torch.empty(B, 2 * H, 2 * W, Cout // 4, dtype=torch.float32, device=x.device)
     b = None if bias is None else bias.detach().float()
     if _tc_route(H, W, Cin, Cout, 1):
-        hi, lo = _split(x, st)
-        w_hi, w_lo = _packed_conv_weight_split(w)
-        _call("muse_conv2d_nhwc_tc", _p(hi), _p(lo), _p(w_hi), _p(w_lo), _p(b), None, _p(y), None, B, H, W, Cin, Cout, 1,
-              _tc_mode(16), st)
+        _conv_tc(_split(x, st), _cached_pack("tc", w, _pack_tc), b, y, B, H, W, Cin, Cout, 1, CONV_TC_PIXEL_SHUFFLE, st)
         return y
-    _call("muse_conv2d_nhwc", _p(x), _p(_packed_conv_weight(w)), _p(b), None, _p(y), B, H, W, Cin, Cout, 1, 16, st)
+    _call("muse_conv2d_nhwc", _p(x), _p(_cached_pack("simt", w, _pack_simt)), _p(b), None, _p(y), B, H, W, Cin, Cout, 1,
+          CONV_PIXEL_SHUFFLE, st)
     return y
