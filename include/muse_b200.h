@@ -7,7 +7,9 @@
  *   - enqueue work on that stream and return immediately (asynchronous, like the torch ops);
  *   - allocate nothing: scratch and outputs are caller-provided;
  *   - return 0 (MUSE_OK) or a non-zero status; muse_last_error() gives the message (thread-local).
- * Dtype codes: 0 = float32, 1 = bfloat16.  "bf16" pointers are 16-bit bfloat16 arrays.
+ * Dtype codes: 0 = float32, 1 = bfloat16, 2 = float8 e4m3 (output of the FP8 producers only, each row stored as
+ * e4m3_rn_satfinite(y / s) with s = amax(|y| over the row) / 448, or 1 for an all-zero row, written to row_scale[row]).
+ * "bf16" pointers are 16-bit bfloat16 arrays.
  * Dropout (nn.Dropout(p) in training mode) is fused into the ops that take `bits`; bits == NULL means no dropout.  Keep
  * masks come from Philox4x32-10 keyed by the 64-bit seed at *seed (device memory, so a captured graph draws a fresh seed per
  * replay) with a per-forward unique site id; the mapping from (seed, site, coordinates) to bits and the rate (p_eff =
@@ -27,7 +29,7 @@ extern "C" {
 #define MUSE_ERR_CUDA 2
 #define MUSE_ERR_UNSUPPORTED 3
 
-#define MUSE_B200_ABI_VERSION 10
+#define MUSE_B200_ABI_VERSION 11
 
 /* library / device plumbing */
 int muse_abi_version(void);
@@ -68,6 +70,14 @@ int muse_get_pdl(void);
  * through the a_mn/b_mn views, their autograd dgrad / wgrad matmuls. */
 int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int M, int N, int K, int lda, int ldb,
                    int ldc, int a_mn, int b_mn, int epilogue, void* stream);
+
+/* FP8 forward GEMM (inference): C bf16 [M,N] (pitch ldc) = bf16(sum_k A[m,k] B[n,k] * sa[m] * sb[n]), A e4m3 row-major
+ * [M,K] (pitch lda bytes), B e4m3 row-major [N,K] (pitch ldb bytes), sa fp32 [M], sb fp32 [N] (8-byte aligned); fp32
+ * accumulation with each 128-wide k-block's partial sum promoted into fp32 registers.  N and ldc multiples of 8; lda / ldb
+ * multiples of 16.  The e4m3 producers: muse_add_norm_mod_fwd, muse_dwconv3x3_norm_fwd, muse_glu_fwd (dtype code 2) and
+ * muse_quantize_rows_e4m3. */
+int muse_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
+                  int ldb, int ldc, void* stream);
 
 /* Weight-gradient GEMM with a run-to-run reproducible result: C fp32 [M,N] = opA(A) * opB(B)^T split over K (= tokens) so
  * that the few output tiles fill the SMs; every split stores its partial tile into `ws` and a second kernel sums the
@@ -161,11 +171,12 @@ int muse_norm2_bwd(const void* d_h2, const float* x2, const float* w2, const flo
                    const float* dres, const void* a, const float* w1, const float* mean1, const float* rstd1, float* dx2,
                    void* d_a, float* dw2, float* dw1, float* ws, int rows, int H, int rms1, int rms2, void* stream);
 
-/* GLU of FeedForward (:789-792): ab bf16 [rows, 2I] = [wi_0(x) | wi_1(x)], out bf16 [rows, I] = gelu(a) * b.
- * bits (nullable): FeedForward.dropout (:797) fused into the pass (the model without the mid norm): out is the dropped
- * output, bits [rows, ceil(I / 32)] written; the backward scales dout by them as it reads it. */
-int muse_glu_fwd(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
-                 long long rows, int I, void* stream);
+/* GLU of FeedForward (:789-792): ab bf16 [rows, 2I] = [wi_0(x) | wi_1(x)], out [rows, I] = gelu(a) * b.
+ * out_dtype 1: bf16.  out_dtype 2: e4m3 with its scales in row_scale fp32 [rows] (required then; a warp per row, I <= 4096;
+ * no dropout).  bits (nullable): FeedForward.dropout (:797) fused into the pass (the model without the mid norm): out is
+ * the dropped output, bits [rows, ceil(I / 32)] written; the backward scales dout by them as it reads it. */
+int muse_glu_fwd(const void* ab, void* out, int out_dtype, float* row_scale, unsigned int* bits,
+                 const unsigned long long* seed, int site, float p, long long rows, int I, void* stream);
 int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
                  void* stream);
 
@@ -208,14 +219,17 @@ int muse_ce_bwd(const void* logits, const long long* labels, const float* lse, c
  * in TransformerLayer / GLUFeedForward (:757-792, :926-951, AdaLNModulation :1025-1037):
  *   r_out = a + r (r NULL: r_out = a; r_out NULL: not stored);  y = norm(r_out) * w  [* (1 + scale_b) + shift_b].
  * scale_shift (nullable) fp32: scale of sample b at [b*ss_stride, +H), shift at [b*ss_stride + H, +H); a row belongs to
- * sample row / rows_per_sample.  H <= 1024, H % 8 == 0. */
+ * sample row / rows_per_sample.  H <= 1024, H % 8 == 0.  y_dtype 2: y is e4m3 with its scales in row_scale fp32 [rows]
+ * (required then, ignored otherwise): the A operand of muse_gemm_fp8. */
 int muse_add_norm_mod_fwd(const void* a, int a_dtype, const float* r, const float* w, const float* scale_shift,
-                          long long ss_stride, int rows_per_sample, float* r_out, void* y, int y_dtype, int rows, int H,
-                          float eps, int rms, void* stream);
+                          long long ss_stride, int rows_per_sample, float* r_out, void* y, int y_dtype, float* row_scale,
+                          int rows, int H, float eps, int rms, void* stream);
 /* ResBlock head (:604-612): depthwise 3x3 'same' conv (groups = C, no bias; output rounded to bf16 like the autocast conv)
- * + Norm2D over channels.  x fp32 [B,h,w,C] token-major, wk fp32 [9, C] (tap-major), norm_w fp32 [C] or NULL -> y bf16. */
-int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* norm_w, void* y, void* conv_out, int B, int h,
-                            int w, int C, float eps, int rms, void* stream);  /* conv_out (nullable) bf16: saved for bwd */
+ * + Norm2D over channels.  x fp32 [B,h,w,C] token-major, wk fp32 [9, C] (tap-major), norm_w fp32 [C] or NULL -> y of
+ * y_dtype 1 (bf16) or 2 (e4m3, one scale per pixel in row_scale fp32 [B*h*w], required then). */
+int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* norm_w, void* y, int y_dtype, float* row_scale,
+                            void* conv_out, int B, int h, int w, int C, float eps, int rms, void* stream);
+                            /* conv_out (nullable) bf16: saved for bwd */
 /* nn.GELU + GlobalResponseNorm (:741-751) on x bf16 [B, HW, C]: g = gelu(x), Gx = ||g||_2 over the HW tokens,
  * Nx = Gx / (mean_c Gx + 1e-6), out = gamma * (g * Nx) + beta + g (bf16).  sumsq_ws (Gx^2) and nx_ws: fp32 [B, C],
  * left filled for muse_grn_bwd.  bits (nullable): the ResBlock's nn.Dropout between GlobalResponseNorm and channelwise[4]
@@ -224,6 +238,11 @@ int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* norm_w
 int muse_grn_fwd(const void* x, const float* gamma, const float* beta, void* out, float* sumsq_ws, float* nx_ws,
                  unsigned int* bits, const unsigned long long* seed, int site, float p, int B, int HW, int C,
                  void* stream);
+/* Per-row e4m3 quantization of a bf16 matrix x [rows, K] (pitch ldx elements): s[r] = amax(|x[r,:]|) / 448 (1 for an
+ * all-zero row), q[r,k] = e4m3_rn_satfinite(x[r,k] / s[r]) (pitch ldq bytes).  K, ldx, ldq multiples of 8, x 16-byte and
+ * q 8-byte aligned.  The weight operands of muse_gemm_fp8, one
+ * scale per output row; graph-capturable, so the FP8 copies can be refreshed after an optimizer step. */
+int muse_quantize_rows_e4m3(const void* x, int ldx, void* q, int ldq, float* scale, int rows, int K, void* stream);
 /* AdaLNModulation at the end of a ResBlock (:617): x fp32 [B*rows_per_sample, C] *= (1 + scale_b), += shift_b, in place. */
 int muse_adaln_apply(float* x, const float* scale_shift, long long ss_stride, int B, int rows_per_sample, int C,
                      void* stream);

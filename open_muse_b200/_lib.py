@@ -26,6 +26,8 @@ SIGNATURES = {
     "muse_set_pdl": (c_int, [_I]),
     "muse_get_pdl": (c_int, []),
     "muse_gemm_bf16": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "muse_gemm_fp8": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "muse_quantize_rows_e4m3": (c_int, [_P, _I, _P, _I, _P, _I, _I, _P]),
     "muse_gemm_splitk_workspace_bytes": (c_longlong, [_I, _I, _I]),
     "muse_gemm_bf16_splitk": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
     "muse_pack_bf16": (c_int, [_P, _I, _L, _P]),
@@ -41,7 +43,7 @@ SIGNATURES = {
     "muse_norm_bwd_workspace_floats": (c_longlong, [_I, _I, _I]),
     "muse_norm2_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _F, _I, _I, _P]),
     "muse_norm2_bwd": (c_int, [_P] * 15 + [_I, _I, _I, _I, _P]),
-    "muse_glu_fwd": (c_int, [_P, _P, _P, _P, _I, _F, _L, _I, _P]),
+    "muse_glu_fwd": (c_int, [_P, _P, _I, _P, _P, _P, _I, _F, _L, _I, _P]),
     "muse_glu_bwd": (c_int, [_P, _P, _P, _F, _P, _L, _I, _P]),
     "muse_attn_fwd": (c_int, [_P] * 7 + [_I, _F] + [_I] * 9 + [_F, _P]),
     "muse_attn_bwd": (c_int, [_P] * 6 + [_F] + [_P] * 4 + [_I] * 12 + [_F, _P]),
@@ -49,8 +51,8 @@ SIGNATURES = {
     "muse_dropout_bwd": (c_int, [_P, _P, _I, _P, _F, _L, _I, _P]),
     "muse_ce_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),
     "muse_ce_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),
-    "muse_add_norm_mod_fwd": (c_int, [_P, _I, _P, _P, _P, _L, _I, _P, _P, _I, _I, _I, _F, _I, _P]),
-    "muse_dwconv3x3_norm_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
+    "muse_add_norm_mod_fwd": (c_int, [_P, _I, _P, _P, _P, _L, _I, _P, _P, _I, _P, _I, _I, _F, _I, _P]),
+    "muse_dwconv3x3_norm_fwd": (c_int, [_P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
     "muse_grn_fwd": (c_int, [_P] * 8 + [_I, _F, _I, _I, _I, _P]),
     "muse_add_norm_mod_bwd": (c_int, [_P, _I, _P, _P, _P, _P, _L, _I, _P, _I, _P, _P, _P, _I, _I, _F, _I, _P]),
     "muse_dwconv3x3_norm_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
@@ -81,7 +83,7 @@ SIGNATURES = {
     "muse_transpose_batched": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 # the mode argument of muse_conv2d_nhwc (enum muse_conv_mode): one geometry plus flags
 CONV_SAME, CONV_UPSAMPLE2X, CONV_STRIDE2, CONV_S2P1, CONV_TRANSPOSE_S2 = 0, 1, 2, 3, 4

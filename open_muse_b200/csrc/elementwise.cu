@@ -1,11 +1,14 @@
 // HBM-bound elementwise / gather kernels of the transformer step:
 //   * multi-tensor fp32 -> bf16 weight packing (one launch for all Linear weights of a model)
 //   * token + position embedding gather (muse/modeling_transformer.py:942-957) and its backward
-//   * GLU: gelu(a) * b (muse/modeling_transformer.py:789-792) forward / backward
+//   * GLU: gelu(a) * b (muse/modeling_transformer.py:789-792) forward / backward; its e4m3 form (a warp per row, which the
+//     row's scale needs) writes the wo operand of the FP8 GEMM
+//   * per-row e4m3 quantization of the bf16 weight operands of the FP8 GEMM
 //   * plain fp32 -> bf16 cast (gradient of the residual stream entering a dgrad GEMM)
 //   * nn.Dropout of the embedding output and of the FFN hidden state (keep bits of philox.cuh) and its backward
 #include "common.cuh"
 #include "philox.cuh"
+#include "row_norm.cuh"
 
 namespace muse {
 namespace {
@@ -360,6 +363,64 @@ dropout_bwd_kernel(const T* dy, T* dx, const uint8_t* __restrict__ bits, float s
   store8(dx + r * cols + 8 * k, v);
 }
 
+// e4m3 GLU: one warp per row holds gelu(a) * b (the fp32 value the bf16 form rounds) as a register row, then stores it
+// with row_store_e4m3.  ab bf16 [rows, 2I], q [rows, I] bytes, row_scale fp32 [rows].
+constexpr int kGluRowWarps = 4;
+template <int CH>
+__global__ void __launch_bounds__(kGluRowWarps * 32)
+glu_fwd_e4m3_kernel(const bf16* __restrict__ ab, uint8_t* __restrict__ q, float* __restrict__ row_scale, long long rows,
+                    int I) {
+  pdl_enter();
+  const int lane = threadIdx.x & 31;
+  const long long r = static_cast<long long>(blockIdx.x) * kGluRowWarps + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  float v[CH][8];
+  row_load(v, I, lane, [&](int col, float (&vc)[8]) {
+    float b[8];
+    load8(ab + r * 2 * I + col, vc);
+    load8(ab + r * 2 * I + I + col, b);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) vc[j] = bf16_round(gelu_f(vc[j])) * b[j];
+  });
+  row_store_e4m3(v, I, lane, q + r * I, row_scale + r);
+}
+
+// Per-row e4m3 quantization, one warp per row, 8 elements (16 bytes in, 8 bytes out) per lane and access: the row's
+// amax over |x| first, then q = e4m3_rn_satfinite(x / s) on a second read of the row (from L1 / L2).
+__global__ void __launch_bounds__(256)
+quantize_rows_e4m3_kernel(const bf16* __restrict__ x, int ldx, uint8_t* __restrict__ q, int ldq, float* __restrict__ scale,
+                          int rows, int K) {
+  pdl_enter();
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  const bf16* xr = x + static_cast<size_t>(r) * ldx;
+  float amax = 0.f;
+  for (int k = lane * 8; k < K; k += 256) {
+    float v[8];
+    load8(xr + k, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(v[j]));
+  }
+  amax = warp_max(amax);
+  const float s = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+  if (lane == 0) scale[r] = s;
+  uint8_t* qr = q + static_cast<size_t>(r) * ldq;
+  for (int k = lane * 8; k < K; k += 256) {
+    float v[8];
+    load8(xr + k, v);
+    uint32_t w[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float* e = &v[4 * h];
+      const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(e[0], s), __fdiv_rn(e[1], s)), __NV_SATFINITE, __NV_E4M3);
+      const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(e[2], s), __fdiv_rn(e[3], s)), __NV_SATFINITE, __NV_E4M3);
+      w[h] = lo | (hi << 16);
+    }
+    *reinterpret_cast<uint2*>(qr + k) = make_uint2(w[0], w[1]);
+  }
+}
+
 }  // namespace
 }  // namespace muse
 
@@ -482,16 +543,44 @@ int muse_embed_bwd_sorted(const long long* order, const long long* bounds, const
 }
 
 // bits == nullptr: no dropout; else FeedForward.dropout fused into the pass, bits [rows, ceil(I / 32)] written.
-int muse_glu_fwd(const void* ab, void* out, unsigned int* bits, const unsigned long long* seed, int site, float p,
-                 long long rows, int I, void* stream) {
+int muse_glu_fwd(const void* ab, void* out, int out_dt, float* row_scale, unsigned int* bits, const unsigned long long* seed,
+                 int site, float p, long long rows, int I, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (I % 8 != 0) { set_last_error("glu_fwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
   if (bits != nullptr && seed == nullptr) { set_last_error("glu_fwd: dropout needs a seed"); return MUSE_ERR_INVALID; }
+  if (out_dt != 1 && out_dt != 2) { set_last_error("glu_fwd: out dtype code %d (bf16 = 1 or e4m3 = 2)", out_dt); return MUSE_ERR_INVALID; }
+  if (out_dt == 2) {
+    if (row_scale == nullptr || bits != nullptr || I > 4096) {
+      set_last_error("glu_fwd: the e4m3 output needs row_scale, takes no dropout and I <= 4096 (I = %d)", I);
+      return MUSE_ERR_INVALID;
+    }
+    if (rows <= 0) return MUSE_OK;
+    const unsigned grid = static_cast<unsigned>(ceil_div_ll(rows, kGluRowWarps));
+    with_row_chunks<1, 2, 4, 8, 12, 16>(I, [&](auto ch) {
+      pdl_launch(grid, kGluRowWarps * 32, 0, s)(glu_fwd_e4m3_kernel<decltype(ch)::value>, reinterpret_cast<const bf16*>(ab),
+                                                reinterpret_cast<uint8_t*>(out), row_scale, rows, I);
+    });
+    return check_launch("glu_fwd_e4m3");
+  }
   const long long n = rows * (I / 8);
   if (n <= 0) return MUSE_OK;
   pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? glu_fwd_kernel<true> : glu_fwd_kernel<false>,
       reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, philox::elem_drop(bits, seed, site, p, I));
   return check_launch("glu_fwd");
+}
+
+int muse_quantize_rows_e4m3(const void* x, int ldx, void* q, int ldq, float* scale, int rows, int K, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (rows <= 0 || K <= 0) return MUSE_OK;
+  if (ldx < K || ldq < K) { set_last_error("quantize_rows_e4m3: pitches %d / %d below K = %d", ldx, ldq, K); return MUSE_ERR_INVALID; }
+  if (K % 8 != 0 || ldx % 8 != 0 || ldq % 8 != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0 ||
+      (reinterpret_cast<uintptr_t>(q) & 7) != 0) {
+    set_last_error("quantize_rows_e4m3: K, ldx and ldq must be multiples of 8, x 16-byte and q 8-byte aligned");
+    return MUSE_ERR_INVALID;
+  }
+  pdl_launch(ceil_div(rows, 8), 256, 0, s)(quantize_rows_e4m3_kernel, reinterpret_cast<const bf16*>(x), ldx,
+                                           reinterpret_cast<uint8_t*>(q), ldq, scale, rows, K);
+  return check_launch("quantize_rows_e4m3");
 }
 
 // bits: those muse_glu_fwd wrote (nullptr: no dropout); dout is scaled by them as it is read.

@@ -11,6 +11,9 @@
 // warpgroup's next tile runs its MMAs; the producer runs up to a ring's worth of k-blocks ahead, so it keeps loading the
 // next tile meanwhile.  The atomic epilogue adds straight from the accumulator registers.
 //
+// FP8 (muse_gemm_fp8, inference): A and B e4m3, both K-major, with fp32 scales per row of A and per row of B (= column
+// of C); the same pipeline with k32 e4m3 MMAs, and the bf16 epilogue stores bf16(acc * sa[m] * sb[n]).
+//
 // Operand "major-ness": an operand is K-major when the reduction dim is contiguous in memory
 // (activations X[T,K], weights W[N,K] in forward) and MN-major when the M/N dim is contiguous
 // (W[N,K] used as the B operand of dgrad; dY[T,N] and X[T,K] as operands of wgrad, where the
@@ -31,21 +34,25 @@ using tc::BM;
 // EPI_SPLITK_F32: deterministic split-K.  Every split stores its fp32 partial tile into a workspace and a second, fully
 // parallel kernel sums the partials in split order and STORES the result, so the output needs no zero fill and is
 // bit-identical from run to run (the atomic variant is order-dependent).
-enum Epi { EPI_BF16 = 0, EPI_F32 = 1, EPI_ATOMIC_F32 = 2, EPI_RESADD_F32 = 3, EPI_SPLITK_F32 = 4 };
+// EPI_FP8_BF16: e4m3 operands (muse_gemm_fp8 only), C bf16 = acc * sa[row] * sb[col].
+enum Epi { EPI_BF16 = 0, EPI_F32 = 1, EPI_ATOMIC_F32 = 2, EPI_RESADD_F32 = 3, EPI_SPLITK_F32 = 4, EPI_FP8_BF16 = 5 };
+
 
 // Epilogue staging buffer: 64 rows x 128 B (a chunk of 64 bf16 or 32 fp32 columns of a warpgroup's half tile), laid out
 // with the 128-byte swizzle of the output tensor map.  Two per consumer warpgroup, then one mbarrier per buffer for the
 // residual loads of EPI_RESADD_F32.
 constexpr int kEpiBuf = 64 * 128;
 
-template <int BN>
-using Ring = tc::Ring<BN, (BN == 256) ? 4 : 6, 4 * kEpiBuf + 4 * 8>;
+template <int BN, typename T = bf16>
+using Ring = tc::Ring<BN, (BN == 256) ? 4 : 6, 4 * kEpiBuf + 4 * 8, T>;
 
 struct GemmParams {
   void* C;  // EPI_ATOMIC_F32 only; the other epilogues store through the output tensor map
   int M, N, K;
   int ldc;
   int num_m, num_n, num_kb, kb_per_split, splits;
+  const float* sa;  // EPI_FP8_BF16: scales of the rows of A [M] and of B [N]
+  const float* sb;
 };
 
 // tmC: the output, box {128 B of columns, 64 rows}: C [M, N] (pitch ldc), or for split-K partial tiles the workspace
@@ -56,7 +63,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
-  Ring<BN> ring(smem_raw);
+  constexpr bool kFp8 = EPI == EPI_FP8_BF16;
+  using R = Ring<BN, std::conditional_t<kFp8, __nv_fp8_e4m3, bf16>>;
+  constexpr int kBK = R::kBK;
+  R ring(smem_raw);
 
   const int wg = threadIdx.x >> 7;
 
@@ -91,14 +101,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int kb = kb0; kb < kb1; ++kb) {
           const auto s = ring.produce();
           if (!A_MN) {
-            ptx::tma_load_2d(s.a, &tmA, s.bar, kb * BK, m0);
+            ptx::tma_load_2d(s.a, &tmA, s.bar, kb * kBK, m0);
           } else {
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i)
               ptx::tma_load_2d(s.a + i * (BK * 128), &tmA, s.bar, m0 + i * 64, kb * BK);
           }
           if (!B_MN) {
-            ptx::tma_load_2d(s.b, &tmB, s.bar, kb * BK, n0);
+            ptx::tma_load_2d(s.b, &tmB, s.bar, kb * kBK, n0);
           } else {
 #pragma unroll
             for (int i = 0; i < BN / 64; ++i)
@@ -118,7 +128,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint64_t* rbar = reinterpret_cast<uint64_t*>(ring.extra() + 4 * kEpiBuf) + 2 * half;
     // A chunk is 128 B of each of the 64 rows; chunk q goes through buffer q & 1.  Every epilogue has an even number of
     // chunks per tile, so each tile starts on buffer 0 and the residual barriers on phase 0.
-    constexpr bool kF32 = EPI != EPI_BF16;
+    constexpr bool kF32 = EPI != EPI_BF16 && !kFp8;
     constexpr int kCols = kF32 ? 32 : 64;
     constexpr int kChunks = BN / kCols;
     constexpr int kJ = kCols / 8;  // 8-column fragment groups per chunk
@@ -143,7 +153,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           ptx::tma_load_2d(ebuf + b * kEpiBuf, &tmR, &rbar[b], ocol + b * kCols, orow);
         }
       }
-      ring.template consume<A_MN, B_MN>(acc, kb0, kb1, half);
+      if constexpr (kFp8) {
+        // the e4m3 MMA keeps fewer accumulator bits than fp32: each k-block's partial sum is promoted into the fp32
+        // registers of acc (DESIGN.md section 4 has the measurement with and without)
+        float part[BN / 2];
+        ring.consume_promoted(acc, part, kb0, kb1, half);
+      } else {
+        ring.template consume<A_MN, B_MN>(acc, kb0, kb1, half);
+      }
+      float sx[2] = {1.f, 1.f};  // EPI_FP8_BF16: scales of the thread's rows fr and fr + 8 (0 past M)
+      if constexpr (kFp8) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int grow = orow + fr + 8 * hr;
+          sx[hr] = grow < p.M ? p.sa[grow] : 0.f;
+        }
+      }
       if constexpr (EPI == EPI_ATOMIC_F32) {
         // ---------------------------------------------------------- fp32 atomics straight from the accumulator registers
         const int lr = half * 64 + fr;
@@ -173,9 +198,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
           for (int jj = 0; jj < kJ; ++jj) {
             const int j = q * kJ + jj;
+            float2 sw = make_float2(1.f, 1.f);  // EPI_FP8_BF16: scales of columns lc, lc + 1 of this 8-column group
+            if constexpr (kFp8) {
+              const int gcol = ocol + q * kCols + 8 * jj + lc;  // N % 8 == 0: both columns are inside or both past N
+              sw = gcol < p.N ? *reinterpret_cast<const float2*>(p.sb + gcol) : make_float2(0.f, 0.f);
+            }
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr) {
-              const float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+              float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+              if constexpr (kFp8) {
+                v0 = v0 * sx[hr] * sw.x;
+                v1 = v1 * sx[hr] * sw.y;
+              }
               const int r = fr + 8 * hr;
               // 16-byte unit u of row r sits at unit u ^ (r & 7): the 128-byte swizzle, so the 8 rows of a warp's store
               // fall into different banks
@@ -247,10 +281,11 @@ struct GemmMaps {
 template <int BN, bool A_MN, bool B_MN, int EPI>
 int launch(const GemmMaps& m, const GemmParams& p, cudaStream_t stream) {
   constexpr auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI>;
-  if (int rc = set_max_dynamic_smem<kern>(Ring<BN>::kSmemBytes)) return rc;
+  constexpr int kSmem = Ring<BN>::kSmemBytes;  // the same for both operand types
+  if (int rc = set_max_dynamic_smem<kern>(kSmem)) return rc;
   const int total = p.num_m * p.num_n * p.splits;
   const int grid = total < num_sms() ? total : num_sms();
-  pdl_launch(grid, tc::kThreads, Ring<BN>::kSmemBytes, stream)(kern, m.a, m.b, m.c, m.r, p);
+  pdl_launch(grid, tc::kThreads, kSmem, stream)(kern, m.a, m.b, m.c, m.r, p);
   return check_launch("gemm_wgmma");
 }
 
@@ -337,6 +372,7 @@ static int gemm_tc(const void* A, const void* B, void* C, const float* res, int 
   p.num_kb = ceil_div(K, BK);
   p.splits = 1;
   p.kb_per_split = p.num_kb;
+  p.sa = p.sb = nullptr;
   if (epi == EPI_ATOMIC_F32 || epi == EPI_SPLITK_F32) {
     int num_m, num_n, num_kb, bn;
     split_plan(M, N, K, &num_m, &num_n, &num_kb, &p.kb_per_split, &p.splits, &bn);
@@ -367,6 +403,40 @@ static int gemm_tc(const void* A, const void* B, void* C, const float* res, int 
   return check_launch("gemm splitk reduce");
 }
 
+// C bf16 [M,N] (ldc) = (A e4m3 [M,K] (lda) * diag(sa)) (B e4m3 [N,K] (ldb) * diag(sb))^T; pitches in elements = bytes.
+static int gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
+                    int ldb, int ldc, cudaStream_t stream) {
+  if (M <= 0 || N <= 0 || K <= 0) return MUSE_OK;
+  if (ldc % 8 != 0 || N % 8 != 0) {
+    set_last_error("gemm_fp8: N=%d and ldc=%d must be multiples of 8 (the TMA stores write whole 16-byte units)", N, ldc);
+    return MUSE_ERR_INVALID;
+  }
+  if ((reinterpret_cast<uintptr_t>(C) & 15) != 0 || sa == nullptr || sb == nullptr ||
+      (reinterpret_cast<uintptr_t>(sb) & 7) != 0) {
+    set_last_error("gemm_fp8: C must be 16B aligned and the scales given, sb 8B aligned");
+    return MUSE_ERR_INVALID;
+  }
+  constexpr int BN = 128;
+  constexpr int kBK = Ring<BN, __nv_fp8_e4m3>::kBK;
+  GemmMaps m;
+  int rc;
+  if ((rc = make_tmap(&m.a, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_UINT8, A, {K, M}, {1LL * lda}, {kBK, BM}))) return rc;
+  if ((rc = make_tmap(&m.b, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_UINT8, B, {K, N}, {1LL * ldb}, {kBK, BN}))) return rc;
+  if ((rc = make_tmap(&m.c, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, C, {N, M}, {2LL * ldc}, {64, 64}))) return rc;
+  m.r = m.c;
+  GemmParams p;
+  p.C = C;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc;
+  p.num_m = ceil_div(M, BM);
+  p.num_n = ceil_div(N, BN);
+  p.num_kb = ceil_div(K, kBK);
+  p.splits = 1;
+  p.kb_per_split = p.num_kb;
+  p.sa = sa;
+  p.sb = sb;
+  return launch<BN, false, false, EPI_FP8_BF16>(m, p, stream);
+}
+
 }  // namespace muse
 
 using namespace muse;
@@ -386,6 +456,11 @@ int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int 
   if (epilogue == MUSE_EPI_RESADD_F32 && res == nullptr) { set_last_error("gemm: RESADD epilogue needs res"); return MUSE_ERR_INVALID; }
   if (epilogue == MUSE_EPI_SPLITK_F32) { set_last_error("gemm: the deterministic split-K epilogue goes through muse_gemm_bf16_splitk"); return MUSE_ERR_INVALID; }
   return gemm_tc(A, B, C, res, M, N, K, lda, ldb, ldc, a_mn, b_mn, epilogue, static_cast<cudaStream_t>(stream), nullptr, 0);
+}
+
+int muse_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
+                  int ldb, int ldc, void* stream) {
+  return gemm_fp8(A, sa, B, sb, C, M, N, K, lda, ldb, ldc, static_cast<cudaStream_t>(stream));
 }
 
 long long muse_gemm_splitk_workspace_bytes(int M, int N, int K) {

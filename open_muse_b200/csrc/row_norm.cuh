@@ -2,8 +2,11 @@
 // One warp owns one row and holds it in registers as float v[CH][8]: chunk c of lane `lane` is the 8 columns starting at
 // row_col(c, lane), and chunks at or past H are zero.  Each helper fixes the order of its floating-point operations, so
 // every kernel built on them produces the same bits for the same row.  The GLU and wide streaming kernels of norm.cu
-// keep their own loops: they do not hold the row as floats (packed bf16 pairs, or no row at all).
+// keep their own loops: they do not hold the row as floats (packed bf16 pairs, or no row at all).  row_store_e4m3 writes
+// a finished row as the e4m3 operand of muse_gemm_fp8, which needs the row's absolute maximum before any element.
 #pragma once
+#include <cuda_fp8.h>
+
 #include <type_traits>
 
 #include "common.cuh"
@@ -65,6 +68,35 @@ __device__ __forceinline__ void row_bwd_sums(float inv_h, int rms, float& s1, fl
 }
 __device__ __forceinline__ float row_dx(float g, float xh, float s1, float s2, float rstd) {
   return rstd * (g - s1 - xh * s2);
+}
+
+// e4m3 form of a finished register row (chunks at or past H hold zeros): s = amax / 448, or 1 for an all-zero row;
+// q[col] = e4m3_rn_satfinite(v / s) with a correctly rounded division, s to row_scale[0] (lane 0).  q: the row's bytes.
+template <int CH>
+__device__ __forceinline__ void row_store_e4m3(const float (&v)[CH][8], int H, int lane, uint8_t* q, float* row_scale) {
+  float amax = 0.f;
+#pragma unroll
+  for (int c = 0; c < CH; ++c)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(v[c][j]));
+  amax = warp_max(amax);
+  const float s = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+  if (lane == 0) *row_scale = s;
+#pragma unroll
+  for (int c = 0; c < CH; ++c) {
+    const int col = row_col(c, lane);
+    if (col < H) {
+      uint32_t w[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float* x = &v[c][4 * h];
+        const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(x[0], s), __fdiv_rn(x[1], s)), __NV_SATFINITE, __NV_E4M3);
+        const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(x[2], s), __fdiv_rn(x[3], s)), __NV_SATFINITE, __NV_E4M3);
+        w[h] = lo | (hi << 16);
+      }
+      *reinterpret_cast<uint2*>(q + col) = make_uint2(w[0], w[1]);
+    }
+  }
 }
 
 // ---- host side

@@ -21,11 +21,12 @@ constexpr int kWarps = 4;
 // a: [rows, H] (TA = bf16 | float), r: fp32 [rows, H] or null, w: fp32 [H] or null,
 // ss: fp32, scale of sample b at ss[b * ss_stride + 0 .. H), shift at ss[b * ss_stride + H .. 2H); null -> no modulation
 // r_out: fp32 [rows, H] or null ; y: TY [rows, H]
-template <typename TA, typename TY, int CH>
+// F8: y is the e4m3 operand of muse_gemm_fp8 (TY = uint8_t) and row_scale [rows] its scales (row_store_e4m3).
+template <typename TA, typename TY, int CH, bool F8>
 __global__ void __launch_bounds__(kWarps * 32)
 add_norm_mod_kernel(const TA* __restrict__ a, const float* __restrict__ r, const float* __restrict__ w,
                     const float* __restrict__ ss, long long ss_stride, int rows_per_sample, float* __restrict__ r_out,
-                    TY* __restrict__ y, int rows, int H, float eps, int rms) {
+                    TY* __restrict__ y, int rows, int H, float eps, int rms, float* __restrict__ row_scale) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kWarps + (threadIdx.x >> 5);
@@ -63,16 +64,24 @@ add_norm_mod_kernel(const TA* __restrict__ a, const float* __restrict__ r, const
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = fmaf(o[j], 1.f + s8[j], h8[j]);
       }
-      store8(y + base + col, o);
+      if constexpr (F8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[c][j] = o[j];
+      } else {
+        store8(y + base + col, o);
+      }
     }
   }
+  if constexpr (F8) row_store_e4m3(v, H, lane, y + base, row_scale + row);
 }
 
 // x fp32 [B, hh, ww, C]; wk fp32 [9][C] (tap-major); nw fp32 [C] or null; y bf16 [B, hh, ww, C].  One warp per pixel.
-template <int CH>
+// F8: y is e4m3 (TY = uint8_t) with one scale per pixel in row_scale (row_store_e4m3).
+template <int CH, bool F8, typename TY = bf16>
 __global__ void __launch_bounds__(kWarps * 32)
 dwconv3x3_norm_kernel(const float* __restrict__ x, const float* __restrict__ wk, const float* __restrict__ nw,
-                      bf16* __restrict__ y, bf16* __restrict__ conv_out, int B, int hh, int ww, int C, float eps, int rms) {
+                      TY* __restrict__ y, bf16* __restrict__ conv_out, int B, int hh, int ww, int C, float eps, int rms,
+                      float* __restrict__ row_scale) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const long long pix = static_cast<long long>(blockIdx.x) * kWarps + (threadIdx.x >> 5);
@@ -109,9 +118,15 @@ dwconv3x3_norm_kernel(const float* __restrict__ x, const float* __restrict__ wk,
       if (nw) load8(nw + col, wv);
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean) * rstd * (nw ? wv[j] : 1.f);
-      store8(y + pix * C + col, o);
+      if constexpr (F8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[c][j] = o[j];
+      } else {
+        store8(y + pix * C + col, o);
+      }
     }
   }
+  if constexpr (F8) row_store_e4m3(v, C, lane, y + pix * C, row_scale + pix);
 }
 
 // GRN pass 1: sumsq[b, c] = sum over the image's tokens of bf16(gelu(x))^2.  grid (C/256, B), 128 threads x 2 channels.
@@ -229,35 +244,47 @@ using namespace muse;
 extern "C" {
 
 int muse_add_norm_mod_fwd(const void* a, int a_dt, const float* r, const float* w, const float* ss, long long ss_stride,
-                          int rows_per_sample, float* r_out, void* y, int y_dt, int rows, int H, float eps, int rms,
-                          void* stream) {
+                          int rows_per_sample, float* r_out, void* y, int y_dt, float* row_scale, int rows, int H,
+                          float eps, int rms, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0) return MUSE_OK;
   if (H % 8 != 0 || H > 1024) { set_last_error("add_norm_mod: H=%d must be a multiple of 8 and <= 1024", H); return MUSE_ERR_UNSUPPORTED; }
   if (ss != nullptr && (rows_per_sample <= 0 || ss_stride % 4 != 0)) { set_last_error("add_norm_mod: bad modulation layout"); return MUSE_ERR_INVALID; }
   if (ss == nullptr) rows_per_sample = 1;
-  return dtype_dispatch("add_norm_mod", [&](auto a_t, auto y_t) {
+  auto run = [&](auto a_t, auto y_t, auto f8) {
     using TA = decltype(a_t);
     using TY = decltype(y_t);
     with_row_chunks<1, 2, 3, 4>(H, [&](auto ch) {
       pdl_launch(ceil_div(rows, kWarps), kWarps * 32, 0, s)(
-          add_norm_mod_kernel<TA, TY, decltype(ch)::value>, reinterpret_cast<const TA*>(a), r, w, ss, ss_stride,
-          rows_per_sample, r_out, reinterpret_cast<TY*>(y), rows, H, eps, rms);
+          add_norm_mod_kernel<TA, TY, decltype(ch)::value, decltype(f8)::value>, reinterpret_cast<const TA*>(a), r, w, ss,
+          ss_stride, rows_per_sample, r_out, reinterpret_cast<TY*>(y), rows, H, eps, rms, row_scale);
     });
     return check_launch("add_norm_mod");
-  }, a_dt, y_dt);
+  };
+  if (y_dt == 2) {
+    if (row_scale == nullptr) { set_last_error("add_norm_mod: the e4m3 output needs row_scale"); return MUSE_ERR_INVALID; }
+    return dtype_dispatch("add_norm_mod", [&](auto a_t) { return run(a_t, uint8_t(), std::true_type()); }, a_dt);
+  }
+  return dtype_dispatch("add_norm_mod", [&](auto a_t, auto y_t) { return run(a_t, y_t, std::false_type()); }, a_dt, y_dt);
 }
 
-int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y, void* conv_out, int B, int hh, int ww,
-                            int C, float eps, int rms, void* stream) {
+int muse_dwconv3x3_norm_fwd(const float* x, const float* wk, const float* nw, void* y, int y_dt, float* row_scale,
+                            void* conv_out, int B, int hh, int ww, int C, float eps, int rms, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const long long pixels = static_cast<long long>(B) * hh * ww;
+  if (y_dt != 1 && y_dt != 2) { set_last_error("dwconv3x3_norm: y dtype code %d (bf16 = 1 or e4m3 = 2)", y_dt); return MUSE_ERR_INVALID; }
+  if (y_dt == 2 && row_scale == nullptr) { set_last_error("dwconv3x3_norm: the e4m3 output needs row_scale"); return MUSE_ERR_INVALID; }
   if (pixels <= 0) return MUSE_OK;
   if (C % 8 != 0 || C > 1024) { set_last_error("dwconv3x3_norm: C=%d must be a multiple of 8 and <= 1024", C); return MUSE_ERR_UNSUPPORTED; }
   const unsigned grid = static_cast<unsigned>(ceil_div_ll(pixels, kWarps));
   with_row_chunks<1, 2, 3, 4>(C, [&](auto ch) {
-    pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<decltype(ch)::value>, x, wk, nw, reinterpret_cast<bf16*>(y),
-                                        reinterpret_cast<bf16*>(conv_out), B, hh, ww, C, eps, rms);
+    constexpr int CH = decltype(ch)::value;
+    if (y_dt == 2)
+      pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<CH, true, uint8_t>, x, wk, nw, reinterpret_cast<uint8_t*>(y),
+                                          reinterpret_cast<bf16*>(conv_out), B, hh, ww, C, eps, rms, row_scale);
+    else
+      pdl_launch(grid, kWarps * 32, 0, s)(dwconv3x3_norm_kernel<CH, false>, x, wk, nw, reinterpret_cast<bf16*>(y),
+                                          reinterpret_cast<bf16*>(conv_out), B, hh, ww, C, eps, rms, row_scale);
   });
   return check_launch("dwconv3x3_norm");
 }

@@ -197,11 +197,13 @@ class _OperandCache:
     ``refresh()`` brings the cache up to date and returns an object whose ``dst_of`` maps a parameter's data_ptr to its bf16
     copy, which the optimizer's pass writes; after the step ``sync()`` recomputes the few operands that are not such a copy
     (``derived``: the transposed depthwise weights, the permuted down / up-sample weights) in place -- graph-capturable
-    copies -- and moves the cache's key to the parameters' new version counters, so the next forward rebuilds nothing."""
+    copies -- and moves the cache's key to the parameters' new version counters, so the next forward rebuilds nothing.
+    In FP8 mode it also re-quantizes the e4m3 weight operands (``quantized``: (bf16 operand, its F8 copy)) from the bf16
+    operands the step has just written, so no FP8 copy is left stale by a step that moves the key without a rebuild."""
 
     def __init__(self, model):
         self.model = model
-        self.dst_of, self.derived = {}, []
+        self.dst_of, self.derived, self.quantized = {}, [], []
 
     def refresh(self):
         self.model._weights()
@@ -213,6 +215,8 @@ class _OperandCache:
             return
         for dst, src in self.derived:
             dst.copy_(src())
+        for src, dst in self.quantized:
+            ops.quantize_rows_e4m3(src, out=dst)
         m._cache_key = m._weights_key()
 
 
@@ -265,6 +269,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
             if isinstance(m, AdaLNModulation):
                 nn.init.constant_(m.mapper.weight, 0)
         self._cache_key, self._cache = None, None
+        self._gemm_precision = "bf16"
         self._packed = _OperandCache(self)  # the fused optimizers' handle on the cache (model=)
         self._debug_stages = None  # tests set this to a dict to receive the block-boundary activations
         self._graph = None         # CUDA graph of one decode-step forward (generate2), keyed by shapes and weight versions
@@ -284,9 +289,38 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
     def generate(self):
         assert False  # (reference :326-328)
 
+    # ------------------------------------------------------------------------------------ GEMM precision
+    def set_gemm_precision(self, mode: str):
+        """"bf16" (default: the reference's autocast recipe) or "fp8": inference only -- forward under torch.no_grad() in
+        eval mode, and generate2 -- with the e4m3 tensor cores for the transformer layers' [q;k;v], cross-attention q,
+        [wi_0;wi_1] and wo GEMMs and the ResBlock / AttentionBlock2D channelwise[0] and q GEMMs.  Their activations come
+        out of the passes that produce them as e4m3 with one scale per row, the weights are quantized per output row; every
+        other GEMM stays bf16 (DESIGN.md section 5).  Not a config key: save_pretrained / from_pretrained do not see it.
+        "fp8" needs hidden_size, block_out_channels[0] and intermediate_size to be multiples of 16 (the e4m3 rows are fed
+        by TMA, whose row pitches are multiples of 16 bytes); bf16 needs multiples of 8."""
+        if mode not in ("bf16", "fp8"):
+            raise ValueError(f"gemm precision must be 'bf16' or 'fp8', got {mode!r}")
+        c = self.config
+        widths = dict(hidden_size=c.hidden_size, block_out_channels=c.block_out_channels[0],
+                      intermediate_size=c.intermediate_size)
+        bad = {k: v for k, v in widths.items() if v % 16}
+        if mode == "fp8" and bad:
+            raise ValueError(f"gemm precision 'fp8' needs widths that are multiples of 16, got {bad}")
+        self._gemm_precision = mode  # part of the operand cache key: the next forward rebuilds the operands
+        return self
+
+    @property
+    def gemm_precision(self) -> str:
+        return self._gemm_precision
+
+    def _check_fp8_inference(self):
+        if self._gemm_precision == "fp8" and (self.training or torch.is_grad_enabled()):
+            raise RuntimeError("MaskGiTUViT_v2 in FP8 GEMM precision is inference only: call model.eval() and run under "
+                               "torch.no_grad(), or set_gemm_precision('bf16') to train")
+
     # ------------------------------------------------------------------------------------ bf16 operand cache
     def _weights_key(self):
-        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+        return (self._gemm_precision,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
 
     def _weights(self):
         """bf16 GEMM operands (fused [k;v], [q;k;v], [wi_0;wi_1], all adaLN mappers stacked into one matrix, logits rows
@@ -295,14 +329,16 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         key = self._weights_key()
         if key == self._cache_key:
             return self._cache
-        W, self._packed.dst_of, self._packed.derived = self._build_weights()
+        W, self._packed.dst_of, self._packed.derived, self._packed.quantized = self._build_weights()
         self._cache_key, self._cache = key, W
         return W
 
     def _build_weights(self):
-        """(W, dst_of, derived): the operand dict; parameter data_ptr -> address of its bf16 copy, for every parameter whose
-        operand is a plain row block of one bf16 matrix; and (destination, source view) of the operands that are not: the
-        transposed fp32 depthwise weights and the permuted down / up-sample weights."""
+        """(W, dst_of, derived, quantized): the operand dict; parameter data_ptr -> address of its bf16 copy, for every
+        parameter whose operand is a plain row block of one bf16 matrix; (destination, source view) of the operands that
+        are not: the transposed fp32 depthwise weights and the permuted down / up-sample weights; and in FP8 mode
+        (bf16 operand, F8 copy) of the FP8 sites, whose W entries are then the F8 copies (the bf16 operands stay, as the
+        fused optimizers' destinations)."""
         dev = next(self.parameters()).device
         dst_of, derived = {}, []
 
@@ -387,7 +423,17 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
                 "wo": bf(l.ffn.wo.weight)})
         W["up"] = block(self.up_blocks[0])
         W["mappers"] = bf(*mappers)
-        return W, dst_of, derived
+        quantized = []
+        if self._gemm_precision == "fp8":
+            def f8(d, k):
+                quantized.append((d[k], ops.quantize_rows_e4m3(d[k])))
+                d[k] = quantized[-1][1]
+
+            for w in W["down"] + W["up"]:
+                f8(w, "cw0"), f8(w["a1"], "q"), f8(w["a2"], "q")
+            for w in W["layers"]:
+                f8(w["sa"], "qkv"), f8(w["ca"], "q"), f8(w, "wi"), f8(w, "wo")
+        return W, dst_of, derived, quantized
 
     # ------------------------------------------------------------------------------------------- forward
     def _forward_tokens(self, input_ids, encoder_hidden_states, cond_embeds, micro_conds, drop=None):
@@ -459,6 +505,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
                 loss_weight=None, _raw_bf16=False):
         c = self.config
         B, S = input_ids.shape
+        self._check_fp8_inference()
         # nn.Dropout is active iff the module is in training mode (also under no_grad), each rate gating its own sites.
         # One seed per forward, drawn on the device from torch's default generator as MaskGitTransformer does:
         # torch.manual_seed reproduces the masks.  Site ids: uvit_v2_train.unit_drop.
@@ -524,6 +571,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         """MaskGIT parallel decoding with classifier-free guidance, semantics of the reference (:330-479); per step one
         doubled-batch forward and ONE fused kernel (guidance mix, categorical sample, confidence, k-th cut, re-mask)."""
         c = self.config
+        self._check_fp8_inference()
         if self.training and (c.hidden_dropout > 0.0 or c.attention_dropout > 0.0):
             # the reference would sample with dropout applied to every forward of the decode loop
             raise RuntimeError("generate2 on a MaskGiTUViT_v2 in training mode would sample with dropout > 0 active; "

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import os
 import weakref
+from typing import NamedTuple
 
 import torch
 
@@ -16,7 +17,20 @@ from ._lib import (CONV_GELU, CONV_PIXEL_SHUFFLE, CONV_S2P1, CONV_SAME, CONV_STR
                    CONV_TC_PER_IMAGE_WEIGHTS, CONV_TC_PIXEL_SHUFFLE, CONV_TC_SAME, CONV_TC_SINGLE_PASS, CONV_TC_UPSAMPLE2X,
                    CONV_TRANSPOSE_S2, CONV_UPSAMPLE2X)
 
-F32, BF16 = 0, 1
+F32, BF16, E4M3 = 0, 1, 2
+FP8 = torch.float8_e4m3fn
+
+
+class F8(NamedTuple):
+    """An e4m3 GEMM operand with one fp32 scale per row: row r stands for q[r] * s[r] (the producers store
+    e4m3_rn_satfinite(y / s) with s = amax(|y[r]|) / 448, or 1 for an all-zero row)."""
+    q: torch.Tensor  # torch.float8_e4m3fn [rows, K]
+    s: torch.Tensor  # fp32 [rows]
+
+    @property
+    def shape(self):
+        return self.q.shape
+
 EPI_BF16, EPI_F32, EPI_ATOMIC_F32, EPI_RESADD_F32 = 0, 1, 2, 3
 
 _state = {"device": None, "launches": 0}
@@ -60,7 +74,22 @@ def _dt(t: torch.Tensor) -> int:
         return F32
     if t.dtype == torch.bfloat16:
         return BF16
+    if t.dtype == FP8:
+        return E4M3
     raise TypeError(f"unsupported dtype {t.dtype}")
+
+
+def _new_out(rows, cols, dtype, device):
+    """(output, its row scales or None): an F8 pair for dtype FP8, else a plain tensor"""
+    y = torch.empty(rows, cols, dtype=dtype, device=device)
+    if dtype != FP8:
+        return y, None
+    s = torch.empty(rows, dtype=torch.float32, device=device)
+    return F8(y, s), s
+
+
+def _data(y):
+    return y.q if isinstance(y, F8) else y
 
 
 def _p(t):
@@ -106,8 +135,40 @@ def gemm(a, b, c, M, N, K, lda, ldb, ldc, a_mn=0, b_mn=0, epi=EPI_BF16, res=None
     return c
 
 
+def gemm_fp8(a: F8, b: F8, c, M, N, K, lda, ldb, ldc):
+    """c bf16 [M,N] = (a.q * a.s[:, None]) @ (b.q * b.s[:, None])^T with the e4m3 tensor cores (fp32 accumulation)."""
+    st = _prep(c)
+    if _prof["on"]:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    _call("muse_gemm_fp8", _p(a.q), _p(a.s), _p(b.q), _p(b.s), _p(c), M, N, K, lda, ldb, ldc, st)
+    if _prof["on"]:
+        e1.record()
+        _prof["events"].append((e0, e1, 2.0 * M * N * K))
+    return c
+
+
+def quantize_rows_e4m3(x, out: F8 | None = None) -> F8:
+    """bf16 [rows, K] -> F8 with one scale per row (the FP8 weight operands); out: an F8 of the same shape to refresh in
+    place (graph-capturable)."""
+    st = _prep(x)
+    rows, K = x.shape
+    if out is None:
+        out = F8(torch.empty(rows, K, dtype=FP8, device=x.device), torch.empty(rows, dtype=torch.float32, device=x.device))
+    _call("muse_quantize_rows_e4m3", _p(x), x.stride(0), _p(out.q), out.q.stride(0), _p(out.s), rows, K, st)
+    return out
+
+
 def linear_fwd(x, w, out_dtype=torch.bfloat16, res=None, n_valid=None):
-    """y[T,N] = x[T,K] @ w[N,K]^T.  res (fp32 [T,N]) selects the fused residual epilogue."""
+    """y[T,N] = x[T,K] @ w[N,K]^T.  res (fp32 [T,N]) selects the fused residual epilogue.  x and w both F8: the FP8
+    GEMM (bf16 output, no residual)."""
+    if isinstance(x, F8):
+        if not isinstance(w, F8) or res is not None or out_dtype != torch.bfloat16:
+            raise TypeError("linear_fwd: an F8 activation needs an F8 weight, a bf16 output and no residual")
+        T, K = x.q.shape
+        N = w.q.shape[0] if n_valid is None else n_valid
+        y = torch.empty(T, N, dtype=torch.bfloat16, device=x.q.device)
+        return gemm_fp8(x, w, y, T, N, K, x.q.stride(0), w.q.stride(0), N)
     T, K = x.shape
     N = w.shape[0] if n_valid is None else n_valid
     if res is not None:
@@ -318,13 +379,14 @@ def norm2_bwd(d_h2, x2, w2, dres, a, w1, stats, rms1=0, rms2=0):
 
 
 # ------------------------------------------------------------------------------------------ GLU
-def glu_fwd(ab, dropout=None):
-    """dropout = (p, seed, site): FeedForward.dropout fused into the pass; then returns (out, bits) (see dropout_fwd)."""
+def glu_fwd(ab, dropout=None, out_dtype=torch.bfloat16):
+    """dropout = (p, seed, site): FeedForward.dropout fused into the pass; then returns (out, bits) (see dropout_fwd).
+    out_dtype FP8: out is an F8 (no dropout)."""
     st = _prep(ab)
     rows, two_i = ab.shape
-    out = torch.empty(rows, two_i // 2, dtype=torch.bfloat16, device=ab.device)
+    out, scale = _new_out(rows, two_i // 2, out_dtype, ab.device)
     bits, seed, site, p = _drop_fwd_args(dropout, ab.device, rows, cols=two_i // 2)
-    _call("muse_glu_fwd", _p(ab), _p(out), _p(bits), _p(seed), site, p, rows, two_i // 2, st)
+    _call("muse_glu_fwd", _p(ab), _p(_data(out)), _dt(_data(out)), _p(scale), _p(bits), _p(seed), site, p, rows, two_i // 2, st)
     return out if bits is None else (out, bits)
 
 
@@ -450,24 +512,25 @@ def ce_bwd(logits_padded, labels, ws, dloss, loss_out, V, label_smoothing, row_s
 # ------------------------------------------------------------------------------------------ U-ViT v2 forward ops
 def add_norm_mod(a, w, eps, rms, out_dtype=torch.bfloat16, residual=None, mod=None, rows_per_sample=1, want_residual=True):
     """(r', y): r' = a + residual (fp32), y = norm(r') * w [* (1 + scale_b) + shift_b].  mod: fp32 [B, 2H] view (scale |
-    shift per sample, row pitch mod.stride(0)) of the batched adaLN mapper output."""
+    shift per sample, row pitch mod.stride(0)) of the batched adaLN mapper output.  out_dtype FP8: y is an F8."""
     st = _prep(a)
     rows, H = a.shape
-    y = torch.empty(rows, H, dtype=out_dtype, device=a.device)
+    y, scale = _new_out(rows, H, out_dtype, a.device)
     r_out = torch.empty(rows, H, dtype=torch.float32, device=a.device) if want_residual else None
     _call("muse_add_norm_mod_fwd", _p(a), _dt(a), _p(residual), _p(w), _p(mod), 0 if mod is None else mod.stride(0),
-          int(rows_per_sample), _p(r_out), _p(y), _dt(y), rows, H, float(eps), int(rms), st)
+          int(rows_per_sample), _p(r_out), _p(_data(y)), _dt(_data(y)), _p(scale), rows, H, float(eps), int(rms), st)
     return r_out, y
 
 
-def dwconv3x3_norm(x, wk, norm_w, B, hh, ww, eps, rms, save_conv=False):
+def dwconv3x3_norm(x, wk, norm_w, B, hh, ww, eps, rms, save_conv=False, out_dtype=torch.bfloat16):
     """x fp32 [B*hh*ww, C] token-major, wk fp32 [9, C] -> bf16 [B*hh*ww, C] = Norm2D(depthwise3x3(x)).
-    save_conv: also return the bf16 conv output (needed by dwconv3x3_norm_bwd)."""
+    save_conv: also return the bf16 conv output (needed by dwconv3x3_norm_bwd).  out_dtype FP8: y is an F8."""
     st = _prep(x)
     C = x.shape[1]
-    y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    conv = torch.empty_like(y) if save_conv else None
-    _call("muse_dwconv3x3_norm_fwd", _p(x), _p(wk), _p(norm_w), _p(y), _p(conv), B, hh, ww, C, float(eps), int(rms), st)
+    y, scale = _new_out(x.shape[0], C, out_dtype, x.device)
+    conv = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if save_conv else None
+    _call("muse_dwconv3x3_norm_fwd", _p(x), _p(wk), _p(norm_w), _p(_data(y)), _dt(_data(y)), _p(scale), _p(conv), B, hh,
+          ww, C, float(eps), int(rms), st)
     return (y, conv) if save_conv else y
 
 

@@ -81,6 +81,13 @@ def _dkw(dr):
     return {} if dr is None else {"dropout": dr}
 
 
+def _form(w):
+    """keywords of the producer of a GEMM's activation: the FP8 output for an e4m3 weight
+    (MaskGiTUViT_v2.set_gemm_precision("fp8")), none for a bf16 one (the producer's default).  The operand form is thus
+    decided in this one place, from the weights the block forward is given."""
+    return {"out_dtype": ops.FP8} if isinstance(w, ops.F8) else {}
+
+
 # ------------------------------------------------------------------------------------------------ attention helper
 def _attn_fwd(y, ctx_in, a, B, S, Skv, fused, drop=None):
     """drop = (p, seed, site) of this attention's probabilities, or None"""
@@ -125,7 +132,7 @@ def _res_block_fwd(h, w, mod_all, B, hw, eps, rms, save=True, drop=None):
     """save=False (inference): no conv output is written and adaLN modulates in place (no copy), so no state is returned.
     drop: the unit's dropout spec -- channelwise[3] is fused into the GRN pass, whose dropped output is the cw4 operand
     (and what the cw4 weight gradient reads)."""
-    out = ops.dwconv3x3_norm(h, w["dw"], w["dw_norm"], B, hw, hw, eps, rms, save_conv=save)
+    out = ops.dwconv3x3_norm(h, w["dw"], w["dw_norm"], B, hw, hw, eps, rms, save_conv=save, **_form(w["cw0"]))
     d, conv = out if save else (out, None)
     g1 = ops.linear_fwd(d, w["cw0"])
     gd = _site(drop, 0, attn=False)
@@ -159,10 +166,10 @@ def _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=None):
         se = ops.silu_bf16(enc)
         encb = ops.linear_fwd(se, w["kvm"])
     ctx_in = enc if encb is None else encb
-    _, y1 = ops.add_norm_mod(h, w["ln1"], eps, rms, want_residual=False)
+    _, y1 = ops.add_norm_mod(h, w["ln1"], eps, rms, **_form(w["a1"]["q"]), want_residual=False)
     c1, s1 = _attn_fwd(y1, ctx_in, w["a1"], B, S, Skv, False, _site(drop, 1, attn=True))
     a1o = ops.linear_fwd(c1, w["a1"]["o"])
-    r2, y2 = ops.add_norm_mod(a1o, w["ln2"], eps, rms, residual=h)
+    r2, y2 = ops.add_norm_mod(a1o, w["ln2"], eps, rms, **_form(w["a2"]["q"]), residual=h)
     c2, s2 = _attn_fwd(y2, ctx_in, w["a2"], B, S, Skv, False, _site(drop, 2, attn=True))
     out = ops.linear_fwd(c2, w["a2"]["o"], res=r2)
     return out, (h, se, ctx_in, y1, c1, s1, r2, y2, c2, s2)
@@ -186,17 +193,20 @@ def _attn_block_bwd(dout, st, w, g, enc, d_enc, B, S, Skv, eps, rms):
 
 def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=None):
     m = lambda k: mod_all[:, w[k][0]:w[k][0] + w[k][1]]
-    r1, y1 = ops.add_norm_mod(x, w["ln1"], eps, rms, residual=r, mod=m("mod1"), rows_per_sample=S)
+    r1, y1 = ops.add_norm_mod(x, w["ln1"], eps, rms, **_form(w["sa"]["qkv"]), residual=r, mod=m("mod1"),
+                              rows_per_sample=S)
     c, s_sa = _attn_fwd(y1, None, w["sa"], B, S, S, True, _site(drop, 0, attn=True))
     a = ops.linear_fwd(c, w["sa"]["o"])
-    r2, y2 = ops.add_norm_mod(a, w["ln2"], eps, rms, residual=r1, mod=m("mod2"), rows_per_sample=S)
+    r2, y2 = ops.add_norm_mod(a, w["ln2"], eps, rms, **_form(w["ca"]["q"]), residual=r1, mod=m("mod2"),
+                              rows_per_sample=S)
     cc, s_ca = _attn_fwd(y2, enc, w["ca"], B, S, Skv, False, _site(drop, 1, attn=True))
     co = ops.linear_fwd(cc, w["ca"]["o"])
-    r3, y3 = ops.add_norm_mod(co, w["ln3"], eps, 0, residual=r2, mod=m("mod3"), rows_per_sample=S)
+    r3, y3 = ops.add_norm_mod(co, w["ln3"], eps, 0, **_form(w["wi"]), residual=r2, mod=m("mod3"),
+                              rows_per_sample=S)
     ab = ops.linear_fwd(y3, w["wi"])
     fd = _site(drop, 2, attn=False)
     if fd is None:
-        gl, fdr = ops.glu_fwd(ab), None
+        gl, fdr = ops.glu_fwd(ab, **_form(w["wo"])), None
     else:  # GLUFeedForward.dropout fused into the GLU pass: gl is the dropped wo operand
         gl, bits = ops.glu_fwd(ab, dropout=fd)
         fdr = (fd[0], bits)
