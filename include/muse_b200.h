@@ -117,6 +117,25 @@ int muse_lion_ema_step(const void* entries_host, int n_entries, float* scal_dev,
                        int ema_update_after_step, int ema_update_every, int ema_use_warmup, float ema_inv_gamma,
                        float ema_power, void* stream);
 
+/* One pass over all parameters: AdamW with block-wise 8-bit moments (the scheme of bitsandbytes' AdamW8bit, the script
+ * train_muse.py's optimizer.name: 8bit_adamw) + the same EMA and bf16 copy as muse_adamw_ema_step, same step counter and
+ * scalar array (one prepare launch per call).  entries_host: HOST array of n_entries {float* p; const float* g; m; v;
+ * float* ema (nullable); bf16* packed (nullable); int64 numel (multiple of 4); int64 reserved; float* absmax1;
+ * float* absmax2} (10 x int64), in chunks of 48 tensors per launch.  absmax1 == NULL: m / v are fp32 moments, updated by
+ * muse_adamw_ema_step's element code.  Otherwise m / v are uint8 codes and absmax1 / absmax2 hold one fp32 value per
+ * 256-element block (blocks start at element 0 of each tensor; the last may be partial).  Per block: decode
+ * m0 = Q1[code] * absmax1, v0 = Q2[code] * absmax2; the AdamW update of (p, m, v) from (p, g, m0, v0) (p takes these
+ * un-requantised moments); absmax1 = max |m|, absmax2 = max v over the block; code = #{k : M[k] < x} with
+ * x = m / absmax (IEEE division; 0 when absmax is 0).  maps_dev: device array of 1612 floats: [Q1 | Q2 | M1 | M2], the
+ * signed and unsigned 256-entry maps and their 255 midpoints (each padded to 256), then three 784-byte tables (signed map
+ * for x >= 0, signed map for x < 0, unsigned map) of the code #{k : M[k] < lowest x of the bucket} for each of 769
+ * buckets of |x| = (bits(|x|) >> 18) - (103 << 5), clamped to [0, 768]. */
+int muse_adamw8bit_ema_step(const void* entries_host, int n_entries, const float* maps_dev, float* scal_dev,
+                            long long* step_dev, const float* lr_dev, float lr_host, float beta1, float beta2, float eps,
+                            float weight_decay, int ema_enabled, float ema_decay, float ema_min_decay,
+                            int ema_update_after_step, int ema_update_every, int ema_use_warmup, float ema_inv_gamma,
+                            float ema_power, void* stream);
+
 /* Embed.forward (muse/modeling_transformer.py:942-957): out[b,s,:] = word[ids[b,s],:] + pos[s,:] (fp32). */
 int muse_embed_fwd(const long long* ids, const float* word, const float* pos, float* out, int B, int S, int H,
                    int vocab, void* stream);

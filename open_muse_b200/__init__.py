@@ -18,4 +18,4 @@ MaskGiTUViT = MaskGiTUViT_v2  # the reference's alias (muse/modeling_transformer
 from .pipeline_muse import PipelineMuse, PipelineMuseInpainting  # noqa: F401
 from .sampling import get_mask_chedule  # noqa: F401
 
-from .optim import FusedAdamW, FusedLion  # noqa: F401,E402
+from .optim import FusedAdamW, FusedAdamW8bit, FusedLion  # noqa: F401,E402

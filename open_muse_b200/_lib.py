@@ -33,6 +33,7 @@ SIGNATURES = {
     "muse_pack_bf16": (c_int, [_P, _I, _L, _P]),
     "muse_adamw_ema_step": (c_int, [_P, _I, _P, _P, _P, _F, _F, _F, _F, _F, _I, _F, _F, _I, _I, _I, _F, _F, _P]),
     "muse_lion_ema_step": (c_int, [_P, _I, _P, _P, _P, _F, _F, _F, _F, _F, _F, _F, _I, _F, _F, _I, _I, _I, _F, _F, _P]),
+    "muse_adamw8bit_ema_step": (c_int, [_P, _I, _P, _P, _P, _P, _F, _F, _F, _F, _F, _I, _F, _F, _I, _I, _I, _F, _F, _P]),
     "muse_cast_bf16": (c_int, [_P, _P, _L, _P]),
     "muse_embed_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "muse_embed_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),

@@ -9,7 +9,8 @@ GEMM operand.  A ``torch.optim.Optimizer`` subclass, so LR schedulers, ``state_d
 the device).
 
 ``FusedLion`` is the reference's ``training/optimizer.py::Lion`` (the scripts' ``optimizer.name: lion``; one moment instead
-of two) on the same machinery.  Both optimizers keep a model's bf16 operand cache current (see ``_FusedOptimizer``)."""
+of two) on the same machinery, and ``FusedAdamW8bit`` is AdamW with block-wise 8-bit moments (train_muse.py's
+``optimizer.name: 8bit_adamw``).  All three keep a model's bf16 operand cache current (see ``_FusedOptimizer``)."""
 from __future__ import annotations
 
 from typing import Optional
@@ -29,15 +30,17 @@ def _check_lr(lr, device=None, who="FusedAdamW"):
 
 
 class _FusedOptimizer(torch.optim.Optimizer):
-    """The launch plan, EMA wiring and operand-cache protocol shared by ``FusedAdamW`` and ``FusedLion``.
+    """The launch plan, EMA wiring and operand-cache protocol shared by ``FusedAdamW``, ``FusedLion`` and
+    ``FusedAdamW8bit``.
 
-    A subclass names its per-parameter moment buffers (``_moments``: the table's m and v slots) and launches its kernel in
-    ``_launch``.  The kernels write parameters through raw pointers, which autograd does not see, so after every step the
-    written parameters' version counters are bumped: a model's operand cache keyed on ``(data_ptr, _version)`` then
-    rebuilds on its next forward.  With ``model=`` the step also writes the bf16 operands itself: ``model._packed``
-    provides ``refresh()`` (bring the cache up to date; returns an object whose ``dst_of`` maps a parameter's data_ptr to
-    its bf16 copy) and ``sync()`` (after the step: refresh the few operands that are not a plain copy of one parameter and
-    move the cache's key to the new versions), so no re-pack follows the step."""
+    A subclass names its per-parameter moment buffers (``_moments``: the table's m and v slots; or overrides
+    ``_state_columns`` for another layout) and launches its kernel in ``_launch``.  The kernels write parameters through
+    raw pointers, which autograd does not see, so after every step the written parameters' version counters are bumped:
+    a model's operand cache keyed on ``(data_ptr, _version)`` then rebuilds on its next forward.  With ``model=`` the
+    step also writes the bf16 operands itself: ``model._packed`` provides ``refresh()`` (bring the cache up to date;
+    returns an object whose ``dst_of`` maps a parameter's data_ptr to its bf16 copy) and ``sync()`` (after the step:
+    refresh the few operands that are not a plain copy of one parameter and move the cache's key to the new versions),
+    so no re-pack follows the step."""
 
     _moments = ()
 
@@ -49,6 +52,16 @@ class _FusedOptimizer(torch.optim.Optimizer):
             flat = [p for g in self.param_groups for p in g["params"]]
             if len(flat) != len(ema.shadow_params) or any(p.shape != s.shape for p, s in zip(flat, ema.shadow_params)):
                 raise ValueError(f"{type(self).__name__}(ema=...): the EMAModel must be built over the same parameter list")
+
+    def _state_columns(self, p):
+        """the table's m and v addresses for p and the columns that follow its fixed eight (none here), creating its moment
+        buffers on first use"""
+        st = self.state[p]
+        for k in self._moments:
+            if k not in st:
+                st[k] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        m, v = (st[k].data_ptr() for k in self._moments) if len(self._moments) == 2 else (st[self._moments[0]].data_ptr(), 0)
+        return m, v, ()
 
     # ---- per-group launch plan (device table), rebuilt when pointers change (new grads storage, .to(device), ...)
     def _packed_cache(self):
@@ -83,12 +96,8 @@ class _FusedOptimizer(torch.optim.Optimizer):
             if sh is not None and (sh.dtype != torch.float32 or sh.device != p.device or sh.shape != p.shape
                                    or not sh.is_contiguous()):
                 raise RuntimeError(f"{name}(ema=...) needs contiguous fp32 EMA shadows shaped and placed like the parameters")
-            st = self.state[p]
-            for k in self._moments:
-                if k not in st:
-                    st[k] = torch.zeros_like(p, memory_format=torch.preserve_format)
-            m, v = (st[k].data_ptr() for k in self._moments) if len(self._moments) == 2 else (st[self._moments[0]].data_ptr(), 0)
-            entries.append((p.data_ptr(), p.grad.data_ptr(), m, v, sh_ptr, packed_ptr, p.numel(), 0))
+            m, v, extra = self._state_columns(p)
+            entries.append((p.data_ptr(), p.grad.data_ptr(), m, v, sh_ptr, packed_ptr, p.numel(), 0, *extra))
         plan = self._plans.get(gi) or {}
         if "step" not in plan:
             # one device-resident step counter per group, shared by the group's parameters' state entries so that
@@ -209,3 +218,145 @@ class FusedLion(_FusedOptimizer):
                   plan["step"].data_ptr(), None if lr_dev is None else lr_dev.data_ptr(),
                   0.0 if lr_dev is not None else float(lr), 1.0 if lr_dev is not None else 1.0 - float(lr) * wd,
                   float(b1), float(b2), 1.0 - float(b1), 1.0 - float(b2), wd, *ema_args, stream)
+
+
+MIN_8BIT_SIZE = 4096  # parameters with fewer elements keep fp32 moments (bitsandbytes' min_8bit_size)
+QBLOCK = 256          # elements per quantisation block (one fp32 absmax each)
+
+
+def dynamic_map(signed: bool) -> torch.Tensor:
+    """The 256-entry dynamic quantisation map of the 8-bit moments, built in fp32 on the CPU: for each decade 10^-6 ..
+    10^0, the midpoints of an evenly spaced grid over [0.1, 1] scaled into it (and their negatives when signed), plus 0
+    and 1, sorted.  Signed (m): zero at index 127, 1.0 last; unsigned (v): zero at index 0."""
+    data = []
+    for i in range(7):
+        n = 2 ** i + 1 if signed else 2 ** (i + 1) + 1
+        b = torch.linspace(0.1, 1, n)
+        means = (b[:-1] + b[1:]) / 2.0
+        data += ((10 ** (-6 + i)) * means).tolist()
+        if signed:
+            data += (-(10 ** (-6 + i)) * means).tolist()
+    data += [0.0, 1.0]
+    return torch.tensor(sorted(data), dtype=torch.float32)
+
+
+def midpoints(q: torch.Tensor) -> torch.Tensor:
+    """the 255 fp32 decision boundaries (q[k] + q[k + 1]) / 2 of a map: a value x encodes to #{k : M[k] < x}"""
+    return (q[:-1] + q[1:]) / 2
+
+
+BUCKETS, BUCKET_BASE, START_BYTES = 769, 103 << 5, 784  # the encoder's first guess (csrc/optim.cu kBuckets, ...)
+
+
+def bucket_starts(mid: torch.Tensor, negative: bool) -> torch.Tensor:
+    """per bucket of |x| (its fp32 bits >> 18, less the bits of 2^-24 >> 18, clamped to [0, 768]), a code no larger than
+    that of any x of the bucket: #{k : mid[k] < lowest x}.  For x >= 0 the lowest x is the bucket's lower bound (0 for
+    bucket 0); for x < 0 it lies above minus the bucket's upper bound (no bound for the last bucket)."""
+    b = torch.arange(BUCKETS, dtype=torch.int32)
+    lo = ((b + BUCKET_BASE) << 18).view(torch.float32).clone()
+    lo[0] = 0.0
+    if not negative:
+        return torch.searchsorted(mid, lo, side="left")
+    hi = torch.cat([lo[1:], torch.tensor([float("inf")])])
+    return torch.searchsorted(mid, -hi, side="left")
+
+
+def _maps_buffer(device) -> torch.Tensor:
+    """what the kernel stages in shared memory: [Q1 | Q2 | M1 | M2] (both maps and their midpoints, each padded to 256
+    entries), then the encoder's start-code tables as bytes (signed map for x >= 0 and for x < 0, unsigned map), each
+    padded to START_BYTES"""
+    q1, q2 = dynamic_map(True), dynamic_map(False)
+    m1, m2 = midpoints(q1), midpoints(q2)
+    pad = torch.tensor([float("inf")])  # never read
+    tables = torch.zeros(3, START_BYTES, dtype=torch.uint8)
+    for row, (mid, neg) in enumerate(((m1, False), (m1, True), (m2, False))):
+        tables[row, :BUCKETS] = bucket_starts(mid, neg).to(torch.uint8)
+    return torch.cat([q1, q2, m1, pad, m2, pad, tables.reshape(-1).view(torch.float32)]).to(device)
+
+
+class FusedAdamW8bit(_FusedOptimizer):
+    """AdamW with block-wise 8-bit moments (the scheme of bitsandbytes' ``AdamW8bit``; train_muse.py's ``optimizer.name:
+    8bit_adamw``) + EMA + bf16 operand packing in one pass.
+
+    A parameter with at least ``MIN_8BIT_SIZE`` elements keeps its moments as uint8 codes shaped like it (``state1``: m
+    against the signed ``dynamic_map``, ``state2``: v against the unsigned one) plus one fp32 absmax per 256-element block
+    (``absmax1`` / ``absmax2``; blocks start at the tensor's first element, the last may be partial).  A step decodes
+    ``Q[code] * absmax``, applies ``FusedAdamW``'s element update (decay before the Adam step, as torch ``AdamW``; the
+    parameter takes the un-requantised moments), sets each block's absmax to max |m| / max v and re-encodes to the
+    nearest map entry (ties to the lower code).  Smaller parameters keep fp32 ``exp_avg`` / ``exp_avg_sq`` and are
+    updated exactly as ``FusedAdamW`` updates them.  Every state also holds its group's device-resident ``step``.  The
+    moments then take about 2 B per parameter instead of 8.  Bit-parity with bitsandbytes is not claimed; it applies
+    decay after the step."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, ema=None, model=None):
+        """``lr`` (a number or a one-element fp32 device tensor), ``ema`` and ``model`` as in ``FusedAdamW``."""
+        _check_lr(lr, who="FusedAdamW8bit")
+        if lr < 0 or eps < 0 or not 0 <= betas[0] < 1 or not 0 <= betas[1] < 1 or weight_decay < 0:
+            raise ValueError("invalid AdamW hyper-parameters")
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), ema, model)
+        self._maps = {}
+
+    @staticmethod
+    def _layout(p):
+        """state key -> (dtype, shape) of p's moments"""
+        if p.numel() < MIN_8BIT_SIZE:
+            return {"exp_avg": (torch.float32, p.shape), "exp_avg_sq": (torch.float32, p.shape)}
+        nblk = -(-p.numel() // QBLOCK)
+        return {"state1": (torch.uint8, p.shape), "state2": (torch.uint8, p.shape),
+                "absmax1": (torch.float32, torch.Size([nblk])), "absmax2": (torch.float32, torch.Size([nblk]))}
+
+    def _init_state(self, p):
+        st = self.state[p]
+        for k, (dtype, shape) in self._layout(p).items():
+            if k not in st:
+                st[k] = torch.zeros(shape, dtype=dtype, device=p.device)
+        return st
+
+    def _state_columns(self, p):
+        st = self._init_state(p)
+        if p.numel() < MIN_8BIT_SIZE:
+            return st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(), (0, 0)
+        return st["state1"].data_ptr(), st["state2"].data_ptr(), (st["absmax1"].data_ptr(), st["absmax2"].data_ptr())
+
+    def load_state_dict(self, state_dict):
+        """checks every parameter's saved moments against the layout its size calls for before loading (the kernel reads
+        the buffers through raw pointers of the layout's dtypes), and keeps the codes uint8 and every buffer dense"""
+        saved = [i for g in state_dict["param_groups"] for i in g["params"]]
+        params = [p for g in self.param_groups for p in g["params"]]
+        if len(saved) != len(params):
+            raise ValueError(f"FusedAdamW8bit.load_state_dict: the state has {len(saved)} parameters, the optimizer "
+                             f"{len(params)}")
+        for n, (i, p) in enumerate(zip(saved, params)):
+            st = state_dict["state"].get(i)
+            if st is None:
+                continue
+            want = self._layout(p)
+            have = {k for k in st if k != "step"}
+            if have and have != set(want):
+                raise ValueError(f"FusedAdamW8bit.load_state_dict: parameter {n} ({p.numel()} elements) needs the state "
+                                 f"{sorted(want)}, the loaded state has {sorted(have)}")
+            for k in have:
+                t, (dtype, shape) = st[k], want[k]
+                if not torch.is_tensor(t) or t.dtype != dtype or t.shape != shape:
+                    got = f"{t.dtype} {tuple(t.shape)}" if torch.is_tensor(t) else type(t).__name__
+                    raise ValueError(f"FusedAdamW8bit.load_state_dict: parameter {n} state {k!r} must be {dtype} "
+                                     f"{tuple(shape)}, got {got}")
+        super().load_state_dict(state_dict)
+        for p in params:
+            # torch casts loaded state to the parameter's dtype (the codes go back to uint8, exactly) and keeps its strides;
+            # the kernel walks every buffer as a dense array in logical order
+            st = self.state.get(p, {})
+            for k, (dtype, _) in self._layout(p).items():
+                if k in st:
+                    st[k] = st[k].to(dtype).contiguous()
+        self._plans = {}  # the next step builds its tables over the loaded buffers and step counters
+
+    def _launch(self, plan, group, lr_dev, ema_args, stream):
+        dev = plan["params"][0].device
+        if dev not in self._maps:
+            self._maps[dev] = _maps_buffer(dev)
+        b1, b2 = group["betas"]
+        ops._call("muse_adamw8bit_ema_step", plan["table"].ctypes.data, plan["n"], self._maps[dev].data_ptr(),
+                  plan["scal"].data_ptr(), plan["step"].data_ptr(), None if lr_dev is None else lr_dev.data_ptr(),
+                  0.0 if lr_dev is not None else float(group["lr"]), float(b1), float(b2), float(group["eps"]),
+                  float(group["weight_decay"]), *ema_args, stream)
