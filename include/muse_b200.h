@@ -199,8 +199,9 @@ int muse_glu_fwd(const void* ab, void* out, int out_dtype, float* row_scale, uns
 int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
                  void* stream);
 
-/* Attention.attention (:221-241) fused: O = softmax(Q K^T * scale) V per (batch, head), head_dim 64 or 48
- * (configs/imagenet.yaml: hidden 768 / 16 heads).  Q/K/V/O are bf16 with row strides (elements) q_rs/k_rs/v_rs/o_rs, head h at
+/* Attention.attention (:221-241) fused: O = softmax(Q K^T * scale) V per (batch, head), head_dim 48, 64, 96
+ * or 128 (48: configs/imagenet.yaml, hidden 768 / 16 heads; 128: hidden 1024 / 8 heads); any other width returns
+ * MUSE_ERR_UNSUPPORTED.  Q/K/V/O are bf16 with row strides (elements) q_rs/k_rs/v_rs/o_rs, head h at
  * column offset h*head_dim,
  * batch b at row offset b*Sq (Q,O) or b*Skv (K,V).  lse fp32 [B,nh,Sq] is saved for backward.
  * bits (nullable): dropout on the probabilities (:236-237), bits [B, nh, Sq, ceil(Skv / 32)] written; the lse is that of
@@ -208,7 +209,7 @@ int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, flo
 int muse_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
                   const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int head_dim,
                   int q_rs, int k_rs, int v_rs, int o_rs, float scale, void* stream);
-/* dvec: fp32 scratch [B,nh,Sq].  bits (nullable): the bits muse_attn_fwd wrote. */
+/* dvec: fp32 scratch [B,nh,Sq].  bits (nullable): the bits muse_attn_fwd wrote.  head_dim 48, 64, 96 or 128. */
 int muse_attn_bwd(const void* q, const void* k, const void* v, const void* d_o, const float* lse,
                   const unsigned int* bits, float p, float* dvec, void* dq, void* dk, void* dv, int B, int nh, int Sq,
                   int Skv, int head_dim, int q_rs, int k_rs, int v_rs, int do_rs, int dq_rs, int dk_rs, int dv_rs,

@@ -1,4 +1,4 @@
-// wgmma / TMA attention for head_dim 64 and 48 (sm_90a): forward, dQ and dK/dV kernels.
+// wgmma / TMA attention for head_dim 64, 48, 128 and 96 (sm_90a): forward, dQ and dK/dV kernels.
 // Replaces the reference's materialised attention (muse/modeling_transformer.py:221-241) and its autograd backward.
 //
 // One CTA = one (batch, head) x one 64-row tile of the "owned" sequence dimension: a consumer warpgroup that issues the
@@ -12,7 +12,8 @@
 //   dQ       : owned = q rows.   S, dP = dO V_j^T -> sweep 1: D = sum P*dP ; sweep 2: dS -> dQ += dS K_j
 //   dK/dV    : owned = kv rows.  S^T = K Q_i^T, dP^T = V dO_i^T -> P^T, dS^T -> dV += P^T dO_i, dK += dS^T Q_i
 // Operands are read straight from the strided [tokens, 3H] QKV projection through 3-D TMA tensor maps
-// {64 head columns, S rows, B} (rows past the end of a sequence are zero-filled by the TMA unit), with the same
+// {64 head columns, S rows, B} (rows past the end of a sequence are zero-filled by the TMA unit; a head wider than 64
+// columns is two such boxes, 8 KB apart in shared memory), with the same
 // 128-byte-swizzled tiles serving as K-major or MN-major MMA operands depending on the product.
 // The owned dimension is cut into ceil(S / 64) tiles of EQUAL height R = ceil(S / tiles) (S = 257 with the class token ->
 // five tiles of 52 rows; S = 256 -> four of 64; the 77 text states of cross-attention -> two of 39): a tile starts at row
@@ -41,6 +42,11 @@ namespace {
 // 64 columns wide (head h starts at column 48 h; the 16 trailing columns belong to the next head or are zero-filled past the
 // tensor) and simply never enter a product: Q K^T / dO V^T run 3 instead of 4 k-steps, and the accumulate MMAs (P V, dS K,
 // dS^T Q, P^T dO) have N = 48, reading the first 48 columns of their MN-major 128-byte rows.
+// HD = 128 and 96 (hidden 1024 / 8 heads, 768 / 6 heads) go past one box: a Q / K / V / dO tile is two 64-column boxes,
+// loaded at columns h HD and h HD + 64 and stored 8 KB apart.  The score products run 8 (HD 128) or 6 (HD 96) k-steps,
+// the K-major descriptors moving to the second box from k-step 4 on; the accumulate MMAs have N = 128 / 96 and read the
+// second box through the MN-major descriptor's 64-column chunk stride (LBO = 8 KB).  For HD = 96 the second box's last
+// 32 columns belong to the next head (or are zero-filled past the tensor) and never enter a product, as for HD = 48.
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
@@ -57,6 +63,9 @@ constexpr int kConsumers = 128;         // threads of the consumer warpgroup; th
 constexpr int kThreads = kConsumers + 32;
 constexpr int kStages = 2;              // ring stages of looped tiles
 constexpr int kTile = 64 * 64 * 2;      // one 64-row x 64-column bf16 TMA box, 8 KB
+// one 64-row Q / K / V / dO tile of head width HD: ceil(HD / 64) boxes, kTile apart
+template <int HD>
+constexpr int kHdTile = (HD + 63) / 64 * kTile;
 
 struct TcParams {
   int Sq, Skv, nh;
@@ -107,14 +116,26 @@ constexpr int kBarBytes = 64;
 // data-dependent branch, and ptxas then serialises every wgmma of the kernel.)  Each step's MMAs are retired before
 // the next step's are issued, for the same reason: ptxas serialises a pipeline stage across which the next step's
 // fragments are defined.
-// d = A B^T for the 64 rows of A and of B, both K-major with 16 KS columns
+// d = A B^T for the 64 rows of A and of B, both K-major with 16 KS columns (k-steps 4 .. 7 in the second box)
 template <int KS>
 __device__ __forceinline__ void issue_scores(float (&d)[32], uint32_t a, uint32_t b) {
+  constexpr int KS0 = KS < 4 ? KS : 4;
 #pragma unroll
-  for (int ks = 0; ks < KS; ++ks) ptx::Wgmma<64, 0, 0>::run(d, ptx::desc_kmajor(a, ks), ptx::desc_kmajor(b, ks), ks > 0);
+  for (int ks = 0; ks < KS0; ++ks) ptx::Wgmma<64, 0, 0>::run(d, ptx::desc_kmajor(a, ks), ptx::desc_kmajor(b, ks), ks > 0);
+#pragma unroll
+  for (int ks = 0; ks < KS - KS0; ++ks)
+    ptx::Wgmma<64, 0, 0>::run(d, ptx::desc_kmajor(a + kTile, ks), ptx::desc_kmajor(b + kTile, ks), 1);
 }
 
-// d += A B: A the bf16 register fragment of a 64 x 64 product (wgmma.cuh), B MN-major with HD columns
+// Loads the 64-row tile of head columns [col, col + HD) at row `row` of batch b: one TMA box per 64 columns.
+template <int HD>
+__device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int col, int row, int b) {
+#pragma unroll
+  for (int x = 0; x < kHdTile<HD> / kTile; ++x) ptx::tma_load_3d(dst + x * kTile, m, bar, col + 64 * x, row, b);
+}
+
+// d += A B: A the bf16 register fragment of a 64 x 64 product (wgmma.cuh), B MN-major with HD columns (past 64 columns
+// the descriptor's LBO steps to the second box)
 template <int HD>
 __device__ __forceinline__ void issue_acc(float (&d)[HD / 2], const uint32_t (&a)[16], uint32_t b) {
 #pragma unroll
@@ -164,19 +185,22 @@ __device__ __forceinline__ bool kept(const uint32_t (&w)[2][2], int i) {
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-// smem: Q 8K | kStages x {K 8K, V 8K} | barriers
-constexpr int FWD_SMEM = kTile + kStages * 2 * kTile + kBarBytes;
+// smem: Q T | kStages x {K T, V T} | barriers, T = kHdTile<HD> (8 KB up to HD 64: three CTAs per SM; 16 KB past it,
+// 80 KB per CTA: two)
+template <int HD>
+constexpr int fwd_smem() { return kHdTile<HD> + kStages * 2 * kHdTile<HD> + kBarBytes; }
 
 template <int HD, bool DROP>
-__global__ void __launch_bounds__(kThreads, 3)
+__global__ void __launch_bounds__(kThreads, HD > 64 ? 2 : 3)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const TcParams p) {
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t smem[];  // 128B-swizzled tiles need 1024 B alignment
   if ((ptx::smem_u32(smem) & 1023u) != 0) __trap();
+  constexpr int T = kHdTile<HD>;
   uint8_t* sQ = smem;
-  uint8_t* sKV = smem + kTile;
-  const Bars bars(sKV + kStages * 2 * kTile);
+  uint8_t* sKV = smem + T;
+  const Bars bars(sKV + kStages * 2 * T);
 
   const int tid = threadIdx.x;
   const int q0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
@@ -188,15 +212,15 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   if (tid >= kConsumers) {  // producer warp: Q once, then K_j / V_j through the ring
     if (tid == kConsumers) {
-      ptx::mbar_expect_tx(bars.own, kTile);
-      ptx::tma_load_3d(sQ, &tmQ, bars.own, h * HD, q0, b);
+      ptx::mbar_expect_tx(bars.own, T);
+      load_tile<HD>(sQ, &tmQ, bars.own, h * HD, q0, b);
       for (int j = 0; j < ntiles; ++j) {
         bars.wait_empty(j);
         uint64_t* full = &bars.full[j % kStages];
-        uint8_t* sK = sKV + (j % kStages) * 2 * kTile;
-        ptx::mbar_expect_tx(full, 2 * kTile);
-        ptx::tma_load_3d(sK, &tmK, full, h * HD, j * kBN, b);
-        ptx::tma_load_3d(sK + kTile, &tmV, full, h * HD, j * kBN, b);
+        uint8_t* sK = sKV + (j % kStages) * 2 * T;
+        ptx::mbar_expect_tx(full, 2 * T);
+        load_tile<HD>(sK, &tmK, full, h * HD, j * kBN, b);
+        load_tile<HD>(sK + T, &tmV, full, h * HD, j * kBN, b);
       }
     }
     return;
@@ -213,7 +237,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   ptx::mbar_wait(bars.own, 0);
   for (int j = 0; j < ntiles; ++j) {
     const int nvalid = min(kBN, p.Skv - j * kBN);
-    const uint32_t sK = ptx::smem_u32(sKV + (j % kStages) * 2 * kTile);
+    const uint32_t sK = ptx::smem_u32(sKV + (j % kStages) * 2 * T);
     float s[32];
     bars.wait_full(j);
     ptx::wgmma_fence();
@@ -275,7 +299,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
     ptx::wgmma_fence();
-    issue_acc<HD>(o, pa, sK + kTile);
+    issue_acc<HD>(o, pa, sK + T);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_operand(o);
@@ -296,21 +320,23 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
 // ------------------------------------------------------------------------------------------------ backward: dQ
 // The ring streams the K/V tiles twice: sweep 1 accumulates D = sum_j P dP per row, sweep 2 forms dS and dQ.
-// smem: Q 8K | dO 8K | kStages x {K_j 8K, V_j 8K} | barriers
-constexpr int DQ_SMEM = 2 * kTile + kStages * 2 * kTile + kBarBytes;
+// smem: Q T | dO T | kStages x {K_j T, V_j T} | barriers (48 KB up to HD 64, three CTAs per SM; 96 KB past it, two)
+template <int HD>
+constexpr int dq_smem() { return 2 * kHdTile<HD> + kStages * 2 * kHdTile<HD> + kBarBytes; }
 
 template <int HD, bool DROP>
-__global__ void __launch_bounds__(kThreads, 3)
+__global__ void __launch_bounds__(kThreads, HD > 64 ? 2 : 3)
 attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const TcParams p) {
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((ptx::smem_u32(smem) & 1023u) != 0) __trap();
+  constexpr int T = kHdTile<HD>;
   uint8_t* sQ = smem;
-  uint8_t* sdO = smem + kTile;
-  uint8_t* sKV = smem + 2 * kTile;
-  const Bars bars(sKV + kStages * 2 * kTile);
+  uint8_t* sdO = smem + T;
+  uint8_t* sKV = smem + 2 * T;
+  const Bars bars(sKV + kStages * 2 * T);
 
   const int tid = threadIdx.x;
   const int q0 = blockIdx.x * p.tile_rows, h = blockIdx.y, b = blockIdx.z;
@@ -323,17 +349,17 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 
   if (tid >= kConsumers) {  // producer warp: Q, dO once, then K_j / V_j twice through the ring
     if (tid == kConsumers) {
-      ptx::mbar_expect_tx(bars.own, 2 * kTile);
-      ptx::tma_load_3d(sQ, &tmQ, bars.own, h * HD, q0, b);
-      ptx::tma_load_3d(sdO, &tmdO, bars.own, h * HD, q0, b);
+      ptx::mbar_expect_tx(bars.own, 2 * T);
+      load_tile<HD>(sQ, &tmQ, bars.own, h * HD, q0, b);
+      load_tile<HD>(sdO, &tmdO, bars.own, h * HD, q0, b);
       for (int st = 0; st < nsteps; ++st) {
         bars.wait_empty(st);
         uint64_t* full = &bars.full[st % kStages];
-        uint8_t* sK = sKV + (st % kStages) * 2 * kTile;
+        uint8_t* sK = sKV + (st % kStages) * 2 * T;
         const int j = st % ntiles;
-        ptx::mbar_expect_tx(full, 2 * kTile);
-        ptx::tma_load_3d(sK, &tmK, full, h * HD, j * kBN, b);
-        ptx::tma_load_3d(sK + kTile, &tmV, full, h * HD, j * kBN, b);
+        ptx::mbar_expect_tx(full, 2 * T);
+        load_tile<HD>(sK, &tmK, full, h * HD, j * kBN, b);
+        load_tile<HD>(sK + T, &tmV, full, h * HD, j * kBN, b);
       }
     }
     return;
@@ -352,7 +378,7 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   for (int st = 0; st < nsteps; ++st) {
     const int j = st % ntiles;
     const int nvalid = min(kBN, p.Skv - j * kBN);
-    const uint32_t sK = ptx::smem_u32(sKV + (st % kStages) * 2 * kTile);
+    const uint32_t sK = ptx::smem_u32(sKV + (st % kStages) * 2 * T);
     float s[32], dp[32];
     uint32_t kw[2][2];  // keep bits of rows r, r + 8 x column halves of tile j, shifted to this thread's column pairs
     if constexpr (DROP) {
@@ -367,7 +393,7 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     bars.wait_full(st);
     ptx::wgmma_fence();
     issue_scores<HD / 16>(s, ptx::smem_u32(sQ), sK);
-    issue_scores<HD / 16>(dp, ptx::smem_u32(sdO), sK + kTile);
+    issue_scores<HD / 16>(dp, ptx::smem_u32(sdO), sK + T);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_operand(s);
@@ -414,22 +440,27 @@ attn_bwd_dq_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 // Same structure as the dQ kernel, looping over 64-row q tiles; dK and dV of the CTA's kv rows in registers.  The producer
 // warp also stages each q tile's lse (x log2 e) and D (x scale) as 64-float vectors next to the ring, read per column.
 // With dropout the producer also stages the q tile's keep bits: 64 q rows x 2 words (the CTA's 64 kv rows).
-// smem: K 8K | V 8K | kStages x {Q_i 8K, dO_i 8K} | kStages x {lse 64, D 64} floats | [kStages x 128 bit words] | barriers
-constexpr int DKDV_SMEM = 2 * kTile + kStages * 2 * kTile + kStages * 2 * kBN * 4 + kBarBytes;
-constexpr int DKDV_DROP_SMEM = DKDV_SMEM + kStages * 2 * kBN * 4;
-
+// smem: K T | V T | kStages x {Q_i T, dO_i T} | kStages x {lse 64, D 64} floats | [kStages x 128 bit words] | barriers
 template <int HD, bool DROP>
-__global__ void __launch_bounds__(kThreads, 2)
+constexpr int dkdv_smem() {
+  return 2 * kHdTile<HD> + kStages * 2 * kHdTile<HD> + kStages * 2 * kBN * 4 + (DROP ? kStages * 2 * kBN * 4 : 0) + kBarBytes;
+}
+
+// Past HD 64 the dK and dV accumulators (HD / 2 floats each) and the two score fragments need up to 245 registers: the
+// kernel keeps its single consumer warpgroup and runs one CTA per SM (two would cap it at 168 registers and spill).
+template <int HD, bool DROP>
+__global__ void __launch_bounds__(kThreads, HD > 64 ? 1 : 2)
 attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                         const TcParams p) {
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((ptx::smem_u32(smem) & 1023u) != 0) __trap();
+  constexpr int T = kHdTile<HD>;
   uint8_t* sK = smem;
-  uint8_t* sV = smem + kTile;
-  uint8_t* sQO = smem + 2 * kTile;
-  float* sLD = reinterpret_cast<float*>(sQO + kStages * 2 * kTile);
+  uint8_t* sV = smem + T;
+  uint8_t* sQO = smem + 2 * T;
+  float* sLD = reinterpret_cast<float*>(sQO + kStages * 2 * T);
   uint32_t* sBits = reinterpret_cast<uint32_t*>(sLD + kStages * 2 * kBN);  // DROP only: [stage][q 64][2 words]
   const Bars bars(reinterpret_cast<uint8_t*>(sLD + kStages * 2 * kBN) + (DROP ? kStages * 2 * kBN * 4 : 0));
 
@@ -445,9 +476,9 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
   if (tid >= kConsumers) {  // producer warp: K, V once, then {Q_i, dO_i, lse_i, D_i} through the ring
     const int lane = tid & 31;
     if (lane == 0) {
-      ptx::mbar_expect_tx(bars.own, 2 * kTile);
-      ptx::tma_load_3d(sK, &tmK, bars.own, h * HD, kv0, b);
-      ptx::tma_load_3d(sV, &tmV, bars.own, h * HD, kv0, b);
+      ptx::mbar_expect_tx(bars.own, 2 * T);
+      load_tile<HD>(sK, &tmK, bars.own, h * HD, kv0, b);
+      load_tile<HD>(sV, &tmV, bars.own, h * HD, kv0, b);
     }
     for (int i = 0; i < ntiles; ++i) {
       bars.wait_empty(i);
@@ -472,10 +503,10 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
       __syncwarp();  // the vectors are written before lane 0's arrival publishes the stage
       if (lane == 0) {
         uint64_t* full = &bars.full[i % kStages];
-        uint8_t* sQ = sQO + (i % kStages) * 2 * kTile;
-        ptx::mbar_expect_tx(full, 2 * kTile);
-        ptx::tma_load_3d(sQ, &tmQ, full, h * HD, i * kBN, b);
-        ptx::tma_load_3d(sQ + kTile, &tmdO, full, h * HD, i * kBN, b);
+        uint8_t* sQ = sQO + (i % kStages) * 2 * T;
+        ptx::mbar_expect_tx(full, 2 * T);
+        load_tile<HD>(sQ, &tmQ, full, h * HD, i * kBN, b);
+        load_tile<HD>(sQ + T, &tmdO, full, h * HD, i * kBN, b);
       }
     }
     return;
@@ -490,14 +521,14 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
   ptx::mbar_wait(bars.own, 0);
   for (int i = 0; i < ntiles; ++i) {
     const int nvalid = min(kBN, p.Sq - i * kBN);
-    const uint32_t sQ = ptx::smem_u32(sQO + (i % kStages) * 2 * kTile);
+    const uint32_t sQ = ptx::smem_u32(sQO + (i % kStages) * 2 * T);
     const float* sL = sLD + (i % kStages) * 2 * kBN;
     const float* sD = sL + kBN;
     float s[32], dp[32];
     bars.wait_full(i);
     ptx::wgmma_fence();
     issue_scores<HD / 16>(s, ptx::smem_u32(sK), sQ);
-    issue_scores<HD / 16>(dp, ptx::smem_u32(sV), sQ + kTile);
+    issue_scores<HD / 16>(dp, ptx::smem_u32(sV), sQ + T);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_operand(s);
@@ -527,7 +558,7 @@ attn_bwd_dkdv_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_co
       }
     }
     ptx::wgmma_fence();
-    issue_acc<HD>(dv, pa, sQ + kTile);  // dV += P^T dO_i
+    issue_acc<HD>(dv, pa, sQ + T);  // dV += P^T dO_i
     issue_acc<HD>(dk, da, sQ);          // dK += dS^T Q_i
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
@@ -589,12 +620,12 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   if ((rc = qkv_tmap(&tq, q, nh * HD, Sq, B, q_rs))) return rc;
   if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs))) return rc;
   if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs))) return rc;
-  if ((rc = set_smem<attn_fwd_tc_kernel<HD, DROP>>(FWD_SMEM))) return rc;
+  if ((rc = set_smem<attn_fwd_tc_kernel<HD, DROP>>(fwd_smem<HD>()))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale; p.tile_rows = tile_rows;
   p.out0 = reinterpret_cast<bf16*>(o); p.out0_rs = o_rs; p.lse = lse;
   if (DROP) set_drop(p, drop, Skv);
-  pdl_launch(dim3(ntile, nh, B), kThreads, FWD_SMEM, s)(attn_fwd_tc_kernel<HD, DROP>, tq, tk, tv, p);
+  pdl_launch(dim3(ntile, nh, B), kThreads, fwd_smem<HD>(), s)(attn_fwd_tc_kernel<HD, DROP>, tq, tk, tv, p);
   return check_launch("attn_fwd_tc");
 }
 
@@ -611,17 +642,17 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* d_o, 
   if ((rc = qkv_tmap(&tdo, d_o, nh * HD, Sq, B, do_rs))) return rc;
   if ((rc = qkv_tmap(&tk, k, nh * HD, Skv, B, k_rs))) return rc;
   if ((rc = qkv_tmap(&tv, v, nh * HD, Skv, B, v_rs))) return rc;
-  if ((rc = set_smem<attn_bwd_dq_tc_kernel<HD, DROP>>(DQ_SMEM))) return rc;
+  if ((rc = set_smem<attn_bwd_dq_tc_kernel<HD, DROP>>(dq_smem<HD>()))) return rc;
   TcParams p{};
   p.Sq = Sq; p.Skv = Skv; p.nh = nh; p.scale = scale;
   p.out0 = reinterpret_cast<bf16*>(dq); p.out0_rs = dq_rs; p.lse = const_cast<float*>(lse); p.dvec = dvec;
   p.tile_rows = tile_rows;
   if (DROP) set_drop(p, drop, Skv);
-  pdl_launch(dim3(ntile, nh, B), kThreads, DQ_SMEM, s)(attn_bwd_dq_tc_kernel<HD, DROP>, tq, tdo, tk, tv, p);
+  pdl_launch(dim3(ntile, nh, B), kThreads, dq_smem<HD>(), s)(attn_bwd_dq_tc_kernel<HD, DROP>, tq, tdo, tk, tv, p);
   if ((rc = check_launch("attn_bwd_dq_tc"))) return rc;
 
   balanced_tiles(Skv, &ntile, &tile_rows);
-  constexpr int smem = DROP ? DKDV_DROP_SMEM : DKDV_SMEM;
+  constexpr int smem = dkdv_smem<HD, DROP>();
   if ((rc = set_smem<attn_bwd_dkdv_tc_kernel<HD, DROP>>(smem))) return rc;
   p.out0 = reinterpret_cast<bf16*>(dk); p.out0_rs = dk_rs; p.out1 = reinterpret_cast<bf16*>(dv); p.out1_rs = dv_rs;
   p.tile_rows = tile_rows;
@@ -630,7 +661,10 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* d_o, 
 }
 
 int check_args(const char* who, int hd, int a, int b, int c) {
-  if (hd != 64 && hd != 48) { set_last_error("%s: head_dim %d unsupported (64 and 48 are built)", who, hd); return MUSE_ERR_UNSUPPORTED; }
+  if (hd != 48 && hd != 64 && hd != 96 && hd != 128) {
+    set_last_error("%s: head_dim %d unsupported (48, 64, 96 and 128 are built)", who, hd);
+    return MUSE_ERR_UNSUPPORTED;
+  }
   if (((a | b | c) & 7) != 0) { set_last_error("%s: row strides must be multiples of 8 elements", who); return MUSE_ERR_INVALID; }
   return MUSE_OK;
 }
@@ -643,7 +677,7 @@ using namespace muse;
 extern "C" {
 
 // Entry points of the C ABI: Attention.attention of the reference (muse/modeling_transformer.py:221-241) and its autograd
-// backward, head_dim 64 or 48, no mask; with bits, nn.Dropout(p) is applied to the probabilities (:236-237) with the keep
+// backward, head_dim 48, 64, 96 or 128, no mask; with bits, nn.Dropout(p) is applied to the probabilities (:236-237) with the keep
 // bits of philox.cuh (the DROP = true kernels).
 int muse_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, unsigned int* bits,
                   const unsigned long long* seed, int site, float p, int B, int nh, int Sq, int Skv, int hd, int q_rs,
@@ -654,11 +688,18 @@ int muse_attn_fwd(const void* q, const void* k, const void* v, void* o, float* l
   int rc = check_args("attn_fwd", hd, q_rs | o_rs, k_rs, v_rs);
   if (rc) return rc;
   const Drop d{bits, seed, site, p};
-  if (bits == nullptr)
-    return hd == 64 ? attn_fwd_impl<64, false>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
-                    : attn_fwd_impl<48, false>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s);
-  return hd == 64 ? attn_fwd_impl<64, true>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
-                  : attn_fwd_impl<48, true>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s);
+#define MUSE_ATTN_FWD(HD, DROP) attn_fwd_impl<HD, DROP>(q, k, v, o, lse, B, nh, Sq, Skv, q_rs, k_rs, v_rs, o_rs, scale, d, s)
+#define MUSE_ATTN_FWD_HD(DROP)                                                                 \
+  switch (hd) {                                                                                \
+    case 48: return MUSE_ATTN_FWD(48, DROP);                                                   \
+    case 64: return MUSE_ATTN_FWD(64, DROP);                                                   \
+    case 96: return MUSE_ATTN_FWD(96, DROP);                                                   \
+    default: return MUSE_ATTN_FWD(128, DROP);                                                  \
+  }
+  if (bits == nullptr) MUSE_ATTN_FWD_HD(false)
+  MUSE_ATTN_FWD_HD(true)
+#undef MUSE_ATTN_FWD_HD
+#undef MUSE_ATTN_FWD
 }
 
 // D is recomputed from (P, dP) inside the dQ kernel, so the backward does not read O.
@@ -672,8 +713,16 @@ int muse_attn_bwd(const void* q, const void* k, const void* v, const void* d_o, 
   const Drop d{const_cast<unsigned int*>(bits), nullptr, 0, p};
 #define MUSE_ATTN_BWD(HD, DROP) \
   attn_bwd_impl<HD, DROP>(q, k, v, d_o, lse, dvec, dq, dk, dv, B, nh, Sq, Skv, q_rs, k_rs, v_rs, do_rs, dq_rs, dk_rs, dv_rs, scale, d, s)
-  if (bits == nullptr) return hd == 64 ? MUSE_ATTN_BWD(64, false) : MUSE_ATTN_BWD(48, false);
-  return hd == 64 ? MUSE_ATTN_BWD(64, true) : MUSE_ATTN_BWD(48, true);
+#define MUSE_ATTN_BWD_HD(DROP)                                                                 \
+  switch (hd) {                                                                                \
+    case 48: return MUSE_ATTN_BWD(48, DROP);                                                   \
+    case 64: return MUSE_ATTN_BWD(64, DROP);                                                   \
+    case 96: return MUSE_ATTN_BWD(96, DROP);                                                   \
+    default: return MUSE_ATTN_BWD(128, DROP);                                                  \
+  }
+  if (bits == nullptr) MUSE_ATTN_BWD_HD(false)
+  MUSE_ATTN_BWD_HD(true)
+#undef MUSE_ATTN_BWD_HD
 #undef MUSE_ATTN_BWD
 }
 

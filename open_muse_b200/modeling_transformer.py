@@ -801,14 +801,14 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
                                       "not supported")
         if use_mlm_layer and not use_mlm_layernorm and not use_conv_in_out:
             raise NotImplementedError("open_muse_b200: use_mlm_layer without use_mlm_layernorm is not supported yet")
-        if hidden_size % num_attention_heads or hidden_size // num_attention_heads not in (64, 48):
+        if hidden_size % num_attention_heads or hidden_size // num_attention_heads not in (48, 64, 96, 128):
             if hidden_size % num_attention_heads:
                 raise ValueError(
                     f"embed_dim must be divisible by num_heads (got `embed_dim`: {hidden_size} and `num_heads`:"
                     f" {num_attention_heads})."
                 )
-            raise NotImplementedError("open_muse_b200: head_dim must be 64 or 48 (the reference configs use 64, and 48 in "
-                                      "configs/imagenet.yaml / imagenet_movq.yaml: hidden 768, 16 heads)")
+            raise NotImplementedError("open_muse_b200: head_dim must be 48, 64, 96 or 128 (the reference configs use 64, "
+                                      "and 48 in configs/imagenet.yaml / imagenet_movq.yaml: hidden 768, 16 heads)")
         self.vocab_size = vocab_size
         self.hidden_size = hidden_size
         self.num_hidden_layers = num_hidden_layers

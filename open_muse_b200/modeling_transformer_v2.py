@@ -91,9 +91,9 @@ class Attention(nn.Module):
         super().__init__()
         if hidden_size % num_heads != 0:
             raise ValueError(f"self.hidden_size: {hidden_size} must be divisible by self.num_heads: {num_heads}")
-        if hidden_size // num_heads not in (64, 48):
-            raise NotImplementedError("open_muse_b200.MaskGiTUViT_v2: head_dim must be 64 (every U-ViT config of the reference) "
-                                      "or 48; the attention kernels are built for these two widths")
+        if hidden_size // num_heads not in (48, 64, 96, 128):
+            raise NotImplementedError("open_muse_b200.MaskGiTUViT_v2: head_dim must be 48, 64, 96 or 128 (every U-ViT config "
+                                      "of the reference uses 64); the attention kernels are built for these four widths")
         self.num_heads = num_heads
         self.query = nn.Linear(hidden_size, hidden_size, bias=False)
         self.key = nn.Linear(context_dim, hidden_size, bias=False)
@@ -382,7 +382,7 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
             return o
 
         def attn(a, fuse_q):
-            hd = a.out.weight.shape[0] // a.num_heads  # 64: scale 0.125 exactly; 48 for 768-wide / 16-head layers
+            hd = a.out.weight.shape[0] // a.num_heads  # 64: scale 0.125 exactly; 48, 96 or 128 otherwise
             d = {"o": bf(a.out.weight), "nh": a.num_heads, "hd": hd, "sc": 1.0 / math.sqrt(hd)}
             if fuse_q:  # self-attention reads k and v from [q;k;v] only: no separate [k;v] copy of the same weights
                 d["qkv"] = bf(a.query.weight, a.key.weight, a.value.weight)

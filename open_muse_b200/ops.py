@@ -403,7 +403,7 @@ def glu_bwd(ab, dout, dropout=None):
 # ------------------------------------------------------------------------------------------ attention
 def attn_fwd(q, k, v, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
     """q: [B*Sq, *] view with head h at columns h*head_dim; k, v: [B*Skv, *] views.  Returns ctx [B*Sq, nh*head_dim], lse.
-    head_dim: 64 (default) or 48 (configs/imagenet.yaml: hidden 768 / 16 heads).
+    head_dim: 64 (default), 48 (configs/imagenet.yaml: hidden 768 / 16 heads), 96 or 128 (hidden 1024 / 8 heads).
     dropout = (p, seed, site): nn.Dropout(p) on the probabilities with the keep bits of (seed: int64 [1] device tensor,
     site) -- see dropout_fwd; then returns (ctx, lse, bits) with bits int32 [B, nh, Sq, ceil(Skv / 32)] for attn_bwd."""
     st = _prep(q)
@@ -418,7 +418,7 @@ def attn_fwd(q, k, v, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
 
 def attn_bwd(q, k, v, o, do, lse, dq, dk, dv, B, nh, Sq, Skv, scale, head_dim=64, dropout=None):
     """dropout = (p, bits): the rate and the keep bits attn_fwd(..., dropout=...) returned.  o is not read: the kernels
-    recompute what they need from q, k, v and lse."""
+    recompute what they need from q, k, v and lse.  head_dim: 48, 64, 96 or 128, as for attn_fwd."""
     st = _prep(q)
     dvec = torch.empty(B, nh, Sq, dtype=torch.float32, device=q.device)
     p, bits = dropout if dropout is not None else (0.0, None)
