@@ -11,7 +11,11 @@
 //   * backward: dx = norm_bwd(dy) (+ dres), so the residual-stream gradient add is free.
 //   * act=2 with dropout: FeedForward.dropout (:797) on the normalised output -- the forward draws the keep bits
 //              (philox.cuh) and writes the dropped bf16 output and the bits, the backward scales dy by them as it reads it
+#include <climits>
+#include <cstdlib>
+
 #include "philox.cuh"
+#include "ptx.cuh"
 #include "row_norm.cuh"
 
 namespace muse {
@@ -107,8 +111,9 @@ __global__ void __launch_bounds__(1024) colsum_ordered_kernel(const float* __res
   }
 }
 
-// L2 prefetch (a hint: no register, no scoreboard entry).  The persistent row-streaming backward kernels are bound by
-// exposed load latency rather than by issue slots or DRAM bandwidth.  A warp walks its rows strictly one after the
+// L2 prefetch (a hint: no register, no scoreboard entry).  The persistent row-streaming backward kernels of the register
+// path are bound by exposed load latency rather than by issue slots or DRAM bandwidth (the row-ring kernels further down
+// take their place wherever they apply).  A warp walks its rows strictly one after the
 // other, so the lines of the row it will touch NEXT are requested from HBM while the current row is processed and the demand
 // loads become L2 hits.  prefetch_row: the lanes of a warp cover the 128-byte lines of one row of H elements.
 // The GLU + LayerNorm backward prefetches two loop iterations ahead instead (see glu_norm_bwd_kernel).
@@ -543,7 +548,8 @@ __device__ __forceinline__ uint32_t bf16x2_mul(uint32_t a, uint32_t b) {  // bf1
 // The row's 2 * CH 16-byte loads are all issued before any math (CH <= 8: 64 registers of loads in flight per lane, two CTAs
 // per SM): with the loads interleaved chunk by chunk only ~24 KB per SM were in flight, which by Little's law capped the
 // kernel at ~3.7 TB/s whatever the instruction count (same-box A/B: 219 -> 193 us at [65 792, 2 x 2048]).  The backward
-// got nothing from the same treatment (362 -> 360 us): it is bound by instruction issue, and keeps three CTAs per SM.
+// got nothing from the same treatment (362 -> 360 us) at three CTAs per SM; its loads go through a shared-memory row ring
+// instead (glu_norm_bwd_ring_kernel).
 template <int CH, bool DROP>
 __global__ void __launch_bounds__(kGluWarps * 32, (CH <= 8) ? 2 : 1)
 glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf16* __restrict__ y,
@@ -796,6 +802,423 @@ glu_norm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, co
   if (dw) flush_cta_dw(s_dw, kGluWarps, H, dw, dw_ws);
 }
 
+// ---- row-ring backward kernels of a transformer layer: norm_bwd with dres (H <= 1024), norm2_bwd (H <= 512) and the GLU
+// backward with the saved y (H <= 2048).  Same rows, same per-row arithmetic and same weight-gradient order as the
+// register-path kernels above, which stay for the other cases, for inputs that are not 16-byte aligned, and as the
+// cross-check of these (MUSE_NORM_BWD_RING=0).
+// The register-path kernels load through registers and are bound by exposed load latency: a warp keeps its current row
+// (plus a prefetch hint) in flight.  Here one producer thread per CTA copies the CTA's input rows, in the order the warps
+// consume them, into a ring of row stages with 1-D bulk copies (a full / empty mbarrier per stage), and refills a stage
+// as soon as its warp releases it.  The bytes in flight are then set by the ring, not by registers, and every input row
+// is read from HBM exactly once (both passes of the GLU backward read dy from the stage).
+// Row mapping: the register path runs G = bwd_grid(rows) CTAs of 8 warps, CTA b warp w taking rows b*8 + w + k*8G.  A
+// ring CTA has 8 consumer warps and walks the "virtual CTAs" b = blockIdx.x, blockIdx.x + gridDim.x, ... < G one after
+// the other with exactly that mapping.  Each warp keeps its weight-gradient partial in registers (a lane owns fixed
+// columns, as norm_bwd_warp_kernel's does) and virtual CTA b's warp-ordered sum goes to dw_ws[b] as before, so dx and dw
+// are bit-identical to the register path.
+constexpr int kRingWarps = 8;                        // one virtual CTA: kBwdWarps == kGluWarps
+constexpr int kRingThreads = (kRingWarps + 1) * 32;  // + the producer warp
+constexpr int kRingStages = kRingWarps;              // see ring_plan
+constexpr int kRingBarBytes = 2 * kRingStages * 8;   // full[], empty[]
+
+struct RowRing {
+  uint64_t* full;
+  uint64_t* empty;
+  uint8_t* stages;
+  int nstages, stage_bytes;
+  __device__ __forceinline__ uint8_t* stage(int n) const { return stages + static_cast<size_t>(n % nstages) * stage_bytes; }
+  __device__ __forceinline__ uint32_t parity(int n) const { return static_cast<uint32_t>(n / nstages) & 1u; }
+};
+
+// Dynamic shared memory: barriers | sum_floats floats (the CTA's weight-gradient sums) | nstages row stages.
+__host__ __device__ __forceinline__ int ring_sum_bytes(int sum_floats) { return (sum_floats * 4 + 127) & ~127; }
+
+__device__ __forceinline__ RowRing ring_setup(uint8_t* smem, int nstages, int stage_bytes, int sum_floats, float*& s_sum) {
+  RowRing r{reinterpret_cast<uint64_t*>(smem), reinterpret_cast<uint64_t*>(smem) + kRingStages,
+            smem + kRingBarBytes + ring_sum_bytes(sum_floats), nstages, stage_bytes};
+  s_sum = reinterpret_cast<float*>(smem + kRingBarBytes);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < nstages; ++i) {
+      ptx::mbar_init(&r.full[i], 1);
+      ptx::mbar_init(&r.empty[i], 1);  // the consuming warp
+    }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+  return r;
+}
+
+// Calls row_fn(n, row) for the CTA's rows in ring order (n counts them): every row for the producer (warp < 0), warp
+// `warp`'s rows for a consumer; end_vb(vb) after each virtual CTA.
+template <typename RowFn, typename EndFn>
+__device__ __forceinline__ void ring_walk(int rows, int G, int warp, RowFn&& row_fn, EndFn&& end_vb) {
+  int n0 = 0;
+  for (int vb = blockIdx.x; vb < G; vb += gridDim.x) {
+    for (int base = vb * kRingWarps; base < rows; base += G * kRingWarps) {
+      const int cnt = min(kRingWarps, rows - base);
+      if (warp < 0) {
+        for (int i = 0; i < cnt; ++i) row_fn(n0 + i, base + i);
+      } else {
+        if (warp < cnt) row_fn(n0 + warp, base + warp);
+        // No consumer starts a round before every row of the previous one is released: with nstages >= kRingWarps the
+        // stage of ring position n has then completed the fill of n - nstages, so the parity wait cannot alias.
+        ptx::named_barrier_sync(1, kRingWarps * 32);
+      }
+      n0 += cnt;
+    }
+    end_vb(vb);
+  }
+}
+
+// Producer side of one row: waits for the stage to be released, arms its full barrier for `bytes` and hands it to
+// copy(stage, bar), which issues the bulk copies.
+template <typename CopyFn>
+__device__ __forceinline__ void ring_produce(const RowRing& r, int n, uint32_t bytes, CopyFn&& copy) {
+  ptx::mbar_wait(&r.empty[n % r.nstages], r.parity(n) ^ 1u);
+  uint64_t* bar = &r.full[n % r.nstages];
+  ptx::mbar_expect_tx(bar, bytes);
+  copy(r.stage(n), bar);
+}
+__device__ __forceinline__ void ring_release(const RowRing& r, int n, int lane) {
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(&r.empty[n % r.nstages]);
+}
+
+// Virtual CTA vb's weight gradient from the consumer warps' register partials (which are reset): summed in warp order
+// starting from 0 (flush_cta_dw's order) in s_sum, then stored to dw_ws[vb] or added to dw.
+template <int CH>
+__device__ __forceinline__ void ring_flush_dw(float (&acc)[CH][8], float* s_sum, int H, int warp, int lane, float* dw,
+                                              float* dw_ws, int vb) {
+  for (int k = 0; k < kRingWarps; ++k) {
+    if (warp == k) {
+#pragma unroll
+      for (int c = 0; c < CH; ++c) {
+        const int col = row_col(c, lane);
+        if (col < H) {
+          float e[8];
+          if (k == 0) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) e[j] = 0.f;
+          } else {
+            load8(s_sum + col, e);
+          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j) { e[j] += acc[c][j]; acc[c][j] = 0.f; }
+          store8(s_sum + col, e);
+        }
+      }
+    }
+    ptx::named_barrier_sync(1, kRingWarps * 32);
+  }
+  for (int i = threadIdx.x; i < H; i += kRingWarps * 32) {
+    if (dw_ws) dw_ws[static_cast<size_t>(vb) * H + i] = s_sum[i];
+    else atomicAdd(&dw[i], s_sum[i]);
+  }
+  ptx::named_barrier_sync(1, kRingWarps * 32);  // s_sum is free for the next virtual CTA
+}
+
+// norm_bwd_warp_kernel on the ring, with dres.  Stage: x | dy | dres.
+template <typename TDY, typename TX, typename TDX, int CH>
+__global__ void __launch_bounds__(kRingThreads, 1)
+norm_bwd_ring_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const float* __restrict__ w,
+                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
+                     const float* __restrict__ dres, TDX* __restrict__ dx, bf16* __restrict__ dx_copy,
+                     float* __restrict__ dw, float* __restrict__ dw_ws, int rows, int H, int act, int rms, int G,
+                     int nstages) {
+  pdl_enter();
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int xb = H * static_cast<int>(sizeof(TX)), db = H * static_cast<int>(sizeof(TDY)), rb = H * 4;
+  float* s_sum;
+  const RowRing ring = ring_setup(smem, nstages, xb + db + rb, dw ? H : 0, s_sum);
+  if (warp == kRingWarps) {
+    if (lane == 0)
+      ring_walk(rows, G, -1, [&](int n, int row) {
+        ring_produce(ring, n, xb + db + rb, [&](uint8_t* st, uint64_t* bar) {
+          ptx::bulk_load_1d(st, x + static_cast<size_t>(row) * H, xb, bar);
+          ptx::bulk_load_1d(st + xb, dy + static_cast<size_t>(row) * H, db, bar);
+          ptx::bulk_load_1d(st + xb + db, dres + static_cast<size_t>(row) * H, rb, bar);
+        });
+      }, [](int) {});
+    return;
+  }
+  float dw_acc[CH][8];
+#pragma unroll
+  for (int c = 0; c < CH; ++c)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) dw_acc[c][j] = 0.f;
+  const float inv_h = 1.0f / static_cast<float>(H);
+  ring_walk(rows, G, warp, [&](int n, int row) {
+    const float mean = rms ? 0.f : mean_in[row];
+    const float rstd = rstd_in[row];
+    ptx::mbar_wait(&ring.full[n % ring.nstages], ring.parity(n));
+    const uint8_t* st = ring.stage(n);
+    const TX* xr = reinterpret_cast<const TX*>(st);
+    const TDY* dyr = reinterpret_cast<const TDY*>(st + xb);
+    const float* drr = reinterpret_cast<const float*>(st + xb + db);
+    // the register path's statements, with the row read from the stage instead of global memory
+    float xh[CH][8], g[CH][8], rs[CH][8];
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        float xv[8], dv[8], wv[8];
+        load8(xr + col, xv);
+        load8(dyr + col, dv);
+        if (drr) load8(drr + col, rs[c]);
+        if (w) load8(w + col, wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float a = act ? gelu_f(xv[j]) : xv[j];
+          xh[c][j] = (a - mean) * rstd;
+          dw_acc[c][j] += dv[j] * xh[c][j];
+          g[c][j] = dv[j] * (w ? wv[j] : 1.f);
+          row_bwd_acc(g[c][j], xh[c][j], s1, s2);
+        }
+      }
+    }
+    row_bwd_sums(inv_h, rms, s1, s2);
+    TDX* dxr = dx + static_cast<size_t>(row) * H;
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        float o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = row_dx(g[c][j], xh[c][j], s1, s2, rstd);
+        if (act) {
+          float xv[8];
+          load8(xr + col, xv);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[j] *= gelu_grad_f(xv[j]);
+        }
+        if (drr) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[j] += rs[c][j];
+        }
+        store8(dxr + col, o);
+        if (dx_copy) store8(dx_copy + static_cast<size_t>(row) * H + col, o);
+      }
+    }
+    ring_release(ring, n, lane);
+  }, [&](int vb) {
+    if (dw) ring_flush_dw(dw_acc, s_sum, H, warp, lane, dw, dw_ws, vb);
+  });
+}
+
+// norm2_bwd_warp_kernel on the ring, H <= 512.  Stage: x2 | dres | d_h2 | a.  (At H = 1024 the register path's four row
+// arrays and two weight-gradient partials spill.)
+template <int CH>
+__global__ void __launch_bounds__(kRingThreads, 1)
+norm2_bwd_ring_kernel(const bf16* __restrict__ d_h2, const float* __restrict__ x2, const float* __restrict__ w2,
+                      const float* __restrict__ mean2_in, const float* __restrict__ rstd2_in, const float* __restrict__ dres,
+                      const bf16* __restrict__ a, const float* __restrict__ w1, const float* __restrict__ mean1_in,
+                      const float* __restrict__ rstd1_in, float* __restrict__ dx2, bf16* __restrict__ d_a,
+                      float* __restrict__ dw2_ws, float* __restrict__ dw1_ws, int rows, int H, int rms1, int rms2, int G,
+                      int nstages) {
+  pdl_enter();
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int fb = H * 4, hb = H * 2;
+  float* s_sum;
+  const RowRing ring = ring_setup(smem, nstages, 2 * fb + 2 * hb, H, s_sum);
+  if (warp == kRingWarps) {
+    if (lane == 0)
+      ring_walk(rows, G, -1, [&](int n, int row) {
+        ring_produce(ring, n, 2 * fb + 2 * hb, [&](uint8_t* st, uint64_t* bar) {
+          const size_t off = static_cast<size_t>(row) * H;
+          ptx::bulk_load_1d(st, x2 + off, fb, bar);
+          ptx::bulk_load_1d(st + fb, dres + off, fb, bar);
+          ptx::bulk_load_1d(st + 2 * fb, d_h2 + off, hb, bar);
+          ptx::bulk_load_1d(st + 2 * fb + hb, a + off, hb, bar);
+        });
+      }, [](int) {});
+    return;
+  }
+  float acc2[CH][8], acc1[CH][8];
+#pragma unroll
+  for (int c = 0; c < CH; ++c)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { acc2[c][j] = 0.f; acc1[c][j] = 0.f; }
+  const float inv_h = 1.0f / static_cast<float>(H);
+  ring_walk(rows, G, warp, [&](int n, int row) {
+    const size_t off = static_cast<size_t>(row) * H;
+    const float mean2 = rms2 ? 0.f : mean2_in[row], rstd2 = rstd2_in[row];
+    const float mean1 = rms1 ? 0.f : mean1_in[row], rstd1 = rstd1_in[row];
+    ptx::mbar_wait(&ring.full[n % ring.nstages], ring.parity(n));
+    const uint8_t* st = ring.stage(n);
+    const float* xr = reinterpret_cast<const float*>(st);
+    const float* rr = reinterpret_cast<const float*>(st + fb);
+    const bf16* dr = reinterpret_cast<const bf16*>(st + 2 * fb);
+    const bf16* ar = reinterpret_cast<const bf16*>(st + 2 * fb + hb);
+    // the register path's statements, with the row read from the stage instead of global memory
+    float xh[CH][8], g[CH][8], rs[CH][8], av[CH][8];
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        float xv[8], dv[8], wv[8];
+        load8(xr + col, xv);
+        load8(dr + col, dv);
+        load8(rr + col, rs[c]);
+        load8(ar + col, av[c]);
+        load8(w2 + col, wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          xh[c][j] = (xv[j] - mean2) * rstd2;
+          acc2[c][j] += dv[j] * xh[c][j];
+          g[c][j] = dv[j] * wv[j];
+          row_bwd_acc(g[c][j], xh[c][j], s1, s2);
+        }
+      }
+    }
+    row_bwd_sums(inv_h, rms2, s1, s2);
+    float t1 = 0.f, t2 = 0.f;
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        float wv[8];
+        load8(w1 + col, wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float d2 = row_dx(g[c][j], xh[c][j], s1, s2, rstd2) + rs[c][j];  // dx2
+          rs[c][j] = d2;
+          const float ah = (av[c][j] - mean1) * rstd1;
+          av[c][j] = ah;
+          acc1[c][j] += d2 * ah;
+          g[c][j] = d2 * wv[j];
+          row_bwd_acc(g[c][j], ah, t1, t2);
+        }
+        store8(dx2 + off + col, rs[c]);
+      }
+    }
+    row_bwd_sums(inv_h, rms1, t1, t2);
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        float o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = row_dx(g[c][j], av[c][j], t1, t2, rstd1);
+        store8(d_a + off + col, o);
+      }
+    }
+    ring_release(ring, n, lane);
+  }, [&](int vb) {
+    ring_flush_dw(acc2, s_sum, H, warp, lane, nullptr, dw2_ws, vb);
+    ring_flush_dw(acc1, s_sum, H, warp, lane, nullptr, dw1_ws, vb);
+  });
+}
+
+// glu_norm_bwd_kernel<HAVE_Y = true> on the ring, for H <= 2048: the saved forward output y gives the first pass its
+// sums, so a row is dy | y | [a | b], 8 H bytes, and dy is read from the stage by both passes.  (The dropout and
+// recompute variants evaluate the GELU in both passes and stay on the register path.)  Products that the register path
+// rounds before adding them -- behind a `w ?` select, or stored for the shared-memory read-modify-write -- are rounded
+// here too (__fmul_rn), where unrolling would otherwise let the compiler fuse them into the add.
+template <int CH>
+__global__ void __launch_bounds__(kRingThreads, 1)
+glu_norm_bwd_ring_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ ab, const float* __restrict__ w,
+                         const float* __restrict__ mean_in, const float* __restrict__ rstd_in, bf16* __restrict__ dab,
+                         float* __restrict__ dw, float* __restrict__ dw_ws, const bf16* __restrict__ yf, int rows, int H,
+                         int rms, int G, int nstages) {
+  pdl_enter();
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int hb = H * 2;
+  float* s_sum;
+  const RowRing ring = ring_setup(smem, nstages, 4 * hb, dw ? H : 0, s_sum);
+  if (warp == kRingWarps) {
+    if (lane == 0)
+      ring_walk(rows, G, -1, [&](int n, int row) {
+        ring_produce(ring, n, 4 * hb, [&](uint8_t* st, uint64_t* bar) {
+          ptx::bulk_load_1d(st, dy + static_cast<size_t>(row) * H, hb, bar);
+          ptx::bulk_load_1d(st + hb, yf + static_cast<size_t>(row) * H, hb, bar);
+          ptx::bulk_load_1d(st + 2 * hb, ab + static_cast<size_t>(row) * 2 * H, 2 * hb, bar);
+        });
+      }, [](int) {});
+    return;
+  }
+  float acc[CH][8];
+#pragma unroll
+  for (int c = 0; c < CH; ++c)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[c][j] = 0.f;
+  const float inv_h = 1.0f / static_cast<float>(H);
+  ring_walk(rows, G, warp, [&](int n, int row) {
+    const float mean = rms ? 0.f : mean_in[row];
+    const float rstd = rstd_in[row];
+    ptx::mbar_wait(&ring.full[n % ring.nstages], ring.parity(n));
+    const uint8_t* st = ring.stage(n);
+    const bf16* dyr = reinterpret_cast<const bf16*>(st);
+    const bf16* yr = reinterpret_cast<const bf16*>(st + hb);
+    const bf16* xr = reinterpret_cast<const bf16*>(st + 2 * hb);
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        float d[8], yv[8], wv[8];
+        load8(dyr + col, d);
+        load8(yr + col, yv);
+        if (w) load8(w + col, wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          s1 += w ? d[j] * wv[j] : d[j];
+          s2 = fmaf(d[j], yv[j], s2);
+        }
+      }
+    }
+    s1 = rms ? 0.f : warp_sum(s1) * inv_h;
+    s2 = warp_sum(s2) * inv_h;
+    bf16* dr = dab + static_cast<size_t>(row) * 2 * H;
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      const int col = row_col(c, lane);
+      if (col < H) {
+        const uint4 au = *reinterpret_cast<const uint4*>(xr + col);
+        const uint4 bu = *reinterpret_cast<const uint4*>(xr + H + col);
+        const uint4 du = *reinterpret_cast<const uint4*>(dyr + col);
+        const uint32_t aw[4] = {au.x, au.y, au.z, au.w}, bw[4] = {bu.x, bu.y, bu.z, bu.w}, dd[4] = {du.x, du.y, du.z, du.w};
+        float wv[8];
+        if (w) load8(w + col, wv);
+        uint4 oa, ob;
+        uint32_t* pa = reinterpret_cast<uint32_t*>(&oa);
+        uint32_t* pb = reinterpret_cast<uint32_t*>(&ob);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 a2 = unpack_bf16(aw[j]);
+          float g0, g1, t0, t1;
+          gelu_eval(a2.x, g0, t0);
+          gelu_eval(a2.y, g1, t1);
+          const uint32_t gp = pack_bf16(g0, g1);
+          const float2 gr = unpack_bf16(gp);  // bf16(gelu(a))
+          const float2 v2 = unpack_bf16(bf16x2_mul(gp, bw[j]));
+          const float2 b2 = unpack_bf16(bw[j]);
+          const float2 d2 = unpack_bf16(dd[j]);
+          const float xh0 = (v2.x - mean) * rstd, xh1 = (v2.y - mean) * rstd;
+          const float q0 = w ? __fmul_rn(d2.x, wv[2 * j]) : d2.x, q1 = w ? __fmul_rn(d2.y, wv[2 * j + 1]) : d2.y;
+          const float o0 = rstd * (q0 - s1 - xh0 * s2), o1 = rstd * (q1 - s1 - xh1 * s2);
+          pa[j] = pack_bf16(o0 * b2.x * t0, o1 * b2.y * t1);
+          pb[j] = pack_bf16(o0 * gr.x, o1 * gr.y);
+          acc[c][2 * j] += __fmul_rn(d2.x, xh0);
+          acc[c][2 * j + 1] += __fmul_rn(d2.y, xh1);
+        }
+        *reinterpret_cast<uint4*>(dr + col) = oa;
+        *reinterpret_cast<uint4*>(dr + H + col) = ob;
+      }
+    }
+    ring_release(ring, n, lane);
+  }, [&](int vb) {
+    if (dw) ring_flush_dw(acc, s_sum, H, warp, lane, dw, dw_ws, vb);
+  });
+}
+
 template <typename TX, typename TY>
 int fwd_dispatch(const void* x, const float* w, const float* res, void* y, float* mean, float* rstd, int rows, int H,
                  float eps, int act, int rms, cudaStream_t s) {
@@ -825,6 +1248,33 @@ int reduce_dw(const float* dw_ws, float* dw, int grid, int H, cudaStream_t s) {
   return check_launch("norm_bwd colsum");
 }
 
+// Launch shape of a row-ring kernel: one CTA per SM, walking the G virtual CTAs, with kRingStages stages.  Eight
+// stages -- one per consumer warp, the fewest ring_walk allows -- measured fastest for the GLU backward on an H100
+// 80GB HBM3 (700 W): 574 us at [65 792, 2 x 2048] against 589 us with 10 and 716 us with 13, which leave the L1 cache
+// (the same 256 KB as shared memory) too little room for the weight vector; the H = 512 passes measured within 3 %
+// of each other from 8 stages up.  MUSE_NORM_BWD_RING=0 selects the register-path kernels instead (the reference the
+// tests compare against).  stages == 0: take the register path.
+struct RingPlan {
+  int stages = 0, grid = 0;
+  size_t smem = 0;
+};
+constexpr int kSms = 132;
+
+RingPlan ring_plan(int G, int stage_bytes, int sum_floats, std::initializer_list<const void*> inputs) {
+  RingPlan p;
+  for (const void* q : inputs)
+    if (reinterpret_cast<uintptr_t>(q) % 16 != 0) return p;  // the bulk copies need 16-byte aligned rows
+  const char* env = getenv("MUSE_NORM_BWD_RING");
+  if (env && env[0] == '0' && env[1] == 0) return p;
+  const size_t smem = static_cast<size_t>(kRingBarBytes + ring_sum_bytes(sum_floats)) +
+                      static_cast<size_t>(kRingStages) * stage_bytes;
+  if (smem > 227 * 1024) return p;
+  p.stages = kRingStages;
+  p.smem = smem;
+  p.grid = G < kSms ? G : kSms;
+  return p;
+}
+
 template <typename TDY, typename TX, typename TDX>
 int bwd_dispatch(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,
                  const float* dres, void* dx, void* dx_copy, float* dw, float* dw_ws, int rows, int H, int act, int rms,
@@ -833,7 +1283,18 @@ int bwd_dispatch(const void* dy, const void* x, const float* w, const float* mea
   const TDY* dyp = reinterpret_cast<const TDY*>(dy);
   const TX* xp = reinterpret_cast<const TX*>(x);
   TDX* dxp = reinterpret_cast<TDX*>(dx);
-  if (H <= 1024) {
+  const int stage_bytes = H * static_cast<int>(sizeof(TX) + sizeof(TDY) + sizeof(float));
+  // the attention pre-norm of every layer (+ dres); the single norms of the embedding and the head stay on the register path
+  const RingPlan rp = (dres && H <= 1024) ? ring_plan(grid, stage_bytes, dw ? H : 0, {dy, x, dres}) : RingPlan{};
+  if (rp.stages) {
+    with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+      constexpr int CH = decltype(ch)::value;
+      allow_dynamic_smem_once<norm_bwd_ring_kernel<TDY, TX, TDX, CH>>(227 * 1024);
+      pdl_launch(rp.grid, kRingThreads, rp.smem, s)(norm_bwd_ring_kernel<TDY, TX, TDX, CH>, dyp, xp, w, mean, rstd, dres,
+                                                    dxp, reinterpret_cast<bf16*>(dx_copy), dw, dw_ws, rows, H, act, rms,
+                                                    grid, rp.stages);
+    });
+  } else if (H <= 1024) {
     const size_t smem = dw ? static_cast<size_t>(kBwdWarps) * H * sizeof(float) : 0;
     with_row_chunks<1, 2, 4>(H, [&](auto ch) {
       pdl_launch(grid, kBwdWarps * 32, smem, s)(norm_bwd_warp_kernel<TDY, TX, TDX, decltype(ch)::value>, dyp, xp, w, mean,
@@ -926,14 +1387,26 @@ int muse_norm2_bwd(const void* d_h2, const float* x2, const float* w2, const flo
   const int grid = bwd_grid(rows, H, 0);
   float* ws2 = ws;
   float* ws1 = ws + static_cast<size_t>(grid) * H;
-  const size_t smem = static_cast<size_t>(2) * kBwdWarps * H * sizeof(float);
-  with_row_chunks<1, 2, 4>(H, [&](auto ch) {
-    constexpr int CH = decltype(ch)::value;
-    allow_dynamic_smem_once<norm2_bwd_warp_kernel<CH>>(2 * kBwdWarps * 1024 * 4);
-    pdl_launch(grid, kBwdWarps * 32, smem, s)(norm2_bwd_warp_kernel<CH>, reinterpret_cast<const bf16*>(d_h2), x2, w2, mean2,
-                                              rstd2, dres, reinterpret_cast<const bf16*>(a), w1, mean1, rstd1, dx2,
-                                              reinterpret_cast<bf16*>(d_a), ws2, ws1, rows, H, rms1, rms2);
-  });
+  const RingPlan rp = H <= 512 ? ring_plan(grid, 12 * H, H, {d_h2, x2, dres, a}) : RingPlan{};
+  if (rp.stages) {
+    with_row_chunks<1, 2>(H, [&](auto ch) {
+      constexpr int CH = decltype(ch)::value;
+      allow_dynamic_smem_once<norm2_bwd_ring_kernel<CH>>(227 * 1024);
+      pdl_launch(rp.grid, kRingThreads, rp.smem, s)(norm2_bwd_ring_kernel<CH>, reinterpret_cast<const bf16*>(d_h2), x2, w2,
+                                                    mean2, rstd2, dres, reinterpret_cast<const bf16*>(a), w1, mean1, rstd1,
+                                                    dx2, reinterpret_cast<bf16*>(d_a), ws2, ws1, rows, H, rms1, rms2, grid,
+                                                    rp.stages);
+    });
+  } else {
+    const size_t smem = static_cast<size_t>(2) * kBwdWarps * H * sizeof(float);
+    with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+      constexpr int CH = decltype(ch)::value;
+      allow_dynamic_smem_once<norm2_bwd_warp_kernel<CH>>(2 * kBwdWarps * 1024 * 4);
+      pdl_launch(grid, kBwdWarps * 32, smem, s)(norm2_bwd_warp_kernel<CH>, reinterpret_cast<const bf16*>(d_h2), x2, w2,
+                                                mean2, rstd2, dres, reinterpret_cast<const bf16*>(a), w1, mean1, rstd1, dx2,
+                                                reinterpret_cast<bf16*>(d_a), ws2, ws1, rows, H, rms1, rms2);
+    });
+  }
   int rc = check_launch("norm2_bwd");
   if (rc) return rc;
   if ((rc = reduce_dw(ws2, dw2, grid, H, s))) return rc;
@@ -967,6 +1440,19 @@ int muse_norm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const floa
     const int grid = bwd_grid(rows, H, act);
     const size_t smem = dw ? static_cast<size_t>(kGluWarps) * H * sizeof(float) : 0;
     const philox::ElemDrop drop = philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, H);
+    const RingPlan rp = (y_fwd && H <= 2048) ? ring_plan(grid, 8 * H, dw ? H : 0, {dy, x, y_fwd}) : RingPlan{};
+    if (rp.stages) {
+      with_row_chunks<1, 2, 4, 8>(H, [&](auto ch) {
+        constexpr int CH = decltype(ch)::value;
+        allow_dynamic_smem_once<glu_norm_bwd_ring_kernel<CH>>(227 * 1024);
+        pdl_launch(rp.grid, kRingThreads, rp.smem, s)(glu_norm_bwd_ring_kernel<CH>, reinterpret_cast<const bf16*>(dy),
+            reinterpret_cast<const bf16*>(x), w, mean, rstd, reinterpret_cast<bf16*>(dx), dw, dw_ws,
+            reinterpret_cast<const bf16*>(y_fwd), rows, H, rms, grid, rp.stages);
+      });
+      rc = check_launch("glu_norm_bwd");
+      if (rc || !dw || !dw_ws) return rc;
+      return reduce_dw(dw_ws, dw, grid, H, s);
+    }
     allow_dynamic_smem_once<glu_norm_bwd_kernel<false, false>, glu_norm_bwd_kernel<true, false>,
                             glu_norm_bwd_kernel<false, true>>(kGluWarps * 4096 * 4);
     if (y_fwd != nullptr)

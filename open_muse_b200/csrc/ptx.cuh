@@ -91,6 +91,15 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// 1D bulk copy global -> shared of `bytes` contiguous bytes, completion signalled on an mbarrier (complete_tx::bytes).
+// Both addresses and the size are multiples of 16 bytes.
+__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
 // 2D tiled store shared -> global.  Elements of the box outside the tensor map's extents are not written.  The source
 // must be visible to the async proxy (fence_proxy_async after the generic-proxy writes) and stay untouched until
 // bulk_wait_read has covered the store's bulk group.
