@@ -429,8 +429,9 @@ class _ConvHeadFn(torch.autograd.Function):
 class _LayerSpec:
     """Static description of one transformer layer handed to the layer Function."""
 
-    def __init__(self, B, S, H, I, nh, eps, rms, normformer, cross, Skv, E, w, enc_op=None, drop=None):
+    def __init__(self, B, S, H, I, nh, eps, rms, normformer, cross, Skv, E, w, enc_op=None, drop=None, ckpt=False):
         self.B, self.S, self.H, self.I, self.nh = B, S, H, I, nh
+        self.ckpt = ckpt  # gradient checkpointing: the backward recomputes the layer's activations from its input
         # dropout of this layer in training mode: (attention p, hidden p, seed tensor, first site id) -- self-attention
         # uses site, cross-attention site + 1, the FFN site + 2; a rate of 0 leaves its site out
         self.p_attn, self.p_hidden, self.seed, self.site = drop if drop is not None else (0.0, 0.0, None, 0)
@@ -466,95 +467,115 @@ class _EncProjFn(torch.autograd.Function):
         return None, None, None, None, g_proj, g_norm
 
 
+def _layer_body(x, enc, s, params, save, out=True):
+    """The forward of one layer: returns (x3, sv).  save=True keeps in sv (and writes the statistics of) every activation
+    the backward reads; save=False computes the same x3 with no statistics written.  out=False stops after ml, the last
+    tensor the backward reads: the recompute of a checkpointed layer does not run the wo GEMM (x3 is then None)."""
+    it = iter(params)
+    w_attn_ln, _, _, _, _ = next(it), next(it), next(it), next(it), next(it)
+    w_post = next(it) if s.normformer else None
+    w_pre, _, _ = next(it), next(it), next(it)
+    w_mid = next(it) if s.normformer else None
+    next(it)
+    if s.cross:
+        w_cln = next(it)
+        next(it), next(it), next(it), next(it)
+        w_cpost = next(it) if s.normformer else None
+    H, I, B, S, nh = s.H, s.I, s.B, s.S, s.nh
+    sv = {}
+    # ---- self attention
+    h1, st1 = ops.norm_fwd(x, _f32(w_attn_ln), s.eps, torch.bfloat16, rms=s.rms, save_stats=save)
+    qkv = ops.linear_fwd(h1, s.w["qkv"])
+    if s.p_attn:
+        ctxt, lse, abits = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh,
+                                        dropout=(s.p_attn, s.seed, s.site))
+        sv["abits"] = abits
+    else:
+        ctxt, lse = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh)
+    fused_norms = s.normformer and not s.cross and H <= 1024  # post-attention norm + FFN pre-norm in one pass
+    h2 = st3 = None
+    if fused_norms:
+        ao = ops.linear_fwd(ctxt, s.w["ao"])
+        x2, h2, st2 = ops.norm2_fwd(ao, x, _f32(w_post), _f32(w_pre), s.eps, rms1=s.rms, rms2=0, save_stats=save)
+    elif s.normformer:
+        ao = ops.linear_fwd(ctxt, s.w["ao"])
+        x2, st2 = ops.norm_fwd(ao, _f32(w_post), s.eps, torch.float32, res=x, rms=s.rms, save_stats=save)
+    else:
+        ao, st2 = None, None
+        x2 = ops.linear_fwd(ctxt, s.w["ao"], res=x)
+    if save:
+        sv.update(x=x, h1=h1, st1=st1, qkv=qkv, ctxt=ctxt, lse=lse, ao=ao, st2=st2, x2=x2)
+    # ---- cross attention (text conditioning, :886-899)
+    if s.cross:
+        hc, stc = ops.norm_fwd(x2, _f32(w_cln), s.eps, torch.bfloat16, rms=s.rms, save_stats=save)
+        qc = ops.linear_fwd(hc, s.w["cq"])
+        enc_op = s.enc_op if s.enc_op is not None else enc  # bf16 GEMM operand (enc itself may be the fp32 projection)
+        kvc = ops.linear_fwd(enc_op, s.w["ckv"])
+        if s.p_attn:
+            cctx, clse, cbits = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh,
+                                             dropout=(s.p_attn, s.seed, s.site + 1))
+            sv["cbits"] = cbits
+        else:
+            cctx, clse = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh)
+        if s.normformer:
+            cao = ops.linear_fwd(cctx, s.w["co"])
+            x2b, stcp = ops.norm_fwd(cao, _f32(w_cpost), s.eps, torch.float32, res=x2, rms=s.rms, save_stats=save)
+        else:
+            cao, stcp = None, None
+            x2b = ops.linear_fwd(cctx, s.w["co"], res=x2)
+        if save:
+            sv.update(hc=hc, stc=stc, qc=qc, kvc=kvc, cctx=cctx, clse=clse, cao=cao, stcp=stcp, enc=enc_op)
+        x2 = x2b
+        if save:
+            sv["x2b"] = x2b
+    # ---- GLU feed-forward (:785-799)
+    if h2 is None:
+        h2, st3 = ops.norm_fwd(x2, _f32(w_pre), s.eps, torch.bfloat16, rms=0, save_stats=save)
+    ab = ops.linear_fwd(h2, s.w["wi"])
+    # FeedForward.dropout (:797) is fused into the pass that writes ml: ml is then the dropped wo operand (which is
+    # also what the wo weight gradient reads), and the keep bits are saved for the backward
+    ffn_drop = (s.p_hidden, s.seed, s.site + 2)
+    if s.normformer and s.p_hidden:
+        ml, st4, sv["fbits"] = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms,
+                                            save_stats=save, dropout=ffn_drop)
+    elif s.normformer:  # GLU product + mid_mlp_layer_norm in one pass; gelu(a)*b is never written to HBM
+        ml, st4 = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms, save_stats=save)
+    elif s.p_hidden:
+        (ml, sv["fbits"]), st4 = ops.glu_fwd(ab, dropout=ffn_drop), None
+    else:
+        ml, st4 = ops.glu_fwd(ab), None
+    x3 = ops.linear_fwd(ml, s.w["wo"], res=x2) if out else None
+    if save:
+        sv.update(h2=h2, st3=st3, ab=ab, ml=ml, st4=st4, fused_norms=fused_norms)
+    return x3, sv
+
+
 class _LayerFn(torch.autograd.Function):
-    """One pre-LN (normformer) transformer layer: reference TransformerLayer.forward (:875-904)."""
+    """One pre-LN (normformer) transformer layer: reference TransformerLayer.forward (:875-904).
+
+    With gradient checkpointing (spec.ckpt) the forward keeps only its input x, the encoder states and the spec (whose seed
+    tensor and site ids reproduce the dropout masks); the backward re-runs ``_layer_body`` on them with saving on.  Every
+    kernel is run-to-run deterministic, so the recomputed activations, and hence the gradients, are bit-identical to the
+    ones a saving forward would have kept."""
 
     @staticmethod
     def forward(ctx, x, enc, spec, *params):
         s = spec
         grad = s.train and any(ctx.needs_input_grad)  # nothing is saved (no statistics written) under no_grad
-        it = iter(params)
-        w_attn_ln, _, _, _, _ = next(it), next(it), next(it), next(it), next(it)
-        w_post = next(it) if s.normformer else None
-        w_pre, _, _ = next(it), next(it), next(it)
-        w_mid = next(it) if s.normformer else None
-        next(it)
-        if s.cross:
-            w_cln = next(it)
-            next(it), next(it), next(it), next(it)
-            w_cpost = next(it) if s.normformer else None
-        H, I, B, S, nh = s.H, s.I, s.B, s.S, s.nh
-        sv = {}
-        # ---- self attention
-        h1, st1 = ops.norm_fwd(x, _f32(w_attn_ln), s.eps, torch.bfloat16, rms=s.rms, save_stats=grad)
-        qkv = ops.linear_fwd(h1, s.w["qkv"])
-        if s.p_attn:
-            ctxt, lse, abits = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh,
-                                            dropout=(s.p_attn, s.seed, s.site))
-            sv["abits"] = abits
-        else:
-            ctxt, lse = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh)
-        fused_norms = s.normformer and not s.cross and H <= 1024  # post-attention norm + FFN pre-norm in one pass
-        h2 = st3 = None
-        if fused_norms:
-            ao = ops.linear_fwd(ctxt, s.w["ao"])
-            x2, h2, st2 = ops.norm2_fwd(ao, x, _f32(w_post), _f32(w_pre), s.eps, rms1=s.rms, rms2=0, save_stats=grad)
-        elif s.normformer:
-            ao = ops.linear_fwd(ctxt, s.w["ao"])
-            x2, st2 = ops.norm_fwd(ao, _f32(w_post), s.eps, torch.float32, res=x, rms=s.rms, save_stats=grad)
-        else:
-            ao, st2 = None, None
-            x2 = ops.linear_fwd(ctxt, s.w["ao"], res=x)
+        recompute = grad and s.ckpt
+        x3, sv = _layer_body(x, enc, s, params, save=grad and not recompute)
         if grad:
-            sv.update(x=x, h1=h1, st1=st1, qkv=qkv, ctxt=ctxt, lse=lse, ao=ao, st2=st2, x2=x2)
-        # ---- cross attention (text conditioning, :886-899)
-        if s.cross:
-            hc, stc = ops.norm_fwd(x2, _f32(w_cln), s.eps, torch.bfloat16, rms=s.rms, save_stats=grad)
-            qc = ops.linear_fwd(hc, s.w["cq"])
-            enc_op = s.enc_op if s.enc_op is not None else enc  # bf16 GEMM operand (enc itself may be the fp32 projection)
-            kvc = ops.linear_fwd(enc_op, s.w["ckv"])
-            if s.p_attn:
-                cctx, clse, cbits = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh,
-                                                 dropout=(s.p_attn, s.seed, s.site + 1))
-                sv["cbits"] = cbits
-            else:
-                cctx, clse = ops.attn_fwd(qc, kvc[:, :H], kvc[:, H:], B, nh, S, s.Skv, s.scale, head_dim=H // nh)
-            if s.normformer:
-                cao = ops.linear_fwd(cctx, s.w["co"])
-                x2b, stcp = ops.norm_fwd(cao, _f32(w_cpost), s.eps, torch.float32, res=x2, rms=s.rms, save_stats=grad)
-            else:
-                cao, stcp = None, None
-                x2b = ops.linear_fwd(cctx, s.w["co"], res=x2)
-            if grad:
-                sv.update(hc=hc, stc=stc, qc=qc, kvc=kvc, cctx=cctx, clse=clse, cao=cao, stcp=stcp, enc=enc_op)
-            x2 = x2b
-            if grad:
-                sv["x2b"] = x2b
-        # ---- GLU feed-forward (:785-799)
-        if h2 is None:
-            h2, st3 = ops.norm_fwd(x2, _f32(w_pre), s.eps, torch.bfloat16, rms=0, save_stats=grad)
-        ab = ops.linear_fwd(h2, s.w["wi"])
-        # FeedForward.dropout (:797) is fused into the pass that writes ml: ml is then the dropped wo operand (which is
-        # also what the wo weight gradient reads), and the keep bits are saved for the backward
-        ffn_drop = (s.p_hidden, s.seed, s.site + 2)
-        if s.normformer and s.p_hidden:
-            ml, st4, sv["fbits"] = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms,
-                                                save_stats=grad, dropout=ffn_drop)
-        elif s.normformer:  # GLU product + mid_mlp_layer_norm in one pass; gelu(a)*b is never written to HBM
-            ml, st4 = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms, save_stats=grad)
-        elif s.p_hidden:
-            (ml, sv["fbits"]), st4 = ops.glu_fwd(ab, dropout=ffn_drop), None
-        else:
-            ml, st4 = ops.glu_fwd(ab), None
-        x3 = ops.linear_fwd(ml, s.w["wo"], res=x2)
-        if grad:
-            sv.update(h2=h2, st3=st3, ab=ab, ml=ml, st4=st4, fused_norms=fused_norms)
-            ctx.sv, ctx.spec, ctx.params = sv, s, params
+            ctx.sv = None if recompute else sv
+            ctx.inputs = (x, enc) if recompute else None
+            ctx.spec, ctx.params = s, params
         return x3
 
     @staticmethod
     def backward(ctx, dx3):
         s, sv, params = ctx.spec, ctx.sv, ctx.params
+        if ctx.inputs is not None:  # checkpointed: recompute the saved set from the layer's input
+            _, sv = _layer_body(*ctx.inputs, s, params, save=True, out=False)
+            ctx.inputs = None
         H, I, B, S, nh = s.H, s.I, s.B, s.S, s.nh
         dev = dx3.device
         dx3 = dx3.contiguous()
@@ -979,7 +1000,8 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
         for i, layer in enumerate(self.transformer_layers):
             spec = _LayerSpec(B, S, H, self.intermediate_size, self.num_attention_heads, c.layer_norm_eps, rms,
                               c.use_normformer, enc is not None, Skv, E, packed.layers[i], enc_op,
-                              drop=(p_attn, p_hidden, seed, 1 + 3 * i) if seed is not None else None)
+                              drop=(p_attn, p_hidden, seed, 1 + 3 * i) if seed is not None else None,
+                              ckpt=self.gradient_checkpointing)
             x = _LayerFn.apply(x, enc, spec, *self._layer_params(layer))
 
         flat_labels = labels.reshape(-1).contiguous().to(torch.int64) if labels is not None else None

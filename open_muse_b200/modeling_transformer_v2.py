@@ -15,6 +15,7 @@ Activations are token-major ``[B*h*w, C]`` throughout -- the NCHW <-> NHWC permu
 from __future__ import annotations
 
 import math
+from functools import partial
 from typing import Tuple
 
 import numpy as np
@@ -285,6 +286,19 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
 
     def _set_gradient_checkpointing(self, module, value=False):
         self.gradient_checkpointing = value
+        if isinstance(module, (DownsampleBlock, UpsampleBlock)):
+            module.gradient_checkpointing = value
+
+    def enable_gradient_checkpointing(self):
+        """Recompute activations in the backward instead of keeping them: every transformer layer, and the res + attention
+        pairs of the down / up stages (each stage's own flag, as the reference's ``_set_gradient_checkpointing`` sets them).
+        The recomputed activations are bit-identical to the saved ones, so the gradients equal those without it (up to the
+        fp32-atomic summation order of the weight gradients, as between any two runs); only training forwards that a
+        backward can follow recompute."""
+        self.apply(partial(self._set_gradient_checkpointing, value=True))
+
+    def disable_gradient_checkpointing(self):
+        self.apply(partial(self._set_gradient_checkpointing, value=False))
 
     def generate(self):
         assert False  # (reference :326-328)

@@ -160,7 +160,9 @@ def _res_block_bwd(dh3, st, w, g, mod_all, d_mod_all, B, hw, eps, rms):
     return ops.dwconv3x3_norm_bwd(dd, conv, h, w["dw"], w["dw_norm"], dh2, g.of("dw"), g.of("dw_norm"), B, hw, hw, eps, rms)
 
 
-def _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=None):
+def _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=None, out=True):
+    """out=False (the recompute of a checkpointed block): the last GEMM, whose output the backward never reads, is skipped
+    and None is returned in its place."""
     se = encb = None
     if w["kvm"] is not None:
         se = ops.silu_bf16(enc)
@@ -171,7 +173,7 @@ def _attn_block_fwd(h, enc, w, B, S, Skv, eps, rms, drop=None):
     a1o = ops.linear_fwd(c1, w["a1"]["o"])
     r2, y2 = ops.add_norm_mod(a1o, w["ln2"], eps, rms, **_form(w["a2"]["q"]), residual=h)
     c2, s2 = _attn_fwd(y2, ctx_in, w["a2"], B, S, Skv, False, _site(drop, 2, attn=True))
-    out = ops.linear_fwd(c2, w["a2"]["o"], res=r2)
+    out = ops.linear_fwd(c2, w["a2"]["o"], res=r2) if out else None
     return out, (h, se, ctx_in, y1, c1, s1, r2, y2, c2, s2)
 
 
@@ -191,7 +193,8 @@ def _attn_block_bwd(dout, st, w, g, enc, d_enc, B, S, Skv, eps, rms):
     return dh
 
 
-def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=None):
+def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=None, out=True):
+    """out=False: as _attn_block_fwd, the wo GEMM is skipped and f is None."""
     m = lambda k: mod_all[:, w[k][0]:w[k][0] + w[k][1]]
     r1, y1 = ops.add_norm_mod(x, w["ln1"], eps, rms, **_form(w["sa"]["qkv"]), residual=r, mod=m("mod1"),
                               rows_per_sample=S)
@@ -210,7 +213,7 @@ def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=None):
     else:  # GLUFeedForward.dropout fused into the GLU pass: gl is the dropped wo operand
         gl, bits = ops.glu_fwd(ab, dropout=fd)
         fdr = (fd[0], bits)
-    f = ops.linear_fwd(gl, w["wo"])
+    f = ops.linear_fwd(gl, w["wo"]) if out else None
     return f, r3, (r is not None, r1, y1, c, s_sa, r2, y2, cc, s_ca, r3, y3, ab, gl, fdr)
 
 
@@ -376,15 +379,25 @@ def block_params(rb, ab):
 
 
 class UBlockFn(torch.autograd.Function):
-    """ResBlock + AttentionBlock2D pair of the down / up stage"""
+    """ResBlock + AttentionBlock2D pair of the down / up stage.  ckpt (gradient checkpointing): the forward keeps only its
+    input h and its adaLN rows mod, and the backward re-runs the pair's forward with saving on; every kernel is
+    deterministic and the dropout masks follow from the seed tensor, so the recomputed state is the one a saving forward
+    would have kept, bit for bit."""
 
     @staticmethod
-    def forward(ctx, sh, model, which, idx, drop, h, enc32, sc32, *params):
+    def forward(ctx, sh, model, which, idx, drop, ckpt, h, enc32, sc32, *params):
         w = sh.W[which][idx]
         wl, w_map = _local_mods(sh, w, ["mod"])
         mod = ops.linear_fwd(sh.sc, w_map, out_dtype=F32)
-        h, s_r = _res_block_fwd(h, wl, mod, sh.B, sh.hw, sh.eps, sh.rms, drop=drop)
-        h, s_a = _attn_block_fwd(h, sh.enc, wl, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop)
+        if ckpt:
+            ctx.inputs = (h, drop)
+            h, _ = _res_block_fwd(h, wl, mod, sh.B, sh.hw, sh.eps, sh.rms, save=False, drop=drop)
+            h, _ = _attn_block_fwd(h, sh.enc, wl, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop)
+            s_r = s_a = None
+        else:
+            ctx.inputs = None
+            h, s_r = _res_block_fwd(h, wl, mod, sh.B, sh.hw, sh.eps, sh.rms, drop=drop)
+            h, s_a = _attn_block_fwd(h, sh.enc, wl, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop)
         ctx.sh, ctx.sv, ctx.key = sh, (wl, w_map, mod, s_r, s_a), (model, which, idx)
         ctx.set_materialize_grads(False)
         return h
@@ -392,6 +405,11 @@ class UBlockFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dh):
         sh, (wl, w_map, mod, s_r, s_a), (model, which, idx) = ctx.sh, ctx.sv, ctx.key
+        if ctx.inputs is not None:  # checkpointed: recompute the saved state from the block's input
+            h, drop = ctx.inputs
+            h, s_r = _res_block_fwd(h, wl, mod, sh.B, sh.hw, sh.eps, sh.rms, drop=drop)
+            _, s_a = _attn_block_fwd(h, sh.enc, wl, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop, out=False)
+            ctx.inputs = None
         stage = model.down_blocks[0] if which == "down" else model.up_blocks[0]
         rb, ab = stage.res_blocks[idx], stage.attention_blocks[idx]
         g, d_enc, d_mod = _G(wl), _z(sh.enc), _z(mod)
@@ -402,7 +420,7 @@ class UBlockFn(torch.autograd.Function):
         grads = [g["dw"].t().contiguous(), g.get("dw_norm"), g["cw0"], g["gamma"], g["beta"], g["cw4"], g_map, g.get("kvm"),
                  g.get("ln1")] + _attn_grads(g["a1"], ab.attention, False) + [g.get("ln2")] + _attn_grads(g["a2"], ab.crossattention, False)
         ctx.sv = None  # release the block's activations now, not when the graph dies
-        return (None, None, None, None, None, dh, d_enc, d_sc32, *_align(params, grads))
+        return (None, None, None, None, None, None, dh, d_enc, d_sc32, *_align(params, grads))
 
 
 def layer_params(l):
@@ -413,18 +431,22 @@ def layer_params(l):
 
 
 class ULayerFn(torch.autograd.Function):
-    """one TransformerLayer carrying (hidden, residual)"""
+    """one TransformerLayer carrying (hidden, residual).  ckpt: as UBlockFn, the forward keeps only x, r and mod."""
 
     @staticmethod
-    def forward(ctx, sh, model, idx, drop, x, r, enc32, sc32, *params):
+    def forward(ctx, sh, model, idx, drop, ckpt, x, r, enc32, sc32, *params):
         w = sh.W["layers"][idx]
         wl, w_map = _local_mods(sh, w, ["mod1", "mod2", "mod3"])
         mod = ops.linear_fwd(sh.sc, w_map, out_dtype=F32)
         f, r3, s_l = _layer_fwd(x, r, sh.enc, wl, mod, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop)
-        s_l = list(s_l)
-        assert s_l[9] is r3
-        s_l[9] = None  # r3 is an OUTPUT of this Function: held through save_for_backward, a ctx attribute would be a cycle
-        ctx.save_for_backward(r3)
+        if ckpt:
+            ctx.inputs, s_l = (x, r, drop), None
+        else:
+            ctx.inputs = None
+            s_l = list(s_l)
+            assert s_l[9] is r3
+            s_l[9] = None  # r3 is an OUTPUT of this Function: held through save_for_backward, a ctx attribute would be a cycle
+            ctx.save_for_backward(r3)
         ctx.sh, ctx.sv, ctx.key = sh, (wl, w_map, mod, s_l), (model, idx)
         ctx.set_materialize_grads(False)
         return f, r3
@@ -432,8 +454,13 @@ class ULayerFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, df, dr3):
         sh, (wl, w_map, mod, s_l), (model, idx) = ctx.sh, ctx.sv, ctx.key
-        s_l = list(s_l)
-        s_l[9] = ctx.saved_tensors[0]
+        if ctx.inputs is not None:  # checkpointed: recompute the saved state (r3 included) from the layer's inputs
+            x, r, drop = ctx.inputs
+            _, _, s_l = _layer_fwd(x, r, sh.enc, wl, mod, sh.B, sh.S, sh.Skv, sh.eps, sh.rms, drop=drop, out=False)
+            ctx.inputs = None
+        else:
+            s_l = list(s_l)
+            s_l[9] = ctx.saved_tensors[0]
         l = model.transformer_layers[idx]
         g, d_enc, d_mod = _G(wl), _z(sh.enc), _z(mod)
         if df is None:
@@ -448,7 +475,7 @@ class ULayerFn(torch.autograd.Function):
             _attn_grads(g["ca"], l.crossattention, False) + [g_map[H2:2 * H2], g.get("ln3"), g_map[2 * H2:], g["wi"][:I], g["wi"][I:],
                                                              g["wo"]]
         ctx.sv = None  # release the block's activations now, not when the graph dies
-        return (None, None, None, None, dx, dr, d_enc, d_sc32, *_align(params, grads))
+        return (None, None, None, None, None, dx, dr, d_enc, d_sc32, *_align(params, grads))
 
 
 class ProjFn(torch.autograd.Function):
@@ -588,15 +615,20 @@ def train_forward(model, input_ids, encoder_hidden_states, cond_embeds, micro_co
         sh = copy.copy(sh_full)  # same operand caches (W, enc, sc), coarse grid
         sh.S, sh.hw = S // 4, sh_full.hw // 2
     R, L = len(down.res_blocks), len(model.transformer_layers)
+    # gradient checkpointing where the reference checkpoints (:276-278, :531-533, :570-572): the transformer layers when the
+    # model's flag is set, a stage's res + attention pairs when that stage's own flag is set
+    ck_down, ck_up = down.training and down.gradient_checkpointing, up.training and up.gradient_checkpointing
+    ck_layers = model.training and model.gradient_checkpointing
     for i, (rb, ab) in enumerate(zip(down.res_blocks, down.attention_blocks)):
-        h = UBlockFn.apply(sh, model, "down", i, unit_drop(drop, i), h, enc32, sc32, *_present(block_params(rb, ab)))
+        h = UBlockFn.apply(sh, model, "down", i, unit_drop(drop, i), ck_down, h, enc32, sc32, *_present(block_params(rb, ab)))
     x = ProjFn.apply(sh, "pth", h, None, model.project_to_hidden_norm.weight, model.project_to_hidden.weight)
     r = None
     for i, l in enumerate(model.transformer_layers):
-        x, r = ULayerFn.apply(sh, model, i, unit_drop(drop, R + i), x, r, enc32, sc32, *_present(layer_params(l)))
+        x, r = ULayerFn.apply(sh, model, i, unit_drop(drop, R + i), ck_layers, x, r, enc32, sc32, *_present(layer_params(l)))
     h = ProjFn.apply(sh, "pfh", x, r, model.project_from_hidden_norm.weight, model.project_from_hidden.weight)
     for i, (rb, ab) in enumerate(zip(up.res_blocks, up.attention_blocks)):
-        h = UBlockFn.apply(sh, model, "up", i, unit_drop(drop, R + L + i), h, enc32, sc32, *_present(block_params(rb, ab)))
+        h = UBlockFn.apply(sh, model, "up", i, unit_drop(drop, R + L + i), ck_up, h, enc32, sc32,
+                           *_present(block_params(rb, ab)))
     if c.force_down_up_sample:  # back to the full grid (:555-559); sh still describes the coarse grid this op reads
         h = ResampleFn.apply(sh, "us", h, up.upsample[0].norm.weight, up.upsample[1].weight)
         sh = sh_full
