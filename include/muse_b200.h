@@ -74,8 +74,8 @@ int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int 
 /* FP8 forward GEMM (inference): C bf16 [M,N] (pitch ldc) = bf16(sum_k A[m,k] B[n,k] * sa[m] * sb[n]), A e4m3 row-major
  * [M,K] (pitch lda bytes), B e4m3 row-major [N,K] (pitch ldb bytes), sa fp32 [M], sb fp32 [N] (8-byte aligned); fp32
  * accumulation with each 128-wide k-block's partial sum promoted into fp32 registers.  N and ldc multiples of 8; lda / ldb
- * multiples of 16.  The e4m3 producers: muse_add_norm_mod_fwd, muse_dwconv3x3_norm_fwd, muse_glu_fwd (dtype code 2) and
- * muse_quantize_rows_e4m3. */
+ * multiples of 16.  The e4m3 producers: muse_add_norm_mod_fwd, muse_dwconv3x3_norm_fwd, muse_glu_fwd, muse_gelu_tanh_fwd
+ * (dtype code 2) and muse_quantize_rows_e4m3. */
 int muse_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
                   int ldb, int ldc, void* stream);
 
@@ -198,6 +198,13 @@ int muse_glu_fwd(const void* ab, void* out, int out_dtype, float* row_scale, uns
                  const unsigned long long* seed, int site, float p, long long rows, int I, void* stream);
 int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
                  void* stream);
+
+/* Activation of FusedGeLUFeedForward (muse/modeling_transformer_v2.py:954-996, use_fused_mlp): pre bf16 [rows, I] =
+ * wi_0(x), out [rows, I] = gelu_tanh(pre) = 0.5 pre (1 + tanh(sqrt(2/pi) (pre + 0.044715 pre^3))) with accurate tanhf.
+ * out_dtype 1: bf16.  out_dtype 2: e4m3 with its scales in row_scale fp32 [rows] (required then; a warp per row,
+ * I <= 4096).  The reference applies no dropout in this block.  Backward: dpre bf16 [rows, I] = dout * gelu_tanh'(pre). */
+int muse_gelu_tanh_fwd(const void* pre, void* out, int out_dtype, float* row_scale, long long rows, int I, void* stream);
+int muse_gelu_tanh_bwd(const void* pre, const void* dout, void* dpre, long long rows, int I, void* stream);
 
 /* Attention.attention (:221-241) fused: O = softmax(Q K^T * scale) V per (batch, head), head_dim 48, 64, 96
  * or 128 (48: configs/imagenet.yaml, hidden 768 / 16 heads; 128: hidden 1024 / 8 heads); any other width returns

@@ -46,6 +46,8 @@ SIGNATURES = {
     "muse_norm2_bwd": (c_int, [_P] * 15 + [_I, _I, _I, _I, _P]),
     "muse_glu_fwd": (c_int, [_P, _P, _I, _P, _P, _P, _I, _F, _L, _I, _P]),
     "muse_glu_bwd": (c_int, [_P, _P, _P, _F, _P, _L, _I, _P]),
+    "muse_gelu_tanh_fwd": (c_int, [_P, _P, _I, _P, _L, _I, _P]),
+    "muse_gelu_tanh_bwd": (c_int, [_P, _P, _P, _L, _I, _P]),
     "muse_attn_fwd": (c_int, [_P] * 7 + [_I, _F] + [_I] * 9 + [_F, _P]),
     "muse_attn_bwd": (c_int, [_P] * 6 + [_F] + [_P] * 4 + [_I] * 12 + [_F, _P]),
     "muse_dropout_fwd": (c_int, [_P, _P, _I, _P, _P, _I, _F, _L, _I, _P]),

@@ -1,8 +1,9 @@
 // HBM-bound elementwise / gather kernels of the transformer step:
 //   * multi-tensor fp32 -> bf16 weight packing (one launch for all Linear weights of a model)
 //   * token + position embedding gather (muse/modeling_transformer.py:942-957) and its backward
-//   * GLU: gelu(a) * b (muse/modeling_transformer.py:789-792) forward / backward; its e4m3 form (a warp per row, which the
-//     row's scale needs) writes the wo operand of the FP8 GEMM
+//   * the FFN activations, one templated pass: GLU gelu(a) * b (muse/modeling_transformer.py:789-792) and the ungated
+//     tanh-GELU of FusedGeLUFeedForward (muse/modeling_transformer_v2.py:954-996), forward / backward; their e4m3 form (a
+//     warp per row, which the row's scale needs) writes the wo operand of the FP8 GEMM
 //   * per-row e4m3 quantization of the bf16 weight operands of the FP8 GEMM
 //   * plain fp32 -> bf16 cast (gradient of the residual stream entering a dgrad GEMM)
 //   * nn.Dropout of the embedding output and of the FFN hidden state (keep bits of philox.cuh) and its backward
@@ -256,26 +257,51 @@ __global__ void __launch_bounds__(512) embed_seg_final_kernel(const int* __restr
   ordered_rows_sum([&](int i) { return ws + static_cast<size_t>(c0 + i) * H; }, nc, H, s_q, out);
 }
 
-// ---------------------------------------------------------------- GLU
-// ab: [rows, 2*I] bf16 (a = cols [0,I), b = cols [I,2I)); out [rows, I] bf16.
+// ---------------------------------------------------------------- FFN activation: GLU / tanh-GELU
+// GATED (GLUFeedForward): ab [rows, 2*I] bf16 (a = cols [0,I), b = cols [I,2I)); out [rows, I] bf16 = bf16(gelu(a)) * b.
 // Rounding points follow the reference under bf16 autocast: gelu(a) is rounded to bf16 before the product.
+// !GATED (FusedGeLUFeedForward, muse/modeling_transformer_v2.py:954-996): ab is the pre-activation [rows, I] bf16 and
+// out = gelu_tanh(pre); the reference's dropout module of that block is never applied, so there is no DROP variant.
 // DROP: FeedForward.dropout (:797) fused -- the forward draws the chunk's keep byte (philox.cuh elementwise mapping), writes
 // the dropped product and the byte (the last chunk of a row also zeroes the pad bytes of the row's last word); the
 // backward scales dout by the stored byte as it reads it.
-template <bool DROP>
+
+// F.gelu(x, approximate="tanh") and its derivative with torch's formula and constants (ATen GeluKernel), accurate tanhf
+constexpr float kGeluTanhBeta = 0.7978845608028654f;  // sqrt(2 / pi)
+constexpr float kGeluTanhKappa = 0.044715f;
+__device__ __forceinline__ float gelu_tanh_f(float x) {
+  const float inner = kGeluTanhBeta * (x + kGeluTanhKappa * (x * x * x));
+  return 0.5f * x * (1.f + tanhf(inner));
+}
+__device__ __forceinline__ float gelu_tanh_grad_f(float x) {
+  const float x_sq = x * x;
+  const float t = tanhf(kGeluTanhBeta * (x + kGeluTanhKappa * (x_sq * x)));
+  const float left = 0.5f * x, right = 1.f + t;
+  return 0.5f * right + left * (1.f - t * t) * kGeluTanhBeta * (1.f + 3.f * kGeluTanhKappa * x_sq);
+}
+
+template <bool GATED, bool DROP>
 __global__ void __launch_bounds__(256)
-glu_fwd_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, long long rows, int I, const philox::ElemDrop dr) {
+ffn_act_fwd_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, long long rows, int I, const philox::ElemDrop dr) {
+  static_assert(GATED || !DROP, "the tanh-GELU pass has no dropout");
   pdl_enter();
   const int chunks = I / 8;
   const long long idx = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (idx >= rows * chunks) return;
   const long long r = idx / chunks;
   const int c = static_cast<int>(idx % chunks) * 8;
-  float a[8], b[8], o[8];
-  load8(ab + r * 2 * I + c, a);
-  load8(ab + r * 2 * I + I + c, b);
+  float a[8], o[8];
+  if constexpr (GATED) {
+    float b[8];
+    load8(ab + r * 2 * I + c, a);
+    load8(ab + r * 2 * I + I + c, b);
 #pragma unroll
-  for (int j = 0; j < 8; ++j) o[j] = bf16_round(gelu_f(a[j])) * b[j];
+    for (int j = 0; j < 8; ++j) o[j] = bf16_round(gelu_f(a[j])) * b[j];
+  } else {
+    load8(ab + r * I + c, a);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = gelu_tanh_f(a[j]);
+  }
   if constexpr (DROP) {
     const uint32_t kb = philox::elem_keep8(*dr.seed, dr.site, static_cast<uint32_t>(r), c / 8, dr.thresh);
 #pragma unroll
@@ -288,34 +314,45 @@ glu_fwd_kernel(const bf16* __restrict__ ab, bf16* __restrict__ out, long long ro
   store8(out + r * I + c, o);
 }
 
-template <bool DROP>
+// GATED: dab = [d a | d b]; !GATED: dab = dpre [rows, I] = dout * gelu_tanh'(pre)
+template <bool GATED, bool DROP>
 __global__ void __launch_bounds__(256)
-glu_bwd_kernel(const bf16* __restrict__ ab, const bf16* __restrict__ dout, bf16* __restrict__ dab, long long rows, int I,
-               const philox::ElemDrop dr) {
+ffn_act_bwd_kernel(const bf16* __restrict__ ab, const bf16* __restrict__ dout, bf16* __restrict__ dab, long long rows, int I,
+                   const philox::ElemDrop dr) {
+  static_assert(GATED || !DROP, "the tanh-GELU pass has no dropout");
   pdl_enter();
   const int chunks = I / 8;
   const long long idx = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (idx >= rows * chunks) return;
   const long long r = idx / chunks;
   const int c = static_cast<int>(idx % chunks) * 8;
-  float a[8], b[8], d[8], da[8], db[8];
-  load8(ab + r * 2 * I + c, a);
-  load8(ab + r * 2 * I + I + c, b);
-  load8(dout + r * I + c, d);
-  if constexpr (DROP) {
-    const uint32_t kb = dr.bits[r * dr.row_bytes + c / 8];
+  if constexpr (GATED) {
+    float a[8], b[8], d[8], da[8], db[8];
+    load8(ab + r * 2 * I + c, a);
+    load8(ab + r * 2 * I + I + c, b);
+    load8(dout + r * I + c, d);
+    if constexpr (DROP) {
+      const uint32_t kb = dr.bits[r * dr.row_bytes + c / 8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) d[j] *= philox::keep_z(kb, j, dr.scale);
-  }
+      for (int j = 0; j < 8; ++j) d[j] *= philox::keep_z(kb, j, dr.scale);
+    }
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float gv, gg;
-    gelu_eval(a[j], gv, gg);
-    da[j] = d[j] * b[j] * gg;
-    db[j] = d[j] * bf16_round(gv);
+    for (int j = 0; j < 8; ++j) {
+      float gv, gg;
+      gelu_eval(a[j], gv, gg);
+      da[j] = d[j] * b[j] * gg;
+      db[j] = d[j] * bf16_round(gv);
+    }
+    store8(dab + r * 2 * I + c, da);
+    store8(dab + r * 2 * I + I + c, db);
+  } else {
+    float a[8], d[8];
+    load8(ab + r * I + c, a);
+    load8(dout + r * I + c, d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) d[j] *= gelu_tanh_grad_f(a[j]);
+    store8(dab + r * I + c, d);
   }
-  store8(dab + r * 2 * I + c, da);
-  store8(dab + r * 2 * I + I + c, db);
 }
 
 // ---------------------------------------------------------------- dropout (elementwise sites)
@@ -363,24 +400,31 @@ dropout_bwd_kernel(const T* dy, T* dx, const uint8_t* __restrict__ bits, float s
   store8(dx + r * cols + 8 * k, v);
 }
 
-// e4m3 GLU: one warp per row holds gelu(a) * b (the fp32 value the bf16 form rounds) as a register row, then stores it
-// with row_store_e4m3.  ab bf16 [rows, 2I], q [rows, I] bytes, row_scale fp32 [rows].
+// e4m3 form of the FFN activation: one warp per row holds the fp32 value the bf16 form rounds (GATED: gelu(a) * b,
+// else gelu_tanh(pre)) as a register row, then stores it with row_store_e4m3.  ab bf16 [rows, 2I] (GATED) or [rows, I],
+// q [rows, I] bytes, row_scale fp32 [rows].
 constexpr int kGluRowWarps = 4;
-template <int CH>
+template <bool GATED, int CH>
 __global__ void __launch_bounds__(kGluRowWarps * 32)
-glu_fwd_e4m3_kernel(const bf16* __restrict__ ab, uint8_t* __restrict__ q, float* __restrict__ row_scale, long long rows,
-                    int I) {
+ffn_act_fwd_e4m3_kernel(const bf16* __restrict__ ab, uint8_t* __restrict__ q, float* __restrict__ row_scale, long long rows,
+                        int I) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const long long r = static_cast<long long>(blockIdx.x) * kGluRowWarps + (threadIdx.x >> 5);
   if (r >= rows) return;
   float v[CH][8];
   row_load(v, I, lane, [&](int col, float (&vc)[8]) {
-    float b[8];
-    load8(ab + r * 2 * I + col, vc);
-    load8(ab + r * 2 * I + I + col, b);
+    if constexpr (GATED) {
+      float b[8];
+      load8(ab + r * 2 * I + col, vc);
+      load8(ab + r * 2 * I + I + col, b);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) vc[j] = bf16_round(gelu_f(vc[j])) * b[j];
+      for (int j = 0; j < 8; ++j) vc[j] = bf16_round(gelu_f(vc[j])) * b[j];
+    } else {
+      load8(ab + r * I + col, vc);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) vc[j] = gelu_tanh_f(vc[j]);
+    }
   });
   row_store_e4m3(v, I, lane, q + r * I, row_scale + r);
 }
@@ -419,6 +463,55 @@ quantize_rows_e4m3_kernel(const bf16* __restrict__ x, int ldx, uint8_t* __restri
     }
     *reinterpret_cast<uint2*>(qr + k) = make_uint2(w[0], w[1]);
   }
+}
+
+// ---------------------------------------------------------------- FFN activation launchers (GLU and tanh-GELU entry points)
+template <bool GATED>
+int ffn_act_fwd(const char* name, const void* ab, void* out, int out_dt, float* row_scale, unsigned int* bits,
+                const unsigned long long* seed, int site, float p, long long rows, int I, cudaStream_t s) {
+  if (I % 8 != 0) { set_last_error("%s: I must be a multiple of 8", name); return MUSE_ERR_INVALID; }
+  if (bits != nullptr && seed == nullptr) { set_last_error("%s: dropout needs a seed", name); return MUSE_ERR_INVALID; }
+  if (out_dt != 1 && out_dt != 2) { set_last_error("%s: out dtype code %d (bf16 = 1 or e4m3 = 2)", name, out_dt); return MUSE_ERR_INVALID; }
+  if (out_dt == 2) {
+    if (row_scale == nullptr || bits != nullptr || I > 4096) {
+      set_last_error("%s: the e4m3 output needs row_scale, takes no dropout and I <= 4096 (I = %d)", name, I);
+      return MUSE_ERR_INVALID;
+    }
+    if (rows <= 0) return MUSE_OK;
+    const unsigned grid = static_cast<unsigned>(ceil_div_ll(rows, kGluRowWarps));
+    with_row_chunks<1, 2, 4, 8, 12, 16>(I, [&](auto ch) {
+      pdl_launch(grid, kGluRowWarps * 32, 0, s)(ffn_act_fwd_e4m3_kernel<GATED, decltype(ch)::value>,
+                                                reinterpret_cast<const bf16*>(ab), reinterpret_cast<uint8_t*>(out), row_scale,
+                                                rows, I);
+    });
+    return check_launch(name);
+  }
+  const long long n = rows * (I / 8);
+  if (n <= 0) return MUSE_OK;
+  const philox::ElemDrop dr = philox::elem_drop(bits, seed, site, p, I);
+  if constexpr (GATED)
+    pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? ffn_act_fwd_kernel<true, true> : ffn_act_fwd_kernel<true, false>,
+        reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, dr);
+  else
+    pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(ffn_act_fwd_kernel<false, false>,
+        reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, dr);
+  return check_launch(name);
+}
+
+template <bool GATED>
+int ffn_act_bwd(const char* name, const void* ab, const void* dout, const unsigned int* bits, float p, void* dab,
+                long long rows, int I, cudaStream_t s) {
+  if (I % 8 != 0) { set_last_error("%s: I must be a multiple of 8", name); return MUSE_ERR_INVALID; }
+  const long long n = rows * (I / 8);
+  if (n <= 0) return MUSE_OK;
+  const philox::ElemDrop dr = philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, I);
+  if constexpr (GATED)
+    pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? ffn_act_bwd_kernel<true, true> : ffn_act_bwd_kernel<true, false>,
+        reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I, dr);
+  else
+    pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(ffn_act_bwd_kernel<false, false>,
+        reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I, dr);
+  return check_launch(name);
 }
 
 }  // namespace
@@ -542,33 +635,6 @@ int muse_embed_bwd_sorted(const long long* order, const long long* bounds, const
   return check_launch("embed_bwd_pos");
 }
 
-// bits == nullptr: no dropout; else FeedForward.dropout fused into the pass, bits [rows, ceil(I / 32)] written.
-int muse_glu_fwd(const void* ab, void* out, int out_dt, float* row_scale, unsigned int* bits, const unsigned long long* seed,
-                 int site, float p, long long rows, int I, void* stream) {
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (I % 8 != 0) { set_last_error("glu_fwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
-  if (bits != nullptr && seed == nullptr) { set_last_error("glu_fwd: dropout needs a seed"); return MUSE_ERR_INVALID; }
-  if (out_dt != 1 && out_dt != 2) { set_last_error("glu_fwd: out dtype code %d (bf16 = 1 or e4m3 = 2)", out_dt); return MUSE_ERR_INVALID; }
-  if (out_dt == 2) {
-    if (row_scale == nullptr || bits != nullptr || I > 4096) {
-      set_last_error("glu_fwd: the e4m3 output needs row_scale, takes no dropout and I <= 4096 (I = %d)", I);
-      return MUSE_ERR_INVALID;
-    }
-    if (rows <= 0) return MUSE_OK;
-    const unsigned grid = static_cast<unsigned>(ceil_div_ll(rows, kGluRowWarps));
-    with_row_chunks<1, 2, 4, 8, 12, 16>(I, [&](auto ch) {
-      pdl_launch(grid, kGluRowWarps * 32, 0, s)(glu_fwd_e4m3_kernel<decltype(ch)::value>, reinterpret_cast<const bf16*>(ab),
-                                                reinterpret_cast<uint8_t*>(out), row_scale, rows, I);
-    });
-    return check_launch("glu_fwd_e4m3");
-  }
-  const long long n = rows * (I / 8);
-  if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? glu_fwd_kernel<true> : glu_fwd_kernel<false>,
-      reinterpret_cast<const bf16*>(ab), reinterpret_cast<bf16*>(out), rows, I, philox::elem_drop(bits, seed, site, p, I));
-  return check_launch("glu_fwd");
-}
-
 int muse_quantize_rows_e4m3(const void* x, int ldx, void* q, int ldq, float* scale, int rows, int K, void* stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows <= 0 || K <= 0) return MUSE_OK;
@@ -583,17 +649,25 @@ int muse_quantize_rows_e4m3(const void* x, int ldx, void* q, int ldq, float* sca
   return check_launch("quantize_rows_e4m3");
 }
 
+// bits == nullptr: no dropout; else FeedForward.dropout fused into the pass, bits [rows, ceil(I / 32)] written.
+int muse_glu_fwd(const void* ab, void* out, int out_dt, float* row_scale, unsigned int* bits, const unsigned long long* seed,
+                 int site, float p, long long rows, int I, void* stream) {
+  return ffn_act_fwd<true>("glu_fwd", ab, out, out_dt, row_scale, bits, seed, site, p, rows, I, static_cast<cudaStream_t>(stream));
+}
+
 // bits: those muse_glu_fwd wrote (nullptr: no dropout); dout is scaled by them as it is read.
 int muse_glu_bwd(const void* ab, const void* dout, const unsigned int* bits, float p, void* dab, long long rows, int I,
                  void* stream) {
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (I % 8 != 0) { set_last_error("glu_bwd: I must be a multiple of 8"); return MUSE_ERR_INVALID; }
-  const long long n = rows * (I / 8);
-  if (n <= 0) return MUSE_OK;
-  pdl_launch(static_cast<unsigned>(ceil_div_ll(n, 256)), 256, 0, s)(bits ? glu_bwd_kernel<true> : glu_bwd_kernel<false>,
-      reinterpret_cast<const bf16*>(ab), reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(dab), rows, I,
-      philox::elem_drop(const_cast<unsigned int*>(bits), nullptr, 0, p, I));
-  return check_launch("glu_bwd");
+  return ffn_act_bwd<true>("glu_bwd", ab, dout, bits, p, dab, rows, I, static_cast<cudaStream_t>(stream));
+}
+
+int muse_gelu_tanh_fwd(const void* pre, void* out, int out_dt, float* row_scale, long long rows, int I, void* stream) {
+  return ffn_act_fwd<false>("gelu_tanh_fwd", pre, out, out_dt, row_scale, nullptr, nullptr, 0, 0.f, rows, I,
+                            static_cast<cudaStream_t>(stream));
+}
+
+int muse_gelu_tanh_bwd(const void* pre, const void* dout, void* dpre, long long rows, int I, void* stream) {
+  return ffn_act_bwd<false>("gelu_tanh_bwd", pre, dout, nullptr, 0.f, dpre, rows, I, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -163,6 +163,19 @@ class GLUFeedForward(nn.Module):
         self.wo = nn.Linear(cfg["intermediate_size"], cfg["hidden_size"], bias=False)
 
 
+class FusedGeLUFeedForward(nn.Module):
+    """use_fused_mlp (:954-996): wo(gelu_tanh(wi_0(x))), no gate.  ``dropout`` is constructed (it fixes the module order)
+    but, as in the reference, never applied."""
+
+    def __init__(self, cfg):
+        super().__init__()
+        self.pre_mlp_layer_norm = LayerNorm(cfg["hidden_size"], cfg["ln_elementwise_affine"])  # always LayerNorm (:957)
+        self.adaLN_modulation = AdaLNModulation(cfg["hidden_size"], cfg)
+        self.wi_0 = nn.Linear(cfg["hidden_size"], cfg["intermediate_size"], bias=False)
+        self.dropout = nn.Dropout(cfg["hidden_dropout"])
+        self.wo = nn.Linear(cfg["intermediate_size"], cfg["hidden_size"], bias=False)
+
+
 class TransformerLayer(nn.Module):
     def __init__(self, cfg):
         super().__init__()
@@ -173,7 +186,7 @@ class TransformerLayer(nn.Module):
         self.crossattn_layer_norm = _norm(H, cfg)
         self.crossattention = Attention(H, H, nh, cfg)
         self.cross_attn_adaLN_modulation = AdaLNModulation(H, cfg)
-        self.ffn = GLUFeedForward(cfg)
+        self.ffn = (FusedGeLUFeedForward if cfg["use_fused_mlp"] else GLUFeedForward)(cfg)  # FeedForward (:919-923)
 
 
 class ConvEmbed(nn.Module):
@@ -235,9 +248,8 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         self.register_to_config(**cfg)
         self.register_to_config(mask_token_id=cfg["vocab_size"] - 1)
         assert len(cfg["block_out_channels"]) == 1
-        for flag in ("use_bias", "use_fused_mlp"):
-            if cfg[flag]:
-                raise NotImplementedError(f"open_muse_b200.MaskGiTUViT_v2: {flag}=True is not supported")
+        if cfg["use_bias"]:
+            raise NotImplementedError("open_muse_b200.MaskGiTUViT_v2: use_bias=True is not supported")
         self.output_size = cfg["codebook_size"]
         H, C = cfg["hidden_size"], cfg["block_out_channels"][0]
 
@@ -307,9 +319,10 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
     def set_gemm_precision(self, mode: str):
         """"bf16" (default: the reference's autocast recipe) or "fp8": inference only -- forward under torch.no_grad() in
         eval mode, and generate2 -- with the e4m3 tensor cores for the transformer layers' [q;k;v], cross-attention q,
-        [wi_0;wi_1] and wo GEMMs and the ResBlock / AttentionBlock2D channelwise[0] and q GEMMs.  Their activations come
-        out of the passes that produce them as e4m3 with one scale per row, the weights are quantized per output row; every
-        other GEMM stays bf16 (DESIGN.md section 5).  Not a config key: save_pretrained / from_pretrained do not see it.
+        [wi_0;wi_1] (wi_0 with use_fused_mlp) and wo GEMMs and the ResBlock / AttentionBlock2D channelwise[0] and q GEMMs.
+        Their activations come out of the passes that produce them as e4m3 with one scale per row, the weights are
+        quantized per output row; every other GEMM stays bf16 (DESIGN.md section 5).  Not a config key: save_pretrained /
+        from_pretrained do not see it.
         "fp8" needs hidden_size, block_out_channels[0] and intermediate_size to be multiples of 16 (the e4m3 rows are fed
         by TMA, whose row pitches are multiples of 16 bytes); bf16 needs multiples of 8."""
         if mode not in ("bf16", "fp8"):
@@ -337,9 +350,9 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
         return (self._gemm_precision,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
 
     def _weights(self):
-        """bf16 GEMM operands (fused [k;v], [q;k;v], [wi_0;wi_1], all adaLN mappers stacked into one matrix, logits rows
-        padded to 64), rebuilt only when a parameter changes -- never inside generate2, and not after a fused optimizer
-        step with ``model=``, which writes them itself (``_packed``)."""
+        """bf16 GEMM operands (fused [k;v], [q;k;v], [wi_0;wi_1] (wi_0 alone with use_fused_mlp), all adaLN mappers
+        stacked into one matrix, logits rows padded to 64), rebuilt only when a parameter changes -- never inside
+        generate2, and not after a fused optimizer step with ``model=``, which writes them itself (``_packed``)."""
         key = self._weights_key()
         if key == self._cache_key:
             return self._cache
@@ -433,7 +446,8 @@ class MaskGiTUViT_v2(ModelMixin, ConfigMixin):
                 "ln1": f32(l.attn_layer_norm.weight), "mod1": mapper(l.self_attn_adaLN_modulation),
                 "sa": attn(l.attention, True), "ln2": f32(l.crossattn_layer_norm.weight), "ca": attn(l.crossattention, False),
                 "mod2": mapper(l.cross_attn_adaLN_modulation), "ln3": f32(l.ffn.pre_mlp_layer_norm.weight),
-                "mod3": mapper(l.ffn.adaLN_modulation), "wi": bf(l.ffn.wi_0.weight, l.ffn.wi_1.weight),
+                "mod3": mapper(l.ffn.adaLN_modulation), "wi": bf(*T._ffn_wi(l.ffn)),
+                "glu": isinstance(l.ffn, GLUFeedForward),  # else FusedGeLUFeedForward: "wi" is wi_0 alone, no gate
                 "wo": bf(l.ffn.wo.weight)})
         W["up"] = block(self.up_blocks[0])
         W["mappers"] = bf(*mappers)

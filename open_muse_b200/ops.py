@@ -378,7 +378,7 @@ def norm2_bwd(d_h2, x2, w2, dres, a, w1, stats, rms1=0, rms2=0):
     return dx2, d_a, dw1, dw2
 
 
-# ------------------------------------------------------------------------------------------ GLU
+# ------------------------------------------------------------------------------------------ GLU / tanh-GELU
 def glu_fwd(ab, dropout=None, out_dtype=torch.bfloat16):
     """dropout = (p, seed, site): FeedForward.dropout fused into the pass; then returns (out, bits) (see dropout_fwd).
     out_dtype FP8: out is an F8 (no dropout)."""
@@ -398,6 +398,25 @@ def glu_bwd(ab, dout, dropout=None):
     p, bits = dropout if dropout is not None else (0.0, None)
     _call("muse_glu_bwd", _p(ab), _p(dout), _p(bits), float(p), _p(dab), rows, two_i // 2, st)
     return dab
+
+
+def gelu_tanh_fwd(pre, out_dtype=torch.bfloat16):
+    """F.gelu(pre, approximate="tanh") of FusedGeLUFeedForward (use_fused_mlp): pre bf16 [rows, I] -> bf16 [rows, I].
+    out_dtype FP8: out is an F8 (I <= 4096), the wo operand of the FP8 GEMM."""
+    st = _prep(pre)
+    rows, I = pre.shape
+    out, scale = _new_out(rows, I, out_dtype, pre.device)
+    _call("muse_gelu_tanh_fwd", _p(pre), _p(_data(out)), _dt(_data(out)), _p(scale), rows, I, st)
+    return out
+
+
+def gelu_tanh_bwd(pre, dout):
+    """dpre bf16 [rows, I] = dout * gelu_tanh'(pre)"""
+    st = _prep(pre)
+    rows, I = pre.shape
+    dpre = torch.empty_like(pre)
+    _call("muse_gelu_tanh_bwd", _p(pre), _p(dout), _p(dpre), rows, I, st)
+    return dpre
 
 
 # ------------------------------------------------------------------------------------------ attention

@@ -61,8 +61,9 @@ def _sub(G, W, key):
 # nn.Dropout in training mode (ops.dropout_record documents the masks).  A block forward receives its unit's spec
 # ``drop = (p_hidden, p_attn, seed, first site)`` or None; unit j (down pairs, then layers, then up pairs) owns the site ids
 # 3 j .. 3 j + 2: a ResBlock + AttentionBlock2D pair uses 3 j for the ResBlock, 3 j + 1 for ``attention`` and 3 j + 2 for
-# ``crossattention``; a transformer layer 3 j for ``attention``, 3 j + 1 for ``crossattention`` and 3 j + 2 for the FFN.
-# A rate of 0 leaves its sites out.  The forward keeps (p, bits) of each active site in the state its backward unpacks.
+# ``crossattention``; a transformer layer 3 j for ``attention``, 3 j + 1 for ``crossattention`` and 3 j + 2 for the FFN
+# (a GLUFeedForward's; FusedGeLUFeedForward applies no dropout, so that site is never drawn).  A rate of 0 leaves its
+# sites out.  The forward keeps (p, bits) of each active site in the state its backward unpacks.
 def unit_drop(drop, j):
     """the spec of unit j from the forward's (p_hidden, p_attn, seed), or None when dropout is inactive"""
     return None if drop is None else (*drop, 3 * j)
@@ -206,9 +207,11 @@ def _layer_fwd(x, r, enc, w, mod_all, B, S, Skv, eps, rms, drop=None, out=True):
     co = ops.linear_fwd(cc, w["ca"]["o"])
     r3, y3 = ops.add_norm_mod(co, w["ln3"], eps, 0, **_form(w["wi"]), residual=r2, mod=m("mod3"),
                               rows_per_sample=S)
-    ab = ops.linear_fwd(y3, w["wi"])
+    ab = ops.linear_fwd(y3, w["wi"])  # [wi_0 | wi_1](x) for the GLU, wi_0(x) for FusedGeLUFeedForward
     fd = _site(drop, 2, attn=False)
-    if fd is None:
+    if not w["glu"]:  # FusedGeLUFeedForward never applies its dropout (:954-996): site 3 j + 2 is not drawn
+        gl, fdr = ops.gelu_tanh_fwd(ab, **_form(w["wo"])), None
+    elif fd is None:
         gl, fdr = ops.glu_fwd(ab, **_form(w["wo"])), None
     else:  # GLUFeedForward.dropout fused into the GLU pass: gl is the dropped wo operand
         gl, bits = ops.glu_fwd(ab, dropout=fd)
@@ -222,7 +225,8 @@ def _layer_bwd(df, dr3, st, w, g, enc, d_enc, mod_all, d_mod_all, B, S, Skv, eps
     m = lambda t, k: t[:, w[k][0]:w[k][0] + w[k][1]]
     gsa, gca = _sub(g, w, "sa"), _sub(g, w, "ca")
     dgl = _lin_bwd(df, gl, w["wo"], g.of("wo"))
-    dy3 = _lin_bwd(ops.glu_bwd(ab, dgl, **_dkw(fdr)), y3, w["wi"], g.of("wi"))
+    dab = ops.glu_bwd(ab, dgl, **_dkw(fdr)) if w["glu"] else ops.gelu_tanh_bwd(ab, dgl)
+    dy3 = _lin_bwd(dab, y3, w["wi"], g.of("wi"))
     dco, dr2 = ops.add_norm_mod_bwd(dy3, dr3, r3, w["ln3"], eps, 0, BF16, mod=m(mod_all, "mod3"), rows_per_sample=S,
                                     dw=g.of("ln3"), dmod=m(d_mod_all, "mod3"))
     dcc = _lin_bwd(dco, cc, w["ca"]["o"], gca.of("o"))
@@ -423,11 +427,16 @@ class UBlockFn(torch.autograd.Function):
         return (None, None, None, None, None, None, dh, d_enc, d_sc32, *_align(params, grads))
 
 
+def _ffn_wi(ffn):
+    """[wi_0, wi_1] of GLUFeedForward, [wi_0] of FusedGeLUFeedForward: the row blocks of the "wi" operand"""
+    return [ffn.wi_0.weight, ffn.wi_1.weight] if hasattr(ffn, "wi_1") else [ffn.wi_0.weight]
+
+
 def layer_params(l):
     return [l.attn_layer_norm.weight, l.self_attn_adaLN_modulation.mapper.weight] + _attn_params(l.attention) + \
         [l.crossattn_layer_norm.weight] + _attn_params(l.crossattention) + \
-        [l.cross_attn_adaLN_modulation.mapper.weight, l.ffn.pre_mlp_layer_norm.weight, l.ffn.adaLN_modulation.mapper.weight,
-         l.ffn.wi_0.weight, l.ffn.wi_1.weight, l.ffn.wo.weight]
+        [l.cross_attn_adaLN_modulation.mapper.weight, l.ffn.pre_mlp_layer_norm.weight, l.ffn.adaLN_modulation.mapper.weight] + \
+        _ffn_wi(l.ffn) + [l.ffn.wo.weight]
 
 
 class ULayerFn(torch.autograd.Function):
@@ -471,9 +480,9 @@ class ULayerFn(torch.autograd.Function):
         H2 = 2 * sh.H
         I = l.ffn.wi_0.weight.shape[0]
         params = layer_params(l)
+        g_wi = [g["wi"][k * I:(k + 1) * I] for k in range(len(_ffn_wi(l.ffn)))]
         grads = [g.get("ln1"), g_map[:H2]] + _attn_grads(g["sa"], l.attention, True) + [g.get("ln2")] + \
-            _attn_grads(g["ca"], l.crossattention, False) + [g_map[H2:2 * H2], g.get("ln3"), g_map[2 * H2:], g["wi"][:I], g["wi"][I:],
-                                                             g["wo"]]
+            _attn_grads(g["ca"], l.crossattention, False) + [g_map[H2:2 * H2], g.get("ln3"), g_map[2 * H2:]] + g_wi + [g["wo"]]
         ctx.sv = None  # release the block's activations now, not when the graph dies
         return (None, None, None, None, None, dx, dr, d_enc, d_sc32, *_align(params, grads))
 
