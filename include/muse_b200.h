@@ -75,9 +75,15 @@ int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int 
  * [M,K] (pitch lda bytes), B e4m3 row-major [N,K] (pitch ldb bytes), sa fp32 [M], sb fp32 [N] (8-byte aligned); fp32
  * accumulation with each 128-wide k-block's partial sum promoted into fp32 registers.  N and ldc multiples of 8; lda / ldb
  * multiples of 16.  The e4m3 producers: muse_add_norm_mod_fwd, muse_dwconv3x3_norm_fwd, muse_glu_fwd, muse_gelu_tanh_fwd
- * (dtype code 2) and muse_quantize_rows_e4m3. */
+ * (dtype code 2), muse_norm_fwd_e4m3, muse_norm2_fwd_e4m3 and muse_quantize_rows_e4m3. */
 int muse_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
                   int ldb, int ldc, void* stream);
+/* muse_gemm_fp8 with the residual add of MUSE_EPI_RESADD_F32 fused into its epilogue (MaskGitTransformer's FP8 wo GEMM):
+ * C fp32 [M,N] = res fp32 [M,N] + bf16(sum_k A[m,k] B[n,k] * sa[m] * sb[n]), res and C with pitch ldc (elements), both
+ * 16-byte aligned; the other arguments and constraints as muse_gemm_fp8.  The A operands: muse_norm_fwd_e4m3 (act 2) and
+ * muse_glu_fwd (dtype code 2). */
+int muse_gemm_fp8_res(const void* A, const float* sa, const void* B, const float* sb, const float* res, float* C, int M,
+                      int N, int K, int lda, int ldb, int ldc, void* stream);
 
 /* Weight-gradient GEMM with a run-to-run reproducible result: C fp32 [M,N] = opA(A) * opB(B)^T split over K (= tokens) so
  * that the few output tiles fill the SMs; every split stores its partial tile into `ws` and a second kernel sums the
@@ -189,6 +195,17 @@ int muse_norm2_fwd(const void* a, const float* res, const float* w1, const float
 int muse_norm2_bwd(const void* d_h2, const float* x2, const float* w2, const float* mean2, const float* rstd2,
                    const float* dres, const void* a, const float* w1, const float* mean1, const float* rstd1, float* dx2,
                    void* d_a, float* dw2, float* dw1, float* ws, int rows, int H, int rms1, int rms2, void* stream);
+
+/* e4m3 forms of muse_norm_fwd and muse_norm2_fwd, the A operands of MaskGitTransformer's FP8 GEMMs: the normalised rows
+ * (y, resp. h2) are stored as q e4m3 [rows, H] with one scale per row in row_scale fp32 [rows] (dtype code 2 above),
+ * from the fp32 values the bf16 forms round; the statistics (nullable) and x2 are the bf16 forms'.
+ * muse_norm_fwd_e4m3: act 0 (fp32 or bf16 x, optional res, H <= 1024) or act 2 (GLU + norm, bf16 x, H <= 4096); no
+ * dropout.  muse_norm2_fwd_e4m3: H <= 1024. */
+int muse_norm_fwd_e4m3(const void* x, int x_dtype, const float* w, const float* res, void* q, float* row_scale, float* mean,
+                       float* rstd, int rows, int H, float eps, int act, int rms, void* stream);
+int muse_norm2_fwd_e4m3(const void* a, const float* res, const float* w1, const float* w2, float* x2, void* q,
+                        float* row_scale, float* mean1, float* rstd1, float* mean2, float* rstd2, int rows, int H, float eps,
+                        int rms1, int rms2, void* stream);
 
 /* GLU of FeedForward (:789-792): ab bf16 [rows, 2I] = [wi_0(x) | wi_1(x)], out [rows, I] = gelu(a) * b.
  * out_dtype 1: bf16.  out_dtype 2: e4m3 with its scales in row_scale fp32 [rows] (required then; a warp per row, I <= 4096;

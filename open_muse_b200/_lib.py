@@ -27,6 +27,7 @@ SIGNATURES = {
     "muse_get_pdl": (c_int, []),
     "muse_gemm_bf16": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "muse_gemm_fp8": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "muse_gemm_fp8_res": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "muse_quantize_rows_e4m3": (c_int, [_P, _I, _P, _I, _P, _I, _I, _P]),
     "muse_gemm_splitk_workspace_bytes": (c_longlong, [_I, _I, _I]),
     "muse_gemm_bf16_splitk": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
@@ -44,6 +45,8 @@ SIGNATURES = {
     "muse_norm_bwd_workspace_floats": (c_longlong, [_I, _I, _I]),
     "muse_norm2_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _F, _I, _I, _P]),
     "muse_norm2_bwd": (c_int, [_P] * 15 + [_I, _I, _I, _I, _P]),
+    "muse_norm_fwd_e4m3": (c_int, [_P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _F, _I, _I, _P]),
+    "muse_norm2_fwd_e4m3": (c_int, [_P] * 11 + [_I, _I, _F, _I, _I, _P]),
     "muse_glu_fwd": (c_int, [_P, _P, _I, _P, _P, _P, _I, _F, _L, _I, _P]),
     "muse_glu_bwd": (c_int, [_P, _P, _P, _F, _P, _L, _I, _P]),
     "muse_gelu_tanh_fwd": (c_int, [_P, _P, _I, _P, _L, _I, _P]),

@@ -12,7 +12,8 @@
 // next tile meanwhile.  The atomic epilogue adds straight from the accumulator registers.
 //
 // FP8 (muse_gemm_fp8, inference): A and B e4m3, both K-major, with fp32 scales per row of A and per row of B (= column
-// of C); the same pipeline with k32 e4m3 MMAs, and the bf16 epilogue stores bf16(acc * sa[m] * sb[n]).
+// of C); the same pipeline with k32 e4m3 MMAs, and the bf16 epilogue stores bf16(acc * sa[m] * sb[n]).  muse_gemm_fp8_res
+// stores res + bf16(acc * sa[m] * sb[n]) in fp32 instead, with the residual prefetch and TMA stores of EPI_RESADD_F32.
 //
 // Operand "major-ness": an operand is K-major when the reduction dim is contiguous in memory
 // (activations X[T,K], weights W[N,K] in forward) and MN-major when the M/N dim is contiguous
@@ -35,7 +36,11 @@ using tc::BM;
 // parallel kernel sums the partials in split order and STORES the result, so the output needs no zero fill and is
 // bit-identical from run to run (the atomic variant is order-dependent).
 // EPI_FP8_BF16: e4m3 operands (muse_gemm_fp8 only), C bf16 = acc * sa[row] * sb[col].
-enum Epi { EPI_BF16 = 0, EPI_F32 = 1, EPI_ATOMIC_F32 = 2, EPI_RESADD_F32 = 3, EPI_SPLITK_F32 = 4, EPI_FP8_BF16 = 5 };
+// EPI_FP8_RESADD_F32: e4m3 operands (muse_gemm_fp8_res only), C fp32 = res + bf16(acc * sa[row] * sb[col]).
+enum Epi {
+  EPI_BF16 = 0, EPI_F32 = 1, EPI_ATOMIC_F32 = 2, EPI_RESADD_F32 = 3, EPI_SPLITK_F32 = 4, EPI_FP8_BF16 = 5,
+  EPI_FP8_RESADD_F32 = 6
+};
 
 
 // Epilogue staging buffer: 64 rows x 128 B (a chunk of 64 bf16 or 32 fp32 columns of a warpgroup's half tile), laid out
@@ -51,19 +56,20 @@ struct GemmParams {
   int M, N, K;
   int ldc;
   int num_m, num_n, num_kb, kb_per_split, splits;
-  const float* sa;  // EPI_FP8_BF16: scales of the rows of A [M] and of B [N]
+  const float* sa;  // FP8 epilogues: scales of the rows of A [M] and of B [N]
   const float* sb;
 };
 
 // tmC: the output, box {128 B of columns, 64 rows}: C [M, N] (pitch ldc), or for split-K partial tiles the workspace
-// [splits * num_m * num_n * BM, BN] fp32.  tmR: the fp32 residual [M, N] (pitch ldc) of EPI_RESADD_F32, same box.
+// [splits * num_m * num_n * BM, BN] fp32.  tmR: the fp32 residual [M, N] (pitch ldc) of the residual epilogues, same box.
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(tc::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
-  constexpr bool kFp8 = EPI == EPI_FP8_BF16;
+  constexpr bool kFp8 = EPI == EPI_FP8_BF16 || EPI == EPI_FP8_RESADD_F32;
+  constexpr bool kRes = EPI == EPI_RESADD_F32 || EPI == EPI_FP8_RESADD_F32;
   using R = Ring<BN, std::conditional_t<kFp8, __nv_fp8_e4m3, bf16>>;
   constexpr int kBK = R::kBK;
   R ring(smem_raw);
@@ -74,7 +80,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
     if (EPI != EPI_ATOMIC_F32) ptx::prefetch_tmap(&tmC);
-    if (EPI == EPI_RESADD_F32) {
+    if (kRes) {
       ptx::prefetch_tmap(&tmR);
       uint64_t* rbar = reinterpret_cast<uint64_t*>(ring.extra() + 4 * kEpiBuf);
       for (int i = 0; i < 4; ++i) ptx::mbar_init(&rbar[i], 1);
@@ -128,7 +134,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint64_t* rbar = reinterpret_cast<uint64_t*>(ring.extra() + 4 * kEpiBuf) + 2 * half;
     // A chunk is 128 B of each of the 64 rows; chunk q goes through buffer q & 1.  Every epilogue has an even number of
     // chunks per tile, so each tile starts on buffer 0 and the residual barriers on phase 0.
-    constexpr bool kF32 = EPI != EPI_BF16 && !kFp8;
+    constexpr bool kF32 = EPI != EPI_BF16 && EPI != EPI_FP8_BF16;
     constexpr int kCols = kF32 ? 32 : 64;
     constexpr int kChunks = BN / kCols;
     constexpr int kJ = kCols / 8;  // 8-column fragment groups per chunk
@@ -145,7 +151,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const bool partial = EPI == EPI_SPLITK_F32 && p.splits > 1;
       const int orow = (partial ? tile * BM : m_idx * BM) + half * 64;
       const int ocol = partial ? 0 : n_idx * BN;
-      if (EPI == EPI_RESADD_F32 && leader) {
+      if (kRes && leader) {
         // the first two residual chunks load during the mainloop, once the previous tile's stores have read the buffers
         ptx::bulk_wait_read<0>();
         for (int b = 0; b < 2; ++b) {
@@ -161,7 +167,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       } else {
         ring.template consume<A_MN, B_MN>(acc, kb0, kb1, half);
       }
-      float sx[2] = {1.f, 1.f};  // EPI_FP8_BF16: scales of the thread's rows fr and fr + 8 (0 past M)
+      float sx[2] = {1.f, 1.f};  // FP8 epilogues: scales of the thread's rows fr and fr + 8 (0 past M)
       if constexpr (kFp8) {
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
@@ -189,7 +195,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
         for (int q = 0; q < kChunks; ++q) {
           uint8_t* buf = ebuf + (q & 1) * kEpiBuf;
-          if (EPI == EPI_RESADD_F32) {
+          if (kRes) {
             ptx::mbar_wait(&rbar[q & 1], (q >> 1) & 1);  // residual chunk q has landed (so the store of q - 2 has read buf)
           } else {
             if (leader) ptx::bulk_wait_read<1>();  // the store of chunk q - 2 has read buf
@@ -198,7 +204,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
           for (int jj = 0; jj < kJ; ++jj) {
             const int j = q * kJ + jj;
-            float2 sw = make_float2(1.f, 1.f);  // EPI_FP8_BF16: scales of columns lc, lc + 1 of this 8-column group
+            float2 sw = make_float2(1.f, 1.f);  // FP8 epilogues: scales of columns lc, lc + 1 of this 8-column group
             if constexpr (kFp8) {
               const int gcol = ocol + q * kCols + 8 * jj + lc;  // N % 8 == 0: both columns are inside or both past N
               sw = gcol < p.N ? *reinterpret_cast<const float2*>(p.sb + gcol) : make_float2(0.f, 0.f);
@@ -217,7 +223,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 *reinterpret_cast<uint32_t*>(buf + r * 128 + ((jj ^ (r & 7)) << 4) + 2 * lc) = pack_bf16(v0, v1);
               } else {
                 float2* dst = reinterpret_cast<float2*>(buf + r * 128 + (((2 * jj + (lc >> 2)) ^ (r & 7)) << 4) + 4 * (lc & 3));
-                if (EPI == EPI_RESADD_F32) {  // out = residual + bf16(acc)  (Linear output is bf16 under autocast)
+                if (kRes) {  // out = residual + bf16(acc)  (Linear output is bf16 under autocast)
                   const float2 rs = *dst;
                   *dst = make_float2(rs.x + bf16_round(v0), rs.y + bf16_round(v1));
                 } else {
@@ -231,7 +237,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (leader) {
             ptx::tma_store_2d(&tmC, buf, ocol + q * kCols, orow);
             ptx::bulk_commit();
-            if (EPI == EPI_RESADD_F32 && q + 2 < kChunks) {
+            if (kRes && q + 2 < kChunks) {
               ptx::bulk_wait_read<0>();
               ptx::mbar_expect_tx(&rbar[q & 1], kEpiBuf);
               ptx::tma_load_2d(buf, &tmR, &rbar[q & 1], ocol + (q + 2) * kCols, orow);
@@ -404,9 +410,14 @@ static int gemm_tc(const void* A, const void* B, void* C, const float* res, int 
 }
 
 // C bf16 [M,N] (ldc) = (A e4m3 [M,K] (lda) * diag(sa)) (B e4m3 [N,K] (ldb) * diag(sb))^T; pitches in elements = bytes.
-static int gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
-                    int ldb, int ldc, cudaStream_t stream) {
+// res given: C fp32 [M,N] (ldc) = res (ldc) + bf16(that product).
+static int gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, const float* res, void* C, int M, int N,
+                    int K, int lda, int ldb, int ldc, cudaStream_t stream) {
   if (M <= 0 || N <= 0 || K <= 0) return MUSE_OK;
+  if (res != nullptr && (reinterpret_cast<uintptr_t>(res) & 15) != 0) {
+    set_last_error("gemm_fp8: the residual must be 16B aligned");
+    return MUSE_ERR_INVALID;
+  }
   if (ldc % 8 != 0 || N % 8 != 0) {
     set_last_error("gemm_fp8: N=%d and ldc=%d must be multiples of 8 (the TMA stores write whole 16-byte units)", N, ldc);
     return MUSE_ERR_INVALID;
@@ -422,8 +433,13 @@ static int gemm_fp8(const void* A, const float* sa, const void* B, const float* 
   int rc;
   if ((rc = make_tmap(&m.a, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_UINT8, A, {K, M}, {1LL * lda}, {kBK, BM}))) return rc;
   if ((rc = make_tmap(&m.b, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_UINT8, B, {K, N}, {1LL * ldb}, {kBK, BN}))) return rc;
-  if ((rc = make_tmap(&m.c, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, C, {N, M}, {2LL * ldc}, {64, 64}))) return rc;
-  m.r = m.c;
+  if (res == nullptr) {
+    if ((rc = make_tmap(&m.c, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, C, {N, M}, {2LL * ldc}, {64, 64}))) return rc;
+    m.r = m.c;
+  } else {
+    if ((rc = make_tmap(&m.c, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, C, {N, M}, {4LL * ldc}, {32, 64}))) return rc;
+    if ((rc = make_tmap(&m.r, "gemm_fp8", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, res, {N, M}, {4LL * ldc}, {32, 64}))) return rc;
+  }
   GemmParams p;
   p.C = C;
   p.M = M; p.N = N; p.K = K; p.ldc = ldc;
@@ -434,7 +450,8 @@ static int gemm_fp8(const void* A, const float* sa, const void* B, const float* 
   p.kb_per_split = p.num_kb;
   p.sa = sa;
   p.sb = sb;
-  return launch<BN, false, false, EPI_FP8_BF16>(m, p, stream);
+  return res == nullptr ? launch<BN, false, false, EPI_FP8_BF16>(m, p, stream)
+                        : launch<BN, false, false, EPI_FP8_RESADD_F32>(m, p, stream);
 }
 
 }  // namespace muse
@@ -460,7 +477,13 @@ int muse_gemm_bf16(const void* A, const void* B, void* C, const float* res, int 
 
 int muse_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, void* C, int M, int N, int K, int lda,
                   int ldb, int ldc, void* stream) {
-  return gemm_fp8(A, sa, B, sb, C, M, N, K, lda, ldb, ldc, static_cast<cudaStream_t>(stream));
+  return gemm_fp8(A, sa, B, sb, nullptr, C, M, N, K, lda, ldb, ldc, static_cast<cudaStream_t>(stream));
+}
+
+int muse_gemm_fp8_res(const void* A, const float* sa, const void* B, const float* sb, const float* res, float* C, int M,
+                      int N, int K, int lda, int ldb, int ldc, void* stream) {
+  if (res == nullptr) { set_last_error("gemm_fp8_res: needs res"); return MUSE_ERR_INVALID; }
+  return gemm_fp8(A, sa, B, sb, res, C, M, N, K, lda, ldb, ldc, static_cast<cudaStream_t>(stream));
 }
 
 long long muse_gemm_splitk_workspace_bytes(int M, int N, int K) {

@@ -26,11 +26,12 @@ constexpr int ACT_NONE = 0, ACT_GELU = 1, ACT_GLU = 2;
 // ---- warp-per-row kernels (H <= 1024, no GLU): the whole row lives in registers (row_norm.cuh), no block barriers
 constexpr int kWarpsPerBlock = 4;
 
-template <typename TX, typename TY, int CH>
+// F8: y is the e4m3 operand of muse_gemm_fp8 (TY = uint8_t) and row_scale [rows] its scales (row_store_e4m3).
+template <typename TX, typename TY, int CH, bool F8>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 norm_fwd_warp_kernel(const TX* __restrict__ x, const float* __restrict__ w, const float* __restrict__ res,
                 TY* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows, int H,
-                float eps, int act, int rms) {
+                float eps, int act, int rms, float* __restrict__ row_scale) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
@@ -67,9 +68,15 @@ norm_fwd_warp_kernel(const TX* __restrict__ x, const float* __restrict__ w, cons
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] += r8[j];
       }
-      store8(yr + col, o);
+      if constexpr (F8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[c][j] = o[j];
+      } else {
+        store8(yr + col, o);
+      }
     }
   }
+  if constexpr (F8) row_store_e4m3(v, H, lane, reinterpret_cast<uint8_t*>(yr), row_scale + row);
 }
 
 // Weight gradients (dw[H] = sum over rows of dy * xhat) are reduced in a FIXED order so that the result is bit-identical
@@ -217,12 +224,15 @@ norm_bwd_warp_kernel(const TDY* __restrict__ dy, const TX* __restrict__ x, const
 // pre_mlp_layer_norm (:787, always LayerNorm).  Separately these are two HBM round trips of the residual stream (x2 is
 // written by the first and read back by the second); fused, the row stays in registers: 12 instead of 16 bytes per element
 // forward, 18 instead of 22 backward.
-template <int CH>
+// F8: h2 is the e4m3 operand of muse_gemm_fp8 (TH = uint8_t) and row_scale [rows] its scales; x2 and the statistics
+// are the same as the bf16 form's.
+template <int CH, bool F8, typename TH = bf16>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 norm2_fwd_warp_kernel(const bf16* __restrict__ a, const float* __restrict__ res, const float* __restrict__ w1,
-                      const float* __restrict__ w2, float* __restrict__ x2, bf16* __restrict__ h2,
+                      const float* __restrict__ w2, float* __restrict__ x2, TH* __restrict__ h2,
                       float* __restrict__ mean1_out, float* __restrict__ rstd1_out, float* __restrict__ mean2_out,
-                      float* __restrict__ rstd2_out, int rows, int H, float eps, int rms1, int rms2) {
+                      float* __restrict__ rstd2_out, int rows, int H, float eps, int rms1, int rms2,
+                      float* __restrict__ row_scale) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
@@ -262,8 +272,19 @@ norm2_fwd_warp_kernel(const bf16* __restrict__ a, const float* __restrict__ res,
       load8(w2 + col, wv);
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean2) * rstd2 * wv[j];
-      store8(h2 + static_cast<size_t>(row) * H + col, o);
+      if constexpr (F8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[c][j] = o[j];
+      } else {
+        store8(h2 + static_cast<size_t>(row) * H + col, o);
+      }
     }
+  }
+  if constexpr (F8) {
+    // the row index passes through a shuffle so that the e4m3 row's addresses are formed here: held from the start of the
+    // kernel, the two 64-bit addresses were spilled to the stack at 2 chunks (264 <= H <= 512)
+    const int r = __shfl_sync(0xffffffffu, row, 0);
+    row_store_e4m3(v, H, lane, h2 + static_cast<size_t>(r) * H, row_scale + r);
   }
 }
 
@@ -550,11 +571,14 @@ __device__ __forceinline__ uint32_t bf16x2_mul(uint32_t a, uint32_t b) {  // bf1
 // kernel at ~3.7 TB/s whatever the instruction count (same-box A/B: 219 -> 193 us at [65 792, 2 x 2048]).  The backward
 // got nothing from the same treatment (362 -> 360 us) at three CTAs per SM; its loads go through a shared-memory row ring
 // instead (glu_norm_bwd_ring_kernel).
-template <int CH, bool DROP>
+// F8 (never with DROP; H <= 4096): y is the e4m3 operand of muse_gemm_fp8 (TY = uint8_t) and row_scale [rows] its
+// scales.  The normalised row is kept as fp32 register chunks (128 values per lane at H = 4096) until its amax is known,
+// then stored with row_store_e4m3.
+template <int CH, bool DROP, bool F8 = false, typename TY = bf16>
 __global__ void __launch_bounds__(kGluWarps * 32, (CH <= 8) ? 2 : 1)
-glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf16* __restrict__ y,
+glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, TY* __restrict__ y,
                     float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows, int H, float eps, int rms,
-                    const philox::ElemDrop drop) {
+                    const philox::ElemDrop drop, float* __restrict__ row_scale) {
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * kGluWarps + (threadIdx.x >> 5);
@@ -617,13 +641,28 @@ glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf
     if (mean_out) mean_out[row] = mean;
     if (rstd_out) rstd_out[row] = rstd;
   }
-  bf16* yr = y + static_cast<size_t>(row) * H;
+  TY* yr = y + static_cast<size_t>(row) * H;
   unsigned long long seed = 0;
   if constexpr (DROP) seed = *drop.seed;
+  float fv[F8 ? CH : 1][8];  // F8: the normalised row, zeros past H
 #pragma unroll
   for (int c = 0; c < CH; ++c) {
     const int col = (c * 32 + lane) * 8;
-    if (col < H) {
+    if constexpr (F8) {
+      if (col < H) {
+        float wv[8];
+        if (w) load8(w + col, wv);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 p = unpack_bf16(vp[c][j]);
+          fv[c][2 * j] = (p.x - mean) * (w ? rstd * wv[2 * j] : rstd);
+          fv[c][2 * j + 1] = (p.y - mean) * (w ? rstd * wv[2 * j + 1] : rstd);
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) fv[c][j] = 0.f;
+      }
+    } else if (col < H) {
       float wv[8];
       if (w) load8(w + col, wv);
       uint32_t kb = 0xFFu;
@@ -646,6 +685,7 @@ glu_norm_fwd_kernel(const bf16* __restrict__ ab, const float* __restrict__ w, bf
       drop.bits[static_cast<size_t>(row) * drop.row_bytes + col / 8] = 0;  // pad bytes of the row's last word
     }
   }
+  if constexpr (F8) row_store_e4m3(fv, H, lane, yr, row_scale + row);
 }
 
 // backward: two streaming passes over the row with the GELU recomputed in the second one (nothing row-sized in
@@ -1227,7 +1267,8 @@ int fwd_dispatch(const void* x, const float* w, const float* res, void* y, float
   if (H <= 1024) {
     with_row_chunks<1, 2, 4>(H, [&](auto ch) {
       pdl_launch(ceil_div(rows, kWarpsPerBlock), kWarpsPerBlock * 32, 0, s)(
-          norm_fwd_warp_kernel<TX, TY, decltype(ch)::value>, xp, w, res, yp, mean, rstd, rows, H, eps, act, rms);
+          norm_fwd_warp_kernel<TX, TY, decltype(ch)::value, false>, xp, w, res, yp, mean, rstd, rows, H, eps, act, rms,
+          nullptr);
     });
   } else {
     pdl_launch(ceil_div(rows, kWideWarps), kWideWarps * 32, 0, s)(norm_fwd_wide_kernel<TX, TY>, xp, w, res, yp, mean, rstd,
@@ -1354,7 +1395,7 @@ int muse_norm_fwd(const void* x, int x_dt, const float* w, const float* res, voi
       constexpr int CH = decltype(ch)::value;
       pdl_launch(ceil_div(rows, kGluWarps), kGluWarps * 32, 0, s)(
           bits ? glu_norm_fwd_kernel<CH, true> : glu_norm_fwd_kernel<CH, false>, reinterpret_cast<const bf16*>(x), w,
-          reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop);
+          reinterpret_cast<bf16*>(y), mean, rstd, rows, H, eps, rms, drop, nullptr);
     });
     return check_launch("glu_norm_fwd");
   }
@@ -1371,10 +1412,60 @@ int muse_norm2_fwd(const void* a, const float* res, const float* w1, const float
   if (H % 8 != 0 || H > 1024 || H < 8) { set_last_error("norm2_fwd: H=%d must be a multiple of 8 in [8, 1024]", H); return MUSE_ERR_UNSUPPORTED; }
   with_row_chunks<1, 2, 4>(H, [&](auto ch) {
     pdl_launch(ceil_div(rows, kWarpsPerBlock), kWarpsPerBlock * 32, 0, s)(
-        norm2_fwd_warp_kernel<decltype(ch)::value>, reinterpret_cast<const bf16*>(a), res, w1, w2, x2,
-        reinterpret_cast<bf16*>(h2), mean1, rstd1, mean2, rstd2, rows, H, eps, rms1, rms2);
+        norm2_fwd_warp_kernel<decltype(ch)::value, false>, reinterpret_cast<const bf16*>(a), res, w1, w2, x2,
+        reinterpret_cast<bf16*>(h2), mean1, rstd1, mean2, rstd2, rows, H, eps, rms1, rms2, nullptr);
   });
   return check_launch("norm2_fwd");
+}
+
+// e4m3 forms of muse_norm_fwd (act 0, H <= 1024; act 2, H <= 4096, no dropout) and muse_norm2_fwd: the operands of the
+// FP8 GEMMs of MaskGitTransformer.  q e4m3 [rows, H], row_scale fp32 [rows]; statistics as the bf16 forms.
+int muse_norm_fwd_e4m3(const void* x, int x_dt, const float* w, const float* res, void* q, float* row_scale, float* mean,
+                       float* rstd, int rows, int H, float eps, int act, int rms, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (rows <= 0) return MUSE_OK;
+  int rc = check_args("norm_fwd_e4m3", H, act, res);
+  if (rc) return rc;
+  if (q == nullptr || row_scale == nullptr) { set_last_error("norm_fwd_e4m3: needs q and row_scale"); return MUSE_ERR_INVALID; }
+  uint8_t* qp = reinterpret_cast<uint8_t*>(q);
+  if (act == ACT_GLU) {
+    if (x_dt != 1) { set_last_error("norm_fwd_e4m3: GLU mode (act 2) takes bf16 x only"); return MUSE_ERR_UNSUPPORTED; }
+    with_row_chunks<1, 2, 4, 8, 16>(H, [&](auto ch) {
+      constexpr int CH = decltype(ch)::value;
+      pdl_launch(ceil_div(rows, kGluWarps), kGluWarps * 32, 0, s)(
+          glu_norm_fwd_kernel<CH, false, true, uint8_t>, reinterpret_cast<const bf16*>(x), w, qp, mean, rstd, rows, H, eps,
+          rms, philox::ElemDrop{}, row_scale);
+    });
+    return check_launch("glu_norm_fwd_e4m3");
+  }
+  if (act != ACT_NONE || H > 1024) {
+    set_last_error("norm_fwd_e4m3: act %d, H %d (act 0 with H <= 1024, or act 2)", act, H);
+    return MUSE_ERR_UNSUPPORTED;
+  }
+  return dtype_dispatch("norm_fwd_e4m3", [&](auto x_t) {
+    using TX = decltype(x_t);
+    with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+      pdl_launch(ceil_div(rows, kWarpsPerBlock), kWarpsPerBlock * 32, 0, s)(
+          norm_fwd_warp_kernel<TX, uint8_t, decltype(ch)::value, true>, reinterpret_cast<const TX*>(x), w, res, qp, mean,
+          rstd, rows, H, eps, act, rms, row_scale);
+    });
+    return check_launch("norm_fwd_e4m3");
+  }, x_dt);
+}
+
+int muse_norm2_fwd_e4m3(const void* a, const float* res, const float* w1, const float* w2, float* x2, void* q,
+                        float* row_scale, float* mean1, float* rstd1, float* mean2, float* rstd2, int rows, int H, float eps,
+                        int rms1, int rms2, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (rows <= 0) return MUSE_OK;
+  if (H % 8 != 0 || H > 1024 || H < 8) { set_last_error("norm2_fwd_e4m3: H=%d must be a multiple of 8 in [8, 1024]", H); return MUSE_ERR_UNSUPPORTED; }
+  if (q == nullptr || row_scale == nullptr) { set_last_error("norm2_fwd_e4m3: needs q and row_scale"); return MUSE_ERR_INVALID; }
+  with_row_chunks<1, 2, 4>(H, [&](auto ch) {
+    pdl_launch(ceil_div(rows, kWarpsPerBlock), kWarpsPerBlock * 32, 0, s)(
+        norm2_fwd_warp_kernel<decltype(ch)::value, true, uint8_t>, reinterpret_cast<const bf16*>(a), res, w1, w2, x2,
+        reinterpret_cast<uint8_t*>(q), mean1, rstd1, mean2, rstd2, rows, H, eps, rms1, rms2, row_scale);
+  });
+  return check_launch("norm2_fwd_e4m3");
 }
 
 // ws: 2 * norm_bwd_workspace_floats(rows, H, 0) floats (dw2 partial rows, then dw1 partial rows); dw2 / dw1 are STORED.

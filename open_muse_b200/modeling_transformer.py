@@ -164,13 +164,26 @@ class ConvMlmLayer(nn.Module):
 class _PackedWeights:
     """Fused bf16 copies of the Linear weights: [q;k;v] -> [3H,H], [wi_0;wi_1] -> [2I,H], padded
     to_logits -> [Vpad,H] ...  Re-packed (one ``muse_pack_bf16`` launch) whenever a parameter's
-    version counter or storage changes, i.e. once per optimizer step and never during ``generate2``."""
+    version counter or storage changes, i.e. once per optimizer step and never during ``generate2``.
+
+    In FP8 GEMM precision (``MaskGitTransformer.set_gemm_precision``) the layer entries of the FP8 sites (``FP8_SITES``)
+    are ``ops.F8`` copies: the per-output-row e4m3 quantization of the bf16 copies, which stay, as the fused optimizers'
+    destinations (``quantized``: (bf16 copy, F8 copy) while in FP8 precision).  The buffers depend on the parameters'
+    storage only, never on the precision: the bf16 copies are allocated once per storage layout, the F8 copies the first
+    time FP8 precision runs on that layout, and both keep their addresses across precision switches (the F8 copies then
+    stay allocated in bf16 precision too).  Every refresh re-packs and, in FP8 precision, re-quantizes in place, so a
+    captured ``generate2`` graph of either precision stays valid.  A new layout drops the model's captured graphs."""
+
+    FP8_SITES = ("qkv", "cq", "wi", "wo")
 
     def __init__(self, model: "MaskGitTransformer"):
         self.model = model
         self.key = None
         self.layers = []
         self.head = {}
+        self.quantized = []
+        self.buffers_key = None
+        self.bf16_layers, self.fp8_layers, self.f8_pairs = [], None, []
 
     def _plan(self):
         m = self.model
@@ -201,12 +214,18 @@ class _PackedWeights:
         return groups
 
     def _key(self, groups):
-        return tuple((p.data_ptr(), p._version, p.dtype) for _, _, ps, _ in groups for p in ps)
+        return (self.model._gemm_precision,) + tuple((p.data_ptr(), p._version, p.dtype) for _, _, ps, _ in groups for p in ps)
+
+    def _quantize(self):
+        for src, dst in self.quantized:
+            ops.quantize_rows_e4m3(src, out=dst)
 
     def sync(self):
-        """after a fused optimizer step that wrote every packed copy through ``dst_of``: the cache is current, so its key
-        follows the parameters' new version counters (no re-pack on the next forward)"""
+        """after a fused optimizer step that wrote every packed copy through ``dst_of``: the cache is current once the F8
+        copies are re-quantized from the new bf16 copies, so its key follows the parameters' new version counters (no
+        re-pack on the next forward)"""
         if self.key is not None:
+            self._quantize()
             self.key = self._key(self._plan())
 
     def refresh(self):
@@ -217,8 +236,9 @@ class _PackedWeights:
         if key == self.key:
             return self
         dev = params[0].device
-        layout_key = tuple(p.data_ptr() for p in params)
-        if getattr(self, "layout_key", None) != layout_key:
+        fp8 = self.model._gemm_precision == "fp8"
+        buffers_key = tuple(p.data_ptr() for p in params)
+        if self.buffers_key != buffers_key:
             total = 0
             offs = []
             for _, _, ps, rows_pad in groups:
@@ -228,14 +248,15 @@ class _PackedWeights:
                 offs.append((total, rows_alloc, cols))
                 total += ((rows_alloc * cols + 127) // 128) * 128  # keep every group 256B aligned
             self.flat = torch.zeros(total, dtype=torch.bfloat16, device=dev)
-            self.layers = [dict() for _ in m.transformer_layers]
+            self.bf16_layers = [dict() for _ in m.transformer_layers]
+            self.fp8_layers, self.f8_pairs = None, []
             self.head = {}
             entries = []
             block = 0
             self.slow = []  # non-fp32 parameters are copied by torch (inference-only convenience)
             for (li, name, ps, _), (off, rows_alloc, cols) in zip(groups, offs):
                 view = self.flat[off: off + rows_alloc * cols].view(rows_alloc, cols)
-                (self.head if li < 0 else self.layers[li])[name] = view
+                (self.head if li < 0 else self.bf16_layers[li])[name] = view
                 r = 0
                 for p in ps:
                     dst = view[r: r + p.shape[0]]
@@ -248,11 +269,25 @@ class _PackedWeights:
             self.n_entries, self.n_blocks = len(entries), block
             self.dst_of = {e[0]: e[1] for e in entries}  # parameter pointer -> bf16 copy (used by the fused optimizers)
             self.table = torch.tensor(entries, dtype=torch.int64).to(dev) if entries else None
-            self.layout_key = layout_key
+            self.buffers_key = buffers_key
+            m.__dict__.pop("_gen_graphs", None)  # graphs captured on the old buffers must never replay
+        if fp8 and self.fp8_layers is None:
+            self.fp8_layers = [dict(d) for d in self.bf16_layers]
+            for d in self.fp8_layers:
+                for name in self.FP8_SITES:
+                    if name in d:
+                        src = d[name]
+                        d[name] = ops.F8(torch.empty(src.shape, dtype=ops.FP8, device=dev),
+                                         torch.empty(src.shape[0], dtype=torch.float32, device=dev))
+                        self.f8_pairs.append((src, d[name]))
+        self.layers = self.fp8_layers if fp8 else self.bf16_layers
+        self.quantized = self.f8_pairs if fp8 else []
+        self.layout_key = (self.model._gemm_precision,) + buffers_key
         if self.table is not None:
             ops.pack_bf16(self.table, self.n_entries, self.n_blocks)
         for p, dst in self.slow:
             dst.copy_(p.detach())
+        self._quantize()
         self.key = key
         return self
 
@@ -467,6 +502,18 @@ class _EncProjFn(torch.autograd.Function):
         return None, None, None, None, g_proj, g_norm
 
 
+def _act_dtype(w):
+    """dtype of the activation the pass producing a GEMM operand writes: e4m3 rows (ops.FP8) for an F8 weight
+    (set_gemm_precision("fp8")), bf16 otherwise"""
+    return ops.FP8 if isinstance(w, ops.F8) else torch.bfloat16
+
+
+def _act_kw(w, key):
+    """_act_dtype as a keyword, for the passes whose bf16 output is the default of `key`: empty for a bf16 weight"""
+    dt = _act_dtype(w)
+    return {} if dt == torch.bfloat16 else {key: dt}
+
+
 def _layer_body(x, enc, s, params, save, out=True):
     """The forward of one layer: returns (x3, sv).  save=True keeps in sv (and writes the statistics of) every activation
     the backward reads; save=False computes the same x3 with no statistics written.  out=False stops after ml, the last
@@ -484,7 +531,7 @@ def _layer_body(x, enc, s, params, save, out=True):
     H, I, B, S, nh = s.H, s.I, s.B, s.S, s.nh
     sv = {}
     # ---- self attention
-    h1, st1 = ops.norm_fwd(x, _f32(w_attn_ln), s.eps, torch.bfloat16, rms=s.rms, save_stats=save)
+    h1, st1 = ops.norm_fwd(x, _f32(w_attn_ln), s.eps, _act_dtype(s.w["qkv"]), rms=s.rms, save_stats=save)
     qkv = ops.linear_fwd(h1, s.w["qkv"])
     if s.p_attn:
         ctxt, lse, abits = ops.attn_fwd(qkv[:, :H], qkv[:, H:2 * H], qkv[:, 2 * H:], B, nh, S, S, s.scale, head_dim=H // nh,
@@ -496,7 +543,8 @@ def _layer_body(x, enc, s, params, save, out=True):
     h2 = st3 = None
     if fused_norms:
         ao = ops.linear_fwd(ctxt, s.w["ao"])
-        x2, h2, st2 = ops.norm2_fwd(ao, x, _f32(w_post), _f32(w_pre), s.eps, rms1=s.rms, rms2=0, save_stats=save)
+        x2, h2, st2 = ops.norm2_fwd(ao, x, _f32(w_post), _f32(w_pre), s.eps, rms1=s.rms, rms2=0, save_stats=save,
+                                    **_act_kw(s.w["wi"], "h2_dtype"))
     elif s.normformer:
         ao = ops.linear_fwd(ctxt, s.w["ao"])
         x2, st2 = ops.norm_fwd(ao, _f32(w_post), s.eps, torch.float32, res=x, rms=s.rms, save_stats=save)
@@ -507,7 +555,7 @@ def _layer_body(x, enc, s, params, save, out=True):
         sv.update(x=x, h1=h1, st1=st1, qkv=qkv, ctxt=ctxt, lse=lse, ao=ao, st2=st2, x2=x2)
     # ---- cross attention (text conditioning, :886-899)
     if s.cross:
-        hc, stc = ops.norm_fwd(x2, _f32(w_cln), s.eps, torch.bfloat16, rms=s.rms, save_stats=save)
+        hc, stc = ops.norm_fwd(x2, _f32(w_cln), s.eps, _act_dtype(s.w["cq"]), rms=s.rms, save_stats=save)
         qc = ops.linear_fwd(hc, s.w["cq"])
         enc_op = s.enc_op if s.enc_op is not None else enc  # bf16 GEMM operand (enc itself may be the fp32 projection)
         kvc = ops.linear_fwd(enc_op, s.w["ckv"])
@@ -530,7 +578,7 @@ def _layer_body(x, enc, s, params, save, out=True):
             sv["x2b"] = x2b
     # ---- GLU feed-forward (:785-799)
     if h2 is None:
-        h2, st3 = ops.norm_fwd(x2, _f32(w_pre), s.eps, torch.bfloat16, rms=0, save_stats=save)
+        h2, st3 = ops.norm_fwd(x2, _f32(w_pre), s.eps, _act_dtype(s.w["wi"]), rms=0, save_stats=save)
     ab = ops.linear_fwd(h2, s.w["wi"])
     # FeedForward.dropout (:797) is fused into the pass that writes ml: ml is then the dropped wo operand (which is
     # also what the wo weight gradient reads), and the keep bits are saved for the backward
@@ -539,12 +587,12 @@ def _layer_body(x, enc, s, params, save, out=True):
         ml, st4, sv["fbits"] = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms,
                                             save_stats=save, dropout=ffn_drop)
     elif s.normformer:  # GLU product + mid_mlp_layer_norm in one pass; gelu(a)*b is never written to HBM
-        ml, st4 = ops.norm_fwd(ab, _f32(w_mid), s.eps, torch.bfloat16, act=2, rms=s.rms, save_stats=save)
+        ml, st4 = ops.norm_fwd(ab, _f32(w_mid), s.eps, _act_dtype(s.w["wo"]), act=2, rms=s.rms, save_stats=save)
     elif s.p_hidden:
         (ml, sv["fbits"]), st4 = ops.glu_fwd(ab, dropout=ffn_drop), None
     else:
-        ml, st4 = ops.glu_fwd(ab), None
-    x3 = ops.linear_fwd(ml, s.w["wo"], res=x2) if out else None
+        ml, st4 = ops.glu_fwd(ab, **_act_kw(s.w["wo"], "out_dtype")), None
+    x3 = ops.linear_fwd(ml, s.w["wo"], res=x2) if out else None  # an F8 ml: res + bf16(ml @ wo^T) in the FP8 epilogue
     if save:
         sv.update(h2=h2, st3=st3, ab=ab, ml=ml, st4=st4, fused_norms=fused_norms)
     return x3, sv
@@ -873,6 +921,7 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
             self.to_logits = nn.Linear(hidden_size, self.output_size, bias=use_bias)
         self.gradient_checkpointing = False
         self.apply(self._init_weights)
+        self._gemm_precision = "bf16"
         self._packed = _PackedWeights(self)
 
     def _init_weights(self, module):
@@ -889,6 +938,38 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
 
     def _set_gradient_checkpointing(self, module, value=False):
         self.gradient_checkpointing = True  # (reference quirk Q6: ``value`` is ignored)
+
+    # ------------------------------------------------------------------ GEMM precision
+    def set_gemm_precision(self, mode: str):
+        """"bf16" (default: the reference's autocast recipe) or "fp8": inference only -- forward under torch.no_grad() in
+        eval mode, and generate2 -- with the e4m3 tensor cores for each layer's [q;k;v], cross-attention q, [wi_0;wi_1]
+        and wo GEMMs (wo with its residual add fused into the FP8 epilogue).  Their activations come out of the norm / GLU
+        passes that produce them as e4m3 with one scale per row, the weights are quantized per output row; every other
+        GEMM stays bf16 (DESIGN.md section 5).  Not a config key: save_pretrained / from_pretrained do not see it.
+        "fp8" needs hidden_size and intermediate_size to be multiples of 16 (the e4m3 rows are fed by TMA, whose row
+        pitches are multiples of 16 bytes), hidden_size <= 1024 (the warp-per-row norm passes) and intermediate_size <=
+        4096 (the GLU + mid-norm pass holds the row in registers)."""
+        if mode not in ("bf16", "fp8"):
+            raise ValueError(f"gemm precision must be 'bf16' or 'fp8', got {mode!r}")
+        H, I = self.hidden_size, self.intermediate_size
+        if mode == "fp8":
+            bad = {k: v for k, v in dict(hidden_size=H, intermediate_size=I).items() if v % 16}
+            if bad:
+                raise ValueError(f"gemm precision 'fp8' needs widths that are multiples of 16, got {bad}")
+            if H > 1024 or I > 4096:
+                raise ValueError(f"gemm precision 'fp8' needs hidden_size <= 1024 and intermediate_size <= 4096, got "
+                                 f"{H} and {I}")
+        self._gemm_precision = mode  # part of the operand cache key: the next forward rebuilds the operands
+        return self
+
+    @property
+    def gemm_precision(self) -> str:
+        return self._gemm_precision
+
+    def _check_fp8_inference(self):
+        if self._gemm_precision == "fp8" and (self.training or torch.is_grad_enabled()):
+            raise RuntimeError("MaskGitTransformer in FP8 GEMM precision is inference only: call model.eval() and run under "
+                               "torch.no_grad(), or set_gemm_precision('bf16') to train")
 
     # ------------------------------------------------------------------ parameter lists (Function order)
     def _layer_params(self, layer):
@@ -939,6 +1020,7 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
             raise TypeError("encoder_attention_mask is not supported (it raises in the reference too: quirk Q2)")
         if not input_ids.is_cuda:
             raise RuntimeError("open_muse_b200.MaskGitTransformer runs on CUDA (sm_90a) only; move inputs to the GPU")
+        self._check_fp8_inference()
         B, S = input_ids.shape
         if _CHECK_IDS:  # debug switch (MUSE_B200_CHECK_IDS=1): torch raises a device assert on out-of-range ids / labels,
             # the kernels clamp silently -- this host-side check (one sync) catches class-offset / vocab mix-ups
@@ -1127,7 +1209,7 @@ class MaskGitTransformer(ModelMixin, ConfigMixin):
         packed = self._packed.refresh()  # outside the graph: replays must see the current weights in the same buffers
         key = (tuple((tuple(a.shape), a.dtype, a.device) if a is not None else None for a in args), sched,
                None if generator is None else id(generator), getattr(packed, "layout_key", None),
-               torch.is_autocast_enabled("cuda"))
+               torch.is_autocast_enabled("cuda"), self._gemm_precision)
         cache = self.__dict__.setdefault("_gen_graphs", {})
         entry = cache.get(key)
         if entry is None:

@@ -148,6 +148,20 @@ def gemm_fp8(a: F8, b: F8, c, M, N, K, lda, ldb, ldc):
     return c
 
 
+def gemm_fp8_res(a: F8, b: F8, res, c, M, N, K, lda, ldb, ldc):
+    """c fp32 [M,N] = res + bf16((a.q * a.s[:, None]) @ (b.q * b.s[:, None])^T): gemm_fp8 with the residual add of
+    EPI_RESADD_F32 fused into its epilogue (res and c fp32 with pitch ldc)."""
+    st = _prep(c)
+    if _prof["on"]:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    _call("muse_gemm_fp8_res", _p(a.q), _p(a.s), _p(b.q), _p(b.s), _p(res), _p(c), M, N, K, lda, ldb, ldc, st)
+    if _prof["on"]:
+        e1.record()
+        _prof["events"].append((e0, e1, 2.0 * M * N * K))
+    return c
+
+
 def quantize_rows_e4m3(x, out: F8 | None = None) -> F8:
     """bf16 [rows, K] -> F8 with one scale per row (the FP8 weight operands); out: an F8 of the same shape to refresh in
     place (graph-capturable)."""
@@ -160,13 +174,16 @@ def quantize_rows_e4m3(x, out: F8 | None = None) -> F8:
 
 
 def linear_fwd(x, w, out_dtype=torch.bfloat16, res=None, n_valid=None):
-    """y[T,N] = x[T,K] @ w[N,K]^T.  res (fp32 [T,N]) selects the fused residual epilogue.  x and w both F8: the FP8
-    GEMM (bf16 output, no residual)."""
+    """y[T,N] = x[T,K] @ w[N,K]^T.  res (fp32 [T,N]) selects the fused residual epilogue (fp32 output).  x and w both
+    F8: the FP8 GEMM, with a bf16 output, or with res the fp32 output res + bf16(x @ w^T)."""
     if isinstance(x, F8):
-        if not isinstance(w, F8) or res is not None or out_dtype != torch.bfloat16:
-            raise TypeError("linear_fwd: an F8 activation needs an F8 weight, a bf16 output and no residual")
+        if not isinstance(w, F8) or (res is None and out_dtype != torch.bfloat16):
+            raise TypeError("linear_fwd: an F8 activation needs an F8 weight, and a bf16 output without a residual")
         T, K = x.q.shape
         N = w.q.shape[0] if n_valid is None else n_valid
+        if res is not None:
+            y = torch.empty(T, N, dtype=torch.float32, device=x.q.device)
+            return gemm_fp8_res(x, w, res, y, T, N, K, x.q.stride(0), w.q.stride(0), N)
         y = torch.empty(T, N, dtype=torch.bfloat16, device=x.q.device)
         return gemm_fp8(x, w, y, T, N, K, x.q.stride(0), w.q.stride(0), N)
     T, K = x.shape
@@ -288,16 +305,25 @@ def embed_bwd_det(ids, dx, vocab, n_pos):
 def norm_fwd(x, w, eps, out_dtype, res=None, act=0, rms=0, save_stats=True, dropout=None):
     """act: 0 none, 1 GELU(x) first, 2 GLU (x is [rows, 2H] = [a | b], the normalised value is gelu(a) * b).
     dropout = (p, seed, site), act 2 with bf16 x and y only: FeedForward.dropout fused into the pass (the output is the
-    dropped one); then returns (y, stats, bits) with bits int32 [rows, ceil(H / 32)] for norm_bwd (see dropout_fwd)."""
+    dropped one); then returns (y, stats, bits) with bits int32 [rows, ceil(H / 32)] for norm_bwd (see dropout_fwd).
+    out_dtype FP8: y is an F8, the A operand of the FP8 GEMMs (act 0 with H <= 1024, or act 2 with H <= 4096; no
+    dropout)."""
     st = _prep(x)
     rows = x.shape[0]
     H = x.shape[1] // 2 if act == 2 else x.shape[1]
-    y = torch.empty(rows, H, dtype=out_dtype, device=x.device)
     if save_stats:
         stats = torch.empty(2, rows, dtype=torch.float32, device=x.device)
         mean, rstd = stats[0], stats[1]
     else:
         stats = mean = rstd = None
+    if out_dtype == FP8:
+        if dropout is not None:
+            raise TypeError("norm_fwd: the e4m3 output takes no dropout")
+        y, scale = _new_out(rows, H, FP8, x.device)
+        _call("muse_norm_fwd_e4m3", _p(x), _dt(x), _p(w), _p(res), _p(y.q), _p(scale), _p(mean), _p(rstd), rows, H,
+              float(eps), act, rms, st)
+        return y, stats
+    y = torch.empty(rows, H, dtype=out_dtype, device=x.device)
     if dropout is not None:
         assert act == 2 and x.dtype == torch.bfloat16 and out_dtype == torch.bfloat16 and res is None
     bits, seed, site, p = _drop_fwd_args(dropout, x.device, rows, cols=H)
@@ -350,14 +376,20 @@ def norm_bwd(dy, x, w, stats, dx_dtype, dw=None, dres=None, act=0, rms=0, y_fwd=
     return (dx, dw) if want_dw else dx
 
 
-def norm2_fwd(a, res, w1, w2, eps, rms1=0, rms2=0, save_stats=True):
-    """x2 = res + norm1(a) * w1 (fp32), h2 = norm2(x2) * w2 (bf16) in one pass; stats = [mean1, rstd1, mean2, rstd2]."""
+def norm2_fwd(a, res, w1, w2, eps, rms1=0, rms2=0, save_stats=True, h2_dtype=torch.bfloat16):
+    """x2 = res + norm1(a) * w1 (fp32), h2 = norm2(x2) * w2 (bf16) in one pass; stats = [mean1, rstd1, mean2, rstd2].
+    h2_dtype FP8: h2 is an F8, the A operand of the FP8 GEMM; x2 and stats are the same as the bf16 form's."""
     st = _prep(a)
     rows, H = a.shape
     x2 = torch.empty(rows, H, dtype=torch.float32, device=a.device)
-    h2 = torch.empty(rows, H, dtype=torch.bfloat16, device=a.device)
     stats = torch.empty(4, rows, dtype=torch.float32, device=a.device) if save_stats else None
     sp = [None] * 4 if stats is None else [stats[i] for i in range(4)]
+    if h2_dtype == FP8:
+        h2, scale = _new_out(rows, H, FP8, a.device)
+        _call("muse_norm2_fwd_e4m3", _p(a), _p(res), _p(w1), _p(w2), _p(x2), _p(h2.q), _p(scale), _p(sp[0]), _p(sp[1]),
+              _p(sp[2]), _p(sp[3]), rows, H, float(eps), int(rms1), int(rms2), st)
+        return x2, h2, stats
+    h2 = torch.empty(rows, H, dtype=torch.bfloat16, device=a.device)
     _call("muse_norm2_fwd", _p(a), _p(res), _p(w1), _p(w2), _p(x2), _p(h2), _p(sp[0]), _p(sp[1]), _p(sp[2]), _p(sp[3]), rows, H,
           float(eps), int(rms1), int(rms2), st)
     return x2, h2, stats
